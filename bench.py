@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — DQN training steps/sec (batch 32, 84x84x4 uint8 states) on N B200s, beside the CPU
+"""bench.py — DQN training steps/sec (batch 32, 84x84x4 uint8 states) on N H100s, beside the CPU
 restatement of the reference path (BASELINE.json metric).
 
 One "step" = one ReplayMemory.getMinibatch() + one DeepQNetwork.train()
@@ -8,14 +8,20 @@ replay 1M x 84x84 u8 (7.06 GB ring in HBM, a 10k-frame random block tiled), batc
 A = 4, terminals ~ Bernoulli(0.005), random.seed(1), Xavier weights (RandomState(1)).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--math fp32|tcgen05]
+                  [--dump-outputs DIR]
 
-N > 1 is launched by the driver through torch.distributed.run (one rank per GPU, NCCL).  Rank 0
+N > 1 is launched through torch.distributed.run (one rank per GPU, NCCL).  Rank 0
 prints ONE JSON line.  `value` times the fused device path with inputs resident in HBM; `e2e`
 times the public drop-in classes from HOST buffers (frames appended with mem.add, the host `random`
 kept in lock-step, cost delivered to the callback inside train()); `roofline` comes from the in-graph
 %globaltimer timeline of the production graph (208 profiled steps regardless of --steps) with the
 replay-gather HBM fraction and the conv-stack tensor fraction as first-class fields;
 `predict_latency` times the agent's action selection — see DESIGN.md §6.
+
+--dump-outputs DIR writes, right after the K timed steps, what the last timed step computed for its caller: the
+step's cost (cost.npy) and the online network's weights and RMSProp state after its update (W0..W4.npy,
+S0..S4.npy), float32.  Frames, replay metadata, initial weights and the sampling stream are all seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -61,12 +67,31 @@ def synthetic_meta(size):
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return dict(hbm_gbs=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained"),
-                    source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): HBM3 bandwidth and dense FP16 tensor rate.  A data-sheet ceiling,
+    # not a measured one: a card run at a lower power limit clocks lower under sustained load.
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=None, source="H100 SXM data sheet (dense fp16)")
+
+
+def gpu_identity(index):
+    """Name, power limit and max SM clock of the card the numbers were measured on (read-only nvidia-smi query)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits",
+                              "-i", str(index)], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clock = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(power), "sm_max_mhz": float(clock)}
+    except (OSError, ValueError, subprocess.SubprocessError):
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "sm_max_mhz": None}
+
+
+def dump_outputs(out_dir, net):
+    """What the last timed step returned to its caller: its cost and the updated online weights + optimizer state."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "cost.npy"), net.last_costs(1).astype(np.float32))
+    ws, ss = net.get_weights()
+    for i, (w, s) in enumerate(zip(ws, ss)):
+        np.save(os.path.join(out_dir, "W%d.npy" % i), np.ascontiguousarray(w, dtype=np.float32))
+        np.save(os.path.join(out_dir, "S%d.npy" % i), np.ascontiguousarray(s, dtype=np.float32))
 
 
 class ClockSampler:
@@ -190,7 +215,7 @@ def workload_config(a, world, comm="NCCL grad all-reduce"):
 # ------------------------------------------------------------------------------------------ GPU arm
 def kernel_model(label, nb, world=1):
     """(bound, algorithmic bytes, algorithmic flops) of one launch of kernel `label` (DESIGN.md §4 kernel table).
-    bound: "tensor" (GEMM-shaped, tcgen05), "hbm" (bytes that must move; L2-resident ones are marked in DESIGN),
+    bound: "tensor" (GEMM-shaped, wgmma), "hbm" (bytes that must move; L2-resident ones are marked in DESIGN),
     "nvlink" (peer stores), "latency" (a few hundred bytes of work: the launch itself is the cost)."""
     f = lambda macs, nets=1: 2.0 * macs * nb * nets
     n_fc1, A = 3136 * 512, NUM_ACTIONS
@@ -325,6 +350,8 @@ def run_b200(a, rank, world, local_rank):
     cost_tail = net.last_costs(min(a.steps, 8))
     assert np.isfinite(cost_tail).all(), cost_tail
     launches = net.launches_per_step() * a.steps
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, net)
 
     # ---- roofline: the in-graph timeline of the production step (same graph, PDL and branches as `value`)
     barrier()
@@ -344,7 +371,7 @@ def run_b200(a, rank, world, local_rank):
     tp = os.path.join(ROOT, "profiles", "ncu_traffic.json")     # dram bytes per launch from the committed ncu capture
     if os.path.exists(tp):
         roof["traffic"] = json.load(open(tp)).get(a.math, {}).get(top)
-    roof["peak_source"] = pk["source"] + ", sustained bf16 figure (kernel timed inside a long step)"
+    roof["peak_source"] = pk["source"] + " (kernel timed inside a long step)"
     roof["us_per_launch"] = dur[top]
     roof["share_of_step"] = dur[top] / span_us if span_us else None
     roof["how"] = ("in-graph %globaltimer timeline of the replayed production graph (first CTA start .. last CTA end, "
@@ -405,7 +432,7 @@ def run_b200(a, rank, world, local_rank):
     costs = []
     net.callback = types.SimpleNamespace(on_train=lambda c: costs.append(c))
     frames = [np.ascontiguousarray(base[i]) for i in range(64)]
-    e2e_steps = max(300, min(a.steps, 1000))          # a fixed floor: the driver runs --steps 20
+    e2e_steps = a.steps
 
     def e2e_loop(n):
         for i in range(n):
@@ -454,11 +481,11 @@ def run_b200(a, rank, world, local_rank):
                                                         "one-shot all-reduce for conv1-3/fc2; comm_p2p.cuh)"
                                                         % os.environ.get("B200DQN_P2P_SCHED", "gather"),
                                                  "nccl": "NCCL grad all-reduce"}.get(comm_mode, comm_mode)),
-            "comm_healthy": bool(comm_ok), "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
+            "gpu": gpu_identity(dev), "comm_healthy": bool(comm_ok), "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
             "roofline": roof, "predict_latency": pred, "last_costs": [float(c) for c in cost_tail]}
     if world > 1:
         line["config"]["global_updates_per_s"] = a.steps / (ms_total * 1e-3)
-        # NVLink bytes each rank SENDS per step (SURVEY §8e asks for the fraction of 770 GB/s per direction)
+        # NVLink bytes each rank SENDS per step, as a fraction of H100 SXM NVLink 4 (450 GB/s per direction)
         n_params = 1683456 + 512 * NUM_ACTIONS
         small = n_params - 3136 * 512                           # conv1..3 + fc2, floats
         if comm_mode == "p2p" and os.environ.get("B200DQN_P2P_SCHED", "gather") == "gather":
@@ -470,7 +497,7 @@ def run_b200(a, rank, world, local_rank):
             how = "reduce-scatter + all-gather of the 6.74 MB gradient"
         gbs = sent / (ms_total / a.steps * 1e-3) / 1e9
         line["nvlink"] = {"sent_bytes_per_step_per_rank": int(sent), "what": how, "GBps_per_rank": gbs,
-                          "frac_of_770GBps_per_dir": gbs / 770.0}
+                          "frac_of_450GBps_per_dir": gbs / 450.0}
     if world == 1 and not a.no_cpu:
         cb, _, _ = cpu_arm(10 ** 9, 3, a.replay, a.batch, max_seconds=a.cpu_seconds)
         line["cpu_baseline"] = cb
@@ -488,14 +515,14 @@ def main():
     ap.add_argument("--replay", type=int, default=1_000_000)
     ap.add_argument("--cpu-seconds", type=float, default=12.0)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32)")
     a = ap.parse_args()
     assert a.warmup >= 3, "timing rules: at least 3 warm-up steps"
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     if a.impl == "reference":
-        if a.steps > 5000:
-            a.steps = 5000
         return run_reference(a, rank, world)
     run_b200(a, rank, world, local_rank)
 

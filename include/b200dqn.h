@@ -1,5 +1,5 @@
 /*
- * b200dqn.h — C-ABI of libb200dqn.so: the B200-native (sm_100a) replay-and-train hot path
+ * b200dqn.h — C-ABI of libb200dqn.so: the H100-native (sm_90a) replay-and-train hot path
  * behind tambetm/simple_dqn's ReplayMemory / DeepQNetwork / StateBuffer call surface.
  *
  * The reference has no FFI of its own (it is pure Python calling Neon); the boundary is the
@@ -41,7 +41,7 @@ enum {
 /* math_mode of b200dqn_net_config */
 enum {
   B200DQN_MATH_FP32_SIMT = 0, /* CUDA-core fp32 FFMA implicit GEMM: exact-fp32 reference mode          */
-  B200DQN_MATH_TCGEN05 = 1    /* tcgen05.mma kind::f16, fp16 hi/lo split operands (3 MMAs), fp32 TMEM */
+  B200DQN_MATH_TCGEN05 = 1    /* wgmma fp16 hi/lo split operands (3 MMAs), fp32 accumulate    */
 };
 
 /* optimizer of b200dqn_net_config — src/deepqnetwork.py:50-61 (--optimizer rmsprop|adam|adadelta, main.py:40) */
@@ -280,7 +280,7 @@ enum {
   B200DQN_NET_PTR_H4            /* (batch,512)                                                         */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
-/* The fused optimizers of the tcgen05 engine never materialise dW4; ask them to keep a copy (tests,
+/* The fused optimizers of the tensor-core engine never materialise dW4; ask them to keep a copy (tests,
  * debugging) before the step whose gradients b200dqn_net_get_grads should return. */
 int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
@@ -288,7 +288,7 @@ int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* strea
 /* Number of kernels one fused train step launches (bench.py's gpu_launches). */
 int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches);
 
-/* Developer aid: clock64() stamps written by CTA (0,0,0) of the tcgen05 kernel whose label equals
+/* Developer aid: clock64() stamps written by CTA (0,0,0) of the tensor-core kernel whose label equals
  * $B200DQN_TRACE_LABEL (slots documented in csrc/umma2.cuh).  Returns the number of slots or -1. */
 int b200dqn_debug_trace(unsigned long long* host_out, int n);
 

@@ -1,4 +1,4 @@
-"""simple_dqn_b200 — the B200-native (sm_100a) replay-and-train hot path behind the call
+"""simple_dqn_b200 — the H100-native (sm_90a) replay-and-train hot path behind the call
 surface of tambetm/simple_dqn's ReplayMemory / DeepQNetwork / StateBuffer.
 
 Importing the package is cheap; the CUDA library is loaded on first use and there is no CPU

@@ -118,7 +118,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             "simple_dqn_b200: %s is missing — build it with `python -m simple_dqn_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback." % LIB_PATH)
+            "(nvcc, sm_90a).  There is no CPU fallback." % LIB_PATH)
     lib = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     lib.b200dqn_last_error.restype = C.c_char_p
     lib.b200dqn_last_error.argtypes = []

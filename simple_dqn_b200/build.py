@@ -1,14 +1,18 @@
-"""In-tree build of libb200dqn.so (nvcc, sm_100a only).  Run: python -m simple_dqn_b200.build"""
+"""In-tree build of libb200dqn.so (nvcc, sm_90a only).  Run: python -m simple_dqn_b200.build"""
 import os
+import shutil
 import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200dqn.so")
+# nvcc from PATH, else from the CUDA toolkit (CUDA_HOME, default /usr/local/cuda)
+NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
 SOURCES = ["capi.cu", "replay.cu", "net.cu", "net_umma.cu", "comm.cu"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-         "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
+                "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
 def _stale():
@@ -21,7 +25,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every CUDA source for sm_100a into simple_dqn_b200/libb200dqn.so."""
+    """Compile every CUDA source for sm_90a into simple_dqn_b200/libb200dqn.so."""
     if not force and not _stale():
         return LIB
     objs = []
@@ -29,7 +33,7 @@ def build(force=False, verbose=False):
     os.makedirs(os.path.join(HERE, "build"), exist_ok=True)
     for src in SOURCES:
         obj = os.path.join(HERE, "build", src.replace(".cu", ".o"))
-        cmd = ["nvcc"] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
+        cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
         objs.append(obj)
     failed = False
@@ -40,7 +44,7 @@ def build(force=False, verbose=False):
         failed |= p.returncode != 0
     if failed:
         raise RuntimeError("nvcc failed")
-    cmd = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + ["-ldl"]
+    cmd = [NVCC] + ARCH + ["-shared", "-o", LIB] + objs + ["-ldl"]
     subprocess.check_call(cmd)
     return LIB
 

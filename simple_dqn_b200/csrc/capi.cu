@@ -170,8 +170,8 @@ extern "C" int b200dqn_device_info(int device, int* sm_count, int* cc_major, int
   B2_CHECK_CUDA(cudaMemGetInfo(&f, &t));
   if (free_bytes) *free_bytes = f;
   if (total_bytes) *total_bytes = t;
-  B2_REQUIRE(prop.major == 10, B200DQN_ECUDA,
-             "device %d is sm_%d%d; libb200dqn.so is built for sm_100a (B200) only", device, prop.major, prop.minor);
+  B2_REQUIRE(prop.major == 9 && prop.minor == 0, B200DQN_ECUDA,
+             "device %d is sm_%d%d; libb200dqn.so is built for sm_90a (H100) only", device, prop.major, prop.minor);
   return B200DQN_OK;
 }
 

@@ -89,8 +89,8 @@ int comm_xchg_range(b200dqn_net* n, int l0, int l1, int chan, cudaStream_t st, c
 constexpr int kXCounterWords = kXChannels * kXMaxBlocks + 1 + 2 * kXChannels + 2 * kXPushChannels + 1;
 
 // B200DQN_HEAD_PUSH=1: the head kernel pushes its dZ4 rows itself (counted arrivals).  OFF by default: parity-clean
-// (tests/test_gpu_multi.py) but MEASURED SLOWER on 2 x B200 — 101 vs 92 us/step: the system-scope fence in front of
-// the arrival counter keeps every head CTA ~15 us on the critical chain (profiles/r2m2_*).
+// (tests/test_gpu_multi.py) but measured slower on two GPUs of an earlier generation (not re-measured on H100): the
+// system-scope fence in front of the arrival counter keeps every head CTA on the critical chain.
 bool comm_head_push(const b200dqn_net* n, cudaStream_t st, HeadPush* out) {
   static const bool enabled = getenv("B200DQN_HEAD_PUSH") && atoi(getenv("B200DQN_HEAD_PUSH")) != 0;
   if (!enabled || !comm_gather_active(n, st)) return false;

@@ -1,5 +1,5 @@
 // common.cuh — error plumbing and small PTX helpers shared by every translation unit of
-// libb200dqn.so (sm_100a only).
+// libb200dqn.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -111,11 +111,10 @@ struct NoPdlScope {
 
 // B200DQN_CARVEOUT=1 (experiment, off by default): every kernel of the library asks for the LARGEST shared-memory
 // carveout, including the ones that use no shared memory at all.  The L1/shared split is an SM-wide setting that can
-// only change while the SM is idle: a streaming kernel (fc1 optimizer: 296 CTAs, 1 KB of shared memory) that configures
-// an SM for "mostly L1" locks the tcgen05 kernels (81-193 KB per CTA) out of that SM until its CTAs have left.
-// Measured (profiles/r2q_periods.txt): with the optimizer at the head of the step (B200DQN_DEFER_FC1=1) one carveout
-// for all kernels lets conv1 start at once (83.2 -> 75.9 us per step); in the default schedule, where the optimizer
-// starts under kernels that have already claimed their SMs, it costs 1.2 us (71.7 -> 72.9), hence off.
+// only change while the SM is idle: a streaming kernel (fc1 optimizer: 1 KB of shared memory per CTA) that configures
+// an SM for "mostly L1" locks the tensor-core kernels (81-193 KB per CTA) out of that SM until its CTAs have left.
+// It helps when the optimizer runs at the head of the step (B200DQN_DEFER_FC1=1) and cost time in the default schedule
+// where it was measured (an earlier GPU generation), hence off; not re-measured on H100.
 void prefer_max_smem_carveout(const void* kernel);   // capi.cu; once per kernel
 template <class K>
 static inline void prefer_max_smem(K* kernel) { prefer_max_smem_carveout(reinterpret_cast<const void*>(kernel)); }
@@ -209,7 +208,7 @@ __device__ __forceinline__ void tma_bulk_wait_read_all() {
 // Programmatic dependent launch: a kernel launched with the programmatic-stream-serialization
 // attribute may begin while its predecessor is still running; pdl_wait() blocks until every
 // prerequisite grid has completed and flushed (no-op without the attribute), pdl_launch_dependents()
-// lets the successor start its own prologue (TMEM alloc, barrier init, index setup) early.
+// lets the successor start its own prologue (barrier init, index setup) early.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // ---- thread-block cluster helpers (split-K partners)
@@ -231,7 +230,7 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr) {
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
-// generic-proxy writes -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }

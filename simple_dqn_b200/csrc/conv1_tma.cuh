@@ -9,12 +9,12 @@
 //   * 8 warps turn the window into the canonical K-major SWIZZLE_128B fp16 tiles of the implicit GEMM (u8 -> fp16
 //     is exact: no lo plane), one [128 pixels x 64 taps] tile per FRAME; a frame shared by both networks is
 //     converted once and multiplied by both networks' weights (online k-block f, target k-block f-1);
-//   * a ninth warp issues tcgen05.mma (M = 128, N = 64 = [W_hi ; W_lo] in one instruction) as tiles become ready;
-//     accumulators of both networks live in TMEM; the epilogue applies 1/255 (the reference's _setInput divide,
+//   * the same two warpgroups issue wgmma (M = 64 per warpgroup, N = 64 = [W_hi ; W_lo] in one instruction) as tiles
+//     become ready; accumulators of both networks live in registers; the epilogue applies 1/255 (the _setInput divide,
 //     src/deepqnetwork.py:100) and Rectlin and writes fp32 + fp16 hi/lo planes;
 //   * the online network's tiles are also shipped to the im2col image conv1_wgrad reads (TMA bulk store).
 //
-// Tiling: one CTA = 5 output rows x 20 columns = 100 pixels of one sample (a 128-row UMMA tile, 100 live rows);
+// Tiling: one CTA = 5 output rows x 20 columns = 100 pixels of one sample (a 128-row tile, 100 live rows);
 // grid = 4 x samples.  Shared memory: the window(s) (12 KB each) + a 3-stage ring of [A tile 16 KB | weight tiles
 // 2 x 8 KB] = 109 KB, so two CTAs share an SM and the next kernels of the PDL chain can still pre-launch.
 #pragma once
@@ -35,7 +35,6 @@ constexpr uint32_t kWTile = 64 * 128;           // [32 hi rows ; 32 lo rows] x 6
 constexpr int kRing = 3;                        // stages: one frame's A tile + the (<= 2) weight tiles that multiply it
 constexpr uint32_t kStage = kATile + 2 * kWTile;   // 32 KB
 constexpr uint32_t kBoxStride = 12288;          // one window (<= 5 frames x 2352 B), 128-byte aligned
-constexpr uint32_t kTmemCols = 128;             // 2 networks x [acc_hi | acc_lo] x 32 channels
 // 109 KB with one window (ring train / predict): two CTAs per SM, and successor kernels of the PDL chain still find
 // room to pre-launch; 121 KB with two windows (staged states)
 static inline uint32_t smem_bytes(int windows) { return kRing * kStage + uint32_t(windows) * kBoxStride + 1024; }
@@ -80,13 +79,10 @@ k_conv1_tma(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CU
             const KTrace kt) {
   using umma2::kLoadThreads;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t s_tmem;
   __shared__ __align__(8) uint64_t s_box[2];          // windows have landed
   __shared__ __align__(8) uint64_t s_full[kRing];     // A tile converted + weight tiles landed
-  __shared__ __align__(8) uint64_t s_empty[kRing];    // the MMAs (and the im2col store) that read the stage are done
-  __shared__ __align__(8) uint64_t s_done;            // all MMAs complete
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int n = blockIdx.x / kTilesPerSample, t = blockIdx.x % kTilesPerSample;
   kt_begin(kt);
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -97,22 +93,14 @@ k_conv1_tma(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CU
   const int box_frames = (nets == 2 && p.shared5) ? kHist + 1 : kHist;
   const int nslots = nboxes * box_frames;          // 4 (predict), 5 (ring train), 8 (staged train)
 
-  if (warp == 8) umma::tmem_alloc(&s_tmem, kTmemCols);
-  if (tid == 32) {
+  if (tid == 0) {
     mbar_init(&s_box[0], 1);
     mbar_init(&s_box[1], 1);
 #pragma unroll
-    for (int s = 0; s < kRing; ++s) {
-      mbar_init(&s_full[s], kLoadThreads + 1);
-      mbar_init(&s_empty[s], 1);
-    }
-    mbar_init(&s_done, 1);
+    for (int s = 0; s < kRing; ++s) mbar_init(&s_full[s], kLoadThreads + 1);
     mbar_fence_init();
   }
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = s_tmem;
 
   // weight tiles of slot j into its stage (thread 0): they do not depend on the predecessor kernel
   auto fetch_weights = [&](int j) {
@@ -139,126 +127,108 @@ k_conv1_tma(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CU
     }
   }
 
-  if (warp == 8) {
-    // ================================================================ MMA issuer
-    constexpr uint32_t idesc = umma::make_idesc_f16(128, 64);
-    for (int j = 0; j < nslots; ++j) {
-      const int s = j % kRing, b = j / box_frames, f = j % box_frames;
-      mbar_wait(&s_full[s], (j / kRing) & 1);
-      fence_proxy_async_smem();
-      umma::fence_after_sync();
-      const uint32_t stage = smem_base + s * kStage;
-      const uint64_t da = umma::make_desc_sw128(stage);
-      if (umma2::elect_one()) {
-        bool dumped = false;
-        for (int z = 0; z < nets; ++z) {
-          const int kb = kb_for(p, nets, b, f, z);
-          if (kb < 0) continue;
-          const uint64_t db = umma::make_desc_sw128(stage + kATile + z * kWTile);
+  // chunk (row, r): the 8 taps of filter row r for output pixel `row` = 8 consecutive bytes of window row 4*pl + r
+  int src_off[4];
+  uint32_t dst_off[4];
+  bool live[4];
 #pragma unroll
-          for (int k = 0; k < 4; ++k) umma::mma_f16(tmem + z * 64, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          if (z == 0 && p.im2col) {   // the online network's tile IS conv1_wgrad's MN-major A operand
-            tma_bulk_s2g(p.im2col + (int64_t(blockIdx.x) * 4 + kb) * kATile, smem_gen + s * kStage, kATile);
-            tma_bulk_commit();
-            dumped = true;
-          }
-        }
-        if (j + kRing < nslots && dumped) tma_bulk_wait_read_all();   // the stage is about to be overwritten
-        umma::mma_commit(&s_empty[s]);
-        if (j == nslots - 1) {
-          umma::mma_commit(&s_done);
-          if (p.im2col) tma_bulk_wait_read_all();
-        }
-      }
-      __syncwarp();
+  for (int i = 0; i < 4; ++i) {
+    const int id = tid + i * kLoadThreads;
+    const int row = id >> 3, r = id & 7;
+    const int pl = row / 20, q = row % 20;
+    live[i] = row < kTileRows;
+    src_off[i] = (4 * pl + r) * kFrameW + 4 * q;
+    dst_off[i] = umma::sw128_off(row, r);
+  }
+  float acc[2][32];   // per network: the N = 64 fragment [acc_hi (32 channels) | acc_lo (32 channels)]
+#pragma unroll
+  for (int z = 0; z < 2; ++z)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[z][i] = 0.f;
+  for (int j = 0; j < nslots; ++j) {
+    const int s = j % kRing, b = j / box_frames, f = j % box_frames;
+    if (f == 0) mbar_wait(&s_box[b], 0);
+    if (j >= kRing) {
+      // both warpgroups are past the wgmma.wait_group that completed slot j - kRing's MMAs (and thread 0 waited for
+      // its im2col store to read the stage): the stage takes slot j
+      umma2::named_bar_sync(1, kLoadThreads);
+      if (tid == 0) fetch_weights(j);
     }
-  } else {
-    // ================================================================ window -> fp16 tiles (8 warps), then epilogue
-    // chunk (row, r): the 8 taps of filter row r for output pixel `row` = 8 consecutive bytes of window row 4*pl + r
-    int src_off[4];
-    uint32_t dst_off[4];
-    bool live[4];
+    // ---- window -> fp16 tile (all 8 warps)
+    const uint8_t* win = smem_gen + (box_base - smem_base) + b * kBoxStride + f * kFrameBoxBytes;
+    uint8_t* tile = smem_gen + s * kStage;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int id = tid + i * kLoadThreads;
-      const int row = id >> 3, r = id & 7;
-      const int pl = row / 20, q = row % 20;
-      live[i] = row < kTileRows;
-      src_off[i] = (4 * pl + r) * kFrameW + 4 * q;
-      dst_off[i] = umma::sw128_off(row, r);
+      uint4 hi = make_uint4(0u, 0u, 0u, 0u);
+      if (live[i]) {
+        const uint32_t x = *reinterpret_cast<const uint32_t*>(win + src_off[i]);
+        const uint32_t y = *reinterpret_cast<const uint32_t*>(win + src_off[i] + 4);
+        // u8 -> fp16 is exact: 0x6400 | v is the half 1024 + v; subtract 1024
+        const __half2 k1024 = __half2half2(__ushort_as_half(0x6400));
+        const uint32_t a0 = 0x64006400u | (x & 0xffu) | ((x & 0xff00u) << 8);
+        const uint32_t a1 = 0x64006400u | ((x >> 16) & 0xffu) | ((x >> 8) & 0xff0000u);
+        const uint32_t a2 = 0x64006400u | (y & 0xffu) | ((y & 0xff00u) << 8);
+        const uint32_t a3 = 0x64006400u | ((y >> 16) & 0xffu) | ((y >> 8) & 0xff0000u);
+        __half2 h0 = __hsub2(*reinterpret_cast<const __half2*>(&a0), k1024);
+        __half2 h1 = __hsub2(*reinterpret_cast<const __half2*>(&a1), k1024);
+        __half2 h2 = __hsub2(*reinterpret_cast<const __half2*>(&a2), k1024);
+        __half2 h3 = __hsub2(*reinterpret_cast<const __half2*>(&a3), k1024);
+        hi = make_uint4(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1),
+                        *reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
+      }
+      *reinterpret_cast<uint4*>(tile + dst_off[i]) = hi;
     }
-    for (int j = 0; j < nslots; ++j) {
-      const int s = j % kRing, b = j / box_frames, f = j % box_frames;
-      if (f == 0) mbar_wait(&s_box[b], 0);
-      if (j >= kRing) {
-        mbar_wait(&s_empty[s], ((j / kRing) - 1) & 1);
-        if (tid == 0) fetch_weights(j);
-      }
-      const uint8_t* win = smem_gen + (box_base - smem_base) + b * kBoxStride + f * kFrameBoxBytes;
-      uint8_t* tile = smem_gen + s * kStage;
+    fence_proxy_async_smem();   // st.shared (generic proxy) -> async proxy, writer side
+    mbar_arrive(&s_full[s]);
+    // ---- MMAs of the slot: each warpgroup multiplies its 64 pixel rows by the weights of every network that uses
+    // this frame (M = 64, N = 64 = [W_hi ; W_lo] in one instruction)
+    mbar_wait(&s_full[s], (j / kRing) & 1);
+    fence_proxy_async_smem();
+    const uint32_t stage = smem_base + s * kStage;
+    const uint64_t da = umma::make_desc_sw128(stage + wg * (umma::kWgM * 128));
+    umma::wgmma_fence();
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 hi = make_uint4(0u, 0u, 0u, 0u);
-        if (live[i]) {
-          const uint32_t x = *reinterpret_cast<const uint32_t*>(win + src_off[i]);
-          const uint32_t y = *reinterpret_cast<const uint32_t*>(win + src_off[i] + 4);
-          // u8 -> fp16 is exact: 0x6400 | v is the half 1024 + v; subtract 1024
-          const __half2 k1024 = __half2half2(__ushort_as_half(0x6400));
-          const uint32_t a0 = 0x64006400u | (x & 0xffu) | ((x & 0xff00u) << 8);
-          const uint32_t a1 = 0x64006400u | ((x >> 16) & 0xffu) | ((x >> 8) & 0xff0000u);
-          const uint32_t a2 = 0x64006400u | (y & 0xffu) | ((y & 0xff00u) << 8);
-          const uint32_t a3 = 0x64006400u | ((y >> 16) & 0xffu) | ((y >> 8) & 0xff0000u);
-          __half2 h0 = __hsub2(*reinterpret_cast<const __half2*>(&a0), k1024);
-          __half2 h1 = __hsub2(*reinterpret_cast<const __half2*>(&a1), k1024);
-          __half2 h2 = __hsub2(*reinterpret_cast<const __half2*>(&a2), k1024);
-          __half2 h3 = __hsub2(*reinterpret_cast<const __half2*>(&a3), k1024);
-          hi = make_uint4(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1),
-                          *reinterpret_cast<uint32_t*>(&h2), *reinterpret_cast<uint32_t*>(&h3));
-        }
-        *reinterpret_cast<uint4*>(tile + dst_off[i]) = hi;
-      }
-      fence_proxy_async_smem();   // st.shared (generic proxy) -> async proxy, writer side
-      mbar_arrive(&s_full[s]);
+    for (int z = 0; z < 2; ++z) {
+      const int kb = z < nets ? kb_for(p, nets, b, f, z) : -1;
+      if (kb < 0) continue;
+      const uint64_t db = umma::make_desc_sw128(stage + kATile + z * kWTile);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) umma::wgmma_f16<64>(acc[z], da + 2 * k, db + 2 * k);
     }
-    pdl_launch_dependents();
-
-    // ---- epilogue: thread <-> (pixel row, 16 channels); x 1/255, Rectlin, fp32 + hi/lo planes
-    mbar_wait(&s_done, 0);
-    umma::fence_after_sync();
-    const int q4 = warp & 3, half = warp >> 2;
-    const int row = q4 * 32 + lane;
-    const uint32_t lane_addr = tmem + (uint32_t(q4 * 32) << 16);
-    for (int z = 0; z < nets; ++z) {
-      float a0[2][8], a1[2][8];
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        umma::tmem_ld8(lane_addr + z * 64 + half * 16 + c * 8, a0[c]);
-        umma::tmem_ld8(lane_addr + z * 64 + 32 + half * 16 + c * 8, a1[c]);
-      }
-      umma::tmem_ld_wait();
-      if (row < kTileRows) {
-        const int64_t pix = int64_t(n) * (kP1 * kP1) + t * kTileRows + row;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          float o[8];
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj)
-            o[jj] = fmaxf(fmaf(a1[c][jj], umma::kLoInv, a0[c][jj]) * (1.0f / 255.0f), 0.f);
-          const int64_t e = pix * kC1 + half * 16 + c * 8;
-          if (p.out[z]) {
-            *reinterpret_cast<float4*>(p.out[z] + e) = make_float4(o[0], o[1], o[2], o[3]);
-            *reinterpret_cast<float4*>(p.out[z] + e + 4) = make_float4(o[4], o[5], o[6], o[7]);
-          }
-          umma2::split8_planes(o, p.out16[z] + e, p.out16[z] + p.lo_off + e);
-        }
+    umma::wgmma_commit();
+    if (tid == 0 && p.im2col) {
+      const int kb = kb_for(p, nets, b, f, 0);
+      if (kb >= 0) {   // the online network's tile IS conv1_wgrad's MN-major A operand
+        tma_bulk_s2g(p.im2col + (int64_t(blockIdx.x) * 4 + kb) * kATile, smem_gen + s * kStage, kATile);
+        tma_bulk_commit();
+        if (j + kRing < nslots) tma_bulk_wait_read_all();   // the stage is about to be overwritten
       }
     }
+    umma::wgmma_wait<1>();
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) {
-    umma::fence_after_sync();
-    umma::tmem_dealloc(tmem, kTmemCols);
+  pdl_launch_dependents();
+  if (tid == 0 && p.im2col) tma_bulk_wait_read_all();   // shared memory must outlive the im2col stores' reads
+
+  // ---- epilogue straight from the accumulator fragments: x 1/255, Rectlin, fp32 + hi/lo planes
+  umma::wgmma_wait<0>();
+#pragma unroll
+  for (int z = 0; z < 2; ++z) {
+    if (z >= nets) break;
+#pragma unroll
+    for (int i = 0; i < 16; i += 2) {   // registers [0, 16) = channels 0..31 of acc_hi; acc_lo 16 registers further
+      const int row = wg * umma::kWgM + umma::frag_row(i, lane, warp), c = umma::frag_col(i, lane);
+      if (row < kTileRows) {
+        const float o0 = fmaxf(fmaf(acc[z][16 + i], umma::kLoInv, acc[z][i]) * (1.0f / 255.0f), 0.f);
+        const float o1 = fmaxf(fmaf(acc[z][17 + i], umma::kLoInv, acc[z][i + 1]) * (1.0f / 255.0f), 0.f);
+        const int64_t e = (int64_t(n) * (kP1 * kP1) + t * kTileRows + row) * kC1 + c;
+        if (p.out[z]) *reinterpret_cast<float2*>(p.out[z] + e) = make_float2(o0, o1);
+        const __half2 hh = __floats2half2_rn(o0, o1);
+        const float2 back = __half22float2(hh);
+        *reinterpret_cast<__half2*>(p.out16[z] + e) = hh;
+        *reinterpret_cast<__half2*>(p.out16[z] + p.lo_off + e) =
+            __floats2half2_rn((o0 - back.x) * umma::kLoScale, (o1 - back.y) * umma::kLoScale);
+      }
+    }
   }
   kt_end(kt);
 }

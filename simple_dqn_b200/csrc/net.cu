@@ -36,7 +36,7 @@ struct HeadTrainArgs {
   float* row_cost;    // [rows]
   float* dz4;         // [rows][512]
   float* dw5_rows;    // [rows][512][A] per-row partials of dW5 (summed in row order by the optimizer)
-  __half* dz4_hi;     // fp16 hi / scaled-lo planes of dZ4 for the tcgen05 dgrad (nullptr in fp32 mode)
+  __half* dz4_hi;     // fp16 hi / scaled-lo planes of dZ4 for the tensor-core dgrad (nullptr in fp32 mode)
   int64_t dz4_lo_off;
   float* adam_l;      // Adam only: this step's scalar l = lr*sqrt(1-beta_2^t)/(1-beta_1^t) for the optimizer kernels
   float adam_lr;
@@ -505,11 +505,10 @@ static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
 //   sC   :                               conv2_wgrad .. [after conv2_dgrad] opt(conv2)
 // In a communicator the update follows one all-reduce of the whole gradient, so the simple
 // serial order is kept.
-// Data-parallel schedule (communicator, tcgen05 engine): the fc gradient (95 % of the bytes) is summed and
+// Data-parallel schedule (communicator, tensor-core engine): the fc gradient (95 % of the bytes) is summed and
 // all-reduced as soon as fc1_wgrad is done, hidden behind the dgrad chain; the three small conv gradients
-// share one all-reduce at the tail.  (Measured on 2x B200: one collective at the tail 190 us/step, this
-// two-collective schedule 144 us/step, one collective per layer 166 us/step — small NCCL all-reduces
-// cost ~15-20 us each inside the graph, so fewer is better once the big one is hidden.)  Both collectives run in this order on one dedicated stream (a NCCL
+// share one all-reduce at the tail: small NCCL all-reduces cost ~15-20 us each inside the graph, so fewer is
+// better once the big one is hidden.  (Multi-GPU schedules have not been re-measured on H100.)  Both collectives run in this order on one dedicated stream (a NCCL
 // communicator must not be used from two streams at once); updates read the reduced gradient from d_g.
 // Peer-memory exchange (comm_p2p.cuh): no shared communicator, so every layer's gradient is reduced
 // the moment its wgrad has finished, on that layer's own branch, and only conv1's 32 KB exchange is left
@@ -617,9 +616,9 @@ static int backward_and_update_gather(b200dqn_net* n, const FrameSource& fs, int
   // experimental: one launch per conv layer for reduce + LL exchange + RMSProp (umma_opt_conv_xll), off by default
   // one launch per conv layer for reduce + LL exchange + update (umma_opt_conv_xll): default since it was validated on
   // hardware at W = 2 (tests/test_gpu_multi.py; ~4.5 us per step); B200DQN_FUSED_XLL=0 restores the three launches
-  // Measured: at W = 2 the fused kernel shortens the traced step (87.7 vs 92 us); at W = 8 its 288 polling CTAs per
-  // layer spin for ~20 us while the peers catch up and delay the chain's own kernels (profiles/r2n8_timeline_w8.txt),
-  // so beyond two ranks the default is the three-launch form with its small polling grid.
+  // At W = 2 the fused kernel shortens the step; at W = 8 its polling CTAs spin while the peers catch up and delay the
+  // chain's own kernels, so beyond two ranks the default is the three-launch form with its small polling grid.
+  // (Chosen on an earlier GPU generation; multi-GPU schedules have not been re-measured on H100.)
   static const int fused_env = getenv("B200DQN_FUSED_XLL") ? atoi(getenv("B200DQN_FUSED_XLL")) : -1;
   const bool fused_xll = fused_env >= 0 ? fused_env != 0 : n->world <= 2;
   B2_CHECK_CUDA(cudaEventRecord(ev[0], st));                 // head done: dZ4 planes, dW5 partials
@@ -1412,9 +1411,9 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
       n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
     }
     // B200DQN_DEFER_FC1=1 (experiment, off by default): several steps in one call -> the fc1 update of step t rides under
-    // the forward of step t+1 (net.cuh).  Parity-clean (profiles/r2p_pytest.log) but slower: the 45 MB the update moves
-    // through L2 stretch whatever runs beside it, and the forward convolutions lose more (conv1 9.2 -> 13.9 us) than
-    // the dgrad chain gains; 75.9 (83.2 with the driver's carveouts) vs 71.7 us per step.
+    // the forward of step t+1 (net.cuh).  Parity-clean but slower where it was measured (an earlier GPU generation):
+    // the 45 MB the update moves through L2 stretch whatever runs beside it, and the forward convolutions lose more
+    // than the dgrad chain gains.  Not re-measured on H100.
     static const bool defer_on = getenv("B200DQN_DEFER_FC1") && atoi(getenv("B200DQN_DEFER_FC1")) != 0;
     const bool deferred = nsteps >= 2 && defer_on && n->use_branches && n->cfg.math_mode == B200DQN_MATH_TCGEN05 &&
                           (n->world == 1 || comm_gather_active(n, st));

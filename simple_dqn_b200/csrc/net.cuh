@@ -28,7 +28,7 @@ struct LayerTable {
 
 struct b200dqn_net {
   int device = 0;
-  int sm_count = 148;      // queried at create; sizes the capped elementwise grids
+  int sm_count = 132;      // queried at create; sizes the capped elementwise grids
   b200dqn_net_config cfg{};
   int nb = 0;  // per-rank minibatch
   int A = 0;
@@ -93,8 +93,9 @@ struct b200dqn_net {
   // Software-pipelined fc1 update (multi-step train_fused, opt-in B200DQN_DEFER_FC1=1 — measured slower, see
   // b200dqn_net_train_fused): the graph of step t applies step t-1's fc1 update on a
   // side branch under its own forward convolutions (joined before fc1_fwd) instead of under the dgrad chain, where its
-  // 296 CTAs compete with the tcgen05 kernels for registers and SM slots; the last step's update is flushed by
-  // train_fused before it returns, so nothing outside that call ever sees a pending update.
+  // 2-CTAs-per-SM grid (264 CTAs on 132 SMs) competes with the tensor-core kernels for registers and SM slots; the
+  // last step's update is flushed by train_fused before it returns, so nothing outside that call ever sees a pending
+  // update.
   cudaGraphExec_t graph_def_exec = nullptr;   // the deferred-update variant of the step graph (same cache keys)
   int graph_def_launches = 0;
   bool defer_fc1 = false;                     // set while that variant is being captured
@@ -105,7 +106,7 @@ struct b200dqn_net {
   cudaStream_t graph_train_stream = nullptr;
   int graph_train_world = 0, graph_train_gen = 0;
 
-  void* umma_state = nullptr;  // tcgen05 engine: fp16 operand planes + weight tile images (net_umma.cu)
+  void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 
   // multi-GPU
   void* nccl_comm = nullptr;

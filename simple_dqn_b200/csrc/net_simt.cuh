@@ -3,7 +3,7 @@
 // One tiled FFMA GEMM kernel, C[M,N] = A[M,K] * B[K,N], whose operands are produced element by
 // element by a "problem" functor, so every GEMM-shaped op of the Nature-DQN step (im2col forward,
 // dgrad, wgrad, dense layers) is the same kernel with a different functor.  It is the exact-fp32
-// mode of the library and the on-device cross-check of the tcgen05 path.
+// mode of the library and the on-device cross-check of the tensor-core path.
 //
 // Geometry is the reference's (src/deepqnetwork.py:77-92): 84x84x4 u8 -> conv 8x8x32 s4 ->
 // conv 4x4x64 s2 -> conv 3x3x64 s1 -> fc 512 -> fc A; no bias, no padding.

@@ -1,5 +1,5 @@
-// net_umma.cu — math_mode TCGEN05: the GEMM-shaped ops of the Nature-DQN step on the 5th-gen
-// tensor cores (tcgen05.mma, TMEM accumulators): forward + dgrad through the K-major kernel of
+// net_umma.cu — math_mode TCGEN05 (the name is historical): the GEMM-shaped ops of the Nature-DQN step on the
+// Hopper tensor cores (wgmma.mma_async, register accumulators): forward + dgrad through the K-major kernel of
 // umma2.cuh, wgrad through the MN-major kernel of umma_mn.cuh, plus the fused optimizer / tile-image
 // kernels.  Same fp32 HBM tensors as the SIMT engine (net_simt.cuh), so every kernel here is checked
 // against its SIMT twin and against the CPU oracle.
@@ -581,7 +581,7 @@ k_opt_conv(const float* __restrict__ part, int splits, float* __restrict__ w, fl
 // one 16-byte chunk of the row-oriented (dgrad) tile image, refreshed in the same pass; the
 // column-oriented (forward) image is rebuilt by k_pack_image right after.  Both kernels are smem-free,
 // light on registers and launched on a CAPPED grid (2 CTAs per SM, grid-stride loop) so that they
-// co-reside with the tcgen05 kernels of the critical chain instead of locking them out of the SMs.
+// co-reside with the tensor-core kernels of the critical chain instead of locking them out of the SMs.
 __global__ void __launch_bounds__(256)
 k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
           const OptArgs opt, const uint32_t* __restrict__ gate, const KTrace kt) {
@@ -626,7 +626,7 @@ int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g, const u
   return B200DQN_OK;
 }
 
-// RMSProp + image refresh of conv layer l (0..2), fused (single-GPU path of the tcgen05 engine).
+// RMSProp + image refresh of conv layer l (0..2), fused (single-GPU path of the tensor-core engine).
 int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* label, bool from_g) {
   UmmaState* u = ust(n);
   const LayerTable& lt = n->lt;
@@ -731,13 +731,13 @@ static inline int fc1_splits_for(int rows) {
   if (forced >= 1 && forced <= kFc1Splits) return forced;
   return rows <= 256 ? 7 : 4;
 }
-// Cluster split-K (umma2.cuh) for the kernels whose tile count leaves most of the 148 SMs idle at batch 32:
+// Cluster split-K (umma2.cuh) for the kernels whose tile count leaves most of the 132 SMs idle at batch 32:
 //   conv2_fwd 42 tiles x 3 partners (8 k-blocks -> 3/3/2),  conv3_fwd 26 x 4 (9 -> 3/2/2/2),
 //   conv3_dgrad 21 x 4,  fc1_dgrad 25 x 4 (8 -> 2 each).
-// OFF by default (B200DQN_SPLITK=1 turns it on): parity-clean, but MEASURED SLOWER inside the step — 85.2 us vs
-// 73.6 us per step on a B200 (profiles/r2c_*): with 100+ CTAs of 193 KB shared memory per kernel the successor of the
-// PDL chain finds no free SM to pre-launch on (its prologue no longer hides behind the predecessor) and the cluster
-// needs all its SMs at once; the few-CTA tiles win because consecutive kernels CO-RESIDE.
+// OFF by default (B200DQN_SPLITK=1 turns it on): parity-clean, but slower inside the step where it was measured (an
+// earlier GPU generation; not re-measured on H100): with 100+ CTAs of 193 KB shared memory per kernel the successor of
+// the PDL chain finds no free SM to pre-launch on and the cluster needs all its SMs at once; the few-CTA tiles win
+// because consecutive kernels CO-RESIDE.
 static const bool g_splitk = getenv("B200DQN_SPLITK") && atoi(getenv("B200DQN_SPLITK")) != 0;
 // Larger minibatches already fill the chip with tiles: split only while the tile count is below the SM count.
 static inline bool use_splitk(int tiles, int ks) { return g_splitk && tiles * ks <= 160; }
@@ -936,9 +936,8 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
 // B200DQN_STAGES2=label,label,...: run that kernel with a 2-stage operand ring (about half the shared memory, so two
 // CTAs of the step's kernels fit on an SM) instead of the deepest ring.
 // Default on ONE GPU: conv2_dgrad — 100 CTAs of 4 k-blocks each; at 81 KB instead of 161 KB they occupy 50 SMs instead
-// of 100 while conv3_wgrad / conv2_wgrad / conv1_wgrad look for SMs (measured period 73.4 -> 71.9 us,
-// profiles/r2o_periods.txt; the conv wgrads themselves are slower with the shallow ring).  With data-parallel learners
-// the same choice costs 12 us per step (2 x B200: 96.0 vs 83.6 us, profiles/r2s_*), so there the default is none.
+// of 100 while conv3_wgrad / conv2_wgrad / conv1_wgrad look for SMs.  With data-parallel learners the same choice was
+// slower, so there the default is none.  (Chosen on an earlier GPU generation; not re-measured on H100.)
 static bool shallow_ring(const b200dqn_net* net, const char* label) {
   static const char* env = getenv("B200DQN_STAGES2");
   const char* list = env ? env : net->world == 1 ? "conv2_dgrad" : "";
@@ -1025,7 +1024,7 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
   }
 }
 
-// fc1 wgrad + RMSProp + image refresh in one kernel (single-GPU tcgen05 path); must follow fc1_dgrad.
+// fc1 wgrad + RMSProp + image refresh in one kernel (single-GPU tensor-core path); must follow fc1_dgrad.
 int umma_fc1_wgrad_fused(b200dqn_net* n, int rows, cudaStream_t st, bool keep_grads) {
   UmmaState* u = ust(n);
   const LayerTable& lt = n->lt;

@@ -13,7 +13,7 @@ namespace b200 {
 
 OptArgs make_opt_args(const b200dqn_net* n, int rows);   // net.cu: optimizer constants of this net
 
-// tcgen05 engine (net_umma.cu)
+// tensor-core engine (net_umma.cu)
 int umma_net_init(b200dqn_net* n);                      // allocate operand images etc. (no-op in SIMT mode)
 void umma_net_destroy(b200dqn_net* n);
 int umma_weights_changed(b200dqn_net* n, cudaStream_t st);  // fp32 master weights were overwritten by the host
@@ -26,7 +26,7 @@ int umma_fc1_splits(int rows);
 // gate != nullptr: the kernel does nothing unless *gate != 0 (software-pipelined update, net.cuh)
 int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false, const uint32_t* gate = nullptr);
 int umma_fc1_wgrad_fused(b200dqn_net* n, int rows, cudaStream_t st, bool keep_grads);
-// fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tcgen05 path
+// fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tensor-core path
 // from_g: read the (all-reduced) gradient from d_g instead of the split-K partials
 int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* label, bool from_g = false);
 // rebuild the fp16 hi/lo tile images of layers [l0, l1] of network `which` (0 online, 1 target)
@@ -54,7 +54,7 @@ int comm_wait_pushes(b200dqn_net* n, cudaStream_t st, int dz_rows = 0);   // dz_
 bool comm_dz4_ll_enabled();
 int comm_gather_dz4_ll(b200dqn_net* n, const void* hi, int64_t lo_off_elems, cudaStream_t st, bool wait_h3);   // LL all-gather of the dZ4 planes
 bool comm_head_push(const b200dqn_net* n, cudaStream_t st, HeadPush* out);   // gather schedule + head-side dZ4 push on?
-// gather schedule hooks of the tcgen05 engine (net_umma.cu)
+// gather schedule hooks of the tensor-core engine (net_umma.cu)
 int umma_push_h3(b200dqn_net* n, cudaStream_t st);       // after conv3_fwd: rows of the online net's H3 planes
 int umma_push_dz4(b200dqn_net* n, cudaStream_t st);      // after the head
 int umma_gather_dz4_ll(b200dqn_net* n, cudaStream_t st); // after the head: LL all-gather of dZ4 (default)

@@ -1,4 +1,4 @@
-// umma2.cuh — tcgen05 implicit-GEMM kernel, engine v2: operands arrive PRE-SPLIT (fp16 hi / scaled
+// umma2.cuh — wgmma implicit-GEMM kernel (sm_90a), engine v2: operands arrive PRE-SPLIT (fp16 hi / scaled
 // fp16 lo planes written once by their producer), so the mainloop is pure data movement:
 //
 //   kAsync : activations / gradients live in HBM as NHWC fp16 hi+lo planes; every 16-byte chunk of
@@ -9,8 +9,8 @@
 //            with ONE TMA bulk copy (cp.async.bulk, SASS UBLKCP) that completes on an mbarrier.
 //   kReg   : the u8 frame window of conv1 is converted in registers (u8 -> fp16 is exact, no lo part).
 //
-// 4-stage ring: loads for k-block i+3 are in flight while the tensor core works on k-block i.
-// Accumulation scheme (3 MMAs / k-step, fp32 in TMEM) as in umma.cuh.
+// 4-stage ring: loads for k-block i+3 are in flight while the tensor cores work on k-block i.
+// Accumulation scheme (2 wgmma per k-step, fp32 accumulators in registers) as in umma.cuh.
 #pragma once
 #include <stdlib.h>
 #include <type_traits>
@@ -121,15 +121,13 @@ struct Cfg2 {
   // that two CTAs — of this or of another kernel of the step — share an SM
   static constexpr int kStages = StagesOf<P>::value ? StagesOf<P>::value : (4 * kStageBytes <= 200 * 1024) ? 4 : 3;
   static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024;
-  static constexpr uint32_t kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128
-                                        : (2 * BN <= 256) ? 256 : 512;
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "UMMA N for M=128 must be a multiple of 16 in [16,256]");
+  static_assert(BN == 32 || BN == 64, "wgmma N = 2*BN (and BN) of the instantiated shapes");
+  static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
   static_assert(!(P::kAMode == kBulk && P::kAExact), "bulk A images always carry hi+lo");
-  static_assert(2 * BN <= 256, "[B_hi ; B_lo] is issued as one N = 2*BN MMA");
 };
 
-// Debug timeline (B200DQN_TRACE_LABEL=<kernel label>): the MMA thread and loader thread 0 of CTA
-// (0,0,0) of the selected kernel stamp clock64() at pipeline events; read with b200dqn_debug_trace().
+// Debug timeline (B200DQN_TRACE_LABEL=<kernel label>): thread 0 of CTA (0,0,0) of the selected kernel stamps
+// clock64() at pipeline events; read with b200dqn_debug_trace().
 constexpr int kTraceSlots = 96;
 __device__ unsigned long long g_trace[kTraceSlots];
 #define B2_TRACE(cond, slot)                                                      \
@@ -141,30 +139,25 @@ __device__ __forceinline__ void cp_async_arrive_noinc(uint64_t* bar) {
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-__device__ __forceinline__ bool elect_one() {   // one lane of a converged warp (CUTLASS elect_one_sync)
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-constexpr int kLoadThreads = 256;            // warps 0..7: operand staging, then the epilogue
-constexpr int kThreads2 = kLoadThreads + 32; // warp 8: MMA issuer
+constexpr int kLoadThreads = 256;            // 2 warpgroups: operand staging, MMAs of their 64 rows, epilogue
+constexpr int kThreads2 = kLoadThreads;
 
-// Warp-specialised pipeline, no CTA-wide barrier inside the k loop:
-//   loaders : for each k-block j: wait empty[j % S] (the MMAs that read that stage S k-blocks ago are
-//             done), issue cp.async / TMA bulk / st.shared for stage j % S, and arrive on full[j % S]
-//             (cp.async.mbarrier.arrive.noinc: the arrive fires when this thread's copies have landed)
-//   MMA warp: wait full[s]; fence.proxy.async (generic-proxy smem writes -> async proxy); issue
-//             2 MMAs per k-step:  [acc0 | acc1] += A_hi x [B_hi ; B_lo]   (one N = 2*BN instruction:
-//             the hi and lo weight tiles are adjacent in shared memory)  and  acc1 += A_lo x B_hi;
-//             tcgen05.commit -> empty[s]
+// Pipeline, every thread in every role (the accumulators of wgmma live in the registers of the issuing warpgroup):
+//   stage j % S is filled S k-blocks ahead (cp.async / TMA bulk / st.shared; cp.async.mbarrier.arrive.noinc fires
+//   when this thread's copies have landed) and completes on full[j % S];
+//   k-block it: wait full[it % S]; fence.proxy.async (generic-proxy smem writes -> async proxy); each warpgroup
+//   issues, on its 64 rows of A, per k-step  [acc0 | acc1] += A_hi x [B_hi ; B_lo]  (one N = 2*BN wgmma: the hi and
+//   lo weight tiles are adjacent in shared memory) and  acc2 += A_lo x B_hi;  then wgmma.wait_group 1 (k-block it-1
+//   has completed in this warpgroup), one named barrier over both warpgroups, and stage (it-1) % S is refilled with
+//   k-block it-1+S while the tensor cores work on k-block it.
 // KS > 1: split-K across a thread-block cluster of KS CTAs along grid x.  Rank r of a cluster walks k-blocks
-// [r*per, (r+1)*per) of its tile into its own TMEM; ranks > 0 park their combined fp32 accumulators in their own
-// shared memory, rank 0 adds them in rank order through DSMEM loads (deterministic) and runs the epilogue.  Gives the
-// 21-56-CTA kernels of the batch-32 step the whole chip: 2-3 k-blocks per CTA instead of 8-9.
+// [r*per, (r+1)*per) of its tile into its own accumulators; every rank parks its combined fp32 tile in its own
+// shared memory, rank 0 adds the partners' tiles in rank order through DSMEM loads (deterministic) and runs the
+// epilogue.  Gives the few-CTA kernels of the batch-32 step the whole chip: 2-3 k-blocks per CTA instead of 8-9.
 template <class P, int KS = 1>
 __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int trace_in, const KTrace kt) {
   using C = Cfg2<P>;
@@ -172,13 +165,9 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   constexpr int BN = C::BN;
   constexpr int S = C::kStages;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t s_tmem;
   __shared__ __align__(8) uint64_t s_full[S];    // operands of the stage have landed
-  __shared__ __align__(8) uint64_t s_empty[S];   // MMAs reading the stage completed
-  __shared__ __align__(8) uint64_t s_done;
-  __shared__ __align__(8) uint64_t s_dumped;     // kDumpA: the bulk stores have finished READING the A tiles
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int z = blockIdx.z;
   const bool trace = trace_in && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   kt_begin(kt);
@@ -202,348 +191,275 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   constexpr bool kAnyBulk = (P::kAMode == kBulk) || (P::kBMode == kBulk);
   constexpr uint32_t kBulkBytes = (P::kAMode == kBulk ? 2 * C::kABytes : 0) + (P::kBMode == kBulk ? 2 * C::kBBytes : 0);
 
-  if (warp == 8) umma::tmem_alloc(&s_tmem, C::kTmemCols);
-  if (tid == 32) {
+  if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&s_full[s], kLoadThreads + (kAnyBulk ? 1 : 0));
-      mbar_init(&s_empty[s], 1);
-    }
-    mbar_init(&s_done, 1);
-    mbar_init(&s_dumped, 1);
+    for (int s = 0; s < S; ++s) mbar_init(&s_full[s], kLoadThreads + (kAnyBulk ? 1 : 0));
     mbar_fence_init();
   }
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
   B2_TRACE(tid == 0, 1);
-  const uint32_t tmem = s_tmem;
 
-  if (warp == 8) {
-    // ================================================================ MMA issuer
-    // The whole warp runs the loop converged; one elected lane issues (keeps descriptors in uniform
-    // registers and avoids the per-instruction re-convergence loop ptxas emits inside divergent code).
-    constexpr bool kAMn = AMnMajor<P>::value;
-    constexpr uint32_t idesc1 = umma::make_idesc_f16(kBM, BN) | (kAMn ? umma::kIdescAMn : 0u);
-    constexpr uint32_t idesc2 = umma::make_idesc_f16(kBM, 2 * BN) | (kAMn ? umma::kIdescAMn : 0u);
-    constexpr uint32_t kAStep = kAMn ? 128 : 2;   // descriptor address units (16 B) per 16 k: 16 k-rows x 128 B or 32 B
-    for (int it = 0; it < nkb; ++it) {
-      const int s = it % S;
-      mbar_wait(&s_full[s], (it / S) & 1);
-      fence_proxy_async_smem();
-      umma::fence_after_sync();
-      B2_TRACE(lane == 0, 8 + it * 4 + 0);
-      const uint32_t sa = smem_base + s * C::kStageBytes;
-      const uint64_t da_hi = kAMn ? umma::make_desc_mn(sa, 64 * 128) : umma::make_desc_sw128(sa);
-      const uint64_t da_lo = kAMn ? umma::make_desc_mn(sa + C::kABytes, 64 * 128) : umma::make_desc_sw128(sa + C::kABytes);
-      const uint64_t db = umma::make_desc_sw128(sa + C::kAStage);   // [B_hi ; B_lo], 2*BN rows
-      if (elect_one()) {
-        if constexpr (P::kDumpA) {
-          // The staged [128 x 64] A_hi tile IS the MN-major operand the wgrad of this layer needs
-          // (row = pixel, 64 contiguous taps): ship it out with one TMA bulk store per k-block.
-          uint8_t* dump = p.a_dump(z, mtile, kb0 + it);
-          if (dump) tma_bulk_s2g(dump, smem_gen + s * C::kStageBytes, C::kABytes);
-        }
+  constexpr int kACh = kBM * 8 / kLoadThreads;
+  constexpr int kBCh = (BN * 8 + kLoadThreads - 1) / kLoadThreads;
+  RowCtx arow[kACh];
+  RowCtx brow[kBCh];
+  Planes apl{nullptr, 0}, bpl{nullptr, 0};
+  if constexpr (P::kAMode == kAsync) {
+    apl = p.a_planes(z);
 #pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          umma::mma_f16(tmem, da_hi + kAStep * k, db + 2 * k, idesc2, (it > 0 || k > 0) ? 1u : 0u);
-          if (!P::kAExact) umma::mma_f16(tmem + BN, da_lo + kAStep * k, db + 2 * k, idesc1, 1u);
-        }
-        umma::mma_commit(&s_empty[s]);
-        if (it == nkb - 1) {
-          umma::mma_commit(&s_done);
-          if constexpr (P::kDumpA) {
-            tma_bulk_commit();
-            tma_bulk_wait_read_all();   // smem may now be reused by the epilogue's staging tile
-            mbar_arrive(&s_dumped);
-          }
+    for (int i = 0; i < kACh; ++i) {
+      const int id = tid + i * kLoadThreads;
+      arow[i] = p.a_row(z, m0 + (P::kARowMajorThreads ? (id >> 3) : (id % kBM)));
+    }
+  }
+  if constexpr (P::kBMode == kAsync) {
+    bpl = p.b_planes(z);
+#pragma unroll
+    for (int i = 0; i < kBCh; ++i) {
+      const int id = tid + i * kLoadThreads;
+      brow[i] = p.b_row(z, n0 + (P::kBRowMajorThreads ? (id >> 3) : (id % BN)));
+    }
+  }
+  // Weight tile images do not depend on the predecessor kernel (they were refreshed by the PREVIOUS step's
+  // optimizer, long finished): the TMA bulk copies of the first S k-blocks are issued ahead of the dependency
+  // wait, so that for the weight-heavy kernels (fc1 forward / dgrad: 32 KB of image per k-block) the first
+  // stages are already full when the activations may be touched.
+  if constexpr (kAnyBulk) {
+    if (tid == 0) {
+#pragma unroll
+      for (int j = 0; j < S; ++j) {
+        if (j < nkb) {
+          uint8_t* st_gen = smem_gen + j * C::kStageBytes;
+          mbar_arrive_expect_tx(&s_full[j], kBulkBytes);
+          issue_bulk_stage<P, C>(p, z, mtile, blockIdx.y, kb0 + j, st_gen, &s_full[j]);
         }
       }
-      __syncwarp();
-      B2_TRACE(lane == 0, 8 + it * 4 + 1);
     }
-    if (nkb == 0 && lane == 0) mbar_arrive(&s_done);   // a partner without k-blocks: nothing to wait for
-    if constexpr (KS > 1) {   // take part in the two cluster barriers of the epilogue's reduction
-      cluster_arrive_release(); cluster_wait_acquire();
-      cluster_arrive_release(); cluster_wait_acquire();
+  }
+  // Everything above (barrier init, the gather index tables, the first weight tiles) overlapped the previous kernel
+  // of the chain; only from here on do we touch its outputs.
+  pdl_wait();
+  if (kt.flags & 1) pdl_launch_dependents();
+  // kReg operands: per-row source pointers, once per kernel (they may depend on upstream data — the
+  // sampled indexes — so they are built after the wait, but not again for every k-block)
+  const uint8_t* areg[kACh];
+  if constexpr (P::kAMode == kReg) {
+#pragma unroll
+    for (int i = 0; i < kACh; ++i) {
+      const int id = tid + i * kLoadThreads;
+      areg[i] = p.a_row_ptr(z, m0 + (P::kARowMajorThreads ? (id >> 3) : (id % kBM)));
     }
-  } else {
-    // ================================================================ loaders
-    constexpr int kACh = kBM * 8 / kLoadThreads;
-    constexpr int kBCh = (BN * 8 + kLoadThreads - 1) / kLoadThreads;
-    RowCtx arow[kACh];
-    RowCtx brow[kBCh];
-    Planes apl{nullptr, 0}, bpl{nullptr, 0};
-    if constexpr (P::kAMode == kAsync) {
-      apl = p.a_planes(z);
+  }
+  // ... and the raw bytes of the first S k-blocks are requested up front: one exposed global-memory
+  // latency for the whole tile instead of one per k-block (the conversion path is synchronous).
+  uint2 araw[S][kACh];
+  if constexpr (P::kAMode == kReg) {
+#pragma unroll
+    for (int j = 0; j < S; ++j)
 #pragma unroll
       for (int i = 0; i < kACh; ++i) {
         const int id = tid + i * kLoadThreads;
-        arow[i] = p.a_row(z, m0 + (P::kARowMajorThreads ? (id >> 3) : (id % kBM)));
+        const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
+        araw[j][i] = (j < nkb) ? p.a_raw8(areg[i], (kb0 + j) * kBK + c * 8) : make_uint2(0u, 0u);
       }
+  }
+  // operands of k-block j into stage j % S (the stage is free: its previous k-block has been consumed)
+  auto stage = [&](int j) {
+    const int s = j % S, kb = kb0 + j, k0 = kb * kBK;
+    B2_TRACE(tid == 0, 8 + j * 4 + 2);
+    const uint32_t st_addr = smem_base + s * C::kStageBytes;
+    uint8_t* st_gen = smem_gen + s * C::kStageBytes;
+    const uint32_t a_hi = st_addr, a_lo = st_addr + C::kABytes, b_hi = st_addr + C::kAStage, b_lo = b_hi + C::kBBytes;
+    if (kAnyBulk && tid == 0 && j >= S) {   // the first S k-blocks' images were requested before the dependency wait
+      mbar_arrive_expect_tx(&s_full[s], kBulkBytes);
+      issue_bulk_stage<P, C>(p, z, mtile, blockIdx.y, kb, st_gen, &s_full[s]);
+    }
+    if constexpr (P::kAMode == kAsync) {
+#pragma unroll
+      for (int i = 0; i < kACh; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int r = P::kARowMajorThreads ? (id >> 3) : (id % kBM);
+        const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
+        int64_t eoff = 0;
+        const bool ok = arow[i].ok && p.a_chunk(z, arow[i], k0 + c * 8, eoff);
+        const uint32_t bytes = ok ? 16u : 0u;
+        const __half* hi = apl.hi + (ok ? eoff : 0);
+        const uint32_t off = umma::sw128_off(r, c);
+        cp_async16(a_hi + off, hi, bytes);
+        if (!P::kAExact) cp_async16(a_lo + off, hi + apl.lo_off, bytes);
+      }
+    } else if constexpr (P::kAMode == kReg) {
+      float av[kACh][8];
+#pragma unroll
+      for (int i = 0; i < kACh; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
+        uint2 raw = make_uint2(0u, 0u);
+        if (j < S) {
+#pragma unroll
+          for (int jj = 0; jj < S; ++jj) if (jj == j) raw = araw[jj][i];   // static indexing keeps araw in registers
+        } else {
+          raw = p.a_raw8(areg[i], k0 + c * 8);
+        }
+        P::cvt8(raw, av[i]);
+      }
+#pragma unroll
+      for (int i = 0; i < kACh; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int r = P::kARowMajorThreads ? (id >> 3) : (id % kBM);
+        const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
+        uint4 hi, lo;
+        umma::split8(av[i], hi, lo);
+        *reinterpret_cast<uint4*>(st_gen + umma::sw128_off(r, c)) = hi;
+        if (!P::kAExact) *reinterpret_cast<uint4*>(st_gen + C::kABytes + umma::sw128_off(r, c)) = lo;
+      }
+      fence_proxy_async_smem();   // st.shared (generic proxy) -> async proxy, writer side
     }
     if constexpr (P::kBMode == kAsync) {
-      bpl = p.b_planes(z);
 #pragma unroll
       for (int i = 0; i < kBCh; ++i) {
         const int id = tid + i * kLoadThreads;
-        brow[i] = p.b_row(z, n0 + (P::kBRowMajorThreads ? (id >> 3) : (id % BN)));
-      }
-    }
-    // Weight tile images do not depend on the predecessor kernel (they were refreshed by the PREVIOUS step's
-    // optimizer, long finished): the TMA bulk copies of the first S k-blocks are issued ahead of the dependency
-    // wait, so that for the weight-heavy kernels (fc1 forward / dgrad: 32 KB of image per k-block) the first
-    // stages are already full when the activations may be touched.
-    if constexpr (kAnyBulk) {
-      if (tid == 0) {
-#pragma unroll
-        for (int j = 0; j < S; ++j) {
-          if (j < nkb) {
-            uint8_t* st_gen = smem_gen + j * C::kStageBytes;
-            mbar_arrive_expect_tx(&s_full[j], kBulkBytes);
-            issue_bulk_stage<P, C>(p, z, mtile, blockIdx.y, kb0 + j, st_gen, &s_full[j]);
-          }
-        }
-      }
-    }
-    // Everything above (TMEM alloc, barrier init, the gather index tables, the first weight tiles) overlapped the
-    // previous kernel of the chain; only from here on do we touch its outputs.  (The MMA warp never reads global memory.)
-    pdl_wait();
-    if (kt.flags & 1) pdl_launch_dependents();
-    // kReg operands: per-row source pointers, once per kernel (they may depend on upstream data — the
-    // sampled indexes — so they are built after the wait, but not again for every k-block)
-    const uint8_t* areg[kACh];
-    if constexpr (P::kAMode == kReg) {
-#pragma unroll
-      for (int i = 0; i < kACh; ++i) {
-        const int id = tid + i * kLoadThreads;
-        areg[i] = p.a_row_ptr(z, m0 + (P::kARowMajorThreads ? (id >> 3) : (id % kBM)));
-      }
-    }
-    // ... and the raw bytes of the first S k-blocks are requested up front: one exposed global-memory
-    // latency for the whole tile instead of one per k-block (the conversion path is synchronous).
-    uint2 araw[S][kACh];
-    if constexpr (P::kAMode == kReg) {
-#pragma unroll
-      for (int j = 0; j < S; ++j)
-#pragma unroll
-        for (int i = 0; i < kACh; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
-          araw[j][i] = (j < nkb) ? p.a_raw8(areg[i], (kb0 + j) * kBK + c * 8) : make_uint2(0u, 0u);
-        }
-    }
-    for (int j = 0; j < nkb; ++j) {
-      const int s = j % S, kb = kb0 + j, k0 = kb * kBK;
-      if (j >= S) mbar_wait(&s_empty[s], ((j / S) - 1) & 1);
-      B2_TRACE(tid == 0, 8 + j * 4 + 2);
-      const uint32_t st_addr = smem_base + s * C::kStageBytes;
-      uint8_t* st_gen = smem_gen + s * C::kStageBytes;
-      const uint32_t a_hi = st_addr, a_lo = st_addr + C::kABytes, b_hi = st_addr + C::kAStage, b_lo = b_hi + C::kBBytes;
-      if (kAnyBulk && tid == 0 && j >= S) {   // the first S k-blocks' images were requested before the dependency wait
-        mbar_arrive_expect_tx(&s_full[s], kBulkBytes);
-        issue_bulk_stage<P, C>(p, z, mtile, blockIdx.y, kb, st_gen, &s_full[s]);
-      }
-      if constexpr (P::kAMode == kAsync) {
-#pragma unroll
-        for (int i = 0; i < kACh; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = P::kARowMajorThreads ? (id >> 3) : (id % kBM);
-          const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
+        if (id < BN * 8) {
+          const int r = P::kBRowMajorThreads ? (id >> 3) : (id % BN);
+          const int c = P::kBRowMajorThreads ? (id & 7) : (id / BN);
           int64_t eoff = 0;
-          const bool ok = arow[i].ok && p.a_chunk(z, arow[i], k0 + c * 8, eoff);
+          const bool ok = brow[i].ok && p.b_chunk(z, brow[i], k0 + c * 8, eoff);
           const uint32_t bytes = ok ? 16u : 0u;
-          const __half* hi = apl.hi + (ok ? eoff : 0);
+          const __half* hi = bpl.hi + (ok ? eoff : 0);
           const uint32_t off = umma::sw128_off(r, c);
-          cp_async16(a_hi + off, hi, bytes);
-          if (!P::kAExact) cp_async16(a_lo + off, hi + apl.lo_off, bytes);
-        }
-      } else if constexpr (P::kAMode == kReg) {
-        float av[kACh][8];
-#pragma unroll
-        for (int i = 0; i < kACh; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = P::kARowMajorThreads ? (id >> 3) : (id % kBM);
-          const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
-          (void)r;
-          uint2 raw = make_uint2(0u, 0u);
-          if (j < S) {
-#pragma unroll
-            for (int jj = 0; jj < S; ++jj) if (jj == j) raw = araw[jj][i];   // static indexing keeps araw in registers
-          } else {
-            raw = p.a_raw8(areg[i], k0 + c * 8);
-          }
-          P::cvt8(raw, av[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < kACh; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = P::kARowMajorThreads ? (id >> 3) : (id % kBM);
-          const int c = P::kARowMajorThreads ? (id & 7) : (id / kBM);
-          uint4 hi, lo;
-          umma::split8(av[i], hi, lo);
-          *reinterpret_cast<uint4*>(st_gen + umma::sw128_off(r, c)) = hi;
-          if (!P::kAExact) *reinterpret_cast<uint4*>(st_gen + C::kABytes + umma::sw128_off(r, c)) = lo;
-        }
-        fence_proxy_async_smem();   // st.shared (generic proxy) -> async proxy, writer side
-      }
-      if constexpr (P::kBMode == kAsync) {
-#pragma unroll
-        for (int i = 0; i < kBCh; ++i) {
-          const int id = tid + i * kLoadThreads;
-          if (id < BN * 8) {
-            const int r = P::kBRowMajorThreads ? (id >> 3) : (id % BN);
-            const int c = P::kBRowMajorThreads ? (id & 7) : (id / BN);
-            int64_t eoff = 0;
-            const bool ok = brow[i].ok && p.b_chunk(z, brow[i], k0 + c * 8, eoff);
-            const uint32_t bytes = ok ? 16u : 0u;
-            const __half* hi = bpl.hi + (ok ? eoff : 0);
-            const uint32_t off = umma::sw128_off(r, c);
-            cp_async16(b_hi + off, hi, bytes);
-            cp_async16(b_lo + off, hi + bpl.lo_off, bytes);
-          }
+          cp_async16(b_hi + off, hi, bytes);
+          cp_async16(b_lo + off, hi + bpl.lo_off, bytes);
         }
       }
-      if constexpr (P::kAMode == kAsync || P::kBMode == kAsync)
-        cp_async_arrive_noinc(&s_full[s]);   // fires when this thread's copies for the stage have landed
-      else
-        mbar_arrive(&s_full[s]);
-      B2_TRACE(tid == 0, 8 + j * 4 + 3);
     }
-    B2_TRACE(tid == 0, 3);
-    // All of this CTA's loads are issued: let the successor kernel pre-launch NOW (it sets up TMEM,
-    // barriers and index tables, then parks at its pdl_wait) — late enough that its parked CTAs
-    // do not hog shared memory for long, early enough to hide its prologue behind our epilogue.
-    pdl_launch_dependents();
+    if constexpr (P::kAMode == kAsync || P::kBMode == kAsync)
+      cp_async_arrive_noinc(&s_full[s]);   // fires when this thread's copies for the stage have landed
+    else
+      mbar_arrive(&s_full[s]);
+    B2_TRACE(tid == 0, 8 + j * 4 + 3);
+  };
 
-    // ================================================================ epilogue (same 8 warps)
-    // Operands of the epilogue that do not depend on the accumulators (Rectlin masks of the dgrads) are
-    // fetched now, while the tensor core is still draining the last k-blocks.
-    constexpr int kStIt = kBM * (BN / 8) / kLoadThreads;         // staged path: (row, chunk) items per thread
-    constexpr int kDirIt = BN / 16;                              // direct path: 8-column chunks per thread
-    float pf[P::kPrefetch ? (P::kStagedEpilogue ? kStIt : kDirIt) : 1][8];
-    if constexpr (P::kPrefetch) {
-      if (crank != 0) {
-        // partners only contribute accumulators
-      } else if constexpr (P::kStagedEpilogue) {
+  for (int j = 0; j < S && j < nkb; ++j) stage(j);
+
+  // ================================================================ mainloop
+  constexpr bool kAMn = AMnMajor<P>::value;
+  constexpr uint32_t kAStep = kAMn ? 128 : 2;        // descriptor address units (16 B) per 16 k: 16 k-rows x 128 B or 32 B
+  constexpr uint32_t kAWg = umma::kWgM * 128;        // this warpgroup's A: 64 rows further (K-major) / the 2nd m chunk (MN)
+  float acc[BN];                                     // N = 2*BN fragment: [acc0 | acc1]
+  float acc2[P::kAExact ? 1 : BN / 2];               // N = BN fragment: A_lo x B_hi
 #pragma unroll
-        for (int i = 0; i < kStIt; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = id / (BN / 8), cc = id % (BN / 8);
-          if (m0 + r < M && n0 + cc * 8 < N) p.prefetch8(z, m0 + r, n0 + cc * 8, pf[i]);
-        }
-      } else {
+  for (int i = 0; i < BN; ++i) acc[i] = 0.f;
 #pragma unroll
-        for (int c = 0; c < kDirIt; ++c) {
-          const int col = (warp >> 2) * (BN / 2) + c * 8;
-          const int m = m0 + (warp & 3) * 32 + lane;
-          if (m < M && n0 + col < N) p.prefetch8(z, m, n0 + col, pf[c]);
-        }
+  for (int i = 0; i < (P::kAExact ? 1 : BN / 2); ++i) acc2[i] = 0.f;
+  for (int it = 0; it < nkb; ++it) {
+    const int s = it % S;
+    mbar_wait(&s_full[s], (it / S) & 1);
+    fence_proxy_async_smem();
+    B2_TRACE(tid == 0, 8 + it * 4 + 0);
+    const uint32_t sa = smem_base + s * C::kStageBytes;
+    if constexpr (P::kDumpA) {
+      // The staged [128 x 64] A_hi tile IS the MN-major operand the wgrad of this layer needs
+      // (row = pixel, 64 contiguous taps): ship it out with one TMA bulk store per k-block.
+      if (tid == 0) {
+        uint8_t* dump = p.a_dump(z, mtile, kb0 + it);
+        if (dump) tma_bulk_s2g(dump, smem_gen + s * C::kStageBytes, C::kABytes);
       }
     }
-    mbar_wait(&s_done, 0);
-    if constexpr (P::kDumpA) mbar_wait(&s_dumped, 0);
-    umma::fence_after_sync();
-    B2_TRACE(tid == 0, 4);
-    {
-      const int q = warp & 3, half = warp >> 2;
-      const int row = q * 32 + lane;
-      const uint32_t lane_addr = tmem + (uint32_t(q * 32) << 16);
-      constexpr int kColsPerHalf = BN / 2;
-      constexpr int kChunks = kColsPerHalf / 8;
-      float a0[kChunks][8], a1[kChunks][8];
+    const uint32_t a_hi = sa + wg * kAWg, a_lo = a_hi + C::kABytes;
+    const uint64_t da_hi = kAMn ? umma::make_desc_mn(a_hi, 64 * 128) : umma::make_desc_sw128(a_hi);
+    const uint64_t da_lo = kAMn ? umma::make_desc_mn(a_lo, 64 * 128) : umma::make_desc_sw128(a_lo);
+    const uint64_t db = umma::make_desc_sw128(sa + C::kAStage);   // [B_hi ; B_lo], 2*BN rows
+    umma::wgmma_fence();
 #pragma unroll
-      for (int c = 0; c < kChunks; ++c) {        // all TMEM loads in flight, one wait
-        const int col = half * kColsPerHalf + c * 8;
-        umma::tmem_ld8(lane_addr + col, a0[c]);
-        umma::tmem_ld8(lane_addr + BN + col, a1[c]);
+    for (int k = 0; k < kBK / 16; ++k) {
+      umma::wgmma_f16<2 * BN, kAMn ? 1 : 0, 0>(acc, da_hi + kAStep * k, db + 2 * k);
+      if constexpr (!P::kAExact) umma::wgmma_f16<BN, kAMn ? 1 : 0, 0>(acc2, da_lo + kAStep * k, db + 2 * k);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait<1>();
+    B2_TRACE(tid == 0, 8 + it * 4 + 1);
+    if (it >= 1 && it - 1 + S < nkb) {
+      named_bar_sync(1, kThreads2);   // both warpgroups are done with k-block it-1: its stage takes k-block it-1+S
+      stage(it - 1 + S);
+    }
+  }
+  B2_TRACE(tid == 0, 3);
+  // All of this CTA's loads are issued: let the successor kernel pre-launch NOW (it sets up its barriers and index
+  // tables, then parks at its pdl_wait) — late enough that its parked CTAs do not hog shared memory for long, early
+  // enough to hide its prologue behind our epilogue.
+  pdl_launch_dependents();
+
+  // ================================================================ epilogue
+  // The combined tile goes through (now idle) stage memory: a thread then owns (row, 8 consecutive columns) items —
+  // row-major items (kStagedEpilogue: 8 CONTIGUOUS outputs of row m, a warp's stores cover whole lines) or lanes along
+  // m (strided outputs).  Row pitch BN*4 + 16 B keeps both phases nearly bank-conflict free.
+  constexpr int kPitch = BN * 4 + 16;
+  constexpr int kChunksPerRow = BN / 8;
+  constexpr int kIt = kBM * kChunksPerRow / kLoadThreads;
+  static_assert(kBM * kPitch <= C::kStages * C::kStageBytes, "staging tile must fit the stage ring");
+  auto item = [&](int i, int& r, int& cc) {
+    const int id = tid + i * kLoadThreads;
+    if constexpr (P::kStagedEpilogue) { r = id / kChunksPerRow; cc = id % kChunksPerRow; }
+    else { r = id % kBM; cc = id / kBM; }
+  };
+  // Operands of the epilogue that do not depend on the accumulators (Rectlin masks of the dgrads) are
+  // fetched now, while the tensor cores are still draining the last k-blocks.
+  float pf[P::kPrefetch ? kIt : 1][8];
+  if constexpr (P::kPrefetch) {
+    if (crank == 0) {   // partners only contribute accumulators
+#pragma unroll
+      for (int i = 0; i < kIt; ++i) {
+        int r, cc;
+        item(i, r, cc);
+        if (m0 + r < M && n0 + cc * 8 < N) p.prefetch8(z, m0 + r, n0 + cc * 8, pf[i]);
       }
-      umma::tmem_ld_wait();
+    }
+  }
+  umma::wgmma_wait<0>();
+  if constexpr (P::kDumpA) {
+    if (tid == 0) {
+      tma_bulk_commit();
+      tma_bulk_wait_read_all();   // smem may now be reused by the staging tile
+    }
+  }
+  named_bar_sync(1, kThreads2);   // every warpgroup's MMAs (and the A dump) have finished reading the stages
+  B2_TRACE(tid == 0, 4);
+  umma::stage_acc<BN>(acc, P::kAExact ? nullptr : acc2, smem_gen, kPitch, wg, warp, lane);
+  if constexpr (KS > 1) {
+    cluster_arrive_release();   // every partner's tile is parked in its own shared memory
+    cluster_wait_acquire();
+  } else {
+    named_bar_sync(1, kThreads2);
+  }
+  if (crank == 0) {
 #pragma unroll
-      for (int c = 0; c < kChunks; ++c)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) a0[c][j] = nkb > 0 ? fmaf(a1[c][j], umma::kLoInv, a0[c][j]) : 0.f;
-      bool emit = true;
+    for (int i = 0; i < kIt; ++i) {
+      int r, cc;
+      item(i, r, cc);
+      uint8_t* src = smem_gen + r * kPitch + cc * 32;
+      const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 16);
+      float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
       if constexpr (KS > 1) {
-        // ---- split-K reduction through distributed shared memory.  A thread owns accumulator row `row`, columns
-        // [half * BN/2, +BN/2): partners park exactly that slice at the same offset of their own (now idle) stage
-        // memory, the leader adds the slices in rank order.
-        constexpr int kRedPitch = BN * 4 + 16;
-        static_assert(kBM * kRedPitch <= C::kStages * C::kStageBytes, "reduction tile must fit the stage ring");
-        uint8_t* mine = smem_gen + row * kRedPitch + half * kColsPerHalf * 4;
-        if (crank != 0) {
+        const uint32_t local = smem_u32(src);
 #pragma unroll
-          for (int c = 0; c < kChunks; ++c) {
-            *reinterpret_cast<float4*>(mine + c * 32) = make_float4(a0[c][0], a0[c][1], a0[c][2], a0[c][3]);
-            *reinterpret_cast<float4*>(mine + c * 32 + 16) = make_float4(a0[c][4], a0[c][5], a0[c][6], a0[c][7]);
-          }
+        for (int rk = 1; rk < KS; ++rk) {   // rank order: deterministic
+          const uint32_t remote = dsmem_addr(local, uint32_t(rk));
+          const float4 w0 = ld_dsmem_f4(remote), w1 = ld_dsmem_f4(remote + 16);
+          v[0] += w0.x; v[1] += w0.y; v[2] += w0.z; v[3] += w0.w;
+          v[4] += w1.x; v[5] += w1.y; v[6] += w1.z; v[7] += w1.w;
         }
-        cluster_arrive_release();
-        cluster_wait_acquire();
-        if (crank == 0) {
-          const uint32_t local = smem_u32(mine);
-#pragma unroll
-          for (int r = 1; r < KS; ++r) {
-            const uint32_t remote = dsmem_addr(local, uint32_t(r));
-#pragma unroll
-            for (int c = 0; c < kChunks; ++c) {
-              const float4 v0 = ld_dsmem_f4(remote + c * 32), v1 = ld_dsmem_f4(remote + c * 32 + 16);
-              a0[c][0] += v0.x; a0[c][1] += v0.y; a0[c][2] += v0.z; a0[c][3] += v0.w;
-              a0[c][4] += v1.x; a0[c][5] += v1.y; a0[c][6] += v1.z; a0[c][7] += v1.w;
-            }
-          }
-        }
-        cluster_arrive_release();   // partners keep their shared memory alive until the leader has read it
-        cluster_wait_acquire();
-        emit = crank == 0;
       }
-      if (!emit) {
-        // partner: done
-      } else if constexpr (P::kStagedEpilogue) {
-        // A thread owns one accumulator ROW; written straight to HBM every store instruction would
-        // touch 32 different lines.  Transpose through (now idle) pipeline smem so each warp store
-        // covers whole lines: row pitch BN*4 + 16 B keeps both phases bank-conflict free.
-        constexpr int kPitch = BN * 4 + 16;
-        static_assert(kBM * kPitch <= C::kStages * C::kStageBytes, "staging tile must fit the stage ring");
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c) {
-          float* dst = reinterpret_cast<float*>(smem_gen + row * kPitch + (half * kColsPerHalf + c * 8) * 4);
-          *reinterpret_cast<float4*>(dst) = make_float4(a0[c][0], a0[c][1], a0[c][2], a0[c][3]);
-          *reinterpret_cast<float4*>(dst + 4) = make_float4(a0[c][4], a0[c][5], a0[c][6], a0[c][7]);
-        }
-        named_bar_sync(1, kLoadThreads);
-        constexpr int kChunksPerRow = BN / 8;
-#pragma unroll
-        for (int i = 0; i < kBM * kChunksPerRow / kLoadThreads; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
-          const float* src = reinterpret_cast<const float*>(smem_gen + r * kPitch + cc * 32);
-          const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
-          const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-          if (m0 + r < M && n0 + cc * 8 < N) {
-            if constexpr (P::kPrefetch) p.store8p(z, m0 + r, n0 + cc * 8, v, pf[i]);
-            else p.store8(z, m0 + r, n0 + cc * 8, v);
-          }
-        }
-      } else {
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c) {
-          const int col = half * kColsPerHalf + c * 8;
-          if (m0 + row < M && n0 + col < N) {
-            if constexpr (P::kPrefetch) p.store8p(z, m0 + row, n0 + col, a0[c], pf[c]);
-            else p.store8(z, m0 + row, n0 + col, a0[c]);
-          }
-        }
+      if (m0 + r < M && n0 + cc * 8 < N) {
+        if constexpr (P::kPrefetch) p.store8p(z, m0 + r, n0 + cc * 8, v, pf[i]);
+        else p.store8(z, m0 + r, n0 + cc * 8, v);
       }
     }
-    B2_TRACE(tid == 0, 5);
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) {
-    umma::fence_after_sync();
-    umma::tmem_dealloc(tmem, C::kTmemCols);
+  if constexpr (KS > 1) {
+    cluster_arrive_release();   // partners keep their shared memory alive until the leader has read it
+    cluster_wait_acquire();
   }
+  B2_TRACE(tid == 0, 5);
   kt_end(kt);
   B2_TRACE(tid == 0, 6);
 }

@@ -1,16 +1,17 @@
-// umma_mn.cuh — tcgen05 kernel for the weight-gradient family: D[M x N] = sum_k A[m][k] * B[n][k]
+// umma_mn.cuh — wgmma kernel (sm_90a) for the weight-gradient family: D[M x N] = sum_k A[m][k] * B[n][k]
 // where the reduction index k runs over (sample, pixel) and BOTH operands are stored with their
 // M / N index contiguous (NHWC activations: one pixel = one contiguous run of channels).  Those are
-// "MN-major" UMMA operands: the 128-byte shared-memory row is a run of 64 consecutive m (or n) for
+// "MN-major" wgmma operands: the 128-byte shared-memory row is a run of 64 consecutive m (or n) for
 // ONE k, eight consecutive k rows form the 1024-byte swizzle atom (cute canonical layout
 // Swizzle<3,4,3> o ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in fp16 elements).  So the gather is again
 // pure cp.async of 16-byte pieces (or an exact u8 -> fp16 convert for the conv1 frame window), no
 // transposition anywhere.
 //
 // Per 64-pixel k-block the stage holds   A_hi [2 chunks x 64 rows x 128 B] (+ A_lo)   and
-//   BN = 64:  B_hi [64 x 128 B] followed by B_lo [64 x 128 B]   -> one N = 128 MMA gives [acc0 | acc1]
-//   BN = 32:  one tile whose rows are [32 hi | 32 lo]            -> one N = 64  MMA gives [acc0 | acc1]
-// and, when A is not exact,  acc1 += A_lo x B_hi  (N = BN).  Split-K over blockIdx.z.
+//   BN = 64:  B_hi [64 x 128 B] followed by B_lo [64 x 128 B]   -> one N = 128 wgmma gives [acc0 | acc1]
+//   BN = 32:  one tile whose rows are [32 hi | 32 lo]            -> one N = 64  wgmma gives [acc0 | acc1]
+// and, when A is not exact,  acc2 += A_lo x B_hi  (N = BN, own accumulator, see umma.cuh); each of the two warpgroups multiplies one 64-wide
+// m chunk of A (wgmma M = 64).  Split-K over blockIdx.z.
 #pragma once
 #include "umma2.cuh"
 
@@ -25,9 +26,6 @@ using umma2::Planes;
 constexpr int kKB = 64;  // reduction rows (pixels) per k-block
 
 using umma::make_desc_mn;   // MN-major SWIZZLE_128B descriptor (umma.cuh)
-__host__ __device__ constexpr uint32_t make_idesc_f16_mn(int M, int N) {
-  return (1u << 4) | (1u << 15) | (1u << 16) | (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
 // byte offset of 16-byte piece j of k-row kr inside one [64 k-rows x 128 B] sub-tile
 __device__ __forceinline__ uint32_t mn_off(int kr, int j) {
   return uint32_t((kr >> 3) * 1024 + (kr & 7) * 128 + ((j ^ (kr & 7)) << 4));
@@ -58,7 +56,7 @@ struct CfgMN {
   static constexpr int kStages = P::kStages;   // 4 for the split-K conv wgrads; 2 for the single-k-block fc1 wgrad
   static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024;
   static_assert(kBM * (BN * 4 + 16) <= kStages * kStageBytes, "epilogue staging tile must fit the stage ring");
-  static constexpr uint32_t kTmemCols = (2 * BN <= 64) ? 64 : 128;
+  static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
 
 template <class P>
@@ -66,13 +64,11 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
   using C = CfgMN<P>;
   constexpr int BN = C::BN;
   constexpr int S = C::kStages;
+  static_assert(P::kAExact || BN == 64, "acc2 += A_lo x B_hi reads B_hi as one whole 64-wide MN chunk");
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint32_t s_tmem;
   __shared__ __align__(8) uint64_t s_full[S];
-  __shared__ __align__(8) uint64_t s_empty[S];
-  __shared__ __align__(8) uint64_t s_done;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int z = blockIdx.z;
   kt_begin(kt);
   const int M = p.M(z), N = p.N(z);
@@ -85,204 +81,179 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
 
-  if (warp == 8) umma::tmem_alloc(&s_tmem, C::kTmemCols);
-  if (tid == 32) {
+  if (tid == 0) {
 #pragma unroll
-    for (int s = 0; s < S; ++s) {
-      mbar_init(&s_full[s], kLoadThreads + (P::kABulk ? 1 : 0));
-      mbar_init(&s_empty[s], 1);
-    }
-    mbar_init(&s_done, 1);
+    for (int s = 0; s < S; ++s) mbar_init(&s_full[s], kLoadThreads + (P::kABulk ? 1 : 0));
     mbar_fence_init();
   }
-  umma::fence_before_sync();
   __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tmem = s_tmem;
 
   if (nkb <= 0) {
     // nothing to reduce in this split: the partial is all zeros
     pdl_wait();
-    if (warp < 8) {
-      const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      for (int id = tid; id < kBM * (BN / 8); id += kLoadThreads) {
-        const int r = id / (BN / 8), cc = id % (BN / 8);
-        if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, zero);
-      }
+    const float zero[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int id = tid; id < kBM * (BN / 8); id += kLoadThreads) {
+      const int r = id / (BN / 8), cc = id % (BN / 8);
+      if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, zero);
     }
-  } else if (warp == 8) {
-    // ================================================================ MMA issuer (converged warp)
-    constexpr uint32_t idesc_full = make_idesc_f16_mn(kBM, 2 * BN);   // A_hi x [B_hi | B_lo]
-    constexpr uint32_t idesc_hi = make_idesc_f16_mn(kBM, BN);         // A_lo x B_hi
-    for (int it = 0; it < nkb; ++it) {
-      const int s = it % S;
-      mbar_wait(&s_full[s], (it / S) & 1);
-      fence_proxy_async_smem();
-      umma::fence_after_sync();
-      const uint32_t sa = smem_base + s * C::kStageBytes;
-      const uint64_t da_hi = make_desc_mn(sa, C::kSub);
-      const uint64_t da_lo = make_desc_mn(sa + C::kAHalf, C::kSub);
-      const uint64_t db = make_desc_mn(sa + C::kAStage, C::kSub);
-      if (umma2::elect_one()) {
+    kt_end(kt);
+    return;
+  }
+
+  // ================================================================ loaders
+  // thread -> k row (tid >> 2) and a quarter (tid & 3) of that row's 16-byte pieces
+  const int kr = tid >> 2, sub = tid & 3;
+  const Planes bpl = p.b_planes(z);
+  Planes apl{nullptr, 0};
+  if constexpr (!P::kARegs && !P::kABulk) apl = p.a_planes(z);
+  pdl_wait();   // the prologue above overlapped the predecessor
+  if (kt.flags & 1) pdl_launch_dependents();
+  auto stage = [&](int j) {
+    const int s = j % S;
+    const uint32_t st_addr = smem_base + s * C::kStageBytes;
+    uint8_t* st_gen = smem_gen + s * C::kStageBytes;
+    const PixCtx px = p.pix(z, (kb0 + j) * kKB + kr);
+    // ---- A: 2 m-chunks x 8 pieces per row; this thread: chunk (sub >> 1), pieces (sub & 1) * 4 .. + 3
+    if constexpr (P::kABulk) {
+      static_assert(P::kAExact, "bulk A sub-tiles carry no lo part");
+      if (tid == 0) {
+        mbar_arrive_expect_tx(&s_full[s], 2 * C::kSub);
+        tma_bulk_g2s(st_gen, p.a_sub(z, blockIdx.x * 2, kb0 + j), C::kSub, &s_full[s]);
+        tma_bulk_g2s(st_gen + C::kSub, p.a_sub(z, blockIdx.x * 2 + 1, kb0 + j), C::kSub, &s_full[s]);
+      }
+    } else {
+      const int mc = sub >> 1, j0 = (sub & 1) * 4;
+      const int mchunk = blockIdx.x * 2 + mc;
+      if constexpr (!P::kARegs) {
+        int64_t eoff = 0;
+        const bool ok = px.ok && p.a_run(z, px, mchunk, eoff);
+        const __half* src = apl.hi + (ok ? eoff : 0);
 #pragma unroll
-        for (int k = 0; k < kKB / 16; ++k) {   // 16 k rows = 2048 bytes = +128 in the address field
-          umma::mma_f16(tmem, da_hi + 128 * k, db + 128 * k, idesc_full, (it > 0 || k > 0) ? 1u : 0u);
-          if (!P::kAExact) umma::mma_f16(tmem + BN, da_lo + 128 * k, db + 128 * k, idesc_hi, 1u);
-        }
-        umma::mma_commit(&s_empty[s]);
-        if (it == nkb - 1) umma::mma_commit(&s_done);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ================================================================ loaders
-    // thread -> k row (tid >> 2) and a quarter (tid & 3) of that row's 16-byte pieces
-    const int kr = tid >> 2, sub = tid & 3;
-    const Planes bpl = p.b_planes(z);
-    Planes apl{nullptr, 0};
-    if constexpr (!P::kARegs && !P::kABulk) apl = p.a_planes(z);
-    pdl_wait();   // prologue above overlapped the predecessor; the MMA warp never reads global memory
-    if (kt.flags & 1) pdl_launch_dependents();
-    for (int j = 0; j < nkb; ++j) {
-      const int s = j % S;
-      if (j >= S) mbar_wait(&s_empty[s], ((j / S) - 1) & 1);
-      const uint32_t st_addr = smem_base + s * C::kStageBytes;
-      uint8_t* st_gen = smem_gen + s * C::kStageBytes;
-      const PixCtx px = p.pix(z, (kb0 + j) * kKB + kr);
-      // ---- A: 2 m-chunks x 8 pieces per row; this thread: chunk (sub >> 1), pieces (sub & 1) * 4 .. + 3
-      if constexpr (P::kABulk) {
-        static_assert(P::kAExact, "bulk A sub-tiles carry no lo part");
-        if (tid == 0) {
-          mbar_arrive_expect_tx(&s_full[s], 2 * C::kSub);
-          tma_bulk_g2s(st_gen, p.a_sub(z, blockIdx.x * 2, kb0 + j), C::kSub, &s_full[s]);
-          tma_bulk_g2s(st_gen + C::kSub, p.a_sub(z, blockIdx.x * 2 + 1, kb0 + j), C::kSub, &s_full[s]);
+        for (int t = 0; t < 4; ++t) {
+          const uint32_t dst = st_addr + mc * C::kSub + mn_off(kr, j0 + t);
+          umma2::cp_async16(dst, src + (j0 + t) * 8, ok ? 16u : 0u);
+          if (!P::kAExact) umma2::cp_async16(dst + C::kAHalf, src + apl.lo_off + (j0 + t) * 8, ok ? 16u : 0u);
         }
       } else {
-        const int mc = sub >> 1, j0 = (sub & 1) * 4;
-        const int mchunk = blockIdx.x * 2 + mc;
-        if constexpr (!P::kARegs) {
-          int64_t eoff = 0;
-          const bool ok = px.ok && p.a_run(z, px, mchunk, eoff);
-          const __half* src = apl.hi + (ok ? eoff : 0);
 #pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            const uint32_t dst = st_addr + mc * C::kSub + mn_off(kr, j0 + t);
-            umma2::cp_async16(dst, src + (j0 + t) * 8, ok ? 16u : 0u);
-            if (!P::kAExact) umma2::cp_async16(dst + C::kAHalf, src + apl.lo_off + (j0 + t) * 8, ok ? 16u : 0u);
-          }
-        } else {
-#pragma unroll
-          for (int t = 0; t < 4; ++t) {
-            float v[8];
-            p.a_piece(z, px, mchunk, j0 + t, v);
-            uint4 hi, lo;
-            umma::split8(v, hi, lo);
-            *reinterpret_cast<uint4*>(st_gen + mc * C::kSub + mn_off(kr, j0 + t)) = hi;
-            if (!P::kAExact) *reinterpret_cast<uint4*>(st_gen + C::kAHalf + mc * C::kSub + mn_off(kr, j0 + t)) = lo;
-          }
+        for (int t = 0; t < 4; ++t) {
+          float v[8];
+          p.a_piece(z, px, mchunk, j0 + t, v);
+          uint4 hi, lo;
+          umma::split8(v, hi, lo);
+          *reinterpret_cast<uint4*>(st_gen + mc * C::kSub + mn_off(kr, j0 + t)) = hi;
+          if (!P::kAExact) *reinterpret_cast<uint4*>(st_gen + C::kAHalf + mc * C::kSub + mn_off(kr, j0 + t)) = lo;
         }
       }
-      // ---- B
-      {
-        const __half* src = bpl.hi + (px.ok ? p.b_off(z, px) + n0 : 0);
-        const uint32_t bytes = px.ok ? 16u : 0u;
-        if constexpr (BN == 64) {   // pieces 0..7 of the hi tile and of the lo tile; this thread: 2 + 2
-#pragma unroll
-          for (int t = 0; t < 2; ++t) {
-            const int jj = sub * 2 + t;
-            const uint32_t dst = st_addr + C::kAStage + mn_off(kr, jj);
-            umma2::cp_async16(dst, src + jj * 8, bytes);
-            umma2::cp_async16(dst + C::kSub, src + bpl.lo_off + jj * 8, bytes);
-          }
-        } else {                    // row = [32 hi | 32 lo]: pieces 0..3 hi, 4..7 lo; this thread: 1 + 1
-          const uint32_t dst = st_addr + C::kAStage;
-          umma2::cp_async16(dst + mn_off(kr, sub), src + sub * 8, bytes);
-          umma2::cp_async16(dst + mn_off(kr, 4 + sub), src + bpl.lo_off + sub * 8, bytes);
-        }
-      }
-      if constexpr (P::kARegs) fence_proxy_async_smem();   // this thread's st.shared -> async proxy
-      umma2::cp_async_arrive_noinc(&s_full[s]);
     }
-
-    pdl_launch_dependents();   // see umma2.cuh: successor pre-launch is deferred to the end of our mainloop
-
-    // ================================================================ epilogue (smem-transposed, see umma2.cuh)
-    mbar_wait(&s_done, 0);
-    umma::fence_after_sync();
+    // ---- B
     {
-      const int q = warp & 3, half = warp >> 2;
-      const int row = q * 32 + lane;
-      const uint32_t lane_addr = tmem + (uint32_t(q * 32) << 16);
-      constexpr int kColsPerHalf = BN / 2;
-      constexpr int kChunks = kColsPerHalf / 8;
-      constexpr int kPitch = BN * 4 + 16;
+      const __half* src = bpl.hi + (px.ok ? p.b_off(z, px) + n0 : 0);
+      const uint32_t bytes = px.ok ? 16u : 0u;
+      if constexpr (BN == 64) {   // pieces 0..7 of the hi tile and of the lo tile; this thread: 2 + 2
 #pragma unroll
-      for (int c = 0; c < kChunks; ++c) {
-        const int col = half * kColsPerHalf + c * 8;
-        float a0[8], a1[8];
-        umma::tmem_ld8(lane_addr + col, a0);
-        umma::tmem_ld8(lane_addr + BN + col, a1);
-        umma::tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 8; ++j) a0[j] = fmaf(a1[j], umma::kLoInv, a0[j]);
-        float* dst = reinterpret_cast<float*>(smem_gen + row * kPitch + col * 4);
-        *reinterpret_cast<float4*>(dst) = make_float4(a0[0], a0[1], a0[2], a0[3]);
-        *reinterpret_cast<float4*>(dst + 4) = make_float4(a0[4], a0[5], a0[6], a0[7]);
+        for (int t = 0; t < 2; ++t) {
+          const int jj = sub * 2 + t;
+          const uint32_t dst = st_addr + C::kAStage + mn_off(kr, jj);
+          umma2::cp_async16(dst, src + jj * 8, bytes);
+          umma2::cp_async16(dst + C::kSub, src + bpl.lo_off + jj * 8, bytes);
+        }
+      } else {                    // row = [32 hi | 32 lo]: pieces 0..3 hi, 4..7 lo; this thread: 1 + 1
+        const uint32_t dst = st_addr + C::kAStage;
+        umma2::cp_async16(dst + mn_off(kr, sub), src + sub * 8, bytes);
+        umma2::cp_async16(dst + mn_off(kr, 4 + sub), src + bpl.lo_off + sub * 8, bytes);
       }
-      umma2::named_bar_sync(1, kLoadThreads);
-      constexpr int kChunksPerRow = BN / 8;
-      if constexpr (!P::kFusedUpdate) {
+    }
+    if constexpr (P::kARegs) fence_proxy_async_smem();   // this thread's st.shared -> async proxy
+    umma2::cp_async_arrive_noinc(&s_full[s]);
+  };
+  for (int j = 0; j < S && j < nkb; ++j) stage(j);
+
+  // ================================================================ mainloop (pipeline as in umma2.cuh)
+  // warpgroup wg multiplies m chunk wg of A (64 m x 64 k-rows); B = [B_hi | B_lo] as 2 chunks (BN = 64, LBO = one
+  // sub-tile) or one chunk of [32 hi | 32 lo] rows (BN = 32)
+  float acc[BN];                           // N = 2*BN fragment: [acc0 | acc1]
+  float acc2[P::kAExact ? 1 : BN / 2];     // N = BN fragment: A_lo x B_hi
 #pragma unroll
-        for (int i = 0; i < kBM * kChunksPerRow / kLoadThreads; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
-          const float* src = reinterpret_cast<const float*>(smem_gen + r * kPitch + cc * 32);
-          const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
-          const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-          if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, v);
-        }
-      } else {
-        // Fused optimizer (no split-K: this tile IS the whole gradient of its weights).
-        // pass 1, thread <-> (row m, 8 consecutive n): RMSProp on W/S in HBM, the updated weights go
-        //         back into the smem tile and into the row-oriented (dgrad) tile image;
-        // pass 2, thread <-> (column n, 8 consecutive m): the column-oriented (forward) tile image.
-        constexpr int kIt = kBM * kChunksPerRow / kLoadThreads;
-        const float l_step = p.step_scalar();
+  for (int i = 0; i < BN; ++i) acc[i] = 0.f;
 #pragma unroll
-        for (int i = 0; i < kIt; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
-          float* src = reinterpret_cast<float*>(smem_gen + r * kPitch + cc * 32);
-          const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
-          const float g[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-          if (m0 + r < M && n0 + cc * 8 < N) {
-            float nw[8];
-            p.update8(z, m0 + r, n0 + cc * 8, l_step, g, nw);
-            *reinterpret_cast<float4*>(src) = make_float4(nw[0], nw[1], nw[2], nw[3]);
-            *reinterpret_cast<float4*>(src + 4) = make_float4(nw[4], nw[5], nw[6], nw[7]);
-          }
-        }
-        umma2::named_bar_sync(1, kLoadThreads);
+  for (int i = 0; i < (P::kAExact ? 1 : BN / 2); ++i) acc2[i] = 0.f;
+  for (int it = 0; it < nkb; ++it) {
+    const int s = it % S;
+    mbar_wait(&s_full[s], (it / S) & 1);
+    fence_proxy_async_smem();
+    const uint32_t sa = smem_base + s * C::kStageBytes;
+    const uint64_t da_hi = make_desc_mn(sa + wg * C::kSub, C::kSub);
+    const uint64_t da_lo = make_desc_mn(sa + C::kAHalf + wg * C::kSub, C::kSub);
+    const uint64_t db = make_desc_mn(sa + C::kAStage, C::kSub);
+    umma::wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < (kBM / 8) * BN / kLoadThreads; ++i) {
-          const int id = tid + i * kLoadThreads;
-          const int nn = id % BN, mg = id / BN;
-          if (m0 + mg * 8 < M && n0 + nn < N) {
-            float wv[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              wv[j] = *reinterpret_cast<const float*>(smem_gen + (mg * 8 + j) * kPitch + nn * 4);
-            p.pack_col8(z, m0 + mg * 8, n0 + nn, wv);
-          }
-        }
-      }
+    for (int k = 0; k < kKB / 16; ++k) {   // 16 k rows = 2048 bytes = +128 in the address field
+      umma::wgmma_f16<2 * BN, 1, 1>(acc, da_hi + 128 * k, db + 128 * k);
+      if constexpr (!P::kAExact) umma::wgmma_f16<BN, 1, 1>(acc2, da_lo + 128 * k, db + 128 * k);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait<1>();
+    if (it >= 1 && it - 1 + S < nkb) {
+      umma2::named_bar_sync(1, kThreads2);   // both warpgroups are done with k-block it-1
+      stage(it - 1 + S);
     }
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 8) {
-    umma::fence_after_sync();
-    umma::tmem_dealloc(tmem, C::kTmemCols);
+  pdl_launch_dependents();   // see umma2.cuh: successor pre-launch is deferred to the end of our mainloop
+
+  // ================================================================ epilogue (smem-transposed, see umma2.cuh)
+  umma::wgmma_wait<0>();
+  umma2::named_bar_sync(1, kThreads2);   // every warpgroup's MMAs have finished reading the stages
+  {
+    constexpr int kPitch = BN * 4 + 16;
+    umma::stage_acc<BN>(acc, P::kAExact ? nullptr : acc2, smem_gen, kPitch, wg, warp, lane);
+    umma2::named_bar_sync(1, kLoadThreads);
+    constexpr int kChunksPerRow = BN / 8;
+    if constexpr (!P::kFusedUpdate) {
+#pragma unroll
+      for (int i = 0; i < kBM * kChunksPerRow / kLoadThreads; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
+        const float* src = reinterpret_cast<const float*>(smem_gen + r * kPitch + cc * 32);
+        const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
+        const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+        if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, v);
+      }
+    } else {
+      // Fused optimizer (no split-K: this tile IS the whole gradient of its weights).
+      // pass 1, thread <-> (row m, 8 consecutive n): RMSProp on W/S in HBM, the updated weights go
+      //         back into the smem tile and into the row-oriented (dgrad) tile image;
+      // pass 2, thread <-> (column n, 8 consecutive m): the column-oriented (forward) tile image.
+      constexpr int kIt = kBM * kChunksPerRow / kLoadThreads;
+      const float l_step = p.step_scalar();
+#pragma unroll
+      for (int i = 0; i < kIt; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
+        float* src = reinterpret_cast<float*>(smem_gen + r * kPitch + cc * 32);
+        const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
+        const float g[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+        if (m0 + r < M && n0 + cc * 8 < N) {
+          float nw[8];
+          p.update8(z, m0 + r, n0 + cc * 8, l_step, g, nw);
+          *reinterpret_cast<float4*>(src) = make_float4(nw[0], nw[1], nw[2], nw[3]);
+          *reinterpret_cast<float4*>(src + 4) = make_float4(nw[4], nw[5], nw[6], nw[7]);
+        }
+      }
+      umma2::named_bar_sync(1, kLoadThreads);
+#pragma unroll
+      for (int i = 0; i < (kBM / 8) * BN / kLoadThreads; ++i) {
+        const int id = tid + i * kLoadThreads;
+        const int nn = id % BN, mg = id / BN;
+        if (m0 + mg * 8 < M && n0 + nn < N) {
+          float wv[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            wv[j] = *reinterpret_cast<const float*>(smem_gen + (mg * 8 + j) * kPitch + nn * 4);
+          p.pack_col8(z, m0 + mg * 8, n0 + nn, wv);
+        }
+      }
+    }
   }
   kt_end(kt);
 }

@@ -1,5 +1,5 @@
 """DeepQNetwork with the reference's call surface (/root/reference/src/deepqnetwork.py:15-192):
-the Neon model/train/predict replaced by hand-written sm_100a kernels (csrc/net*.cu)."""
+the Neon model/train/predict replaced by hand-written sm_90a kernels (csrc/net*.cu)."""
 import ctypes as C
 import logging
 import pickle
@@ -36,13 +36,13 @@ class DeepQNetwork:
         self.batch_norm = _arg(args, "batch_norm", False)
         # flags of the reference this build accepts but does not implement (SURVEY §8 a17 note)
         if self.batch_norm:
-            raise NotImplementedError("--batch_norm is not implemented on the B200 path")
+            raise NotImplementedError("--batch_norm is not implemented in this library")
         self.optimizer = _arg(args, "optimizer", "rmsprop")
         assert self.optimizer in _OPTIMIZERS, "Unknown optimizer"       # :60-61
         if np.dtype(_arg(args, "datatype", "float32")) != np.float32:
-            raise NotImplementedError("only --datatype float32 is implemented on the B200 path")
+            raise NotImplementedError("only --datatype float32 is implemented in this library")
         if _arg(args, "stochastic_round", False):
-            raise NotImplementedError("--stochastic_round is not implemented on the B200 path")
+            raise NotImplementedError("--stochastic_round is not implemented in this library")
         self.device = _arg(args, "device_id", 0) if device is None else device
         self._stream_obj = stream            # keep the stream alive as long as this object uses it
         self._stream = L.stream_ptr(stream)

@@ -1,5 +1,5 @@
 """ReplayMemory with the reference's call surface (/root/reference/src/replay_memory.py:6-79),
-backed by a ring buffer in HBM and hand-written sm_100a kernels (csrc/replay.cu)."""
+backed by a ring buffer in HBM and hand-written sm_90a kernels (csrc/replay.cu)."""
 import ctypes as C
 import logging
 import random

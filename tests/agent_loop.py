@@ -4,12 +4,12 @@ environment; VERDICT r1 N2).
 Two interchangeable drivers produce the same :class:`Trace`:
 
   * :func:`run_reference_loop` — the REFERENCE's own `Agent` + `Statistics` (src/agent.py, src/statistics.py,
-    converted in a temp dir by tests/ref_convert.py; build container only) driven through the schedule of
-    src/main.py:130-162;
-  * :func:`run_restated_loop` — an independent restatement of that loop written for this repository (the GPU box
-    has no /root/reference).  tests/test_agent_loop.py proves, in the build container, that both drivers produce
-    bit-identical traces on the same classes; the GPU test then runs the restatement on the PRODUCT classes
-    against the golden trace the reference loop produced on the oracle classes.
+    converted by tests/ref_convert.py) driven through the schedule of src/main.py:130-162; used only by
+    tests/golden/make_agent_golden.py, which needs the reference's sources, to record agent_loop_golden.npz;
+  * :func:`run_restated_loop` — an independent restatement of that loop written for this repository (the
+    reference's sources are not part of it).  tests/test_agent_loop.py shows that it reproduces the stored traces
+    of the reference loop on the oracle classes; the GPU test runs it on the PRODUCT classes against the same
+    traces.
 
 Whatever `mem`, `net`, `buf` objects are passed in (reference files, oracle classes, product classes) are used only
 through the reference's call surface (SURVEY §8b)."""

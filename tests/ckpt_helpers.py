@@ -1,5 +1,5 @@
-"""Checkpoint fixtures shared by the CPU and GPU tests: the reference's snapshot weights (data) and a writer that
-rebuilds a checkpoint FILE with the reference's own pickle structure around them."""
+"""Checkpoint fixtures shared by the CPU and GPU tests: a seeded stand-in for a trained snapshot and a writer that
+rebuilds a checkpoint FILE with the reference's own pickle structure around any weights."""
 import json
 import os
 import pickle
@@ -9,9 +9,24 @@ import numpy as np
 from conftest import GOLDEN
 
 
+def snapshot_weights(num_actions, seed=77):
+    """Weights and RMSProp state of a snapshot's shapes, seeded: W ~ N(0, 2 / fan_in) (so Q values are O(1-10) like a
+    trained net's), S = saturated second moments in [0, 1e-2).  (With S much smaller than g^2 the RMSProp step is ~sign(g)
+    and two correct fp32 implementations drift apart by percents within 5 steps.)"""
+    from oracle import dqn_oracle as O
+    rs = np.random.RandomState(seed)
+    ws, ss = [], []
+    for shp in O.layer_shapes(num_actions):
+        ws.append((rs.standard_normal(shp) * np.sqrt(2.0 / shp[0])).astype(np.float32))
+        ss.append((rs.random_sample(shp) * 1e-2).astype(np.float32))
+    return ws, ss
+
+
 def fixture():
-    g = np.load(os.path.join(GOLDEN, "snapshot_breakout_77.npz"))
-    return [g["W%d" % i] for i in range(5)], [g["S%d" % i] for i in range(5)], g["q_kat"]
+    """(W, S) of the A = 4 stand-in snapshot and q_kat: the numpy oracle's Q rows for it on the KAT states
+    (RandomState(1234) uint8 states), stored when the fixture was made (tests/golden/make_snapshot_fixture.py)."""
+    ws, ss = snapshot_weights(4)
+    return ws, ss, np.load(os.path.join(GOLDEN, "snapshot_q_kat.npz"))["q_kat"]
 
 
 def rebuild(skel, arrays):

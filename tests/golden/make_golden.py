@@ -1,4 +1,4 @@
-"""Generate tests/golden/replay_golden.npz by running the UNMODIFIED reference files
+"""Generate tests/golden/replay_golden.npz and replay_live_golden.npz by running the UNMODIFIED reference files
 /root/reference/src/replay_memory.py and /root/reference/src/state_buffer.py.
 
 Run in the build container only (the GPU box has no /root/reference):
@@ -92,6 +92,27 @@ def main():
     out["statebuffer/crc"] = crc(buf.getStateMinibatch())
     out["names"] = np.array(names)
     path = os.path.join(HERE, "replay_golden.npz")
+    np.savez_compressed(path, **out)
+    print("wrote", path, os.path.getsize(path), "bytes")
+    live_case(replay_memory)
+
+
+def live_case(replay_memory):
+    """replay_live_golden.npz: ring 500, 1300 env steps (terminal_p 0.03, seed 3), random.seed(99), 20 minibatches —
+    every output array of getMinibatch (frames as CRCs) and the `random` state after them."""
+    args = types.SimpleNamespace(screen_height=84, screen_width=84, history_length=4, batch_size=32)
+    mem = replay_memory.ReplayMemory(500, args)
+    for (a, r, s, t) in indexed_episode_stream(1300, seed=3, terminal_p=0.03):
+        mem.add(a, r, s, t)
+    random.seed(99)
+    out = {"pre_crc": [], "post_crc": [], "actions": [], "rewards": [], "terminals": []}
+    for _ in range(20):
+        pre, a, r, post, t = mem.getMinibatch()
+        out["pre_crc"].append(crc(pre)); out["post_crc"].append(crc(post))
+        out["actions"].append(a.copy()); out["rewards"].append(r.copy()); out["terminals"].append(t.copy())
+    out = {k: np.array(v, dtype=np.uint32) if k.endswith("crc") else np.stack(v) for k, v in out.items()}
+    out["mt_after"] = np.array(random.getstate()[1], dtype=np.uint32)
+    path = os.path.join(HERE, "replay_live_golden.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, os.path.getsize(path), "bytes")
 

@@ -1,16 +1,16 @@
-"""Generate tests/golden/snapshot_breakout_77.npz and snapshot_layouts.json from the reference's
-shipped checkpoints (/root/reference/snapshots/*.pkl).  Build container only:
+"""Generate tests/golden/snapshot_q_kat.npz and, given the reference's shipped checkpoints (SNAP below),
+snapshot_layouts.json:
 
-    python tests/golden/make_snapshot_fixture.py
+    python tests/golden/make_snapshot_fixture.py [--layouts]
 
 What is kept (data only — no reference source):
-  * breakout_77.pkl (pre-1.0 ``layer_params_states`` layout): the fp32 W and RMSProp state of all five
-    layers, bit for bit, plus the fp32 Q-values the numpy oracle computes from them on the KAT input of
-    SURVEY §8(c) (RandomState(1234) states) — the known answer the device must reproduce;
-  * seaquest_178.pkl (neon 1.3.0 layout): the pickle's SKELETON — every key, type string and config
-    dict of the 9-entry layer list with the arrays replaced by (shape, dtype, crc32) — so that tests can
-    rebuild a byte-faithful 1.3.0-layout checkpoint around any weights and check that the product's
-    writer emits the same structure; plus the CRCs of both files' arrays for the container-only live test.
+  * snapshot_q_kat.npz: the fp32 Q-values the numpy oracle computes on the KAT input of SURVEY §8(c)
+    (RandomState(1234) states) from the seeded stand-in snapshot of tests/ckpt_helpers.py — the known answer
+    the device must reproduce.  (A trained snapshot's weights are 13 MB, too large to keep as test data.)
+  * --layouts: the SKELETONS of breakout_77.pkl (pre-1.0 ``layer_params_states`` layout) and seaquest_178.pkl
+    (neon 1.3.0 layout) — every key, type string and config dict with the arrays replaced by (shape, dtype,
+    crc32) — so that tests can rebuild a byte-faithful checkpoint in either layout around any weights and check
+    that the product's writer emits the same structure.
 """
 import json
 import os
@@ -50,16 +50,13 @@ def skeleton(obj):
 
 
 def main():
-    ws, ss = O.load_snapshot(os.path.join(SNAP, "breakout_77.pkl"))
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from ckpt_helpers import snapshot_weights
+    ws, _ = snapshot_weights(4)
     states = np.random.RandomState(1234).randint(0, 256, (32, 4, 84, 84)).astype(np.uint8)
-    q = O.forward(ws, states)
-    assert np.allclose(q[0], [4.052785, 3.199721, 5.557730, 4.043888], atol=2e-5)   # SURVEY §8(c) KAT
-    out = {"q_kat": q.astype(np.float32)}
-    for i, (w, s) in enumerate(zip(ws, ss)):
-        out["W%d" % i] = np.asarray(w, np.float32)
-        out["S%d" % i] = np.asarray(s, np.float32)
-    np.savez_compressed(os.path.join(HERE, "snapshot_breakout_77.npz"), **out)
-
+    np.savez_compressed(os.path.join(HERE, "snapshot_q_kat.npz"), q_kat=O.forward(ws, states).astype(np.float32))
+    if "--layouts" not in sys.argv:
+        return
     with open(os.path.join(SNAP, "breakout_77.pkl"), "rb") as f:
         old = pickle.load(f, encoding="latin1")
     with open(os.path.join(SNAP, "seaquest_178.pkl"), "rb") as f:
@@ -71,7 +68,6 @@ def main():
                              "note": "backend.rng_state (NervanaGPU RNG words) omitted from the skeleton"}}
     with open(os.path.join(HERE, "snapshot_layouts.json"), "w") as f:
         json.dump(meta, f, indent=1, sort_keys=True)
-    print("wrote", os.path.getsize(os.path.join(HERE, "snapshot_breakout_77.npz")), "bytes of weights")
 
 
 if __name__ == "__main__":

@@ -55,14 +55,21 @@ def test_config_default_matches_reference_flags(lib):
     assert (cfg.min_reward, cfg.max_reward, cfg.target_steps) == (-1, 1, 10000)
 
 
-def test_binary_is_blackwell_native():
-    """The shipped cubin targets sm_100a and the gather uses the TMA bulk-copy engine."""
-    if not shutil.which("cuobjdump"):
+def test_binary_is_hopper_native():
+    """The shipped cubin targets sm_90a (and nothing else), the GEMM-shaped kernels run on warpgroup MMAs, conv1
+    gathers its frames by tensor-map TMA, and the replay gather uses the TMA bulk-copy engine."""
+    from simple_dqn_b200.build import NVCC
+    cuobjdump = shutil.which("cuobjdump") or os.path.join(os.path.dirname(NVCC), "cuobjdump")
+    if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     from simple_dqn_b200 import _lib as L
-    elf = subprocess.check_output(["cuobjdump", "-lelf", L.LIB_PATH], text=True)
-    assert "sm_100a" in elf
-    sass = subprocess.check_output(["cuobjdump", "-sass", L.LIB_PATH], text=True, stderr=subprocess.STDOUT)
+    elf = subprocess.check_output([cuobjdump, "-lelf", L.LIB_PATH], text=True)
+    archs = set(re.findall(r"\.(sm_\w+)\.cubin", elf))
+    assert archs == {"sm_90a"}, archs
+    sass = subprocess.check_output([cuobjdump, "-sass", L.LIB_PATH], text=True, stderr=subprocess.STDOUT)
+    for shape in ("64x32x16", "64x64x16", "64x128x16"):
+        assert "HGMMA.%s.F32" % shape in sass, shape
+    assert "UTMALDG.3D" in sass
     gather = sass[sass.index("k_gather"):]
     gather = gather[:gather.index(".....", 200) if "....." in gather[200:] else len(gather)]
     assert "UBLKCP" in gather

@@ -1,11 +1,11 @@
-"""§8 a17 / f2: the reference's shipped checkpoints through the PRODUCT on the device.
+"""§8 a17 / f2: checkpoints in the reference's file layouts through the PRODUCT on the device.
 
-tests/golden/snapshot_breakout_77.npz holds the fp32 W and RMSProp state of /root/reference/snapshots/
-breakout_77.pkl bit for bit (generator: tests/golden/make_snapshot_fixture.py); snapshot_layouts.json holds the
-structure of both pickle layouts found in snapshots/.  The tests rebuild a checkpoint file in EACH layout around
-those weights, load it with DeepQNetwork.load_weights (src/deepqnetwork.py:188-189) and hold the device to the
-Q-value known answer of SURVEY §8(c); then train on the trained weights (every other GPU test runs on Xavier
-weights) and round-trip through save_weights (:191-192)."""
+tests/golden/snapshot_layouts.json holds the structure of both pickle layouts found in the reference's snapshots/;
+tests/ckpt_helpers.py makes a seeded stand-in for a trained snapshot (large weights, saturated RMSProp state) and
+tests/golden/snapshot_q_kat.npz the numpy oracle's Q-values for it on the KAT states of SURVEY §8(c).  The tests
+rebuild a checkpoint file in EACH layout around those weights, load it with DeepQNetwork.load_weights
+(src/deepqnetwork.py:188-189) and hold the device to the Q-value known answer; then train on those weights (every
+other GPU test runs on Xavier weights) and round-trip through save_weights (:191-192)."""
 import json
 import os
 import pickle
@@ -13,17 +13,15 @@ import pickle
 import numpy as np
 import pytest
 
-from conftest import GOLDEN, needs_reference
+from conftest import GOLDEN
 from helpers import make_args, random_minibatch, rel_l2
 from oracle import dqn_oracle as O
 
 pytestmark = pytest.mark.gpu
 MODES = ["fp32", "tcgen05"]
-KAT_Q0 = [4.052785, 3.199721, 5.557730, 4.043888]          # SURVEY §8(c), breakout_77 weights
-KAT_Q31 = [0.752620, 0.125157, 4.278520, 2.264925]
 
 
-from ckpt_helpers import fixture as _fixture, write_checkpoint as _write_checkpoint
+from ckpt_helpers import fixture as _fixture, snapshot_weights as _snapshot_weights, write_checkpoint as _write_checkpoint
 
 
 def _net(mode, **kw):
@@ -44,14 +42,15 @@ def test_load_reference_layouts_and_q_kat(tmp_path, mode, layout):
         assert (w1[l] == ws[l]).all() and (s1[l] == ss[l]).all(), l           # weights AND optimizer state, bit for bit
     states = np.random.RandomState(1234).randint(0, 256, (32, 4, 84, 84)).astype(np.uint8)
     q = net.predict(states)
-    assert np.allclose(q[0], KAT_Q0, atol=2e-5 * 5.6) and np.allclose(q[31], KAT_Q31, atol=2e-5 * 5.6), (q[0], q[31])
+    tol = 2e-5 * np.abs(q_kat).max()
+    assert np.allclose(q[0], q_kat[0], atol=tol) and np.allclose(q[31], q_kat[31], atol=tol), (q[0], q[31])
     assert np.abs(q - q_kat).max() <= 1e-3 * np.abs(q_kat).max()             # north_star's bar; measured ~1e-5
     assert np.abs(q - q_kat).max() <= 5e-5 * np.abs(q_kat).max(), np.abs(q - q_kat).max() / np.abs(q_kat).max()
 
 
 @pytest.mark.parametrize("mode", MODES)
 def test_train_on_trained_weights(mode):
-    """One step and a 5-step trajectory starting from the reference's trained (W, S): the regime the published
+    """One step and a 5-step trajectory starting from the stand-in snapshot's (W, S): the regime the published
     runs spend their time in (large Q, saturated second moments), unlike Xavier x 3."""
     from simple_dqn_b200 import Stream
     ws, ss, _ = _fixture()
@@ -116,13 +115,14 @@ def test_save_weights_structure_matches_reference_layout(tmp_path, layout):
         assert (l["params"]["W"] == w).all() and (l["states"][0] == s).all()
 
 
-@needs_reference
-@pytest.mark.parametrize("name,actions", [("breakout_77", 4), ("seaquest_178", 18), ("pong_141", 3),
-                                          ("space_invaders_126", 6)])
-def test_live_reference_snapshots(name, actions):
-    """Build container + GPU only: the real files (both layouts, four action counts) through load_weights."""
+@pytest.mark.parametrize("layout,actions", [("pre-1.0", 4), ("neon-1.3.0", 18), ("neon-1.3.0", 3),
+                                            ("neon-1.3.0", 6)])
+def test_rebuilt_snapshots_of_every_action_count(tmp_path, layout, actions):
+    """Checkpoint files in both layouts for the four action counts of the reference's snapshots (Breakout 4,
+    Seaquest 18, Pong 3, Space Invaders 6) through load_weights, against the oracle on what the file holds."""
     from simple_dqn_b200 import DeepQNetwork
-    path = "/root/reference/snapshots/%s.pkl" % name
+    path = str(tmp_path / "snap.pkl")
+    _write_checkpoint(path, layout, *_snapshot_weights(actions, seed=100 + actions))
     net = DeepQNetwork(actions, make_args(), math_mode="tcgen05")
     net.load_weights(path)
     ws, ss = O.load_snapshot(path)

@@ -1,4 +1,4 @@
-"""Developer tool: print the in-kernel timeline of one tcgen05 kernel (B200DQN_TRACE_LABEL=conv3_fwd ...)."""
+"""Developer tool: print the in-kernel timeline of one tensor-core kernel (B200DQN_TRACE_LABEL=conv3_fwd ...)."""
 import os, sys, types
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
