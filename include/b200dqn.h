@@ -280,8 +280,8 @@ enum {
   B200DQN_NET_PTR_H4            /* (batch,512)                                                         */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
-/* The fused optimizers of the tensor-core engine never materialise dW4; ask them to keep a copy (tests,
- * debugging) before the step whose gradients b200dqn_net_get_grads should return. */
+/* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well
+ * (tests, debugging). */
 int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
 int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream);

@@ -1,6 +1,4 @@
 // capi.cu — library-wide entry points: error text, version, device probe.
-#include <mutex>
-#include <unordered_set>
 #include <stdarg.h>
 #include <stdlib.h>
 
@@ -60,19 +58,6 @@ struct KtState {
 } g_kt;
 }  // namespace
 
-void prefer_max_smem_carveout(const void* kernel) {
-  static const bool on = getenv("B200DQN_CARVEOUT") && atoi(getenv("B200DQN_CARVEOUT")) != 0;
-  if (!on) return;
-  static std::mutex mu;
-  static std::unordered_set<const void*> done;
-  std::lock_guard<std::mutex> lock(mu);
-  if (!done.insert(kernel).second) return;
-  // a preference, not a requirement: ignore the (never observed) failure rather than fail the launch
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) !=
-      cudaSuccess)
-    cudaGetLastError();
-}
-
 static int early_trigger_flag(const char* label) {
   static const char* list = getenv("B200DQN_EARLY_TRIGGER");
   if (!list) return 0;
@@ -106,7 +91,6 @@ static KTrace ktrace_slot_plain(const char* label) {
 __global__ void k_kt_tick(unsigned long long* buf) { buf[kKtGate] += 1; }
 bool ktrace_tick(cudaStream_t st) {
   if (!g_kt.on || !g_kt.gated) return false;
-  prefer_max_smem(k_kt_tick);
   k_kt_tick<<<1, 1, 0, st>>>(g_kt.d_buf);
   return true;
 }
@@ -197,14 +181,7 @@ extern "C" int b200dqn_stream_create(int device, void** out_stream) {
   B2_REQUIRE(out_stream, B200DQN_EINVAL, "stream_create: null argument");
   b200::DeviceGuard g(device);
   cudaStream_t st;
-  const char* sp = getenv("B200DQN_STREAM_PRIO");            // experiment knob: "hi" = highest priority
-  if (sp && !strcmp(sp, "hi")) {
-    int prio_lo = 0, prio_hi = 0;
-    B2_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-    B2_CHECK_CUDA(cudaStreamCreateWithPriority(&st, cudaStreamNonBlocking, prio_hi));
-  } else {
-    B2_CHECK_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  }
+  B2_CHECK_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   *out_stream = st;
   return B200DQN_OK;
 }

@@ -567,7 +567,6 @@ extern "C" int b200dqn_net_comm_destroy(b200dqn_net* n) {
   cudaDeviceSynchronize();
   // captured steps hold nodes of this communicator
   if (n->graph_exec) { cudaGraphExecDestroy(n->graph_exec); n->graph_exec = nullptr; }
-  if (n->graph_def_exec) { cudaGraphExecDestroy(n->graph_def_exec); n->graph_def_exec = nullptr; }
   if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
   comm_destroy(n);
   return B200DQN_OK;

@@ -109,49 +109,25 @@ struct NoPdlScope {
   ~NoPdlScope() { g_pdl_suppressed = prev; }
 };
 
-// B200DQN_CARVEOUT=1 (experiment, off by default): every kernel of the library asks for the LARGEST shared-memory
-// carveout, including the ones that use no shared memory at all.  The L1/shared split is an SM-wide setting that can
-// only change while the SM is idle: a streaming kernel (fc1 optimizer: 1 KB of shared memory per CTA) that configures
-// an SM for "mostly L1" locks the tensor-core kernels (81-193 KB per CTA) out of that SM until its CTAs have left.
-// It helps when the optimizer runs at the head of the step (B200DQN_DEFER_FC1=1) and cost time in the default schedule
-// where it was measured (an earlier GPU generation), hence off; not re-measured on H100.
-void prefer_max_smem_carveout(const void* kernel);   // capi.cu; once per kernel
-template <class K>
-static inline void prefer_max_smem(K* kernel) { prefer_max_smem_carveout(reinterpret_cast<const void*>(kernel)); }
-
-// cluster_x > 1: thread-block clusters of that many CTAs along grid x (split-K partners reducing through DSMEM)
 template <class... KArgs, class... Args>
-static inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem,
-                                             cudaStream_t st, int cluster_x, Args&&... args) {
+static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                     Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int na = 0;
   if (g_use_pdl && !g_pdl_suppressed) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
     ++na;
   }
-  if (cluster_x > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = unsigned(cluster_x);
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
   cfg.attrs = attr;
   cfg.numAttrs = na;
   ++g_launch_count;
-  prefer_max_smem(kernel);
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-template <class... KArgs, class... Args>
-static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                                     Args&&... args) {
-  return launch_pdl_cluster(kernel, grid, block, smem, st, 1, static_cast<Args&&>(args)...);
 }
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -211,25 +187,6 @@ __device__ __forceinline__ void tma_bulk_wait_read_all() {
 // lets the successor start its own prologue (barrier init, index setup) early.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-// ---- thread-block cluster helpers (split-K partners)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_arrive_release() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait_acquire() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
-// shared::cluster address of `local_smem_addr` in the CTA of rank `rank`
-__device__ __forceinline__ uint32_t dsmem_addr(uint32_t local_smem_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
-  return v;
-}
 // generic-proxy writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");

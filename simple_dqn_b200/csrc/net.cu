@@ -396,7 +396,7 @@ enum BwdOp { kFc1Wgrad, kFc1Dgrad, kConv3Wgrad, kConv3Dgrad, kConv2Wgrad, kConv2
 static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cudaStream_t st) {
   const LayerTable& lt = n->lt;
   const float* w = n->d_w;
-  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05 && umma_has_backward())
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
     return umma_backward_op(n, int(op), fs.src[0], fs.idx[0], fs.shift[0], rows, st);
   switch (op) {
     case kFc1Wgrad: {
@@ -513,39 +513,8 @@ static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
 // Peer-memory exchange (comm_p2p.cuh): no shared communicator, so every layer's gradient is reduced
 // the moment its wgrad has finished, on that layer's own branch, and only conv1's 32 KB exchange is left
 // on the critical chain:  wgrad -> partial sums -> exchange (in place, all ranks) -> RMSProp from d_g.
-// ---- software-pipelined fc1 update (net.cuh: graph_def_exec) ----------------------------------------------------
-// In the deferred variant of the step graph the fc1 optimizer does not run where dW4 becomes available; the step
-// only marks the update as pending ...
-static int fc1_update_deferred(b200dqn_net* n, cudaStream_t branch) {
-  B2_CHECK_CUDA(cudaMemsetAsync(n->d_fc1_pending, 1, sizeof(uint32_t), branch));   // != 0
-  return B200DQN_OK;
-}
-// ... the NEXT step applies it first thing, on a side branch under its forward convolutions (joined before fc1_fwd) ...
-static int fc1_update_leading(b200dqn_net* n, cudaStream_t st) {
-  cudaStream_t sA = n->side[0];
-  B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(sA, n->ev[15], 0));
-  {
-    NoPdlScope side;
-    B2_TRY(umma_opt_fc1(n, n->nb, sA, false, n->d_fc1_pending));
-  }
-  B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sA));
-  return B200DQN_OK;
-}
-// ... and train_fused applies the last one before it returns.
-static int fc1_update_flush(b200dqn_net* n, cudaStream_t st) {
-  if (!n->fc1_pending) return B200DQN_OK;
-  {
-    NoPdlScope plain;
-    B2_TRY(umma_opt_fc1(n, n->nb, st, false, n->d_fc1_pending));
-  }
-  B2_CHECK_CUDA(cudaMemsetAsync(n->d_fc1_pending, 0, sizeof(uint32_t), st));
-  n->fc1_pending = false;
-  return B200DQN_OK;
-}
 static void destroy_step_graphs(b200dqn_net* n) {
   if (n->graph_exec) { cudaGraphExecDestroy(n->graph_exec); n->graph_exec = nullptr; }
-  if (n->graph_def_exec) { cudaGraphExecDestroy(n->graph_def_exec); n->graph_def_exec = nullptr; }
 }
 
 static int backward_and_update_xchg(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
@@ -649,8 +618,7 @@ static int backward_and_update_gather(b200dqn_net* n, const FrameSource& fs, int
   {
     NoPdlScope side;
     B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
-    if (n->defer_fc1) B2_TRY(fc1_update_deferred(n, sA));    // applied under the next step's forward (net.cuh)
-    else B2_TRY(umma_opt_fc1(n, rows, sA));                  // dW4 is already the global sum
+    B2_TRY(umma_opt_fc1(n, rows, sA));                       // dW4 is already the global sum
     B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
     B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB));
     if (!fused_xll) {
@@ -791,53 +759,29 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   cudaStream_t sN = g_prof_on ? st : n->side[3];
   cudaEvent_t* ev = n->ev;
   const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
-  static const bool fc1_fused_epilogue = getenv("B200DQN_FC1_FUSED") != nullptr;   // experimental alternative
-  // experiment knobs: bit op of B200DQN_NOPDL_OPS launches that chain kernel without the programmatic dependency;
-  // B200DQN_WGRAD_ONE_STREAM puts conv2_wgrad / opt_conv2 on conv3_wgrad's branch
-  static const int nopdl_ops = getenv("B200DQN_NOPDL_OPS") ? int(strtol(getenv("B200DQN_NOPDL_OPS"), nullptr, 0)) : 0;
-  if (getenv("B200DQN_WGRAD_ONE_STREAM") && !g_prof_on) sC = sB;
-  auto chain_op = [&](BwdOp op) -> int {
-    if (nopdl_ops >> int(op) & 1) {
-      NoPdlScope plain;
-      return bwd_op(n, fs, rows, op, st);
-    }
-    return bwd_op(n, fs, rows, op, st);
-  };
   B2_CHECK_CUDA(cudaEventRecord(ev[0], st));                 // dZ4, the dW5 partials and the per-sample costs are ready
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[0], 0));
   B2_CHECK_CUDA(cudaStreamWaitEvent(sN, ev[0], 0));
   {
     NoPdlScope side;
-    if (!(tc && fc1_fused_epilogue)) B2_TRY(bwd_op(n, fs, rows, kFc1Wgrad, sA));   // overlaps fc1_dgrad (few CTAs)
+    B2_TRY(bwd_op(n, fs, rows, kFc1Wgrad, sA));             // overlaps fc1_dgrad (few CTAs)
     // fourth branch: the scalar cost and the 512 x A layer — nothing later in the step reads W5, and nothing here
     // sits in front of the fc1 optimizer any more
     B2_TRY(cost_finish_on(n, rows, sN));
     if (tc) B2_TRY(opt_fc2_small(n, rows, sN));
   }
-  B2_TRY(chain_op(kFc1Dgrad));
+  B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st));
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
-  // experiment knob B200DQN_OPT_FC1_WHEN: "ev2" / "ev3" = also wait for conv3_dgrad / conv2_dgrad, "last" = same
-  // dependencies but captured after every other node of the step, "skip" = not launched (timing studies only)
-  static const char* fc1_when_env = getenv("B200DQN_OPT_FC1_WHEN");
-  const int fc1_when = !fc1_when_env || g_prof_on ? 0 : !strcmp(fc1_when_env, "ev2") ? 2 : !strcmp(fc1_when_env, "ev3") ? 3
-                       : !strcmp(fc1_when_env, "last") ? 4 : !strcmp(fc1_when_env, "skip") ? 5 : 0;
-  auto opt_fc1_now = [&]() -> int {
-    NoPdlScope side;
-    if (tc && fc1_fused_epilogue) return umma_fc1_wgrad_fused(n, rows, sA, n->keep_grads);
-    if (tc && n->defer_fc1) return fc1_update_deferred(n, sA);   // applied under the next step's forward (net.cuh)
-    if (tc) return umma_opt_fc1(n, rows, sA);                // smem-free: co-resides with the dgrad chain
-    return optimizer_range(n, 3, 4, 1 | 4, rows, sA, "opt_fc");
-  };
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
-  if (fc1_when == 0) B2_TRY(opt_fc1_now());
+  {
+    NoPdlScope side;
+    if (tc) B2_TRY(umma_opt_fc1(n, rows, sA));               // smem-free: co-resides with the dgrad chain
+    else B2_TRY(optimizer_range(n, 3, 4, 1 | 4, rows, sA, "opt_fc"));
+  }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
-  B2_TRY(chain_op(kConv3Dgrad));
+  B2_TRY(bwd_op(n, fs, rows, kConv3Dgrad, st));
   B2_CHECK_CUDA(cudaEventRecord(ev[2], st));                 // dZ2 ready, W3 no longer needed
-  if (fc1_when == 2) {
-    B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[2], 0));
-    B2_TRY(opt_fc1_now());
-  }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[2], 0));
   {
     NoPdlScope side;
@@ -846,22 +790,17 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[2], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv2Wgrad, sC)); }
-  B2_TRY(chain_op(kConv2Dgrad));
+  B2_TRY(bwd_op(n, fs, rows, kConv2Dgrad, st));
   B2_CHECK_CUDA(cudaEventRecord(ev[3], st));                 // dZ1 ready, W2 no longer needed
-  if (fc1_when == 3) {
-    B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[3], 0));
-    B2_TRY(opt_fc1_now());
-  }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[3], 0));
   {
     NoPdlScope side;
     if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 1, rows, sC, "opt_conv2"));
     else B2_TRY(optimizer_range(n, 1, 1, 1 | 4, rows, sC, "opt_conv2"));
   }
-  B2_TRY(chain_op(kConv1Wgrad));
+  B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st));
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 0, rows, st, "opt_conv1"));
   else B2_TRY(optimizer_range(n, 0, 0, 1 | 4, rows, st, "opt_conv1"));
-  if (fc1_when == 4) B2_TRY(opt_fc1_now());
   B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));
   B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
   B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
@@ -1051,17 +990,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   {
     int prio_lo = 0, prio_hi = 0;   // numerically larger = lower priority
     B2_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-    const char* sp = getenv("B200DQN_SIDE_PRIO");            // experiment knob: "hi" / "lo" for all four
-    for (int i = 0; i < 4; ++i) {
-      int prio = i < 3 ? prio_lo : prio_hi;
-      if (sp && !strcmp(sp, "hi")) prio = prio_hi;
-      if (sp && !strcmp(sp, "lo")) prio = prio_lo;
-      B2_CHECK_CUDA(cudaStreamCreateWithPriority(&n->side[i], cudaStreamNonBlocking, prio));
-    }
+    for (int i = 0; i < 4; ++i)   // the three wgrad/optimizer branches low, the collective stream high
+      B2_CHECK_CUDA(cudaStreamCreateWithPriority(&n->side[i], cudaStreamNonBlocking, i < 3 ? prio_lo : prio_hi));
   }
   for (auto& e : n->ev) B2_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  B2_CHECK_CUDA(cudaMalloc(&n->d_fc1_pending, sizeof(uint32_t)));
-  B2_CHECK_CUDA(cudaMemset(n->d_fc1_pending, 0, sizeof(uint32_t)));
   n->use_graph = getenv("B200DQN_NO_GRAPH") == nullptr;
   n->use_branches = getenv("B200DQN_NO_BRANCHES") == nullptr;
   int rc = umma_net_init(n);
@@ -1079,7 +1011,6 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   umma_net_destroy(n);
   destroy_step_graphs(n);
   if (n->graph_train_exec) cudaGraphExecDestroy(n->graph_train_exec);
-  cudaFree(n->d_fc1_pending);
   if (n->graph_predict_exec) cudaGraphExecDestroy(n->graph_predict_exec);
   for (auto& sd : n->side) if (sd) cudaStreamDestroy(sd);
   for (auto& e : n->ev) if (e) cudaEventDestroy(e);
@@ -1193,7 +1124,6 @@ extern "C" int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_sta
     B2_CHECK_CUDA(cudaMemcpyAsync(dev_q, n->d_q[0], size_t(live_rows) * n->A * sizeof(float),
                                   cudaMemcpyDeviceToDevice, st));
   if (live_rows < n->nb) {
-    prefer_max_smem(k_zero_rows);
     k_zero_rows<<<cdiv((n->nb - live_rows) * n->A, 128), 128, 0, st>>>(dev_q, live_rows, n->nb, n->A);
     B2_LAUNCH_CHECK();
   }
@@ -1239,7 +1169,6 @@ extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* de
     HeadTrainArgs no_td{};
     int rc = forward(n, fs, 1, live_rows, st, no_td);
     if (!rc) {
-      prefer_max_smem(k_publish_q_counter);
       k_publish_q_counter<<<1, 64, 0, st>>>(n->d_q[0], count, n->h_res, n->d_optscal_u32());
       if (cudaGetLastError() != cudaSuccess) rc = B200DQN_ECUDA;
     }
@@ -1410,40 +1339,25 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
       destroy_step_graphs(n);
       n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
     }
-    // B200DQN_DEFER_FC1=1 (experiment, off by default): several steps in one call -> the fc1 update of step t rides under
-    // the forward of step t+1 (net.cuh).  Parity-clean but slower where it was measured (an earlier GPU generation):
-    // the 45 MB the update moves through L2 stretch whatever runs beside it, and the forward convolutions lose more
-    // than the dgrad chain gains.  Not re-measured on H100.
-    static const bool defer_on = getenv("B200DQN_DEFER_FC1") && atoi(getenv("B200DQN_DEFER_FC1")) != 0;
-    const bool deferred = nsteps >= 2 && defer_on && n->use_branches && n->cfg.math_mode == B200DQN_MATH_TCGEN05 &&
-                          (n->world == 1 || comm_gather_active(n, st));
-    cudaGraphExec_t* exec = deferred ? &n->graph_def_exec : &n->graph_exec;
-    if (!*exec) {
+    if (!n->graph_exec) {
       cudaGraph_t graph = nullptr;
       B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
       const long long launches_before = g_launch_count;
-      n->defer_fc1 = deferred;
       {
         const bool prev = g_pdl_suppressed;
         if (ktrace_tick(st)) g_pdl_suppressed = true;   // the sampler must not start ahead of the tick
-        rc = deferred ? fc1_update_leading(n, st) : B200DQN_OK;
-        if (!rc) rc = launch_sample(r, st);
+        rc = launch_sample(r, st);
         g_pdl_suppressed = prev;
       }
       if (!rc) rc = train_on_ring(n, r, st);
-      n->defer_fc1 = false;
-      (deferred ? n->graph_def_launches : n->graph_launches) = int(g_launch_count - launches_before);
+      n->graph_launches = int(g_launch_count - launches_before);
       cudaError_t e = cudaStreamEndCapture(st, &graph);
       if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
       B2_CHECK_CUDA(e);
-      B2_CHECK_CUDA(cudaGraphInstantiate(exec, graph, 0));
+      B2_CHECK_CUDA(cudaGraphInstantiate(&n->graph_exec, graph, 0));
       cudaGraphDestroy(graph);
     }
-    for (int i = 0; i < nsteps; ++i) B2_CHECK_CUDA(cudaGraphLaunch(*exec, st));
-    if (deferred) {
-      n->fc1_pending = true;
-      B2_TRY(fc1_update_flush(n, st));
-    }
+    for (int i = 0; i < nsteps; ++i) B2_CHECK_CUDA(cudaGraphLaunch(n->graph_exec, st));
   } else {
     for (int i = 0; i < nsteps; ++i) {
       const bool prev = g_pdl_suppressed;
@@ -1558,9 +1472,6 @@ extern "C" int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep) {
 
 extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream) {
   B2_REQUIRE(n && host_dW && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_get_grads: bad argument");
-  B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || n->world > 1 || n->keep_grads ||
-                 getenv("B200DQN_FC1_FUSED") == nullptr,
-             B200DQN_ESTATE, "net_get_grads: call b200dqn_net_set_keep_grads(net, 1) before the step (fused optimizer)");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
   const int64_t n4 = n->n_params / 4;
@@ -1582,9 +1493,7 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
   B2_REQUIRE(n && launches, B200DQN_EINVAL, "null argument");
   // Counted at the launch sites while the step was captured into its CUDA graph; before the first
   // fused step: the static schedule (sample, 4 forward, head, 7 backward GEMMs, per-layer optimizers).
-  if (n->graph_def_launches > 0) {          // the multi-step graph (one gated fc1 update at its head)
-    *launches = n->graph_def_launches;
-  } else if (n->graph_launches > 0) {
+  if (n->graph_launches > 0) {
     *launches = n->graph_launches;
   } else {
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;

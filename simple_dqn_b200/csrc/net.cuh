@@ -81,26 +81,15 @@ struct b200dqn_net {
   // step scheduling: side streams / events for the independent wgrad + optimizer branches, and the
   // captured CUDA graph of one fused step
   cudaStream_t side[4] = {};   // three wgrad/optimizer branches + the collective stream
-  cudaEvent_t ev[17] = {};
+  cudaEvent_t ev[15] = {};
   bool use_graph = true, use_branches = true;
-  bool keep_grads = false;   // fused optimizers also write dW for b200dqn_net_get_grads (tests)
+  bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
   cudaGraphExec_t graph_exec = nullptr;
   b200dqn_replay* graph_replay = nullptr;
   cudaStream_t graph_stream = nullptr;
   int graph_world = 0;
   int graph_trace_gen = 0;
   int graph_launches = 0;   // kernels launched by one captured step
-  // Software-pipelined fc1 update (multi-step train_fused, opt-in B200DQN_DEFER_FC1=1 — measured slower, see
-  // b200dqn_net_train_fused): the graph of step t applies step t-1's fc1 update on a
-  // side branch under its own forward convolutions (joined before fc1_fwd) instead of under the dgrad chain, where its
-  // 2-CTAs-per-SM grid (264 CTAs on 132 SMs) competes with the tensor-core kernels for registers and SM slots; the
-  // last step's update is flushed by train_fused before it returns, so nothing outside that call ever sees a pending
-  // update.
-  cudaGraphExec_t graph_def_exec = nullptr;   // the deferred-update variant of the step graph (same cache keys)
-  int graph_def_launches = 0;
-  bool defer_fc1 = false;                     // set while that variant is being captured
-  bool fc1_pending = false;                   // host view: a deferred step was launched since the last flush
-  uint32_t* d_fc1_pending = nullptr;          // device view, read by the gated optimizer kernel
   cudaGraphExec_t graph_train_exec = nullptr;   // same step without the sampler (train on pre-sampled indexes)
   b200dqn_replay* graph_train_replay = nullptr;
   cudaStream_t graph_train_stream = nullptr;

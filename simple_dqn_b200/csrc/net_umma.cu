@@ -272,12 +272,12 @@ struct V2ConvDgrad {
 // ---- wgrad (MN-major operands, umma_mn.cuh) -----------------------------------------------------
 // conv2 / conv3: dW[(r,s,c)][ko] = sum_{n,p,q} X[n, p*ST+r, q*ST+s, c] * dZ[n,p,q,ko]
 // One 64-wide m chunk is a contiguous run of the NHWC input: (s, c) are adjacent dims and R*C % 64 == 0.
-template <int H, int C, int R, int ST, int KO, int STG = 4>
+template <int H, int C, int R, int ST, int KO>
 struct WConvWgrad {
   static constexpr int P = (H - R) / ST + 1, KW = R * R * C;
   static_assert((R * C) % 64 == 0 && KO == 64, "64-element runs must not straddle a filter row");
-  static constexpr int kBN = 64, kStages = STG;   // 4 stages = 193 KB (one CTA per SM), 2 stages = 97 KB (two)
-  static constexpr bool kAExact = false, kARegs = false, kABulk = false, kFusedUpdate = false;
+  static constexpr int kBN = 64, kStages = 4;   // 193 KB: one CTA per SM
+  static constexpr bool kAExact = false, kABulk = false;
   PlanePair x16;    // [rows][H][H][C]
   PlanePair dz16;   // [rows][P][P][KO]
   float* part;      // [splits][KW][KO]
@@ -309,7 +309,7 @@ struct WConvWgrad {
 // (V2Conv1Fwd::kDumpA) and this kernel fetches each [64 pixels x 64 taps] sub-tile with ONE TMA bulk copy.
 struct WConv1Wgrad {
   static constexpr int kBN = 32, kStages = 4;
-  static constexpr bool kAExact = true, kARegs = false, kABulk = true, kFusedUpdate = false;
+  static constexpr bool kAExact = true, kABulk = true;
   const uint8_t* im2col;   // [pixel tile of 128][c = 4][128 x 128 B]
   PlanePair dz16;          // dZ1 [rows][20][20][32]
   float* part;             // [splits][256][32]
@@ -347,7 +347,7 @@ struct WConv1Wgrad {
 // fc1: dW4[m][n] = sum_b H3[b][m] * dZ4[b][n]; the reduction rows are the batch samples.
 struct WFc1Wgrad {
   static constexpr int kBN = 64, kStages = 2;
-  static constexpr bool kAExact = false, kARegs = false, kABulk = false, kFusedUpdate = false;
+  static constexpr bool kAExact = false, kABulk = false;
   PlanePair h3_16;   // [rows][3136]
   PlanePair dz4_16;  // [rows][512]
   float* dw4;        // [3136][512]
@@ -370,7 +370,7 @@ struct WFc1Wgrad {
 // k_xpush fills (comm_p2p.cuh); the parity of the current push epoch selects the area.
 struct WFc1WgradGather {
   static constexpr int kBN = 64, kStages = 2;
-  static constexpr bool kAExact = false, kARegs = false, kABulk = false, kFusedUpdate = false;
+  static constexpr bool kAExact = false, kABulk = false;
   const __half* h3g;   // [parity][hi | lo][rows][3136]
   const __half* dzg;   // [parity][hi | lo][rows][512]
   int64_t h3_parity, h3_lo, dz_parity, dz_lo;   // elements
@@ -389,47 +389,6 @@ struct WFc1WgradGather {
   __device__ umma2::Planes b_planes(int) const { return {dzg + int64_t(epoch[1] & 1) * dz_parity, dz_lo}; }
   __device__ int64_t b_off(int, const umma_mn::PixCtx& px) const { return int64_t(px.n) * kHidden; }
   __device__ void store8(int, int m, int n0, const float v[8]) const { st8(dw4 + int64_t(m) * kHidden + n0, v); }
-};
-
-// fc1 wgrad with the optimizer fused into its epilogue (single GPU): the tile of dW4 never leaves the
-// SM — RMSProp is applied in place and both fp16 tile images of W4 are refreshed.  Must run after
-// fc1_dgrad (which still reads the old dgrad image).
-struct WFc1WgradFused {
-  static constexpr int kBN = 64, kStages = 2;
-  static constexpr bool kAExact = false, kARegs = false, kABulk = false, kFusedUpdate = true;
-  PlanePair h3_16;
-  PlanePair dz4_16;
-  float* w;           // W4 [3136][512]
-  float* s;           // RMSProp state
-  float* dw_out;      // optional copy of dW4 (b200dqn_net_get_grads), nullptr in production
-  uint8_t* img_dgr;   // [25 m-tiles][8 kb][hi 128x128 | lo] — the one fc1 image (forward reads it MN-major)
-  int rows;
-  OptArgs opt;
-  __device__ int M(int) const { return kFlat; }
-  __device__ int N(int) const { return kHidden; }
-  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = (rows + 63) / 64; }
-  __device__ umma_mn::PixCtx pix(int, int b) const { return {b, 0, 0, b < rows}; }
-  __device__ umma2::Planes a_planes(int) const { return {h3_16.hi, h3_16.lo_off}; }
-  __device__ bool a_run(int, const umma_mn::PixCtx& px, int mchunk, int64_t& off) const {
-    off = int64_t(px.n) * kFlat + mchunk * 64;
-    return mchunk * 64 < kFlat;
-  }
-  __device__ umma2::Planes b_planes(int) const { return {dz4_16.hi, dz4_16.lo_off}; }
-  __device__ int64_t b_off(int, const umma_mn::PixCtx& px) const { return int64_t(px.n) * kHidden; }
-  __device__ void store8(int, int, int, const float*) const {}
-  __device__ float step_scalar() const { return opt_step_scalar(opt); }
-  __device__ void update8(int, int m, int n0, float l, const float g[8], float nw[8]) const {
-    const int64_t i = int64_t(m) * kHidden + n0;
-    if (dw_out) st8(dw_out + i, g);
-    opt_update_vec<8>(opt, l, g, nw, w + i, s + i);   // the configured Neon optimizer (optim.cuh)
-    uint4 hi, lo;
-    umma::split8(nw, hi, lo);
-    uint8_t* base = img_dgr + (int64_t(m / 128) * (kHidden / 64) + n0 / 64) * (128 * 256) +
-                    umma::sw128_off(m % 128, (n0 % 64) / 8);
-    *reinterpret_cast<uint4*>(base) = hi;
-    *reinterpret_cast<uint4*>(base + 128 * 128) = lo;
-  }
-  __device__ void pack_col8(int, int, int, const float*) const {}   // no column-oriented image any more
 };
 
 // ---- weight tile-image sources (k_pack_image) --------------------------------------------------
@@ -584,14 +543,10 @@ k_opt_conv(const float* __restrict__ part, int splits, float* __restrict__ w, fl
 // co-reside with the tensor-core kernels of the critical chain instead of locking them out of the SMs.
 __global__ void __launch_bounds__(256)
 k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
-          const OptArgs opt, const uint32_t* __restrict__ gate, const KTrace kt) {
+          const OptArgs opt, const KTrace kt) {
   kt_begin(kt);
   pdl_wait();
   pdl_launch_dependents();
-  if (gate && *gate == 0) {   // nothing pending (first step after a flush): uniform across the grid
-    kt_end(kt);
-    return;
-  }
   constexpr int kNB = kHidden / 8;
   const float l_step = opt_step_scalar(opt);
   for (int id = blockIdx.x * blockDim.x + threadIdx.x; id < kFlat * kNB; id += gridDim.x * blockDim.x) {
@@ -610,18 +565,17 @@ k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict
   kt_end(kt);
 }
 
-int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g, const uint32_t* gate) {
+int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g) {
   UmmaState* u = ust(n);
   const LayerTable& lt = n->lt;
   const float* dw = from_g ? n->d_g + lt.off[3] : n->d_part + lt.part_off[3];
   // One kernel, one image: the update refreshes the row-oriented tile image in the same pass, and the forward reads
   // that image too (MN-major) — the column-oriented forward image and its re-pack kernel (round 1-2: 6.4 MB read +
   // 6.4 MB written per step, 5 us at the end of the fc1 branch) are gone.
-  // capped grid (CTAs per SM, grid-stride): the kernel shares the SMs — and the L2 — with the dgrad chain
-  static const int per_sm = getenv("B200DQN_OPT_FC1_CTAS") ? atoi(getenv("B200DQN_OPT_FC1_CTAS")) : 2;
-  const int ctas = per_sm > 0 ? per_sm * n->sm_count : n->sm_count / (-per_sm > 0 ? -per_sm : 1);
+  // capped grid (2 CTAs per SM, grid-stride): the kernel shares the SMs — and the L2 — with the dgrad chain
+  const int ctas = 2 * n->sm_count;
   B2_CHECK_CUDA(launch_pdl(k_opt_fc1, dim3(ctas), dim3(256), 0, st, dw, n->d_w + lt.off[3],
-                           n->d_s + lt.off[3], u->img_dgr[0], make_opt_args(n, rows), gate, ktrace_slot("opt_fc1")));
+                           n->d_s + lt.off[3], u->img_dgr[0], make_opt_args(n, rows), ktrace_slot("opt_fc1")));
   B2_PROF("opt_fc1", st);
   return B200DQN_OK;
 }
@@ -726,26 +680,18 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
 // fc1 forward split-K over blockIdx.z (the head kernel sums the partials): 49 k-blocks of 64 -> 7 per CTA,
 // 4 M-tiles x 7 x 2 nets = 56 CTAs at batch 32; large minibatches bring their own tiles, so fewer splits keep the
 // partial-sum traffic down.  (13 splits = 104 CTAs was measured: fc1_fwd 6.3 -> 12 us inside the step — see below.)
+// B200DQN_FC1_SPLITS=n overrides: on an H100 80GB HBM3 at 700 W, 4 splits were 2 % faster at batch 256, the same at 32.
 static inline int fc1_splits_for(int rows) {
   static const int forced = getenv("B200DQN_FC1_SPLITS") ? atoi(getenv("B200DQN_FC1_SPLITS")) : 0;
   if (forced >= 1 && forced <= kFc1Splits) return forced;
   return rows <= 256 ? 7 : 4;
 }
-// Cluster split-K (umma2.cuh) for the kernels whose tile count leaves most of the 132 SMs idle at batch 32:
-//   conv2_fwd 42 tiles x 3 partners (8 k-blocks -> 3/3/2),  conv3_fwd 26 x 4 (9 -> 3/2/2/2),
-//   conv3_dgrad 21 x 4,  fc1_dgrad 25 x 4 (8 -> 2 each).
-// OFF by default (B200DQN_SPLITK=1 turns it on): parity-clean, but slower inside the step where it was measured (an
-// earlier GPU generation; not re-measured on H100): with 100+ CTAs of 193 KB shared memory per kernel the successor of
-// the PDL chain finds no free SM to pre-launch on and the cluster needs all its SMs at once; the few-CTA tiles win
-// because consecutive kernels CO-RESIDE.
-static const bool g_splitk = getenv("B200DQN_SPLITK") && atoi(getenv("B200DQN_SPLITK")) != 0;
-// Larger minibatches already fill the chip with tiles: split only while the tile count is below the SM count.
-static inline bool use_splitk(int tiles, int ks) { return g_splitk && tiles * ks <= 160; }
 constexpr int kUWgradKb = 4;      // minimum k-blocks (of 64 pixels) per wgrad split
 
 // k-blocks (of 64 pixels) per wgrad split: at least kUWgradKb, and few enough splits (<= 48) for the
 // one-pass reduction of k_opt_conv
 // conv1 through tensor-map TMA (conv1_tma.cuh) unless B200DQN_CONV1=ldg selects the register-path gather of umma2.cuh
+// (on an H100 80GB HBM3 at 700 W the ldg path was 3 % faster at batch 32 and 6 % at batch 256)
 static const bool g_conv1_tma = !(getenv("B200DQN_CONV1") && strcmp(getenv("B200DQN_CONV1"), "ldg") == 0);
 static inline int conv1_pixels_padded(int rows) { return g_conv1_tma ? rows * conv1tma::kTilesPerSample * 128 : rows * kP1 * kP1; }
 
@@ -891,10 +837,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the target network's fp32 activations
     }
     p.rows = rows;
-    const int tiles = (rows * kP2 * kP2 + 127) / 128 * nets;
-    if (use_splitk(tiles, 3)) rc = umma2::launch_umma2<P, 3>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st);
-    else rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st);
-    if (rc) return rc;
+    if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
   }
   {
     using P = V2ConvFwd<kP2, kC2, 3, 1, kC3>;
@@ -904,10 +847,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       p.out[z] = z ? nullptr : n->d_h3[z];
     }
     p.rows = rows;
-    const int tiles = (rows * kP3 * kP3 + 127) / 128 * nets;
-    if (use_splitk(tiles, 4)) rc = umma2::launch_umma2<P, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st);
-    else rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st);
-    if (rc) return rc;
+    if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
     // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
     if (nets == 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
   }
@@ -915,36 +855,9 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     V2Fc1Fwd p;
     for (int z = 0; z < 2; ++z) { p.in16[z] = planes(2, z); p.wimg[z] = u->img_fwd[z][3]; }
     p.part = n->d_fc1part; p.rows = rows; p.splits = fc1_splits_for(rows);
-    if (n->defer_fc1) {
-      // the previous step's fc1 update (side branch since the start of this step) must have refreshed the image; the
-      // kernel then has two parents, so it is launched as an ordinary node (its pre-wait weight prefetch would
-      // otherwise run ahead of the join)
-      static const bool keep_pdl = getenv("B200DQN_DEFER_PDL") != nullptr;
-      B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[16], 0));
-      if (keep_pdl) {
-        rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st);
-      } else {
-        NoPdlScope plain;
-        rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st);
-      }
-      if (rc) return rc;
-    } else if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st))) return rc;
+    if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st))) return rc;
   }
   return B200DQN_OK;
-}
-
-// B200DQN_STAGES2=label,label,...: run that kernel with a 2-stage operand ring (about half the shared memory, so two
-// CTAs of the step's kernels fit on an SM) instead of the deepest ring.
-// Default on ONE GPU: conv2_dgrad — 100 CTAs of 4 k-blocks each; at 81 KB instead of 161 KB they occupy 50 SMs instead
-// of 100 while conv3_wgrad / conv2_wgrad / conv1_wgrad look for SMs.  With data-parallel learners the same choice was
-// slower, so there the default is none.  (Chosen on an earlier GPU generation; not re-measured on H100.)
-static bool shallow_ring(const b200dqn_net* net, const char* label) {
-  static const char* env = getenv("B200DQN_STAGES2");
-  const char* list = env ? env : net->world == 1 ? "conv2_dgrad" : "";
-  const size_t n = strlen(label);
-  for (const char* p = list; (p = strstr(p, label)) != nullptr; p += n)
-    if ((p == list || p[-1] == ',') && (p[n] == 0 || p[n] == ',')) return true;
-  return false;
 }
 
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,
@@ -963,18 +876,11 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       // the fp32 copies of dZ3/dZ2/dZ1 have no reader in this engine (wgrads and dgrads take the fp16 planes)
       V2Fc1Dgrad p{u->img_dgr[0], PlanePair{u->dz16[0], u->dz_elems[0]}, n->d_h3[0], n->keep_grads ? n->d_dz3 : nullptr,
                    PlanePair{u->dz16[1], u->dz_elems[1]}, rows};
-      if (use_splitk(25 * ((rows + 31) / 32), 4)) return umma2::launch_umma2<V2Fc1Dgrad, 4>("fc1_dgrad", p, kFlat, rows, 1, st);
       return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows, 1, st);
     }
     case 2: {
       UmmaState* u = ust(n);
       using P = WConvWgrad<kP2, kC2, 3, 1, kC3>;
-      using P2 = WConvWgrad<kP2, kC2, 3, 1, kC3, 2>;
-      if (shallow_ring(n, "conv3_wgrad")) {
-        P2 p{PlanePair{u->h16[1][0], u->h_elems[1]}, PlanePair{u->dz16[1], u->dz_elems[1]},
-             n->d_part + lt.part_off[2], rows, umma_wgrad_kb(2, rows)};
-        return umma_mn::launch_umma_mn("conv3_wgrad", p, P::KW, kC3, lt.splits[2], st);
-      }
       P p{PlanePair{u->h16[1][0], u->h_elems[1]}, PlanePair{u->dz16[1], u->dz_elems[1]},
           n->d_part + lt.part_off[2], rows, umma_wgrad_kb(2, rows)};
       return umma_mn::launch_umma_mn("conv3_wgrad", p, P::KW, kC3, lt.splits[2], st);
@@ -984,19 +890,11 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       using P = V2ConvDgrad<kP2, kC2, 3, 1, kC3>;
       P p{PlanePair{u->dz16[1], u->dz_elems[1]}, u->img_dgr[1], n->d_h2[0], n->keep_grads ? n->d_dz2 : nullptr,
           PlanePair{u->dz16[2], u->dz_elems[2]}, rows};
-      if (use_splitk((rows * P::HC * P::HC + 127) / 128, 4))
-        return umma2::launch_umma2<P, 4>("conv3_dgrad", p, rows * P::HC * P::HC, kC2, 1, st);
       return umma2::launch_umma2("conv3_dgrad", p, rows * P::HC * P::HC, kC2, 1, st);
     }
     case 4: {
       UmmaState* u = ust(n);
       using P = WConvWgrad<kP1, kC1, 4, 2, kC2>;
-      using P2 = WConvWgrad<kP1, kC1, 4, 2, kC2, 2>;
-      if (shallow_ring(n, "conv2_wgrad")) {
-        P2 p{PlanePair{u->h16[0][0], u->h_elems[0]}, PlanePair{u->dz16[2], u->dz_elems[2]},
-             n->d_part + lt.part_off[1], rows, umma_wgrad_kb(1, rows)};
-        return umma_mn::launch_umma_mn("conv2_wgrad", p, P::KW, kC2, lt.splits[1], st);
-      }
       P p{PlanePair{u->h16[0][0], u->h_elems[0]}, PlanePair{u->dz16[2], u->dz_elems[2]},
           n->d_part + lt.part_off[1], rows, umma_wgrad_kb(1, rows)};
       return umma_mn::launch_umma_mn("conv2_wgrad", p, P::KW, kC2, lt.splits[1], st);
@@ -1005,7 +903,12 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       UmmaState* u = ust(n);
       using P = V2ConvDgrad<kP1, kC1, 4, 2, kC2>;
       using P2 = V2ConvDgrad<kP1, kC1, 4, 2, kC2, 2>;
-      if (shallow_ring(n, "conv2_dgrad")) {   // 81 KB per CTA: the 100 CTAs take 50 SMs instead of 100
+      // One GPU: a 2-stage operand ring, 81 KB per CTA instead of 161 KB, so the 100 CTAs take 50 SMs instead of 100
+      // while conv3_wgrad / conv2_wgrad / conv1_wgrad look for SMs.  On an H100 80GB HBM3 at 700 W this is 1.5 %
+      // faster than the deepest ring at batch 256 and the same at 32; shallow rings for the conv3/conv2 wgrads as
+      // well cost 1-2 %.  With data-parallel learners the deepest ring was faster (on an earlier GPU generation;
+      // multi-GPU schedules have not been re-measured on H100).
+      if (n->world == 1) {
         P2 p{PlanePair{u->dz16[2], u->dz_elems[2]}, u->img_dgr[2], n->d_h1[0], n->keep_grads ? n->d_dz1 : nullptr,
              PlanePair{u->dz16[3], u->dz_elems[3]}, rows};
         return umma2::launch_umma2("conv2_dgrad", p, rows * P::HC * P::HC, kC1, 4, st);
@@ -1024,18 +927,7 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
   }
 }
 
-// fc1 wgrad + RMSProp + image refresh in one kernel (single-GPU tensor-core path); must follow fc1_dgrad.
-int umma_fc1_wgrad_fused(b200dqn_net* n, int rows, cudaStream_t st, bool keep_grads) {
-  UmmaState* u = ust(n);
-  const LayerTable& lt = n->lt;
-  WFc1WgradFused p{PlanePair{u->h16[2][0], u->h_elems[2]}, PlanePair{u->dz16[0], u->dz_elems[0]},
-                   n->d_w + lt.off[3], n->d_s + lt.off[3], keep_grads ? n->d_part + lt.part_off[3] : nullptr,
-                   u->img_dgr[0], rows, make_opt_args(n, rows)};
-  return umma_mn::launch_umma_mn("fc1_wgrad+opt", p, kFlat, kHidden, 1, st);
-}
-
 int umma_fc1_splits(int rows) { return fc1_splits_for(rows); }
-bool umma_has_backward() { return true; }
 // ---- gather schedule hooks (data-parallel learners, comm_p2p.cuh) ---------------------------------------
 int umma_push_h3(b200dqn_net* n, cudaStream_t st) {
   UmmaState* u = ust(n);
@@ -1062,9 +954,6 @@ int umma_fc1_wgrad_gathered(b200dqn_net* n, cudaStream_t st) {
                     n->d_xpush_epoch, n->d_part + n->lt.part_off[3], n->nb * n->world};
   return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st);
 }
-
-int umma_forward_launches() { return 4; }
-int umma_backward_launches() { return 7; }
 
 }  // namespace b200
 

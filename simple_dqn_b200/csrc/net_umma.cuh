@@ -22,10 +22,8 @@ int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
                  const int64_t nframes[2], int nets, int rows, cudaStream_t st);
 int umma_fc1_splits(int rows);
-// RMSProp of the fc1 layer + refresh of both of its tile images in one smem-free kernel
-// gate != nullptr: the kernel does nothing unless *gate != 0 (software-pipelined update, net.cuh)
-int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false, const uint32_t* gate = nullptr);
-int umma_fc1_wgrad_fused(b200dqn_net* n, int rows, cudaStream_t st, bool keep_grads);
+// RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel
+int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false);
 // fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tensor-core path
 // from_g: read the (all-reduced) gradient from d_g instead of the split-K partials
 int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* label, bool from_g = false);
@@ -34,12 +32,9 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
 // fp16 hi plane of dZ4 and the offset of its lo plane (nullptr when math_mode != TCGEN05)
 void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
 int umma_wgrad_splits(int layer, int rows);   // split-K factor of the conv wgrad of `layer` (0..2)
-bool umma_has_backward();
 // op: 0 fc1_wgrad, 1 fc1_dgrad, 2 conv3_wgrad, 3 conv3_dgrad, 4 conv2_wgrad, 5 conv2_dgrad, 6 conv1_wgrad
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,
                      cudaStream_t st);
-int umma_forward_launches();
-int umma_backward_launches();
 
 // NCCL glue (comm.cu)
 int comm_allreduce_grads(b200dqn_net* n, cudaStream_t st);

@@ -92,7 +92,6 @@ __global__ void k_publish_words(const uint32_t* __restrict__ words, volatile uin
 }
 
 int replay_publish_words(b200dqn_replay* r, cudaStream_t st) {
-  prefer_max_smem(k_publish_words);
   k_publish_words<<<1, 1, 0, st>>>(r->d_words, r->h_words);
   B2_LAUNCH_CHECK();
   return B200DQN_OK;
@@ -108,7 +107,6 @@ int replay_flush(b200dqn_replay* r, cudaStream_t st) {
   if (first < n)
     B2_CHECK_CUDA(cudaMemcpyAsync(r->d_screens, r->h_bank[b] + first * r->frame_bytes, (n - first) * r->frame_bytes,
                                   cudaMemcpyHostToDevice, st));
-  prefer_max_smem(k_add_meta_batch);
   k_add_meta_batch<<<1, 32, 0, st>>>(r->d_actions, r->d_rewards, r->d_terminals, r->d_cursor, pos0, r->size, n,
                                      r->bank_actions(b), r->bank_rewards(b), r->bank_terminals(b), r->count,
                                      r->current);
@@ -552,12 +550,10 @@ extern "C" int b200dqn_statebuf_add(b200dqn_statebuf* s, const uint8_t* host_scr
   B2_CHECK_CUDA(cudaEventRecord(s->slot_done[slot], st));
   if (s->frame_bytes % 16 == 0) {
     const int64_t n = s->frame_bytes / 16;
-    prefer_max_smem(k_statebuf_shift<uint4>);
     k_statebuf_shift<uint4><<<unsigned((n + 127) / 128), 128, 0, st>>>(
         reinterpret_cast<uint4*>(s->d_buf), reinterpret_cast<const uint4*>(d_fresh), s->hist, n);
   } else {
     const int64_t n = s->frame_bytes;
-    prefer_max_smem(k_statebuf_shift<uint8_t>);
     k_statebuf_shift<uint8_t><<<unsigned((n + 255) / 256), 256, 0, st>>>(s->d_buf, d_fresh, s->hist, n);
   }
   B2_LAUNCH_CHECK();

@@ -154,14 +154,9 @@ constexpr int kThreads2 = kLoadThreads;
 //   lo weight tiles are adjacent in shared memory) and  acc2 += A_lo x B_hi;  then wgmma.wait_group 1 (k-block it-1
 //   has completed in this warpgroup), one named barrier over both warpgroups, and stage (it-1) % S is refilled with
 //   k-block it-1+S while the tensor cores work on k-block it.
-// KS > 1: split-K across a thread-block cluster of KS CTAs along grid x.  Rank r of a cluster walks k-blocks
-// [r*per, (r+1)*per) of its tile into its own accumulators; every rank parks its combined fp32 tile in its own
-// shared memory, rank 0 adds the partners' tiles in rank order through DSMEM loads (deterministic) and runs the
-// epilogue.  Gives the few-CTA kernels of the batch-32 step the whole chip: 2-3 k-blocks per CTA instead of 8-9.
-template <class P, int KS = 1>
+template <class P>
 __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int trace_in, const KTrace kt) {
   using C = Cfg2<P>;
-  static_assert(KS >= 1 && KS <= 8 && !(KS > 1 && P::kDumpA), "cluster split-K: 1..8 partners, not with the A dump");
   constexpr int BN = C::BN;
   constexpr int S = C::kStages;
   extern __shared__ uint8_t smem_raw[];
@@ -173,17 +168,11 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   kt_begin(kt);
   B2_TRACE(tid == 0, 0);
   const int M = p.M(z), N = p.N(z);
-  const int crank = KS > 1 ? int(cluster_ctarank()) : 0;
-  const int mtile = KS > 1 ? int(blockIdx.x) / KS : int(blockIdx.x);
+  const int mtile = blockIdx.x;
   const int m0 = mtile * kBM, n0 = blockIdx.y * BN;
-  if (m0 >= M || n0 >= N) return;      // the same for every partner of a cluster
+  if (m0 >= M || n0 >= N) return;
   int kb0, kb1;
   p.krange(z, kb0, kb1);
-  if constexpr (KS > 1) {
-    const int per = (kb1 - kb0 + KS - 1) / KS;
-    kb0 = min(kb0 + crank * per, kb1);
-    kb1 = min(kb0 + per, kb1);
-  }
   const int nkb = kb1 - kb0;
 
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -406,13 +395,11 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   // fetched now, while the tensor cores are still draining the last k-blocks.
   float pf[P::kPrefetch ? kIt : 1][8];
   if constexpr (P::kPrefetch) {
-    if (crank == 0) {   // partners only contribute accumulators
 #pragma unroll
-      for (int i = 0; i < kIt; ++i) {
-        int r, cc;
-        item(i, r, cc);
-        if (m0 + r < M && n0 + cc * 8 < N) p.prefetch8(z, m0 + r, n0 + cc * 8, pf[i]);
-      }
+    for (int i = 0; i < kIt; ++i) {
+      int r, cc;
+      item(i, r, cc);
+      if (m0 + r < M && n0 + cc * 8 < N) p.prefetch8(z, m0 + r, n0 + cc * 8, pf[i]);
     }
   }
   umma::wgmma_wait<0>();
@@ -425,39 +412,18 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   named_bar_sync(1, kThreads2);   // every warpgroup's MMAs (and the A dump) have finished reading the stages
   B2_TRACE(tid == 0, 4);
   umma::stage_acc<BN>(acc, P::kAExact ? nullptr : acc2, smem_gen, kPitch, wg, warp, lane);
-  if constexpr (KS > 1) {
-    cluster_arrive_release();   // every partner's tile is parked in its own shared memory
-    cluster_wait_acquire();
-  } else {
-    named_bar_sync(1, kThreads2);
-  }
-  if (crank == 0) {
+  named_bar_sync(1, kThreads2);
 #pragma unroll
-    for (int i = 0; i < kIt; ++i) {
-      int r, cc;
-      item(i, r, cc);
-      uint8_t* src = smem_gen + r * kPitch + cc * 32;
-      const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 16);
-      float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-      if constexpr (KS > 1) {
-        const uint32_t local = smem_u32(src);
-#pragma unroll
-        for (int rk = 1; rk < KS; ++rk) {   // rank order: deterministic
-          const uint32_t remote = dsmem_addr(local, uint32_t(rk));
-          const float4 w0 = ld_dsmem_f4(remote), w1 = ld_dsmem_f4(remote + 16);
-          v[0] += w0.x; v[1] += w0.y; v[2] += w0.z; v[3] += w0.w;
-          v[4] += w1.x; v[5] += w1.y; v[6] += w1.z; v[7] += w1.w;
-        }
-      }
-      if (m0 + r < M && n0 + cc * 8 < N) {
-        if constexpr (P::kPrefetch) p.store8p(z, m0 + r, n0 + cc * 8, v, pf[i]);
-        else p.store8(z, m0 + r, n0 + cc * 8, v);
-      }
+  for (int i = 0; i < kIt; ++i) {
+    int r, cc;
+    item(i, r, cc);
+    uint8_t* src = smem_gen + r * kPitch + cc * 32;
+    const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 16);
+    float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+    if (m0 + r < M && n0 + cc * 8 < N) {
+      if constexpr (P::kPrefetch) p.store8p(z, m0 + r, n0 + cc * 8, v, pf[i]);
+      else p.store8(z, m0 + r, n0 + cc * 8, v);
     }
-  }
-  if constexpr (KS > 1) {
-    cluster_arrive_release();   // partners keep their shared memory alive until the leader has read it
-    cluster_wait_acquire();
   }
   B2_TRACE(tid == 0, 5);
   kt_end(kt);
@@ -469,19 +435,18 @@ static inline int read_trace(unsigned long long* out, int n) {
   return cudaMemcpyFromSymbol(out, g_trace, n * sizeof(unsigned long long)) == cudaSuccess ? n : -1;
 }
 
-template <class P, int KS = 1>
+template <class P>
 static int launch_umma2(const char* label, const P& p, int M, int N, int Z, cudaStream_t st) {
   using C = Cfg2<P>;
   static bool configured = false;
   if (!configured) {
-    B2_CHECK_CUDA(cudaFuncSetAttribute(k_umma2<P, KS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
+    B2_CHECK_CUDA(cudaFuncSetAttribute(k_umma2<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
     configured = true;
   }
-  dim3 grid(((M + kBM - 1) / kBM) * KS, (N + C::BN - 1) / C::BN, Z);
+  dim3 grid((M + kBM - 1) / kBM, (N + C::BN - 1) / C::BN, Z);
   static const char* trace_label = getenv("B200DQN_TRACE_LABEL");
   const int trace = (trace_label && strcmp(trace_label, label) == 0) ? 1 : 0;
-  B2_CHECK_CUDA(launch_pdl_cluster(k_umma2<P, KS>, grid, dim3(kThreads2), C::kSmemBytes, st, KS, p, trace,
-                                   ktrace_slot(label)));
+  B2_CHECK_CUDA(launch_pdl(k_umma2<P>, grid, dim3(kThreads2), C::kSmemBytes, st, p, trace, ktrace_slot(label)));
   B2_PROF(label, st);
   return B200DQN_OK;
 }

@@ -4,8 +4,7 @@
 // "MN-major" wgmma operands: the 128-byte shared-memory row is a run of 64 consecutive m (or n) for
 // ONE k, eight consecutive k rows form the 1024-byte swizzle atom (cute canonical layout
 // Swizzle<3,4,3> o ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in fp16 elements).  So the gather is again
-// pure cp.async of 16-byte pieces (or an exact u8 -> fp16 convert for the conv1 frame window), no
-// transposition anywhere.
+// pure cp.async of 16-byte pieces (or TMA bulk copies of ready-made sub-tiles), no transposition anywhere.
 //
 // Per 64-pixel k-block the stage holds   A_hi [2 chunks x 64 rows x 128 B] (+ A_lo)   and
 //   BN = 64:  B_hi [64 x 128 B] followed by B_lo [64 x 128 B]   -> one N = 128 wgmma gives [acc0 | acc1]
@@ -37,10 +36,9 @@ struct PixCtx {   // decoded reduction index (one per thread per k-block)
 };
 
 // Problem P:
-//   static constexpr int kBN (32 or 64); static constexpr bool kAExact, kARegs;
+//   static constexpr int kBN (32 or 64); static constexpr bool kAExact, kABulk;
 //   int M(z), N(z); void krange(z, kb0, kb1);  PixCtx pix(z, kpix);
-//   !kARegs: Planes a_planes(z); bool a_run(z, pix, mchunk, int64_t& off)     64 contiguous fp16 of A for this pixel
-//    kARegs: void a_piece(z, pix, mchunk, j, float v[8])                       (exact values, e.g. u8 pixels)
+//   !kABulk: Planes a_planes(z); bool a_run(z, pix, mchunk, int64_t& off)     64 contiguous fp16 of A for this pixel
 //    kABulk: const uint8_t* a_sub(z, mchunk, kb)   ready-made [64 k-rows x 128 B] sub-tile image (exact A only)
 //   Planes b_planes(z); int64_t b_off(z, pix)                                  BN contiguous fp16 of B for this pixel
 //   void store8(z, m, n0, const float v[8])
@@ -105,7 +103,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
   const int kr = tid >> 2, sub = tid & 3;
   const Planes bpl = p.b_planes(z);
   Planes apl{nullptr, 0};
-  if constexpr (!P::kARegs && !P::kABulk) apl = p.a_planes(z);
+  if constexpr (!P::kABulk) apl = p.a_planes(z);
   pdl_wait();   // the prologue above overlapped the predecessor
   if (kt.flags & 1) pdl_launch_dependents();
   auto stage = [&](int j) {
@@ -124,26 +122,14 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
     } else {
       const int mc = sub >> 1, j0 = (sub & 1) * 4;
       const int mchunk = blockIdx.x * 2 + mc;
-      if constexpr (!P::kARegs) {
-        int64_t eoff = 0;
-        const bool ok = px.ok && p.a_run(z, px, mchunk, eoff);
-        const __half* src = apl.hi + (ok ? eoff : 0);
+      int64_t eoff = 0;
+      const bool ok = px.ok && p.a_run(z, px, mchunk, eoff);
+      const __half* src = apl.hi + (ok ? eoff : 0);
 #pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          const uint32_t dst = st_addr + mc * C::kSub + mn_off(kr, j0 + t);
-          umma2::cp_async16(dst, src + (j0 + t) * 8, ok ? 16u : 0u);
-          if (!P::kAExact) umma2::cp_async16(dst + C::kAHalf, src + apl.lo_off + (j0 + t) * 8, ok ? 16u : 0u);
-        }
-      } else {
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          float v[8];
-          p.a_piece(z, px, mchunk, j0 + t, v);
-          uint4 hi, lo;
-          umma::split8(v, hi, lo);
-          *reinterpret_cast<uint4*>(st_gen + mc * C::kSub + mn_off(kr, j0 + t)) = hi;
-          if (!P::kAExact) *reinterpret_cast<uint4*>(st_gen + C::kAHalf + mc * C::kSub + mn_off(kr, j0 + t)) = lo;
-        }
+      for (int t = 0; t < 4; ++t) {
+        const uint32_t dst = st_addr + mc * C::kSub + mn_off(kr, j0 + t);
+        umma2::cp_async16(dst, src + (j0 + t) * 8, ok ? 16u : 0u);
+        if (!P::kAExact) umma2::cp_async16(dst + C::kAHalf, src + apl.lo_off + (j0 + t) * 8, ok ? 16u : 0u);
       }
     }
     // ---- B
@@ -164,7 +150,6 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
         umma2::cp_async16(dst + mn_off(kr, 4 + sub), src + bpl.lo_off + sub * 8, bytes);
       }
     }
-    if constexpr (P::kARegs) fence_proxy_async_smem();   // this thread's st.shared -> async proxy
     umma2::cp_async_arrive_noinc(&s_full[s]);
   };
   for (int j = 0; j < S && j < nkb; ++j) stage(j);
@@ -209,50 +194,14 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
     umma::stage_acc<BN>(acc, P::kAExact ? nullptr : acc2, smem_gen, kPitch, wg, warp, lane);
     umma2::named_bar_sync(1, kLoadThreads);
     constexpr int kChunksPerRow = BN / 8;
-    if constexpr (!P::kFusedUpdate) {
 #pragma unroll
-      for (int i = 0; i < kBM * kChunksPerRow / kLoadThreads; ++i) {
-        const int id = tid + i * kLoadThreads;
-        const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
-        const float* src = reinterpret_cast<const float*>(smem_gen + r * kPitch + cc * 32);
-        const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
-        const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-        if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, v);
-      }
-    } else {
-      // Fused optimizer (no split-K: this tile IS the whole gradient of its weights).
-      // pass 1, thread <-> (row m, 8 consecutive n): RMSProp on W/S in HBM, the updated weights go
-      //         back into the smem tile and into the row-oriented (dgrad) tile image;
-      // pass 2, thread <-> (column n, 8 consecutive m): the column-oriented (forward) tile image.
-      constexpr int kIt = kBM * kChunksPerRow / kLoadThreads;
-      const float l_step = p.step_scalar();
-#pragma unroll
-      for (int i = 0; i < kIt; ++i) {
-        const int id = tid + i * kLoadThreads;
-        const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
-        float* src = reinterpret_cast<float*>(smem_gen + r * kPitch + cc * 32);
-        const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
-        const float g[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
-        if (m0 + r < M && n0 + cc * 8 < N) {
-          float nw[8];
-          p.update8(z, m0 + r, n0 + cc * 8, l_step, g, nw);
-          *reinterpret_cast<float4*>(src) = make_float4(nw[0], nw[1], nw[2], nw[3]);
-          *reinterpret_cast<float4*>(src + 4) = make_float4(nw[4], nw[5], nw[6], nw[7]);
-        }
-      }
-      umma2::named_bar_sync(1, kLoadThreads);
-#pragma unroll
-      for (int i = 0; i < (kBM / 8) * BN / kLoadThreads; ++i) {
-        const int id = tid + i * kLoadThreads;
-        const int nn = id % BN, mg = id / BN;
-        if (m0 + mg * 8 < M && n0 + nn < N) {
-          float wv[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            wv[j] = *reinterpret_cast<const float*>(smem_gen + (mg * 8 + j) * kPitch + nn * 4);
-          p.pack_col8(z, m0 + mg * 8, n0 + nn, wv);
-        }
-      }
+    for (int i = 0; i < kBM * kChunksPerRow / kLoadThreads; ++i) {
+      const int id = tid + i * kLoadThreads;
+      const int r = id / kChunksPerRow, cc = id % kChunksPerRow;
+      const float* src = reinterpret_cast<const float*>(smem_gen + r * kPitch + cc * 32);
+      const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 4);
+      const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+      if (m0 + r < M && n0 + cc * 8 < N) p.store8(z, m0 + r, n0 + cc * 8, v);
     }
   }
   kt_end(kt);

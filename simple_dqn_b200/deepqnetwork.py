@@ -145,7 +145,7 @@ class DeepQNetwork:
         return out
 
     def keep_grads(self, keep=True):
-        """Make the fused optimizers keep a copy of dW so :meth:`get_grads` works (tests / debugging)."""
+        """Make the tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 next to their fp16 planes (tests / debugging)."""
         L.call("b200dqn_net_set_keep_grads", self._h, int(bool(keep)))
 
     def get_grads(self):

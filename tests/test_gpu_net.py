@@ -60,7 +60,7 @@ def _paired(num_actions, mode, seed=3, batch=32, stream=None, optimizer="rmsprop
         ss = [[f(1e-5, w, True), f(1e-9, w, True), f(1e-4, w)] for w in ws]
     net.set_weights(ws, ss)
     net.update_target_network()
-    net.keep_grads(True)            # the fused optimizers otherwise never materialise dW4
+    net.keep_grads(True)            # the fp32 dZ copies as well as the fp16 planes
     orc = O.DQNOracle(num_actions, batch_size=batch, weights=ws, states=ss, optimizer=optimizer)
     return net, orc
 
