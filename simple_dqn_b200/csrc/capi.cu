@@ -58,23 +58,7 @@ struct KtState {
 } g_kt;
 }  // namespace
 
-static int early_trigger_flag(const char* label) {
-  static const char* list = getenv("B200DQN_EARLY_TRIGGER");
-  if (!list) return 0;
-  const size_t n = strlen(label);
-  for (const char* p = list; (p = strstr(p, label)) != nullptr; p += n)
-    if ((p == list || p[-1] == ',') && (p[n] == 0 || p[n] == ',')) return 1;
-  return 0;
-}
-
-static KTrace ktrace_slot_plain(const char* label);
 KTrace ktrace_slot(const char* label) {
-  KTrace kt = ktrace_slot_plain(label);
-  kt.flags = early_trigger_flag(label);
-  return kt;
-}
-
-static KTrace ktrace_slot_plain(const char* label) {
   if (!g_kt.on) return KTrace{nullptr, 0};
   // a gated trace records one step only, so launches of later steps (eager replay re-launches every kernel)
   // share the slot of their label instead of exhausting the table

@@ -66,8 +66,6 @@ extern bool g_prof_on;
 struct KTrace {
   unsigned long long* buf;   // [slot][2] = {start_ns, end_ns}; nullptr = off
   int slot;
-  int flags = 0;             // bit 0: release the dependents right after the dependency wait (experiment knob
-                             // B200DQN_EARLY_TRIGGER=label,label,...; rides here because every kernel gets a KTrace)
 };
 KTrace ktrace_slot(const char* label);   // host: slot for this launch (registers the label), {nullptr,0} when off
 extern int g_ktrace_gen;                 // bumped whenever tracing is switched, invalidates captured graphs

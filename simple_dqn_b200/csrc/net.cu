@@ -343,7 +343,8 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
   const float* w[2] = {n->d_w, n->d_tw};
   int rc;
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
-    rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.nframes, nets, rows, st);
+    // one GPU: the forward launches are links of the critical chain (umma_forward picks the ones that release early)
+    rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.nframes, nets, rows, st, n->world == 1);
     if (rc) return rc;
   } else {
     {
@@ -392,12 +393,15 @@ static int wgrad_chunk(int kred, int base) {
 
 enum BwdOp { kFc1Wgrad, kFc1Dgrad, kConv3Wgrad, kConv3Dgrad, kConv2Wgrad, kConv2Dgrad, kConv1Wgrad };
 
-// One GEMM-shaped backward op on stream `st`, on whichever engine math_mode selects.
-static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cudaStream_t st) {
+// One GEMM-shaped backward op on stream `st`, on whichever engine math_mode selects.  release_early (tensor-core
+// engine): the op is a link of the single-GPU critical chain and lets its successor pre-launch right after its own
+// dependency wait.
+static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cudaStream_t st,
+                  bool release_early = false) {
   const LayerTable& lt = n->lt;
   const float* w = n->d_w;
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
-    return umma_backward_op(n, int(op), fs.src[0], fs.idx[0], fs.shift[0], rows, st);
+    return umma_backward_op(n, int(op), fs.src[0], fs.idx[0], fs.shift[0], rows, st, release_early);
   switch (op) {
     case kFc1Wgrad: {
       Fc1Wgrad p{n->d_h3[0], n->d_dz4, n->d_part + lt.part_off[3], rows};
@@ -770,7 +774,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     B2_TRY(cost_finish_on(n, rows, sN));
     if (tc) B2_TRY(opt_fc2_small(n, rows, sN));
   }
-  B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st));
+  B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
   {
@@ -780,7 +784,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
-  B2_TRY(bwd_op(n, fs, rows, kConv3Dgrad, st));
+  B2_TRY(bwd_op(n, fs, rows, kConv3Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[2], st));                 // dZ2 ready, W3 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[2], 0));
   {
@@ -790,7 +794,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[2], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv2Wgrad, sC)); }
-  B2_TRY(bwd_op(n, fs, rows, kConv2Dgrad, st));
+  B2_TRY(bwd_op(n, fs, rows, kConv2Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[3], st));                 // dZ1 ready, W2 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[3], 0));
   {
@@ -798,7 +802,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 1, rows, sC, "opt_conv2"));
     else B2_TRY(optimizer_range(n, 1, 1, 1 | 4, rows, sC, "opt_conv2"));
   }
-  B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st));
+  B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st, true));
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 0, rows, st, "opt_conv1"));
   else B2_TRY(optimizer_range(n, 0, 0, 1 | 4, rows, st, "opt_conv1"));
   B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));

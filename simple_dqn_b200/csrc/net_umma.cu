@@ -688,19 +688,24 @@ static inline int fc1_splits_for(int rows) {
 }
 constexpr int kUWgradKb = 4;      // minimum k-blocks (of 64 pixels) per wgrad split
 
-// k-blocks (of 64 pixels) per wgrad split: at least kUWgradKb, and few enough splits (<= 48) for the
-// one-pass reduction of k_opt_conv
-// conv1 through tensor-map TMA (conv1_tma.cuh) unless B200DQN_CONV1=ldg selects the register-path gather of umma2.cuh
-// (on an H100 80GB HBM3 at 700 W the ldg path was 3 % faster at batch 32 and 6 % at batch 256)
-static const bool g_conv1_tma = !(getenv("B200DQN_CONV1") && strcmp(getenv("B200DQN_CONV1"), "ldg") == 0);
+// conv1 gathers its frames on the register path of umma2.cuh (V2Conv1Fwd, plain loads) unless B200DQN_CONV1=tma selects
+// the tensor-map TMA twin (conv1_tma.cuh).  On an H100 80GB HBM3 the register path made the step 3 % (700 W) to 5 %
+// (400 W) faster at batch 32 and 5-6 % faster at batch 256.
+static const bool g_conv1_tma = getenv("B200DQN_CONV1") && strcmp(getenv("B200DQN_CONV1"), "tma") == 0;
+// rows of conv1's im2col image (= conv1_wgrad's reduction length): dense 128-row tiles on the register path, 4 tiles
+// of 100 live rows per sample on the TMA path
 static inline int conv1_pixels_padded(int rows) { return g_conv1_tma ? rows * conv1tma::kTilesPerSample * 128 : rows * kP1 * kP1; }
 
+// k-blocks (of 64 pixels) per wgrad split: at least kUWgradKb, and few enough splits (<= 48) for the
+// one-pass reduction of k_opt_conv
 int umma_wgrad_kb(int layer, int rows) {
   const int kred = layer == 0 ? conv1_pixels_padded(rows) : layer == 1 ? rows * kP2 * kP2 : rows * kP3 * kP3;
   const int kbs = (kred + 63) / 64;
   int per = (kbs + 47) / 48;
-  if (layer == 0 && per < 8) per = 8;   // conv1: A tiles arrive by TMA bulk copies; 8 k-blocks per CTA keep the split count (and
-                                        // the optimizer's partial-sum loads) down: measured 43 splits -> opt_conv1 +1.5 us
+  // conv1: at least 8 k-blocks per split (25 splits at batch 32).  On an H100 80GB HBM3 (400 W) the batch-32 step took
+  // 92.5 / 92.1 / 89.3 / 90.9 / 89.8 us with 5 / 6 / 8 / 10 / 13 k-blocks per split (40 / 34 / 25 / 20 / 16 splits,
+  // each partial read back by opt_conv1).
+  if (layer == 0 && per < 8) per = 8;
   return per > kUWgradKb ? per : kUWgradKb;
 }
 int umma_wgrad_splits(int layer, int rows) {
@@ -739,7 +744,7 @@ int umma_net_init(b200dqn_net* n) {
       B2_CHECK_CUDA(cudaMemset(u->img_fwd[z][l], 0, u->img_fwd_bytes[l]));
     }
   }
-  B2_CHECK_CUDA(cudaMalloc(&u->im2col1, int64_t(nb) * conv1tma::kTilesPerSample * (kK1 / 64) * 128 * 128));
+  B2_CHECK_CUDA(cudaMalloc(&u->im2col1, int64_t((conv1_pixels_padded(nb) + 127) / 128) * (kK1 / 64) * 128 * 128));
   u->img_dgr[0] = u->img_fwd[0][3];   // fc1: ONE row-oriented image serves the dgrad (K-major) and the forward (MN-major)
   const int64_t dgr_bytes[3] = {0, int64_t(kK3 / 64) * kC2 * 256, int64_t(4) * (256 / 64) * kC1 * 256};
   for (int i = 1; i < 3; ++i) {
@@ -788,7 +793,9 @@ void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
 }
 
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 const int64_t nframes[2], int nets, int rows, cudaStream_t st) {
+                 const int64_t nframes[2], int nets, int rows, cudaStream_t st, bool release_early) {
+  // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
+  // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.
   UmmaState* u = ust(n);
   int rc;
   auto planes = [&](int i, int z) { return PlanePair{u->h16[i][z], u->h_elems[i]}; };
@@ -827,7 +834,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     }
     p.rows = rows;
     p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
-    if ((rc = umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st))) return rc;
+    if ((rc = umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early))) return rc;
   }
   {
     using P = V2ConvFwd<kP1, kC1, 4, 2, kC2>;
@@ -837,7 +844,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the target network's fp32 activations
     }
     p.rows = rows;
-    if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
+    if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st, false))) return rc;
   }
   {
     using P = V2ConvFwd<kP2, kC2, 3, 1, kC3>;
@@ -847,7 +854,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       p.out[z] = z ? nullptr : n->d_h3[z];
     }
     p.rows = rows;
-    if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
+    if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st, release_early))) return rc;
     // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
     if (nets == 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
   }
@@ -855,13 +862,13 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     V2Fc1Fwd p;
     for (int z = 0; z < 2; ++z) { p.in16[z] = planes(2, z); p.wimg[z] = u->img_fwd[z][3]; }
     p.part = n->d_fc1part; p.rows = rows; p.splits = fc1_splits_for(rows);
-    if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st))) return rc;
+    if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st, false))) return rc;
   }
   return B200DQN_OK;
 }
 
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,
-                     cudaStream_t st) {
+                     cudaStream_t st, bool release_early) {
   const LayerTable& lt = n->lt;
   const float* w = n->d_w;
   switch (op) {
@@ -869,35 +876,35 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       UmmaState* u = ust(n);
       WFc1Wgrad p{PlanePair{u->h16[2][0], u->h_elems[2]}, PlanePair{u->dz16[0], u->dz_elems[0]},
                   n->d_part + lt.part_off[3], rows};
-      return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st);
+      return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st, release_early);
     }
     case 1: {
       UmmaState* u = ust(n);
       // the fp32 copies of dZ3/dZ2/dZ1 have no reader in this engine (wgrads and dgrads take the fp16 planes)
       V2Fc1Dgrad p{u->img_dgr[0], PlanePair{u->dz16[0], u->dz_elems[0]}, n->d_h3[0], n->keep_grads ? n->d_dz3 : nullptr,
                    PlanePair{u->dz16[1], u->dz_elems[1]}, rows};
-      return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows, 1, st);
+      return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows, 1, st, release_early);
     }
     case 2: {
       UmmaState* u = ust(n);
       using P = WConvWgrad<kP2, kC2, 3, 1, kC3>;
       P p{PlanePair{u->h16[1][0], u->h_elems[1]}, PlanePair{u->dz16[1], u->dz_elems[1]},
           n->d_part + lt.part_off[2], rows, umma_wgrad_kb(2, rows)};
-      return umma_mn::launch_umma_mn("conv3_wgrad", p, P::KW, kC3, lt.splits[2], st);
+      return umma_mn::launch_umma_mn("conv3_wgrad", p, P::KW, kC3, lt.splits[2], st, release_early);
     }
     case 3: {
       UmmaState* u = ust(n);
       using P = V2ConvDgrad<kP2, kC2, 3, 1, kC3>;
       P p{PlanePair{u->dz16[1], u->dz_elems[1]}, u->img_dgr[1], n->d_h2[0], n->keep_grads ? n->d_dz2 : nullptr,
           PlanePair{u->dz16[2], u->dz_elems[2]}, rows};
-      return umma2::launch_umma2("conv3_dgrad", p, rows * P::HC * P::HC, kC2, 1, st);
+      return umma2::launch_umma2("conv3_dgrad", p, rows * P::HC * P::HC, kC2, 1, st, release_early);
     }
     case 4: {
       UmmaState* u = ust(n);
       using P = WConvWgrad<kP1, kC1, 4, 2, kC2>;
       P p{PlanePair{u->h16[0][0], u->h_elems[0]}, PlanePair{u->dz16[2], u->dz_elems[2]},
           n->d_part + lt.part_off[1], rows, umma_wgrad_kb(1, rows)};
-      return umma_mn::launch_umma_mn("conv2_wgrad", p, P::KW, kC2, lt.splits[1], st);
+      return umma_mn::launch_umma_mn("conv2_wgrad", p, P::KW, kC2, lt.splits[1], st, release_early);
     }
     case 5: {
       UmmaState* u = ust(n);
@@ -911,18 +918,18 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       if (n->world == 1) {
         P2 p{PlanePair{u->dz16[2], u->dz_elems[2]}, u->img_dgr[2], n->d_h1[0], n->keep_grads ? n->d_dz1 : nullptr,
              PlanePair{u->dz16[3], u->dz_elems[3]}, rows};
-        return umma2::launch_umma2("conv2_dgrad", p, rows * P::HC * P::HC, kC1, 4, st);
+        return umma2::launch_umma2("conv2_dgrad", p, rows * P::HC * P::HC, kC1, 4, st, release_early);
       }
       P p{PlanePair{u->dz16[2], u->dz_elems[2]}, u->img_dgr[2], n->d_h1[0], n->keep_grads ? n->d_dz1 : nullptr,
           PlanePair{u->dz16[3], u->dz_elems[3]}, rows};
-      return umma2::launch_umma2("conv2_dgrad", p, rows * P::HC * P::HC, kC1, 4, st);
+      return umma2::launch_umma2("conv2_dgrad", p, rows * P::HC * P::HC, kC1, 4, st, release_early);
     }
     default: {
       UmmaState* u = ust(n);
       (void)src; (void)idx; (void)shift;   // the frames were already gathered by conv1_fwd (im2col image)
       WConv1Wgrad p{u->im2col1, PlanePair{u->dz16[3], u->dz_elems[3]}, n->d_part + lt.part_off[0], rows,
                     umma_wgrad_kb(0, rows), g_conv1_tma ? conv1tma::kTileRows : 128};
-      return umma_mn::launch_umma_mn("conv1_wgrad", p, kK1, kC1, lt.splits[0], st);
+      return umma_mn::launch_umma_mn("conv1_wgrad", p, kK1, kC1, lt.splits[0], st, release_early);
     }
   }
 }
@@ -952,7 +959,7 @@ int umma_fc1_wgrad_gathered(b200dqn_net* n, cudaStream_t st) {
                     reinterpret_cast<const __half*>(n->d_xbuf + n->x_dz_off),
                     n->x_h3_parity / 2, n->x_h3_lo, n->x_dz_parity / 2, n->x_dz_lo,
                     n->d_xpush_epoch, n->d_part + n->lt.part_off[3], n->nb * n->world};
-  return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st);
+  return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st, false);
 }
 
 }  // namespace b200

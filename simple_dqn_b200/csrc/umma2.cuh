@@ -154,8 +154,11 @@ constexpr int kThreads2 = kLoadThreads;
 //   lo weight tiles are adjacent in shared memory) and  acc2 += A_lo x B_hi;  then wgmma.wait_group 1 (k-block it-1
 //   has completed in this warpgroup), one named barrier over both warpgroups, and stage (it-1) % S is refilled with
 //   k-block it-1+S while the tensor cores work on k-block it.
+//   release_early: the successor may pre-launch as soon as this kernel has passed its dependency wait (links of the
+//   single-GPU critical chain), instead of once this CTA's mainloop has issued all its loads.
 template <class P>
-__global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int trace_in, const KTrace kt) {
+__global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int trace_in, const bool release_early,
+                                                        const KTrace kt) {
   using C = Cfg2<P>;
   constexpr int BN = C::BN;
   constexpr int S = C::kStages;
@@ -228,7 +231,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   // Everything above (barrier init, the gather index tables, the first weight tiles) overlapped the previous kernel
   // of the chain; only from here on do we touch its outputs.
   pdl_wait();
-  if (kt.flags & 1) pdl_launch_dependents();
+  if (release_early) pdl_launch_dependents();
   // kReg operands: per-row source pointers, once per kernel (they may depend on upstream data — the
   // sampled indexes — so they are built after the wait, but not again for every k-block)
   const uint8_t* areg[kACh];
@@ -375,7 +378,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   B2_TRACE(tid == 0, 3);
   // All of this CTA's loads are issued: let the successor kernel pre-launch NOW (it sets up its barriers and index
   // tables, then parks at its pdl_wait) — late enough that its parked CTAs do not hog shared memory for long, early
-  // enough to hide its prologue behind our epilogue.
+  // enough to hide its prologue behind our epilogue.  (A no-op when release_early already did it.)
   pdl_launch_dependents();
 
   // ================================================================ epilogue
@@ -436,7 +439,7 @@ static inline int read_trace(unsigned long long* out, int n) {
 }
 
 template <class P>
-static int launch_umma2(const char* label, const P& p, int M, int N, int Z, cudaStream_t st) {
+static int launch_umma2(const char* label, const P& p, int M, int N, int Z, cudaStream_t st, bool release_early) {
   using C = Cfg2<P>;
   static bool configured = false;
   if (!configured) {
@@ -446,7 +449,8 @@ static int launch_umma2(const char* label, const P& p, int M, int N, int Z, cuda
   dim3 grid((M + kBM - 1) / kBM, (N + C::BN - 1) / C::BN, Z);
   static const char* trace_label = getenv("B200DQN_TRACE_LABEL");
   const int trace = (trace_label && strcmp(trace_label, label) == 0) ? 1 : 0;
-  B2_CHECK_CUDA(launch_pdl(k_umma2<P>, grid, dim3(kThreads2), C::kSmemBytes, st, p, trace, ktrace_slot(label)));
+  B2_CHECK_CUDA(launch_pdl(k_umma2<P>, grid, dim3(kThreads2), C::kSmemBytes, st, p, trace, release_early,
+                           ktrace_slot(label)));
   B2_PROF(label, st);
   return B200DQN_OK;
 }

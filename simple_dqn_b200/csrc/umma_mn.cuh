@@ -57,8 +57,9 @@ struct CfgMN {
   static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
 };
 
+// release_early: as in umma2.cuh's k_umma2
 template <class P>
-__global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrace kt) {
+__global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const bool release_early, const KTrace kt) {
   using C = CfgMN<P>;
   constexpr int BN = C::BN;
   constexpr int S = C::kStages;
@@ -105,7 +106,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
   Planes apl{nullptr, 0};
   if constexpr (!P::kABulk) apl = p.a_planes(z);
   pdl_wait();   // the prologue above overlapped the predecessor
-  if (kt.flags & 1) pdl_launch_dependents();
+  if (release_early) pdl_launch_dependents();
   auto stage = [&](int j) {
     const int s = j % S;
     const uint32_t st_addr = smem_base + s * C::kStageBytes;
@@ -208,7 +209,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const KTrac
 }
 
 template <class P>
-static int launch_umma_mn(const char* label, const P& p, int M, int N, int Z, cudaStream_t st) {
+static int launch_umma_mn(const char* label, const P& p, int M, int N, int Z, cudaStream_t st, bool release_early) {
   using C = CfgMN<P>;
   static bool configured = false;
   if (!configured) {
@@ -216,7 +217,8 @@ static int launch_umma_mn(const char* label, const P& p, int M, int N, int Z, cu
     configured = true;
   }
   dim3 grid((M + kBM - 1) / kBM, (N + C::BN - 1) / C::BN, Z);
-  B2_CHECK_CUDA(launch_pdl(k_umma_mn<P>, grid, dim3(kThreads2), C::kSmemBytes, st, p, ktrace_slot(label)));
+  B2_CHECK_CUDA(launch_pdl(k_umma_mn<P>, grid, dim3(kThreads2), C::kSmemBytes, st, p, release_early,
+                           ktrace_slot(label)));
   B2_PROF(label, st);
   return B200DQN_OK;
 }
