@@ -137,6 +137,291 @@ struct V2ConvFwd {
   }
 };
 
+// ---- conv2 + conv3 forward, one CTA per (sample, network) ------------------------------------------
+// conv3's receptive field never leaves a sample, so one CTA runs conv2 on its sample (81 live rows of a 128-row tile,
+// the k_umma2 pipeline), keeps H2 in shared memory as fp16 hi/lo rows and runs conv3 on it (49 live rows of one
+// 64-row wgmma tile, one k-block per filter tap): no CTA waits on another, and the conv2 -> conv3 link of the chain
+// (grid drain, dependency release, first loads) is gone.  Operand bits, k-block order and the MMAs each output
+// element sees are those of the two V2ConvFwd launches, so the results are the same bits.
+struct Conv23Fwd {
+  using C2 = V2ConvFwd<kP1, kC1, 4, 2, kC2>;   // conv2: gather addressing of H1; out / out16 = H2 of the online net
+  using C3 = V2ConvFwd<kP2, kC2, 3, 1, kC3>;   // conv3: wimg, out / out16 = H3 (in16 unused: H2 stays on chip)
+  C2 c2;
+  C3 c3;
+};
+
+namespace conv23 {
+constexpr int kStages = 4;                               // conv2 ring
+constexpr int kM2 = kP2 * kP2, kM3 = kP3 * kP3;          // live rows: 81 of 128, 49 of 64
+constexpr int kKb2 = kK2 / 64, kKb3 = kK3 / 64;          // 8, 9
+constexpr uint32_t kA2 = umma::kBM * 128;                // conv2 A_hi tile (A_lo follows)
+constexpr uint32_t kB2 = kC2 * 128;                      // conv2 B_hi tile (B_lo follows)
+constexpr uint32_t kStage2 = 2 * kA2 + 2 * kB2;          // 48 KB
+constexpr uint32_t kB3 = kC3 * 256;                      // conv3 weight image of one tap: [hi 64 rows | lo 64 rows]
+constexpr uint32_t kA3 = umma::kWgM * 128;               // conv3 A_hi tile (A_lo follows)
+// Shared memory, from the 1024-aligned base: the conv2 ring; once a conv2 stage is retired it takes the weight images
+// of three conv3 taps (stages 0-2 hold all nine), while stage 3 takes conv2's epilogue tile and then conv3's 3-deep
+// A ring; behind the ring the H2 rows of the sample, [hi 81 x 128 B | lo 81 x 128 B].
+constexpr uint32_t kStaging = 3 * kStage2;
+constexpr uint32_t kH2 = kStages * kStage2;
+constexpr uint32_t kPitch2 = kC2 * 4 + 16, kPitch3 = kC3 * 4 + 16;   // epilogue tile rows (bytes)
+constexpr uint32_t kSmemBytes = kH2 + 2 * kM2 * 128 + 1024;
+static_assert(kKb3 * kB3 == 3 * kStage2, "stages 0-2 of the conv2 ring hold the nine conv3 weight images");
+static_assert(kStaging + umma::kBM * kPitch2 <= kH2 && kStaging + 3 * 2 * kA3 <= kH2, "stage 3: epilogue tile, A ring");
+static_assert(umma::kWgM * kPitch3 <= kStaging, "conv3 epilogue tile over the retired weight images");
+static_assert(kSmemBytes <= 227 * 1024, "H100: at most 227 KB of shared memory per block");
+}  // namespace conv23
+
+// Trace stamps (B200DQN_TRACE_LABEL=conv23_fwd): 0 start, 1 barriers ready, 3 conv2 MMAs issued, 4 conv2 accumulators
+// ready, 2 H2 in shared memory, 7 conv3 accumulators ready, 5 H3 stored, 6 end; k-block rows 8 + 4 * it as in
+// k_umma2, conv2's it = 0..7 and conv3's it = 8..16 (conv3 stamps [it][2] when it starts copying its A tile).
+__global__ void __launch_bounds__(umma2::kThreads2, 1) k_conv23_fwd(const Conv23Fwd p, const int trace_in,
+                                                                    const KTrace kt) {
+  using namespace conv23;
+  using umma2::g_trace;
+  using umma2::kTraceSlots;
+  constexpr int S = kStages;
+  constexpr int kThreads = umma2::kThreads2;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t s_full[S];      // conv2: operands of the stage have landed
+  __shared__ __align__(8) uint64_t s_w3[kKb3];     // conv3: weight image of tap kb has landed
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+  const int n = blockIdx.x, z = blockIdx.y;
+  const bool trace = trace_in && n == 0 && z == 0;
+  kt_begin(kt);
+  B2_TRACE(tid == 0, 0);
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
+  uint8_t* h2 = smem_gen + kH2;
+  const uint8_t* wimg2 = z ? p.c2.wimg[1] : p.c2.wimg[0];
+  const uint8_t* wimg3 = z ? p.c3.wimg[1] : p.c3.wimg[0];
+
+  if (tid == 0) {
+#pragma unroll
+    for (int s = 0; s < S; ++s) mbar_init(&s_full[s], kThreads + 1);
+#pragma unroll
+    for (int kb = 0; kb < kKb3; ++kb) mbar_init(&s_w3[kb], 1);
+    mbar_fence_init();
+  }
+  __syncthreads();
+  B2_TRACE(tid == 0, 1);
+
+  // conv2 gather rows of this thread (sample-local row m = id >> 3; rows 81..127 are zero-filled)
+  constexpr int kACh = umma::kBM * 8 / kThreads;
+  umma2::RowCtx arow[kACh];
+  const umma2::Planes apl = p.c2.a_planes(z);
+#pragma unroll
+  for (int i = 0; i < kACh; ++i) {
+    const int m = (tid + i * kThreads) >> 3;
+    arow[i] = p.c2.a_row(z, n * kM2 + m);
+    arow[i].ok = m < kM2;
+  }
+  // conv2's first S weight tiles do not depend on the predecessor kernel: in flight before the dependency wait
+  if (tid == 0) {
+#pragma unroll
+    for (int j = 0; j < S; ++j) {
+      mbar_arrive_expect_tx(&s_full[j], 2 * kB2);
+      tma_bulk_g2s(smem_gen + j * kStage2 + 2 * kA2, wimg2 + j * (2 * kB2), 2 * kB2, &s_full[j]);
+    }
+  }
+  pdl_wait();
+
+  // conv2 operands of k-block j into stage j % S
+  auto stage2 = [&](int j) {
+    const int s = j % S, k0 = j * umma::kBK;
+    B2_TRACE(tid == 0, 8 + j * 4 + 2);
+    const uint32_t a_hi = smem_base + s * kStage2, a_lo = a_hi + kA2;
+    if (tid == 0 && j >= S) {
+      mbar_arrive_expect_tx(&s_full[s], 2 * kB2);
+      tma_bulk_g2s(smem_gen + s * kStage2 + 2 * kA2, wimg2 + j * (2 * kB2), 2 * kB2, &s_full[s]);
+    }
+#pragma unroll
+    for (int i = 0; i < kACh; ++i) {
+      const int id = tid + i * kThreads, r = id >> 3, c = id & 7;
+      int64_t eoff = 0;
+      const bool ok = arow[i].ok && p.c2.a_chunk(z, arow[i], k0 + c * 8, eoff);
+      const uint32_t bytes = ok ? 16u : 0u;
+      const __half* hi = apl.hi + (ok ? eoff : 0);
+      const uint32_t off = umma::sw128_off(r, c);
+      umma2::cp_async16(a_hi + off, hi, bytes);
+      umma2::cp_async16(a_lo + off, hi + apl.lo_off, bytes);
+    }
+    umma2::cp_async_arrive_noinc(&s_full[s]);
+    B2_TRACE(tid == 0, 8 + j * 4 + 3);
+  };
+  for (int j = 0; j < S; ++j) stage2(j);
+
+  // ================================================================ conv2 mainloop (as k_umma2, BN = 64)
+  float acc[kC2];          // N = 128 fragment: [A_hi x B_hi | A_hi x B_lo]
+  float acc2[kC2 / 2];     // N = 64 fragment: A_lo x B_hi
+#pragma unroll
+  for (int i = 0; i < kC2; ++i) acc[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < kC2 / 2; ++i) acc2[i] = 0.f;
+  for (int it = 0; it < kKb2; ++it) {
+    const int s = it % S;
+    mbar_wait(&s_full[s], (it / S) & 1);
+    fence_proxy_async_smem();
+    B2_TRACE(tid == 0, 8 + it * 4 + 0);
+    const uint32_t sa = smem_base + s * kStage2;
+    const uint64_t da_hi = umma::make_desc_sw128(sa + wg * umma::kWgM * 128);
+    const uint64_t da_lo = umma::make_desc_sw128(sa + kA2 + wg * umma::kWgM * 128);
+    const uint64_t db = umma::make_desc_sw128(sa + 2 * kA2);
+    umma::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < umma::kBK / 16; ++k) {
+      umma::wgmma_f16<2 * kC2>(acc, da_hi + 2 * k, db + 2 * k);
+      umma::wgmma_f16<kC2>(acc2, da_lo + 2 * k, db + 2 * k);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait<1>();
+    B2_TRACE(tid == 0, 8 + it * 4 + 1);
+    if (it >= 1) {
+      umma2::named_bar_sync(1, kThreads);   // both warpgroups are done with k-block it-1: its stage is free
+      const int freed = (it - 1) % S;
+      if (it - 1 + S < kKb2) {
+        stage2(it - 1 + S);
+      } else if (tid == 0) {              // conv2 is done with stage `freed`: it takes the images of conv3 taps 3*freed..+2
+#pragma unroll
+        for (int t = 0; t < 3; ++t) {
+          const int kb = 3 * freed + t;
+          mbar_arrive_expect_tx(&s_w3[kb], kB3);
+          tma_bulk_g2s(smem_gen + kb * kB3, wimg3 + kb * kB3, kB3, &s_w3[kb]);
+        }
+      }
+    }
+  }
+  B2_TRACE(tid == 0, 3);
+  // Every load of the kernel has been issued: fc1_fwd may pre-launch.  On an H100 80GB HBM3 (400 W) this was 0.5 us
+  // faster at batch 32 than releasing right after the dependency wait.
+  pdl_launch_dependents();
+
+  // ================================================================ conv2 epilogue: H2 -> shared memory (+ HBM)
+  umma::wgmma_wait<0>();
+  umma2::named_bar_sync(1, kThreads);     // stage 3 (the epilogue tile) is no longer read by the MMAs
+  B2_TRACE(tid == 0, 4);
+  umma::stage_acc<kC2>(acc, acc2, smem_gen + kStaging, kPitch2, wg, warp, lane);
+  umma2::named_bar_sync(1, kThreads);
+  {
+    float* out = p.c2.out[0];
+    const PlanePair pl = p.c2.out16[0];
+#pragma unroll
+    for (int i = 0; i < umma::kBM * 8 / kThreads; ++i) {
+      const int id = tid + i * kThreads, r = id >> 3, cc = id & 7;
+      if (r < kM2) {
+        const uint8_t* src = smem_gen + kStaging + r * kPitch2 + cc * 32;
+        const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 16);
+        const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = fmaxf(v[j], 0.f);
+        uint4 hi, lo;
+        umma::split8(o, hi, lo);
+        *reinterpret_cast<uint4*>(h2 + r * 128 + cc * 16) = hi;
+        *reinterpret_cast<uint4*>(h2 + kM2 * 128 + r * 128 + cc * 16) = lo;
+        if (z == 0) {   // conv2_dgrad reads the fp32 H2 (Rectlin mask), conv3_wgrad the planes; the target's H2 has no reader
+          const int64_t e = int64_t(n * kM2 + r) * kC2 + cc * 8;
+          if (out) st8(out + e, o);
+          *reinterpret_cast<uint4*>(pl.hi + e) = hi;
+          *reinterpret_cast<uint4*>(pl.hi + pl.lo_off + e) = lo;
+        }
+      }
+    }
+  }
+  umma2::named_bar_sync(1, kThreads);     // H2 complete; the epilogue tile is free for the A ring
+  B2_TRACE(tid == 0, 2);
+
+  // ================================================================ conv3 mainloop
+  // Tap kb = (r, s): A row m = (p, q) is H2 row (p + r, q + s), copied into a SW128 tile (rows 49..63 zero).  Each
+  // warpgroup takes 32 output channels: per k-step three N = 32 wgmmas, A_hi x B_hi, A_hi x B_lo and A_lo x B_hi.
+  float acc3[kC3 / 2];     // [A_hi x B_hi | A_hi x B_lo] laid out as one N = 64 fragment (stage_acc<32>)
+  float acc3l[kC3 / 4];    // A_lo x B_hi
+#pragma unroll
+  for (int i = 0; i < kC3 / 2; ++i) acc3[i] = 0.f;
+#pragma unroll
+  for (int i = 0; i < kC3 / 4; ++i) acc3l[i] = 0.f;
+  for (int it = 0; it < kKb3; ++it) {
+    const int r = it / 3, s = it % 3;
+    const uint32_t a_off = kStaging + (it % 3) * (2 * kA3);
+    B2_TRACE(tid == 0, 8 + (kKb2 + it) * 4 + 2);
+    // buffer it % 3 was last read by tap it-3, complete in both warpgroups (wgmma.wait_group 1 of tap it-2, then the
+    // barrier of tap it-1)
+#pragma unroll
+    for (int i = 0; i < umma::kWgM * 8 / kThreads; ++i) {
+      const int id = tid + i * kThreads, m = id >> 3, c = id & 7;
+      uint4 hi = make_uint4(0u, 0u, 0u, 0u), lo = hi;
+      if (m < kM3) {
+        const int src = (m / kP3 + r) * kP2 + m % kP3 + s;
+        hi = *reinterpret_cast<const uint4*>(h2 + src * 128 + c * 16);
+        lo = *reinterpret_cast<const uint4*>(h2 + kM2 * 128 + src * 128 + c * 16);
+      }
+      *reinterpret_cast<uint4*>(smem_gen + a_off + umma::sw128_off(m, c)) = hi;
+      *reinterpret_cast<uint4*>(smem_gen + a_off + kA3 + umma::sw128_off(m, c)) = lo;
+    }
+    fence_proxy_async_smem();               // st.shared (generic proxy) -> wgmma operand reads (async proxy)
+    umma2::named_bar_sync(1, kThreads);     // both warpgroups read the whole A tile
+    mbar_wait(&s_w3[it], 0);
+    B2_TRACE(tid == 0, 8 + (kKb2 + it) * 4 + 0);
+    const uint64_t da_hi = umma::make_desc_sw128(smem_base + a_off);
+    const uint64_t da_lo = umma::make_desc_sw128(smem_base + a_off + kA3);
+    const uint32_t b = smem_base + it * kB3 + wg * 32 * 128;   // this warpgroup's 32 rows: 1024-byte aligned
+    const uint64_t db_hi = umma::make_desc_sw128(b), db_lo = umma::make_desc_sw128(b + kC3 * 128);
+    umma::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < umma::kBK / 16; ++k) {
+      umma::wgmma_f16<32>(acc3, da_hi + 2 * k, db_hi + 2 * k);
+      umma::wgmma_f16<32>(acc3 + kC3 / 4, da_hi + 2 * k, db_lo + 2 * k);
+      umma::wgmma_f16<32>(acc3l, da_lo + 2 * k, db_hi + 2 * k);
+    }
+    umma::wgmma_commit();
+    umma::wgmma_wait<1>();
+    B2_TRACE(tid == 0, 8 + (kKb2 + it) * 4 + 1);
+  }
+
+  // ================================================================ conv3 epilogue (V2ConvFwd::store8 of conv3_fwd)
+  umma::wgmma_wait<0>();
+  umma2::named_bar_sync(1, kThreads);     // the weight images are no longer read: the epilogue tile goes over them
+  B2_TRACE(tid == 0, 7);
+  umma::stage_acc<32>(acc3, acc3l, smem_gen + wg * 32 * 4, kPitch3, 0, warp, lane);
+  umma2::named_bar_sync(1, kThreads);
+#pragma unroll
+  for (int i = 0; i < umma::kWgM * 8 / kThreads; ++i) {
+    const int id = tid + i * kThreads, m = id >> 3, cc = id & 7;
+    if (m < kM3) {
+      const uint8_t* src = smem_gen + m * kPitch3 + cc * 32;
+      const float4 v0 = *reinterpret_cast<const float4*>(src), v1 = *reinterpret_cast<const float4*>(src + 16);
+      const float v[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
+      p.c3.store8(z, n * kM3 + m, cc * 8, v);
+    }
+  }
+  B2_TRACE(tid == 0, 5);
+  kt_end(kt);
+  B2_TRACE(tid == 0, 6);
+}
+
+// Up to this many samples the forward runs conv2 and conv3 as conv23_fwd, beyond it as the two V2ConvFwd launches.
+// Small minibatches leave most SMs idle and pay for each link of the chain; large ones fill the GPU, and there the
+// per-sample tiles (81 of 128 conv2 rows, 49 of 64 conv3 rows live) cost more than the link saves.  tools/period.py on
+// an H100 80GB HBM3 at 400 W, median us per step, two-kernel against fused: 88.1 / 84.9 at batch 32,
+// 120.4-120.5 / 119.7-122.5 at 64, 191.9-194.9 / 199.5-200.8 at 128, 262.5-262.7 / 274.3-275.3 at 192 and
+// 343.6-344.3 / 353.3-354.2 at 256.
+constexpr int kConv23MaxRows = 64;
+
+static int launch_conv23(const Conv23Fwd& p, int rows, int nets, cudaStream_t st) {
+  static bool configured = false;
+  if (!configured) {
+    B2_CHECK_CUDA(cudaFuncSetAttribute(k_conv23_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, conv23::kSmemBytes));
+    configured = true;
+  }
+  static const char* trace_label = getenv("B200DQN_TRACE_LABEL");
+  const int trace = (trace_label && strcmp(trace_label, "conv23_fwd") == 0) ? 1 : 0;
+  B2_CHECK_CUDA(launch_pdl(k_conv23_fwd, dim3(rows, nets), dim3(umma2::kThreads2), conv23::kSmemBytes, st, p, trace,
+                           ktrace_slot("conv23_fwd")));
+  B2_PROF("conv23_fwd", st);
+  return B200DQN_OK;
+}
+
 struct V2Fc1Fwd {
   static constexpr int kBN = 32;
   static constexpr bool kAExact = false, kARowMajorThreads = false, kBRowMajorThreads = true;
@@ -795,7 +1080,8 @@ void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
                  const int64_t nframes[2], int nets, int rows, cudaStream_t st, bool release_early) {
   // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
-  // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.
+  // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.  conv23_fwd keeps
+  // its own release point.
   UmmaState* u = ust(n);
   int rc;
   auto planes = [&](int i, int z) { return PlanePair{u->h16[i][z], u->h_elems[i]}; };
@@ -836,28 +1122,40 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
     if ((rc = umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early))) return rc;
   }
-  {
-    using P = V2ConvFwd<kP1, kC1, 4, 2, kC2>;
-    P p;
+  if (rows <= kConv23MaxRows) {
+    Conv23Fwd p{};
     for (int z = 0; z < 2; ++z) {
-      p.in16[z] = planes(0, z); p.wimg[z] = u->img_fwd[z][1]; p.out16[z] = planes(1, z);
-      p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the target network's fp32 activations
+      p.c2.in16[z] = planes(0, z); p.c2.wimg[z] = u->img_fwd[z][1];
+      p.c3.wimg[z] = u->img_fwd[z][2]; p.c3.out16[z] = planes(2, z);
+      p.c3.out[z] = z ? nullptr : n->d_h3[z];   // nothing reads the target network's fp32 activations
     }
-    p.rows = rows;
-    if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st, false))) return rc;
-  }
-  {
-    using P = V2ConvFwd<kP2, kC2, 3, 1, kC3>;
-    P p;
-    for (int z = 0; z < 2; ++z) {
-      p.in16[z] = planes(1, z); p.wimg[z] = u->img_fwd[z][2]; p.out16[z] = planes(2, z);
-      p.out[z] = z ? nullptr : n->d_h3[z];
+    p.c2.out[0] = n->d_h2[0]; p.c2.out16[0] = planes(1, 0);   // the kernel stores H2 of the online net only
+    p.c2.rows = p.c3.rows = rows;
+    if ((rc = launch_conv23(p, rows, nets, st))) return rc;
+  } else {
+    {
+      using P = V2ConvFwd<kP1, kC1, 4, 2, kC2>;
+      P p;
+      for (int z = 0; z < 2; ++z) {
+        p.in16[z] = planes(0, z); p.wimg[z] = u->img_fwd[z][1]; p.out16[z] = planes(1, z);
+        p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the target network's fp32 activations
+      }
+      p.rows = rows;
+      if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st, false))) return rc;
     }
-    p.rows = rows;
-    if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st, release_early))) return rc;
-    // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
-    if (nets == 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
+    {
+      using P = V2ConvFwd<kP2, kC2, 3, 1, kC3>;
+      P p;
+      for (int z = 0; z < 2; ++z) {
+        p.in16[z] = planes(1, z); p.wimg[z] = u->img_fwd[z][2]; p.out16[z] = planes(2, z);
+        p.out[z] = z ? nullptr : n->d_h3[z];
+      }
+      p.rows = rows;
+      if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st, release_early))) return rc;
+    }
   }
+  // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
+  if (nets == 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
   {
     V2Fc1Fwd p;
     for (int z = 0; z < 2; ++z) { p.in16[z] = planes(2, z); p.wimg[z] = u->img_fwd[z][3]; }
@@ -939,7 +1237,7 @@ int umma_fc1_splits(int rows) { return fc1_splits_for(rows); }
 int umma_push_h3(b200dqn_net* n, cudaStream_t st) {
   UmmaState* u = ust(n);
   cudaStream_t sN = n->side[3];
-  B2_CHECK_CUDA(cudaEventRecord(n->ev[13], st));          // conv3_fwd done: the online net's H3 planes are final
+  B2_CHECK_CUDA(cudaEventRecord(n->ev[13], st));          // conv23_fwd done: the online net's H3 planes are final
   B2_CHECK_CUDA(cudaStreamWaitEvent(sN, n->ev[13], 0));
   const int rc = comm_push_planes(n, 0, u->h16[2][0], u->h_elems[2], sN);
   if (rc) return rc;

@@ -53,7 +53,7 @@ bool comm_dz4_ll_enabled();
 int comm_gather_dz4_ll(b200dqn_net* n, const void* hi, int64_t lo_off_elems, cudaStream_t st, bool wait_h3);   // LL all-gather of the dZ4 planes
 bool comm_head_push(const b200dqn_net* n, cudaStream_t st, HeadPush* out);   // gather schedule + head-side dZ4 push on?
 // gather schedule hooks of the tensor-core engine (net_umma.cu)
-int umma_push_h3(b200dqn_net* n, cudaStream_t st);       // after conv3_fwd: rows of the online net's H3 planes
+int umma_push_h3(b200dqn_net* n, cudaStream_t st);       // after conv23_fwd: rows of the online net's H3 planes
 int umma_push_dz4(b200dqn_net* n, cudaStream_t st);      // after the head
 int umma_gather_dz4_ll(b200dqn_net* n, cudaStream_t st); // after the head: LL all-gather of dZ4 (default)
 int umma_fc1_wgrad_gathered(b200dqn_net* n, cudaStream_t st);   // dW4 over all world x nb rows
