@@ -174,7 +174,8 @@ int b200dqn_statebuf_device_ptr(b200dqn_statebuf* s, void** dev_ptr, size_t* byt
 typedef struct b200dqn_net_config {
   int num_actions;       /* DeepQNetwork(num_actions, args)        deepqnetwork.py:16-18 */
   int batch_size;        /* args.batch_size (per-rank minibatch)   :19                   */
-  int history_length;    /* args.history_length                    :21                   */
+  int history_length;    /* args.history_length                    :21; 1..16 frames, the
+                          * input channels of conv1 (< 1: EINVAL, > 16: ENOTIMPL)        */
   int screen_h, screen_w;/* args.screen_height / width             :22                   */
   double discount_rate;  /* :20  (a Python float: the TD target is formed in double, :141-143) */
   double learning_rate;  /* :51  RMSProp                                                  */

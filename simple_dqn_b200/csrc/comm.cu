@@ -475,6 +475,10 @@ extern "C" int b200dqn_net_comm_init(b200dqn_net* n, const void* id128, int rank
   B2_REQUIRE(n && id128 && world_size >= 1 && rank >= 0 && rank < world_size, B200DQN_EINVAL,
              "net_comm_init: bad argument");
   B2_REQUIRE(!n->nccl_comm, B200DQN_ESTATE, "net_comm_init: communicator already initialised");
+  // conv1's exchange (k_opt_conv<..., XCHG>, the LL line counts) has only been validated for 4-frame windows
+  B2_REQUIRE(n->cfg.history_length == kHist, B200DQN_ENOTIMPL,
+             "net_comm_init: data-parallel learners are implemented for history_length %d only (got %d)", kHist,
+             n->cfg.history_length);
   int rc = nccl_load();
   if (rc) return rc;
   DeviceGuard g(n->device);

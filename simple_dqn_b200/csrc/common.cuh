@@ -179,6 +179,11 @@ __device__ __forceinline__ void tma_bulk_wait_all() { asm volatile("cp.async.bul
 __device__ __forceinline__ void tma_bulk_wait_read_all() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
+// until at most N of the most recently committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void tma_bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
 // Programmatic dependent launch: a kernel launched with the programmatic-stream-serialization
 // attribute may begin while its predecessor is still running; pdl_wait() blocks until every
 // prerequisite grid has completed and flushed (no-op without the attribute), pdl_launch_dependents()

@@ -354,6 +354,7 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
         p.w[z] = w[z] + lt.off[0]; p.out[z] = n->d_h1[z];
       }
       p.nb = rows;
+      p.k1 = lt.rows[0];
       if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st))) return rc;
     }
     {
@@ -433,8 +434,8 @@ static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cud
     }
     default: {
       Conv1Wgrad p{fs.src[0], fs.idx[0], fs.shift[0], n->d_dz1, n->d_part + lt.part_off[0], rows,
-                   wgrad_chunk(rows * kP1 * kP1, 512)};
-      return launch_gemm<Conv1Wgrad, 64, 32, 16, 4, 2>("conv1_wgrad", p, kK1, kC1, lt.splits[0], st);
+                   wgrad_chunk(rows * kP1 * kP1, 512), lt.rows[0]};
+      return launch_gemm<Conv1Wgrad, 64, 32, 16, 4, 2>("conv1_wgrad", p, lt.rows[0], kC1, lt.splits[0], st);
     }
   }
 }
@@ -887,14 +888,19 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   B2_REQUIRE(cfg->num_actions >= 1 && cfg->num_actions <= kMaxActions, B200DQN_EINVAL,
              "net_create: num_actions %d not in [1,%d]", cfg->num_actions, kMaxActions);
   B2_REQUIRE(cfg->batch_size >= 1 && cfg->batch_size <= 4096, B200DQN_EINVAL, "net_create: batch_size");
-  B2_REQUIRE(cfg->screen_h == kFrameH && cfg->screen_w == kFrameW && cfg->history_length == kHist,
-             B200DQN_ENOTIMPL,
-             "net_create: only the reference's 84x84x4 Nature-DQN geometry is implemented (got %dx%dx%d)",
-             cfg->screen_h, cfg->screen_w, cfg->history_length);
+  B2_REQUIRE(cfg->history_length >= 1, B200DQN_EINVAL, "net_create: history_length %d < 1", cfg->history_length);
+  B2_REQUIRE(cfg->screen_h == kFrameH && cfg->screen_w == kFrameW, B200DQN_ENOTIMPL,
+             "net_create: only the reference's 84x84 Nature-DQN screen is implemented (got %dx%d)", cfg->screen_h,
+             cfg->screen_w);
+  B2_REQUIRE(cfg->history_length <= kMaxHist, B200DQN_ENOTIMPL,
+             "net_create: history_length %d not implemented (history lengths 1..%d are)", cfg->history_length, kMaxHist);
   B2_REQUIRE(cfg->math_mode == B200DQN_MATH_FP32_SIMT || cfg->math_mode == B200DQN_MATH_TCGEN05, B200DQN_EINVAL,
              "net_create: unknown math_mode %d", cfg->math_mode);
   B2_REQUIRE(cfg->optimizer >= B200DQN_OPT_RMSPROP && cfg->optimizer <= B200DQN_OPT_ADADELTA, B200DQN_EINVAL,
              "net_create: unknown optimizer %d", cfg->optimizer);   // deepqnetwork.py:61 `assert false, "Unknown optimizer"`
+  B2_REQUIRE(cfg->math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma() || cfg->history_length == kHist,
+             B200DQN_ENOTIMPL, "net_create: the B200DQN_CONV1=tma conv1 gathers %d-frame windows only (history_length %d)",
+             kHist, cfg->history_length);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -904,9 +910,9 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->cfg = *cfg;
   n->nb = cfg->batch_size;
   n->A = cfg->num_actions;
-  const int nb = n->nb, A = n->A;
+  const int nb = n->nb, A = n->A, hist = cfg->history_length;
   LayerTable& lt = n->lt;
-  const int rows_[kLayers] = {kK1, kK2, kK3, kFlat, kHidden};
+  const int rows_[kLayers] = {64 * hist, kK2, kK3, kFlat, kHidden};   // conv1: one 64-tap k-block per frame
   const int cols_[kLayers] = {kC1, kC2, kC3, kHidden, A};
   lt.off[0] = 0;
   for (int l = 0; l < kLayers; ++l) {
@@ -973,7 +979,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   B2_CHECK_CUDA(cudaMalloc(&n->d_step, sizeof(uint32_t)));
   B2_CHECK_CUDA(cudaMemset(n->d_step, 0, sizeof(uint32_t)));
   B2_CHECK_CUDA(fmalloc(&n->d_rowcost, nb));
-  const size_t state_bytes = size_t(nb) * kHist * kFrameBytes;
+  const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
   B2_CHECK_CUDA(cudaMalloc(&n->d_pre, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_post, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_act, nb));
@@ -981,7 +987,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   B2_CHECK_CUDA(cudaMalloc(&n->d_rew, nb * sizeof(int64_t)));
   B2_CHECK_CUDA(cudaMalloc(&n->d_iota1, nb * sizeof(int32_t)));
   B2_CHECK_CUDA(cudaMalloc(&n->d_iota4, nb * sizeof(int32_t)));
-  k_iota<<<cdiv(nb, 128), 128>>>(n->d_iota1, n->d_iota4, nb, kHist);
+  k_iota<<<cdiv(nb, 128), 128>>>(n->d_iota1, n->d_iota4, nb, hist);
   B2_LAUNCH_CHECK();
   n->pin_bytes = 2 * state_bytes + size_t(nb) * 16 + size_t(nb) * A * sizeof(float) + 256;
   B2_CHECK_CUDA(cudaMallocHost(&n->h_pin, n->pin_bytes));
@@ -1036,7 +1042,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
 extern "C" int b200dqn_net_layer_shape(const b200dqn_net* n, int layer, int* rows, int* cols) {
   B2_REQUIRE(n && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_layer_shape: bad layer");
   // NEON shapes: conv (C*R*S, K); linear (nout, nin)
-  const int r[kLayers] = {kK1, kK2, kK3, kHidden, n->A};
+  const int r[kLayers] = {n->lt.rows[0], kK2, kK3, kHidden, n->A};
   const int c[kLayers] = {kC1, kC2, kC3, kFlat, kHidden};
   if (rows) *rows = r[layer];
   if (cols) *cols = c[layer];
@@ -1119,7 +1125,7 @@ extern "C" int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_sta
              "net_predict_device: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
-  const int64_t state_frames = int64_t(n->nb) * kHist;
+  const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
   FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
   HeadTrainArgs no_td{};
   int rc = forward(n, fs, 1, live_rows, st, no_td);
@@ -1168,7 +1174,7 @@ extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* de
     if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }
     cudaGraph_t graph = nullptr;
     B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int64_t state_frames = int64_t(n->nb) * kHist;
+    const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
     FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
     HeadTrainArgs no_td{};
     int rc = forward(n, fs, 1, live_rows, st, no_td);
@@ -1199,7 +1205,7 @@ extern "C" int b200dqn_net_predict(b200dqn_net* n, const uint8_t* host_states, f
   B2_REQUIRE(n && host_states && host_q, B200DQN_EINVAL, "net_predict: null argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
-  const size_t state_bytes = size_t(n->nb) * kHist * kFrameBytes;
+  const size_t state_bytes = size_t(n->nb) * n->cfg.history_length * kFrameBytes;
   memcpy(n->h_pin, host_states, state_bytes);
   B2_CHECK_CUDA(cudaMemcpyAsync(n->d_pre, n->h_pin, state_bytes, cudaMemcpyHostToDevice, st));
   int rc = b200dqn_net_predict_device(n, n->d_pre, n->nb, n->d_q[0], stream);
@@ -1217,7 +1223,7 @@ extern "C" int b200dqn_net_train_device(b200dqn_net* n, const uint8_t* dev_pre, 
   B2_REQUIRE(n && dev_pre && dev_actions && dev_rewards && dev_post && dev_terminals, B200DQN_EINVAL,
              "net_train_device: null argument");
   DeviceGuard g(n->device);
-  const int64_t state_frames = int64_t(n->nb) * kHist;
+  const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
   FrameSource fs{{dev_pre, dev_post}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
   B2_TRY(train_step(n, fs, dev_actions, dev_rewards, dev_terminals, n->d_iota1, as_stream(stream)));
   n->train_iterations += 1;
@@ -1233,7 +1239,7 @@ extern "C" int b200dqn_net_train(b200dqn_net* n, const uint8_t* host_pre, const 
     B2_REQUIRE(host_actions[i] < n->A, B200DQN_EINVAL, "net_train: action %d >= num_actions %d", host_actions[i], n->A);
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
-  const size_t sb = size_t(n->nb) * kHist * kFrameBytes;
+  const size_t sb = size_t(n->nb) * n->cfg.history_length * kFrameBytes;
   uint8_t* p = n->h_pin;
   memcpy(p, host_pre, sb);
   memcpy(p + sb, host_post, sb);
@@ -1255,8 +1261,9 @@ extern "C" int b200dqn_net_train(b200dqn_net* n, const uint8_t* host_pre, const 
 
 static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
   B2_REQUIRE(r->device == n->device, B200DQN_EINVAL, "train_fused: replay and net live on different devices");
-  B2_REQUIRE(r->h == kFrameH && r->w == kFrameW && r->hist == kHist, B200DQN_EINVAL,
-             "train_fused: replay geometry differs from the network's");
+  B2_REQUIRE(r->h == kFrameH && r->w == kFrameW && r->hist == n->cfg.history_length, B200DQN_EINVAL,
+             "train_fused: replay geometry (%dx%dx%d) differs from the network's (%dx%dx%d)", r->h, r->w, r->hist,
+             kFrameH, kFrameW, n->cfg.history_length);
   B2_REQUIRE(r->batch == n->nb * n->world, B200DQN_EINVAL,
              "train_fused: replay batch (%d) must equal the global minibatch %d x %d", r->batch, n->nb, n->world);
   return B200DQN_OK;
@@ -1264,8 +1271,9 @@ static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
 
 static int train_on_ring(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   const int32_t* my_idx = r->d_idx + n->rank * n->nb;  // this rank's slice of the global minibatch
-  // prestates = frames index-4 .. index-1, poststates = index-3 .. index (src/replay_memory.py:71-72)
-  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-kHist, -kHist + 1}, {r->size, r->size}};
+  // prestates = frames index-H .. index-1, poststates = index-H+1 .. index (src/replay_memory.py:71-72)
+  const int hist = n->cfg.history_length;
+  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-hist, -hist + 1}, {r->size, r->size}};
   n->step_replay = r;
   const int rc = train_step(n, fs, r->d_actions, r->d_rewards, r->d_terminals, my_idx, st);
   n->step_replay = nullptr;

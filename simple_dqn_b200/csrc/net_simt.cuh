@@ -5,27 +5,28 @@
 // dgrad, wgrad, dense layers) is the same kernel with a different functor.  It is the exact-fp32
 // mode of the library and the on-device cross-check of the tensor-core path.
 //
-// Geometry is the reference's (src/deepqnetwork.py:77-92): 84x84x4 u8 -> conv 8x8x32 s4 ->
-// conv 4x4x64 s2 -> conv 3x3x64 s1 -> fc 512 -> fc A; no bias, no padding.
+// Geometry is the reference's (src/deepqnetwork.py:77-92): 84x84xH u8 (H = history_length frames as input
+// channels) -> conv 8x8x32 s4 -> conv 4x4x64 s2 -> conv 3x3x64 s1 -> fc 512 -> fc A; no bias, no padding.
 //
 // Internal layouts (HBM):
 //   activations  NHWC fp32:  H1[n][20][20][32]  H2[n][9][9][64]  H3[n][7][7][64]  H4[n][512]
 //   weights      [K][N] fp32 with N (output feature) contiguous and K ordered to match the
-//                producer's NHWC patch: W1[(c,r,s)][32] (== Neon CRSK), W2[(r,s,c)][64],
+//                producer's NHWC patch: W1[(c,r,s)][32] (64*H rows, == Neon CRSK), W2[(r,s,c)][64],
 //                W3[(r,s,c)][64], W4[(p,q,c)][512], W5[512][A]
 #pragma once
 #include "common.cuh"
 
 namespace b200 {
 
-constexpr int kFrameH = 84, kFrameW = 84, kHist = 4;
+constexpr int kFrameH = 84, kFrameW = 84;
+constexpr int kHist = 4;                        // the reference's default history length (main.py:34)
+constexpr int kMaxHist = 16;                    // history lengths 1..kMaxHist are implemented
 constexpr int kFrameBytes = kFrameH * kFrameW;  // 7056 = 441 * 16
 constexpr int kP1 = 20, kC1 = 32;               // conv1 output
 constexpr int kP2 = 9, kC2 = 64;                // conv2 output
 constexpr int kP3 = 7, kC3 = 64;                // conv3 output
 constexpr int kFlat = kP3 * kP3 * kC3;          // 3136
 constexpr int kHidden = 512;
-constexpr int kK1 = kHist * 8 * 8;              // 256
 constexpr int kK2 = 4 * 4 * kC1;                // 512
 constexpr int kK3 = 3 * 3 * kC2;                // 576
 
@@ -96,8 +97,8 @@ __global__ void __launch_bounds__((BM / TM) * (BN / TN)) k_simt_gemm(const P p) 
 // Forward problems.  z selects the network: 0 = online (prestates), 1 = target (poststates).
 // ------------------------------------------------------------------------------------------
 
-// conv1: A = u8 frames read in place (ring or staged states), k = (c, r, s); the /255 of
-// _setInput (src/deepqnetwork.py:100) is applied to the fp32 accumulator, ReLU fused.
+// conv1: A = u8 frames read in place (ring or staged states), k = (c, r, s) with c the frame of the
+// history window; the /255 of _setInput (src/deepqnetwork.py:100) is applied to the fp32 accumulator, ReLU fused.
 struct Conv1Fwd {
   const uint8_t* src[2];   // base of the frame array
   const int32_t* idx[2];   // per-sample frame index
@@ -105,10 +106,11 @@ struct Conv1Fwd {
   const float* w[2];
   float* out[2];
   int nb;
+  int k1;                  // 64 * history_length
   static constexpr bool kAKContig = true, kBKContig = false;
   __device__ int M(int) const { return nb * kP1 * kP1; }
   __device__ int N(int) const { return kC1; }
-  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = kK1; }
+  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = k1; }
   __device__ float a(int z, int m, int k) const {
     const int n = m / (kP1 * kP1), pq = m % (kP1 * kP1), p = pq / kP1, q = pq % kP1;
     const int c = k >> 6, r = (k >> 3) & 7, s = k & 7;
@@ -271,10 +273,11 @@ struct Conv1Wgrad {
   const int32_t* idx;
   int shift;
   const float* dz;  // dZ1 [nb][20][20][32]
-  float* part;      // [splits][256][32]
+  float* part;      // [splits][k1][32]
   int nb, kchunk;
+  int k1;           // 64 * history_length
   static constexpr bool kAKContig = false, kBKContig = false;
-  __device__ int M(int) const { return kK1; }
+  __device__ int M(int) const { return k1; }
   __device__ int N(int) const { return kC1; }
   __device__ void krange(int z, int& kb, int& ke) const {
     kb = z * kchunk;
@@ -287,7 +290,7 @@ struct Conv1Wgrad {
     return static_cast<float>(src[f * kFrameBytes + (p * 4 + r) * kFrameW + q * 4 + s]);
   }
   __device__ float b(int, int k, int n) const { return dz[k * kC1 + n]; }
-  __device__ void store(int z, int m, int n, float v) const { part[(z * kK1 + m) * kC1 + n] = v * (1.0f / 255.0f); }
+  __device__ void store(int z, int m, int n, float v) const { part[(z * k1 + m) * kC1 + n] = v * (1.0f / 255.0f); }
 };
 
 }  // namespace b200

@@ -38,10 +38,24 @@ struct UmmaState {
   // weight tile images ([hi | lo] per (tile, k-block))
   uint8_t* img_fwd[2][4] = {};  // conv1, conv2, conv3, fc1  x  (online, target)
   int64_t img_fwd_bytes[4] = {};
-  uint8_t* im2col1 = nullptr;   // conv1_fwd's A_hi tiles of the online net: [ceil(nb*400/128)][4][16 KB]
+  uint8_t* im2col1 = nullptr;   // conv1_fwd's A_hi tiles of the online net: [ceil(nb*400/128)][H][16 KB]
   uint8_t* img_dgr[3] = {};     // fc1_dgrad (A operand), conv3_dgrad (B), conv2_dgrad (B, 4 parity classes)
 };
 static inline UmmaState* ust(b200dqn_net* n) { return static_cast<UmmaState*>(n->umma_state); }
+
+// f(std::integral_constant<int, H>{}) for H = hist in 1..kMaxHist: conv1's kernels take the history length as a template
+// argument, so its k-block count, M extent and parameter count are compile-time constants.  One source path for every H;
+// a run-time H made conv1_fwd's refill path live for every H (72 -> 110 registers) and the batch-32 step 0.6 us slower
+// at H = 4 (H100 80GB HBM3, 400 W).
+template <int H = 1, class F>
+static auto with_hist(int hist, F&& f) -> decltype(f(std::integral_constant<int, 1>{})) {
+  if constexpr (H == kMaxHist) {
+    return f(std::integral_constant<int, H>{});   // net_create admits 1..kMaxHist only
+  } else {
+    if (hist == H) return f(std::integral_constant<int, H>{});
+    return with_hist<H + 1>(hist, f);
+  }
+}
 
 struct PlanePair {
   __half* hi;
@@ -54,22 +68,25 @@ __device__ __forceinline__ void store_f32_and_planes(float* f32, const PlanePair
 }
 
 // ---- forward -----------------------------------------------------------------------------
+// H = history_length, a template argument (see with_hist): H k-blocks of 64 taps (8x8 pixels), one per frame.  Up to
+// kStages frames every k-block has its own ring stage, and the loads of later k-blocks compile away.
+template <int H>
 struct V2Conv1Fwd {
   static constexpr int kBN = 32;
   static constexpr bool kAExact = true, kARowMajorThreads = true, kBRowMajorThreads = false;
   static constexpr int kAMode = umma2::kReg, kBMode = umma2::kBulk;
   static constexpr bool kStagedEpilogue = true, kDumpA = true, kPrefetch = false;
-  uint8_t* im2col;          // online net only: [mtile][4 kb][128 x 128 B] A_hi tiles for conv1_wgrad (nullptr = off)
+  uint8_t* im2col;          // online net only: [mtile][H kb][128 x 128 B] A_hi tiles for conv1_wgrad (nullptr = off)
   const uint8_t* src[2];
   const int32_t* idx[2];
   int shift[2];
-  const uint8_t* wimg[2];   // [4 kb][hi 32x128 | lo 32x128]
+  const uint8_t* wimg[2];   // [H kb][hi 32x128 | lo 32x128]
   float* out[2];
   PlanePair out16[2];
   int rows;
   __device__ int M(int) const { return rows * kP1 * kP1; }
   __device__ int N(int) const { return kC1; }
-  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = kK1 / 64; }
+  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = H; }
   // first byte of output pixel m's receptive field in frame 0 of its sample (nullptr = padding row)
   __device__ const uint8_t* a_row_ptr(int z, int m) const {
     if (m >= rows * kP1 * kP1) return nullptr;
@@ -92,7 +109,7 @@ struct V2Conv1Fwd {
   }
   __device__ const uint8_t* b_tile(int z, int, int kb) const { return (z ? wimg[1] : wimg[0]) + kb * (kC1 * 256); }
   __device__ uint8_t* a_dump(int z, int mtile, int kb) const {
-    return (z == 0 && im2col) ? im2col + (int64_t(mtile) * (kK1 / 64) + kb) * (128 * 128) : nullptr;
+    return (z == 0 && im2col) ? im2col + (int64_t(mtile) * H + kb) * (128 * 128) : nullptr;
   }
   __device__ void store8(int z, int m, int n0, const float v[8]) const {
     float o[8];
@@ -592,15 +609,17 @@ struct WConvWgrad {
 // conv1: the A operand (row = output pixel, 64 contiguous taps (r,s) of frame c, exact u8 values) is
 // exactly the tile conv1_fwd staged for its own MMA, so conv1_fwd ships those tiles to an im2col image
 // (V2Conv1Fwd::kDumpA) and this kernel fetches each [64 pixels x 64 taps] sub-tile with ONE TMA bulk copy.
+// M = 64 H rows (c, r, s): each 64-row m chunk is one frame c, so for odd H the last 128-row M tile has one live chunk.
+template <int H>
 struct WConv1Wgrad {
   static constexpr int kBN = 32, kStages = 4;
   static constexpr bool kAExact = true, kABulk = true;
-  const uint8_t* im2col;   // [pixel tile of 128][c = 4][128 x 128 B]
+  const uint8_t* im2col;   // [pixel tile of 128][c = H][128 x 128 B]
   PlanePair dz16;          // dZ1 [rows][20][20][32]
-  float* part;             // [splits][256][32]
+  float* part;             // [splits][64 H][32]
   int rows, kb_per_split;
   int tile_rows;           // live rows per 128-row im2col tile: 128 (dense tiling) or 100 (conv1_tma.cuh: 4 tiles/sample)
-  __device__ int M(int) const { return kK1; }
+  __device__ int M(int) const { return 64 * H; }
   __device__ int N(int) const { return kC1; }
   __device__ int total_kb() const {
     return tile_rows == 128 ? (rows * kP1 * kP1 + 63) / 64 : rows * conv1tma::kTilesPerSample * 2;
@@ -616,8 +635,9 @@ struct WConv1Wgrad {
     const int tile = kpix >> 7, local = kpix & 127;
     return {tile * tile_rows + local, 0, 0, local < tile_rows && tile < rows * conv1tma::kTilesPerSample};
   }
-  __device__ const uint8_t* a_sub(int, int c, int kb) const {   // kb = global 64-pixel block
-    return im2col + (int64_t(kb >> 1) * (kK1 / 64) + c) * (128 * 128) + (kb & 1) * (64 * 128);
+  __device__ const uint8_t* a_sub(int, int c, int kb) const {   // kb = global 64-pixel block; nullptr: c >= H
+    if (c >= H) return nullptr;
+    return im2col + (int64_t(kb >> 1) * H + c) * (128 * 128) + (kb & 1) * (64 * 128);
   }
   __device__ umma2::Planes b_planes(int) const { return {dz16.hi, dz16.lo_off}; }
   __device__ int64_t b_off(int, const umma_mn::PixCtx& px) const { return int64_t(px.n) * kC1; }
@@ -625,7 +645,7 @@ struct WConv1Wgrad {
     float o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = v[j] * (1.0f / 255.0f);
-    st8(part + (int64_t(z) * kK1 + m) * kC1 + n0, o);
+    st8(part + (int64_t(z) * 64 * H + m) * kC1 + n0, o);
   }
 };
 
@@ -880,8 +900,11 @@ int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* 
   cudaError_t e;
   const XllArgs none{};
   if (l == 0)
-    e = launch_pdl(k_opt_conv<kK1, kC1, false, 4, 8, 4>, grid, block, 0, st, part, nsplits, w, s, u->img_fwd[0][0],
-                   (uint8_t*)nullptr, opt, none, ktrace_slot(label));
+    e = with_hist(n->cfg.history_length, [&](auto h) {
+      constexpr int H = decltype(h)::value;
+      return launch_pdl(k_opt_conv<64 * H, kC1, false, 4, 8, 4>, grid, block, 0, st, part, nsplits, w, s,
+                        u->img_fwd[0][0], (uint8_t*)nullptr, opt, none, ktrace_slot(label));
+    });
   else if (l == 1)
     e = launch_pdl(k_opt_conv<kK2, kC2, true, kC1, 4, 2>, grid, block, 0, st, part, nsplits, w, s, u->img_fwd[0][1],
                    u->img_dgr[2], opt, none, ktrace_slot(label));
@@ -910,8 +933,10 @@ int umma_opt_conv_xll(b200dqn_net* n, int l, int rows, cudaStream_t st, const ch
   const int64_t size = lt.off[l + 1] - lt.off[l];
   const dim3 grid(unsigned((size / 4 + 31) / 32)), block(256);
   cudaError_t e;
+  // data-parallel learners run 4-frame windows only (b200dqn_net_comm_init)
+  B2_REQUIRE(lt.rows[0] == 64 * kHist, B200DQN_ENOTIMPL, "opt_conv_xll: history_length %d", n->cfg.history_length);
   if (l == 0)
-    e = launch_pdl(k_opt_conv<kK1, kC1, false, 4, 8, 4, true>, grid, block, 0, st, part, lt.splits[l], w, s,
+    e = launch_pdl(k_opt_conv<64 * kHist, kC1, false, 4, 8, 4, true>, grid, block, 0, st, part, lt.splits[l], w, s,
                    u->img_fwd[0][0], (uint8_t*)nullptr, opt, x, ktrace_slot(label));
   else if (l == 1)
     e = launch_pdl(k_opt_conv<kK2, kC2, true, kC1, 4, 2, true>, grid, block, 0, st, part, lt.splits[l], w, s,
@@ -924,9 +949,9 @@ int umma_opt_conv_xll(b200dqn_net* n, int l, int rows, cudaStream_t st, const ch
   return B200DQN_OK;
 }
 
-static int64_t fwd_image_bytes(int layer) {
+static int64_t fwd_image_bytes(int layer, int hist) {
   switch (layer) {
-    case 0: return int64_t(kK1 / 64) * kC1 * 256;
+    case 0: return int64_t(hist) * kC1 * 256;
     case 1: return int64_t(kK2 / 64) * kC2 * 256;
     case 2: return int64_t(kK3 / 64) * kC3 * 256;
     default: return int64_t((kFlat + 127) / 128) * (kHidden / 64) * 128 * 256;   // fc1: the row-oriented image
@@ -942,7 +967,12 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
   int rc = 0;
   for (int l = l0; l <= l1 && !rc; ++l) {
     switch (l) {
-      case 0: rc = umma2::launch_pack("pack_c1", PackFwdConv<kK1, kC1>{w + lt.off[0]}, u->img_fwd[which][0], st); break;
+      case 0:
+        rc = with_hist(n->cfg.history_length, [&](auto h) {
+          constexpr int H = decltype(h)::value;
+          return umma2::launch_pack("pack_c1", PackFwdConv<64 * H, kC1>{w + lt.off[0]}, u->img_fwd[which][0], st);
+        });
+        break;
       case 1:
         rc = umma2::launch_pack("pack_c2f", PackFwdConv<kK2, kC2>{w + lt.off[1]}, u->img_fwd[which][1], st);
         if (!rc && !which)
@@ -980,6 +1010,7 @@ static const bool g_conv1_tma = getenv("B200DQN_CONV1") && strcmp(getenv("B200DQ
 // rows of conv1's im2col image (= conv1_wgrad's reduction length): dense 128-row tiles on the register path, 4 tiles
 // of 100 live rows per sample on the TMA path
 static inline int conv1_pixels_padded(int rows) { return g_conv1_tma ? rows * conv1tma::kTilesPerSample * 128 : rows * kP1 * kP1; }
+bool umma_conv1_tma() { return g_conv1_tma; }
 
 // k-blocks (of 64 pixels) per wgrad split: at least kUWgradKb, and few enough splits (<= 48) for the
 // one-pass reduction of k_opt_conv
@@ -1022,14 +1053,15 @@ int umma_net_init(b200dqn_net* n) {
     B2_CHECK_CUDA(cudaMemset(u->dz16[i], 0, 2 * u->dz_elems[i] * sizeof(__half)));
   }
   for (int l = 0; l < 4; ++l) {
-    u->img_fwd_bytes[l] = fwd_image_bytes(l);
+    u->img_fwd_bytes[l] = fwd_image_bytes(l, n->cfg.history_length);
     for (int z = 0; z < 2; ++z) {
       if (z == 1 && n->d_tw == n->d_w) { u->img_fwd[1][l] = u->img_fwd[0][l]; continue; }
       B2_CHECK_CUDA(cudaMalloc(&u->img_fwd[z][l], u->img_fwd_bytes[l]));
       B2_CHECK_CUDA(cudaMemset(u->img_fwd[z][l], 0, u->img_fwd_bytes[l]));
     }
   }
-  B2_CHECK_CUDA(cudaMalloc(&u->im2col1, int64_t((conv1_pixels_padded(nb) + 127) / 128) * (kK1 / 64) * 128 * 128));
+  B2_CHECK_CUDA(cudaMalloc(&u->im2col1,
+                           int64_t((conv1_pixels_padded(nb) + 127) / 128) * n->cfg.history_length * 128 * 128));
   u->img_dgr[0] = u->img_fwd[0][3];   // fc1: ONE row-oriented image serves the dgrad (K-major) and the forward (MN-major)
   const int64_t dgr_bytes[3] = {0, int64_t(kK3 / 64) * kC2 * 256, int64_t(4) * (256 / 64) * kC1 * 256};
   for (int i = 1; i < 3; ++i) {
@@ -1113,14 +1145,18 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
                              smem, st, m0, m1, p, ktrace_slot("conv1_fwd")));
     B2_PROF("conv1_fwd", st);
   } else {
-    V2Conv1Fwd p;
-    for (int z = 0; z < 2; ++z) {
-      p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
-      p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z]; p.out16[z] = planes(0, z);
-    }
-    p.rows = rows;
-    p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
-    if ((rc = umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early))) return rc;
+    rc = with_hist(n->cfg.history_length, [&](auto h) {
+      constexpr int H = decltype(h)::value;
+      V2Conv1Fwd<H> p;
+      for (int z = 0; z < 2; ++z) {
+        p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
+        p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z]; p.out16[z] = planes(0, z);
+      }
+      p.rows = rows;
+      p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
+      return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early);
+    });
+    if (rc) return rc;
   }
   if (rows <= kConv23MaxRows) {
     Conv23Fwd p{};
@@ -1225,9 +1261,12 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
     default: {
       UmmaState* u = ust(n);
       (void)src; (void)idx; (void)shift;   // the frames were already gathered by conv1_fwd (im2col image)
-      WConv1Wgrad p{u->im2col1, PlanePair{u->dz16[3], u->dz_elems[3]}, n->d_part + lt.part_off[0], rows,
-                    umma_wgrad_kb(0, rows), g_conv1_tma ? conv1tma::kTileRows : 128};
-      return umma_mn::launch_umma_mn("conv1_wgrad", p, kK1, kC1, lt.splits[0], st, release_early);
+      return with_hist(n->cfg.history_length, [&](auto h) {
+        constexpr int H = decltype(h)::value;
+        WConv1Wgrad<H> p{u->im2col1, PlanePair{u->dz16[3], u->dz_elems[3]}, n->d_part + lt.part_off[0], rows,
+                           umma_wgrad_kb(0, rows), g_conv1_tma ? conv1tma::kTileRows : 128};
+        return umma_mn::launch_umma_mn("conv1_wgrad", p, 64 * H, kC1, lt.splits[0], st, release_early);
+      });
     }
   }
 }

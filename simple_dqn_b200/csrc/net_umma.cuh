@@ -34,6 +34,7 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
 // fp16 hi plane of dZ4 and the offset of its lo plane (nullptr when math_mode != TCGEN05)
 void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
 int umma_wgrad_splits(int layer, int rows);   // split-K factor of the conv wgrad of `layer` (0..2)
+bool umma_conv1_tma();   // B200DQN_CONV1=tma: conv1 runs the tensor-map TMA twin (4-frame windows only)
 // op: 0 fc1_wgrad, 1 fc1_dgrad, 2 conv3_wgrad, 3 conv3_dgrad, 4 conv2_wgrad, 5 conv2_dgrad, 6 conv1_wgrad
 // release_early: as for umma_forward
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,

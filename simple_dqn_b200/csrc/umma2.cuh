@@ -74,8 +74,8 @@ __device__ __forceinline__ void split8_planes(const float v[8], __half* hi_dst, 
 //           as two [64 k-rows x 128 B] sub-tiles per half,  a_sub(z, mtile, kb, chunk) -> hi sub-tile, the lo
 //           sub-tile kAMnLoOffset bytes behind it
 //   void store8(z, m, n0, const float v[8])
-//   static constexpr bool kDumpA: after k-block kb is staged, bulk-store the A_hi tile to a_dump(z, mtile, kb)
-//        (needs every k-block in its own stage: nkb <= kStages)
+//   static constexpr bool kDumpA: after k-block kb is staged, bulk-store the A_hi tile to a_dump(z, mtile, kb); one
+//        bulk group per k-block, and a stage is refilled only once its dump has finished reading it
 //   static constexpr bool kStagedEpilogue: store8 writes 8 CONTIGUOUS outputs of row m (NHWC tensors) ->
 //        the tile is transposed through smem so that a warp's stores are whole cache lines
 template <class P, class = void>
@@ -355,6 +355,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
       if (tid == 0) {
         uint8_t* dump = p.a_dump(z, mtile, kb0 + it);
         if (dump) tma_bulk_s2g(dump, smem_gen + s * C::kStageBytes, C::kABytes);
+        tma_bulk_commit();
       }
     }
     const uint32_t a_hi = sa + wg * kAWg, a_lo = a_hi + C::kABytes;
@@ -371,6 +372,8 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
     umma::wgmma_wait<1>();
     B2_TRACE(tid == 0, 8 + it * 4 + 1);
     if (it >= 1 && it - 1 + S < nkb) {
+      // more k-blocks than stages (conv1 with H > S frames): k-block it-1's dump must have read its stage
+      if (P::kDumpA && tid == 0) tma_bulk_wait_read<1>();
       named_bar_sync(1, kThreads2);   // both warpgroups are done with k-block it-1: its stage takes k-block it-1+S
       stage(it - 1 + S);
     }
@@ -407,10 +410,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   }
   umma::wgmma_wait<0>();
   if constexpr (P::kDumpA) {
-    if (tid == 0) {
-      tma_bulk_commit();
-      tma_bulk_wait_read_all();   // smem may now be reused by the staging tile
-    }
+    if (tid == 0) tma_bulk_wait_read_all();   // smem may now be reused by the staging tile
   }
   named_bar_sync(1, kThreads2);   // every warpgroup's MMAs (and the A dump) have finished reading the stages
   B2_TRACE(tid == 0, 4);

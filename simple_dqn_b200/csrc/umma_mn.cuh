@@ -39,7 +39,9 @@ struct PixCtx {   // decoded reduction index (one per thread per k-block)
 //   static constexpr int kBN (32 or 64); static constexpr bool kAExact, kABulk;
 //   int M(z), N(z); void krange(z, kb0, kb1);  PixCtx pix(z, kpix);
 //   !kABulk: Planes a_planes(z); bool a_run(z, pix, mchunk, int64_t& off)     64 contiguous fp16 of A for this pixel
-//    kABulk: const uint8_t* a_sub(z, mchunk, kb)   ready-made [64 k-rows x 128 B] sub-tile image (exact A only)
+//    kABulk: const uint8_t* a_sub(z, mchunk, kb)   ready-made [64 k-rows x 128 B] sub-tile image (exact A only);
+//            nullptr for the second m chunk of a tile whose rows 64..127 lie beyond M (not fetched: those
+//            accumulator rows are never stored)
 //   Planes b_planes(z); int64_t b_off(z, pix)                                  BN contiguous fp16 of B for this pixel
 //   void store8(z, m, n0, const float v[8])
 template <class P>
@@ -116,9 +118,10 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma_mn(const P p, const bool 
     if constexpr (P::kABulk) {
       static_assert(P::kAExact, "bulk A sub-tiles carry no lo part");
       if (tid == 0) {
-        mbar_arrive_expect_tx(&s_full[s], 2 * C::kSub);
+        const uint8_t* a1 = p.a_sub(z, blockIdx.x * 2 + 1, kb0 + j);
+        mbar_arrive_expect_tx(&s_full[s], (a1 ? 2 : 1) * C::kSub);
         tma_bulk_g2s(st_gen, p.a_sub(z, blockIdx.x * 2, kb0 + j), C::kSub, &s_full[s]);
-        tma_bulk_g2s(st_gen + C::kSub, p.a_sub(z, blockIdx.x * 2 + 1, kb0 + j), C::kSub, &s_full[s]);
+        if (a1) tma_bulk_g2s(st_gen + C::kSub, a1, C::kSub, &s_full[s]);
       }
     } else {
       const int mc = sub >> 1, j0 = (sub & 1) * 4;

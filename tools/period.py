@@ -10,11 +10,20 @@ torch.cuda.set_stream(st)
 replay = 50000
 base, actions, rewards, terminals = synthetic_meta(replay)
 B = int(os.environ.get("BATCH", "32"))
-mem = ReplayMemory(replay, make_args(B), stream=st, rng="device")
+HIST = int(os.environ.get("HIST", "4"))   # --history_length: frames per state, conv1's input channels
+
+
+def args():
+    a = make_args(B)
+    a.history_length = HIST
+    return a
+
+
+mem = ReplayMemory(replay, args(), stream=st, rng="device")
 for s in range(0, replay, 10000):
     mem.add_batch(actions[s:s + 10000], rewards[s:s + 10000], base, terminals[s:s + 10000])
 mem.set_cursor(replay, 1234)
-net = DeepQNetwork(NUM_ACTIONS, make_args(B), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
+net = DeepQNetwork(NUM_ACTIONS, args(), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
 net.update_target_network()
 random.seed(1); mem.seed_device_rng(random)
 net.train_fused(mem, 300); st.synchronize()
@@ -32,4 +41,5 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("period_us min %.2f median %.2f  all %s" % (min(res), float(np.median(res)), " ".join("%.2f" % r for r in res)))
+print("batch %d hist %d period_us min %.2f median %.2f  all %s" % (B, HIST, min(res), float(np.median(res)),
+                                                                  " ".join("%.2f" % r for r in res)))
