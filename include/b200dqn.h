@@ -278,7 +278,14 @@ enum {
   B200DQN_NET_PTR_H1,           /* online activations of the last forward, NHWC fp32: (batch,20,20,32) */
   B200DQN_NET_PTR_H2,           /* (batch,9,9,64)                                                      */
   B200DQN_NET_PTR_H3,           /* (batch,7,7,64)                                                      */
-  B200DQN_NET_PTR_H4            /* (batch,512)                                                         */
+  B200DQN_NET_PTR_H4,           /* (batch,512)                                                         */
+  /* Online-network gradients at each layer's pre-activation (Rectlin mask applied) of the last train step, NHWC
+   * fp32.  DZ4 is always written.  DZ3..DZ1 are always written by the FP32_SIMT engine; the tensor-core engine writes
+   * them only while b200dqn_net_set_keep_grads is on, otherwise they hold whatever was there before. */
+  B200DQN_NET_PTR_DZ4,          /* (batch,512)                                                         */
+  B200DQN_NET_PTR_DZ3,          /* (batch,7,7,64)                                                      */
+  B200DQN_NET_PTR_DZ2,          /* (batch,9,9,64)                                                      */
+  B200DQN_NET_PTR_DZ1           /* (batch,20,20,32)                                                    */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

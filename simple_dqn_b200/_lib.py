@@ -13,7 +13,7 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
 (PTR_SCREENS, PTR_ACTIONS, PTR_REWARDS, PTR_TERMINALS, PTR_PRESTATES, PTR_POSTSTATES, PTR_MB_ACTIONS,
  PTR_MB_REWARDS, PTR_MB_TERMINALS, PTR_INDEXES, PTR_WORDS_CONSUMED, PTR_MT_STATE) = range(12)
 (NET_PTR_Q_ONLINE, NET_PTR_Q_TARGET, NET_PTR_DELTAS, NET_PTR_GRADS, NET_PTR_WEIGHTS, NET_PTR_COST, NET_PTR_H1,
- NET_PTR_H2, NET_PTR_H3, NET_PTR_H4) = range(10)
+ NET_PTR_H2, NET_PTR_H3, NET_PTR_H4, NET_PTR_DZ4, NET_PTR_DZ3, NET_PTR_DZ2, NET_PTR_DZ1) = range(14)
 
 
 class B200DQNError(RuntimeError):

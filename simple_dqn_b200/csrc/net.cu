@@ -1467,6 +1467,10 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_H2: p = n->d_h2[0]; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_H3: p = n->d_h3[0]; b = size_t(n->nb) * kFlat * 4; break;
     case B200DQN_NET_PTR_H4: p = n->d_h4[0]; b = size_t(n->nb) * kHidden * 4; break;
+    case B200DQN_NET_PTR_DZ4: p = n->d_dz4; b = size_t(n->nb) * kHidden * 4; break;
+    case B200DQN_NET_PTR_DZ3: p = n->d_dz3; b = size_t(n->nb) * kFlat * 4; break;
+    case B200DQN_NET_PTR_DZ2: p = n->d_dz2; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
+    case B200DQN_NET_PTR_DZ1: p = n->d_dz1; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;

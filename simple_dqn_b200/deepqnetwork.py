@@ -178,6 +178,16 @@ class DeepQNetwork:
         h4 = self._read_f32(L.NET_PTR_H4, (b, 512))
         return h1, h2, h3, h4
 
+    def last_dz(self):
+        """Online-network gradients at the pre-activations of the last train() as NCHW arrays (dZ1, dZ2, dZ3, dZ4),
+        Rectlin masks applied.  On the tensor-core engine dZ1..dZ3 are only written while keep_grads() is on."""
+        b = self.batch_size
+        dz1 = self._read_f32(L.NET_PTR_DZ1, (b, 20, 20, 32)).transpose(0, 3, 1, 2)
+        dz2 = self._read_f32(L.NET_PTR_DZ2, (b, 9, 9, 64)).transpose(0, 3, 1, 2)
+        dz3 = self._read_f32(L.NET_PTR_DZ3, (b, 7, 7, 64)).transpose(0, 3, 1, 2)
+        dz4 = self._read_f32(L.NET_PTR_DZ4, (b, 512))
+        return dz1, dz2, dz3, dz4
+
     def last_deltas(self):
         return self._read_f32(L.NET_PTR_DELTAS, (self.batch_size, self.num_actions))
 

@@ -76,7 +76,8 @@ def test_xavier_init_matches_oracle_draw_order(mode):
 
 
 @pytest.mark.parametrize("mode", MODES)
-@pytest.mark.parametrize("num_actions,batch", [(4, 32), (18, 32), (4, 1), (6, 8), (4, 40), (4, 256)])
+@pytest.mark.parametrize("num_actions,batch", [(4, 32), (18, 32), (4, 1), (6, 8), (4, 40), (4, 64), (4, 65), (4, 256),
+                                               (4, 257)])
 def test_predict_parity(mode, num_actions, batch):
     """net_create takes any batch 1..4096 (tile tails, partial M tiles): every size is held to the same bar."""
     net, orc = _paired(num_actions, mode, batch=batch)
