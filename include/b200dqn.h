@@ -285,12 +285,24 @@ enum {
   B200DQN_NET_PTR_DZ4,          /* (batch,512)                                                         */
   B200DQN_NET_PTR_DZ3,          /* (batch,7,7,64)                                                      */
   B200DQN_NET_PTR_DZ2,          /* (batch,9,9,64)                                                      */
-  B200DQN_NET_PTR_DZ1           /* (batch,20,20,32)                                                    */
+  B200DQN_NET_PTR_DZ1,          /* (batch,20,20,32)                                                    */
+  /* The online network's Q on the poststates of the last Double DQN train step, (batch,A) f32: the row whose first
+   * maximum picks the action the target network values.  With target_steps = 0 it is the Q_TARGET buffer (the two
+   * networks are one). */
+  B200DQN_NET_PTR_Q_ONLINE_POST
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well
  * (tests, debugging). */
 int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
+/* Double DQN target (van Hasselt et al., 2016; new capability, no reference counterpart), off by default:
+ *   a*_i = argmax_a Q_online(s'_i, a)  (first index of the maximum),  y_i = r_i + discount * Q_target(s'_i, a*_i)
+ * in place of max_a Q_target(s'_i, a) (deepqnetwork.py:124,140-143); terminals, reward and error clipping, the cost,
+ * the backward and the optimizers are unchanged, and predict is not affected.  The train-step forward runs the online
+ * network on the poststates as a third slot of its launches.  The first switch-on allocates that slot's buffers
+ * (synchronises the device).  Captured step graphs are rebuilt.  ENOTIMPL once b200dqn_net_comm_init has run and, on
+ * the tensor-core engine, under B200DQN_CONV1=tma; b200dqn_net_comm_init returns ENOTIMPL while it is on. */
+int b200dqn_net_set_double_q(b200dqn_net* n, int on);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
 int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream);
 /* Number of kernels one fused train step launches (bench.py's gpu_launches). */

@@ -13,7 +13,8 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
 (PTR_SCREENS, PTR_ACTIONS, PTR_REWARDS, PTR_TERMINALS, PTR_PRESTATES, PTR_POSTSTATES, PTR_MB_ACTIONS,
  PTR_MB_REWARDS, PTR_MB_TERMINALS, PTR_INDEXES, PTR_WORDS_CONSUMED, PTR_MT_STATE) = range(12)
 (NET_PTR_Q_ONLINE, NET_PTR_Q_TARGET, NET_PTR_DELTAS, NET_PTR_GRADS, NET_PTR_WEIGHTS, NET_PTR_COST, NET_PTR_H1,
- NET_PTR_H2, NET_PTR_H3, NET_PTR_H4, NET_PTR_DZ4, NET_PTR_DZ3, NET_PTR_DZ2, NET_PTR_DZ1) = range(14)
+ NET_PTR_H2, NET_PTR_H3, NET_PTR_H4, NET_PTR_DZ4, NET_PTR_DZ3, NET_PTR_DZ2, NET_PTR_DZ1,
+ NET_PTR_Q_ONLINE_POST) = range(15)
 
 
 class B200DQNError(RuntimeError):
@@ -96,6 +97,7 @@ SIGNATURES = {
     "b200dqn_net_train_iterations": [_P, _i64p],
     "b200dqn_net_device_ptr": [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_size_t)],
     "b200dqn_net_set_keep_grads": [_P, C.c_int],
+    "b200dqn_net_set_double_q": [_P, C.c_int],
     "b200dqn_net_get_grads": [_P, C.c_int, _P, _P],
     "b200dqn_net_launches_per_step": [_P, C.POINTER(C.c_int)],
     "b200dqn_debug_trace": [_P, C.c_int],

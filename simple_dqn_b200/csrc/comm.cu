@@ -479,6 +479,9 @@ extern "C" int b200dqn_net_comm_init(b200dqn_net* n, const void* id128, int rank
   B2_REQUIRE(n->cfg.history_length == kHist, B200DQN_ENOTIMPL,
              "net_comm_init: data-parallel learners are implemented for history_length %d only (got %d)", kHist,
              n->cfg.history_length);
+  // the data-parallel schedules exchange and gather the two-slot forward's tensors only
+  B2_REQUIRE(!n->double_q, B200DQN_ENOTIMPL,
+             "net_comm_init: the Double DQN target is implemented for a single learner only (switch double Q off first)");
   int rc = nccl_load();
   if (rc) return rc;
   DeviceGuard g(n->device);

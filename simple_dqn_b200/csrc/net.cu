@@ -21,6 +21,9 @@ namespace b200 {
 // float32 array; we do the same arithmetic in fp64 and round once.  The per-sample cost
 // 0.5*sum_a delta^2 (BEFORE the clip) goes to row_cost; the batch mean is formed off the critical
 // chain by k_cost_finish.  grid = rows, block = 512 (one thread per hidden unit).
+// kSlots = 3 (Double DQN, van Hasselt et al. 2016; nets = 3): slot 2 is the online network on the poststates.  Its Q row
+// goes to q_online_post, and the target takes the target network's Q at the first index of that row's maximum (as
+// np.argmax / torch.argmax) instead of the maximum of the target row.  kSlots = 2 serves every other forward.
 // ------------------------------------------------------------------------------------------
 struct HeadTrainArgs {
   int enable;
@@ -45,12 +48,14 @@ struct HeadTrainArgs {
   HeadPush push;      // data-parallel gather schedule: this CTA's dZ4 row goes straight to every rank (world = 0: off)
 };
 
+template <int kSlots>
 __global__ void __launch_bounds__(kHidden)
 k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4_online, float* h4_target,
        const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
-       float* q_target, int A, const HeadTrainArgs td, const KTrace kt) {
-  __shared__ float red[2][kHidden / 32][kMaxActions];
-  __shared__ float s_q[2][kMaxActions];
+       float* q_target, float* q_online_post, int A, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  __shared__ float red[kSlots][kHidden / 32][kMaxActions];
+  __shared__ float s_q[kSlots][kMaxActions];
   __shared__ float s_d;
   __shared__ int s_a;
   __shared__ __align__(16) __half s_row[2][kHidden];   // hi / lo of this sample's dZ4 row (peer push)
@@ -78,20 +83,20 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
   }
   pdl_wait();
   pdl_launch_dependents();
-  float h[2] = {0.f, 0.f};
+  float h[kSlots] = {};
 #pragma unroll
-  for (int z = 0; z < 2; ++z) {
+  for (int z = 0; z < kSlots; ++z) {
     if (z < nets) {
       float acc = 0.f;
       for (int s = 0; s < splits; ++s) acc += part[((z * splits + s) * rows + b) * kHidden + t];
       h[z] = fmaxf(acc, 0.f);
-      (z ? h4_target : h4_online)[b * kHidden + t] = h[z];
+      if (z < 2) (z ? h4_target : h4_online)[b * kHidden + t] = h[z];   // slot 2's H4 has no reader
     }
   }
 #pragma unroll
-  for (int z = 0; z < 2; ++z) {
+  for (int z = 0; z < kSlots; ++z) {
     if (z < nets) {
-      const float* w5 = z ? w5_target : w5_online;
+      const float* w5 = z == 1 ? w5_target : w5_online;
       for (int a = 0; a < A; ++a) {
         float v = h[z] * w5[t * A + a];
 #pragma unroll
@@ -106,7 +111,7 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
     float v = 0.f;
 #pragma unroll
     for (int wI = 0; wI < kHidden / 32; ++wI) v += red[z][wI][a];
-    (z ? q_target : q_online)[b * A + a] = v;
+    (z == 0 ? q_online : (kSlots == 3 && z == 2) ? q_online_post : q_target)[b * A + a] = v;
     s_q[z][a] = v;
   }
   if (!td.enable) {
@@ -118,8 +123,16 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
     const int a = td_a;
     int64_t r = td_r;
     r = r < td.min_reward ? td.min_reward : (r > td.max_reward ? td.max_reward : r);     // np.clip (:136)
-    float maxq = s_q[1][0];
-    for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);                            // be.max(postq) (:124)
+    float maxq;
+    if constexpr (kSlots == 3) {   // Double DQN: a* = argmax_a Q_online(s', a), valued by the target network
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (s_q[2][j] > s_q[2][best]) best = j;
+      maxq = s_q[1][best];
+    } else {
+      maxq = s_q[1][0];
+      for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);                          // be.max(postq) (:124)
+    }
     const double y = td_term ? double(r) : double(r) + td.discount * double(maxq);          // :140-143
     const float target = static_cast<float>(y);
     float d = s_q[0][a] - target;                                                         // SumSquared grad (:149)
@@ -336,11 +349,12 @@ struct FrameSource {
   int64_t nframes[2];   // frames in each source array
 };
 
-// Model.fprop for `nets` networks (z = 0 online, z = 1 target) on `rows` samples.
+// Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
+// for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
                    const HeadTrainArgs& td) {
   const LayerTable& lt = n->lt;
-  const float* w[2] = {n->d_w, n->d_tw};
+  const float* w[3] = {n->d_w, n->d_tw, n->d_w};
   int rc;
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
     // one GPU: the forward launches are links of the critical chain (umma_forward picks the ones that release early)
@@ -349,8 +363,9 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
   } else {
     {
       Conv1Fwd p;
-      for (int z = 0; z < 2; ++z) {
-        p.src[z] = fs.src[z]; p.idx[z] = fs.idx[z]; p.shift[z] = fs.shift[z];
+      for (int z = 0; z < 3; ++z) {
+        const int f = z ? 1 : 0;   // slot 2 reads slot 1's frames
+        p.src[z] = fs.src[f]; p.idx[z] = fs.idx[f]; p.shift[z] = fs.shift[f];
         p.w[z] = w[z] + lt.off[0]; p.out[z] = n->d_h1[z];
       }
       p.nb = rows;
@@ -360,28 +375,28 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     {
       using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
       P p;
-      for (int z = 0; z < 2; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
       p.nb = rows;
       if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
     }
     {
       using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
       P p;
-      for (int z = 0; z < 2; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
       p.nb = rows;
       if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
     }
     {
       Fc1Fwd p;
-      for (int z = 0; z < 2; ++z) { p.in[z] = n->d_h3[z]; p.w[z] = w[z] + lt.off[3]; }
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h3[z]; p.w[z] = w[z] + lt.off[3]; }
       p.part = n->d_fc1part; p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
       if ((rc = launch_gemm<Fc1Fwd, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, kHidden, nets * kFc1Splits, st))) return rc;
     }
   }
   const int fc1_splits = n->cfg.math_mode == B200DQN_MATH_TCGEN05 ? umma_fc1_splits(rows) : kFc1Splits;
-  B2_CHECK_CUDA(launch_pdl(k_head, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_fc1part, fc1_splits, rows, nets,
-                           n->d_h4[0], n->d_h4[1], w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->A,
-                           td, ktrace_slot("head")));
+  B2_CHECK_CUDA(launch_pdl(nets == 3 ? k_head<3> : k_head<2>, dim3(rows), dim3(kHidden), 0, st,
+                           (const float*)n->d_fc1part, fc1_splits, rows, nets, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
+                           w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, td, ktrace_slot("head")));
   B2_PROF(td.enable ? "head(fc2+td+fc2_bwd)" : "fc2_fwd", st);
   return B200DQN_OK;
 }
@@ -828,7 +843,11 @@ static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* acti
                    reinterpret_cast<uint32_t*>(n->d_cost + kCostRing + 1), HeadPush{}};
   umma_dz4_planes(n, &td.dz4_hi, &td.dz4_lo_off);
   comm_head_push(n, st, &td.push);
-  B2_TRY(forward(n, fs, 2, rows, st, td));
+  // Double DQN adds the online network on the poststates as a third slot of the same launches.  With target_steps = 0
+  // the target network IS the online network, so slot 1 already holds that forward and a* = argmax of the same row:
+  // the vanilla step is the Double DQN step, bit for bit.
+  const int nets = (n->double_q && n->d_tw != n->d_w) ? 3 : 2;
+  B2_TRY(forward(n, fs, nets, rows, st, td));
   return backward_and_update(n, fs, rows, st, true);
 }
 
@@ -967,8 +986,8 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(fmalloc(&n->d_h2[z], size_t(nb) * kP2 * kP2 * kC2));
     B2_CHECK_CUDA(fmalloc(&n->d_h3[z], size_t(nb) * kFlat));
     B2_CHECK_CUDA(fmalloc(&n->d_h4[z], size_t(nb) * kHidden));
-    B2_CHECK_CUDA(fmalloc(&n->d_q[z], size_t(nb) * A));
   }
+  for (int z = 0; z < 3; ++z) B2_CHECK_CUDA(fmalloc(&n->d_q[z], size_t(nb) * A));
   B2_CHECK_CUDA(fmalloc(&n->d_fc1part, size_t(2) * kFc1Splits * nb * kHidden));
   B2_CHECK_CUDA(fmalloc(&n->d_delta, size_t(nb) * A));
   B2_CHECK_CUDA(fmalloc(&n->d_dz4, size_t(nb) * kHidden));
@@ -1027,9 +1046,10 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   if (n->d_tw != n->d_w) { cudaFree(n->d_tw); cudaFree(n->d_ts); }
   cudaFree(n->d_optscal);
   cudaFree(n->d_w); cudaFree(n->d_s); cudaFree(n->d_g); cudaFree(n->d_part); cudaFree(n->d_xepoch);
-  for (int z = 0; z < 2; ++z) {
-    cudaFree(n->d_h1[z]); cudaFree(n->d_h2[z]); cudaFree(n->d_h3[z]); cudaFree(n->d_h4[z]); cudaFree(n->d_q[z]);
+  for (int z = 0; z < 3; ++z) {
+    cudaFree(n->d_h1[z]); cudaFree(n->d_h2[z]); cudaFree(n->d_h3[z]); cudaFree(n->d_q[z]);
   }
+  for (int z = 0; z < 2; ++z) cudaFree(n->d_h4[z]);
   cudaFree(n->d_fc1part); cudaFree(n->d_delta); cudaFree(n->d_dz4); cudaFree(n->d_dz3); cudaFree(n->d_dz2);
   cudaFree(n->d_dz1); cudaFree(n->d_cost); cudaFree(n->d_step); cudaFree(n->d_rowcost); cudaFree(n->d_pre); cudaFree(n->d_post);
   cudaFree(n->d_act); cudaFree(n->d_term); cudaFree(n->d_rew); cudaFree(n->d_iota1); cudaFree(n->d_iota4);
@@ -1471,6 +1491,10 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_DZ3: p = n->d_dz3; b = size_t(n->nb) * kFlat * 4; break;
     case B200DQN_NET_PTR_DZ2: p = n->d_dz2; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_DZ1: p = n->d_dz1; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
+    case B200DQN_NET_PTR_Q_ONLINE_POST:   // target_steps = 0: the target forward is the online one (train_step)
+      p = n->d_tw == n->d_w ? n->d_q[1] : n->d_q[2];
+      b = size_t(n->nb) * n->A * 4;
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -1482,6 +1506,49 @@ extern "C" int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep) {
   B2_REQUIRE(n, B200DQN_EINVAL, "null net");
   n->keep_grads = keep != 0;
   destroy_step_graphs(n);   // parameters are baked in
+  if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
+  return B200DQN_OK;
+}
+
+// Buffers of the third network slot, made the first time Double DQN is switched on: the fc1 split-K partials grow to
+// three slots, the SIMT engine gets fp32 activations for slot 2 and the tensor-core engine fp16 planes.
+static int double_q_alloc(b200dqn_net* n) {
+  if (n->double_q_alloc) return B200DQN_OK;
+  DeviceGuard g(n->device);
+  B2_CHECK_CUDA(cudaDeviceSynchronize());   // no step or predict in flight still reads the old partial buffer
+  const size_t nb = size_t(n->nb);
+  float* part = nullptr;
+  B2_CHECK_CUDA(cudaMalloc(&part, size_t(3) * kFc1Splits * nb * kHidden * sizeof(float)));
+  B2_CHECK_CUDA(cudaMemset(part, 0, size_t(3) * kFc1Splits * nb * kHidden * sizeof(float)));
+  cudaFree(n->d_fc1part);
+  n->d_fc1part = part;
+  if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
+    int rc = umma_double_q_alloc(n);
+    if (rc) return rc;
+  } else {
+    const size_t elems[3] = {nb * kP1 * kP1 * kC1, nb * kP2 * kP2 * kC2, nb * kFlat};
+    float** dst[3] = {&n->d_h1[2], &n->d_h2[2], &n->d_h3[2]};
+    for (int i = 0; i < 3; ++i) {
+      B2_CHECK_CUDA(cudaMalloc(dst[i], elems[i] * sizeof(float)));
+      B2_CHECK_CUDA(cudaMemset(*dst[i], 0, elems[i] * sizeof(float)));
+    }
+  }
+  n->double_q_alloc = true;
+  return B200DQN_OK;
+}
+
+extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
+  B2_REQUIRE(n, B200DQN_EINVAL, "null net");
+  if (on) {
+    B2_REQUIRE(!n->nccl_comm, B200DQN_ENOTIMPL,
+               "net_set_double_q: the Double DQN target is implemented for a single learner only (comm_init has run)");
+    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
+               "net_set_double_q: the B200DQN_CONV1=tma conv1 has no Double DQN slot");
+    B2_TRY(double_q_alloc(n));
+  }
+  n->double_q = on != 0;
+  destroy_step_graphs(n);   // the number of network slots is baked in
   if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
   return B200DQN_OK;
 }

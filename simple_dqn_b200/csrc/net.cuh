@@ -48,10 +48,11 @@ struct b200dqn_net {
   float* d_part = nullptr;  // split-K partials
   int64_t part_elems = 0;
 
-  // activations: [0] online, [1] target
-  float* d_h1[2] = {}, *d_h2[2] = {}, *d_h3[2] = {}, *d_h4[2] = {};
-  float* d_fc1part = nullptr;  // [2*splits][nb][512]
-  float* d_q[2] = {};          // [nb][A]
+  // activations: [0] online, [1] target, [2] online on the poststates (Double DQN; SIMT engine only, allocated
+  // when double Q is first switched on)
+  float* d_h1[3] = {}, *d_h2[3] = {}, *d_h3[3] = {}, *d_h4[2] = {};
+  float* d_fc1part = nullptr;  // [2*splits][nb][512], [3*splits][nb][512] once double Q has been switched on
+  float* d_q[3] = {};          // [nb][A]: preq, postq, Q_online_post (Double DQN)
   float* d_delta = nullptr;    // [nb][A] clipped
   float* d_dz4 = nullptr, *d_dz3 = nullptr, *d_dz2 = nullptr, *d_dz1 = nullptr;
   float* d_cost = nullptr;     // cost ring [kCostRing]
@@ -84,6 +85,8 @@ struct b200dqn_net {
   cudaEvent_t ev[15] = {};
   bool use_graph = true, use_branches = true;
   bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
+  bool double_q = false;     // Double DQN target: the online net picks the poststate action, the target net values it
+  bool double_q_alloc = false;   // the third network slot's buffers exist
   cudaGraphExec_t graph_exec = nullptr;
   b200dqn_replay* graph_replay = nullptr;
   cudaStream_t graph_stream = nullptr;

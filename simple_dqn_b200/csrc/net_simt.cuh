@@ -93,18 +93,27 @@ __global__ void __launch_bounds__((BM / TM) * (BN / TN)) k_simt_gemm(const P p) 
     }
 }
 
+// Network slot z of a forward launch: 0 = online weights on the prestates, 1 = target weights on the poststates,
+// 2 = online weights on the poststates (Double DQN's action choice, launched only when it is on).  Per-slot kernel
+// parameters are picked with selects, never indexed by z, so they stay in the parameter bank instead of a local copy.
+template <class T>
+__device__ __forceinline__ T slot3(const T (&x)[3], int z) { return z == 2 ? x[2] : z ? x[1] : x[0]; }
+template <class T>   // weights of slot z where only two networks exist: the target's for slot 1, the online's otherwise
+__device__ __forceinline__ T wslot(const T (&x)[2], int z) { return z == 1 ? x[1] : x[0]; }
+
 // ------------------------------------------------------------------------------------------
-// Forward problems.  z selects the network: 0 = online (prestates), 1 = target (poststates).
+// Forward problems.  z selects the network slot: 0 = online (prestates), 1 = target (poststates), 2 = online on the
+// poststates (the Double DQN action choice; only launched when it is on).
 // ------------------------------------------------------------------------------------------
 
 // conv1: A = u8 frames read in place (ring or staged states), k = (c, r, s) with c the frame of the
 // history window; the /255 of _setInput (src/deepqnetwork.py:100) is applied to the fp32 accumulator, ReLU fused.
 struct Conv1Fwd {
-  const uint8_t* src[2];   // base of the frame array
-  const int32_t* idx[2];   // per-sample frame index
-  int shift[2];            // first frame of sample n is idx[n] + shift
-  const float* w[2];
-  float* out[2];
+  const uint8_t* src[3];   // base of the frame array
+  const int32_t* idx[3];   // per-sample frame index
+  int shift[3];            // first frame of sample n is idx[n] + shift
+  const float* w[3];
+  float* out[3];
   int nb;
   int k1;                  // 64 * history_length
   static constexpr bool kAKContig = true, kBKContig = false;
@@ -114,20 +123,22 @@ struct Conv1Fwd {
   __device__ float a(int z, int m, int k) const {
     const int n = m / (kP1 * kP1), pq = m % (kP1 * kP1), p = pq / kP1, q = pq % kP1;
     const int c = k >> 6, r = (k >> 3) & 7, s = k & 7;
-    const int64_t f = static_cast<int64_t>(idx[z][n]) + shift[z] + c;
-    return static_cast<float>(src[z][f * kFrameBytes + (p * 4 + r) * kFrameW + q * 4 + s]);
+    const int64_t f = static_cast<int64_t>(slot3(idx, z)[n]) + slot3(shift, z) + c;
+    return static_cast<float>(slot3(src, z)[f * kFrameBytes + (p * 4 + r) * kFrameW + q * 4 + s]);
   }
-  __device__ float b(int z, int k, int n) const { return w[z][k * kC1 + n]; }
-  __device__ void store(int z, int m, int n, float v) const { out[z][m * kC1 + n] = fmaxf(v * (1.0f / 255.0f), 0.f); }
+  __device__ float b(int z, int k, int n) const { return slot3(w, z)[k * kC1 + n]; }
+  __device__ void store(int z, int m, int n, float v) const {
+    slot3(out, z)[m * kC1 + n] = fmaxf(v * (1.0f / 255.0f), 0.f);
+  }
 };
 
 // conv2 / conv3: NHWC fp32 input, k = (r, s, c) so one filter row is (S*C) contiguous floats.
 template <int H, int C, int R, int ST, int KO>
 struct ConvFwd {
   static constexpr int P = (H - R) / ST + 1, K = R * R * C;
-  const float* in[2];
-  const float* w[2];
-  float* out[2];
+  const float* in[3];
+  const float* w[3];
+  float* out[3];
   int nb;
   static constexpr bool kAKContig = true, kBKContig = false;
   __device__ int M(int) const { return nb * P * P; }
@@ -136,18 +147,18 @@ struct ConvFwd {
   __device__ float a(int z, int m, int k) const {
     const int n = m / (P * P), pq = m % (P * P), p = pq / P, q = pq % P;
     const int r = k / (R * C), sc = k % (R * C);
-    return in[z][((n * H + p * ST + r) * H + q * ST) * C + sc];
+    return slot3(in, z)[((n * H + p * ST + r) * H + q * ST) * C + sc];
   }
-  __device__ float b(int z, int k, int n) const { return w[z][k * KO + n]; }
-  __device__ void store(int z, int m, int n, float v) const { out[z][m * KO + n] = fmaxf(v, 0.f); }
+  __device__ float b(int z, int k, int n) const { return slot3(w, z)[k * KO + n]; }
+  __device__ void store(int z, int m, int n, float v) const { slot3(out, z)[m * KO + n] = fmaxf(v, 0.f); }
 };
 
 // fc1 forward with split-K: z = net * splits + split; partial[z][m][n].  ReLU is applied by the
 // consumer (k_fc2_fwd) after it sums the splits.
 struct Fc1Fwd {
-  const float* in[2];   // H3 flat [nb][3136]
-  const float* w[2];    // W4 [3136][512]
-  float* part;          // [2*splits][nb][512]
+  const float* in[3];   // H3 flat [nb][3136]
+  const float* w[3];    // W4 [3136][512]
+  float* part;          // [nets*splits][nb][512]
   int nb, splits, kchunk;
   static constexpr bool kAKContig = true, kBKContig = false;
   __device__ int M(int) const { return nb; }
@@ -156,8 +167,8 @@ struct Fc1Fwd {
     kb = (z % splits) * kchunk;
     ke = min(kb + kchunk, kFlat);
   }
-  __device__ float a(int z, int m, int k) const { return in[z / splits][m * kFlat + k]; }
-  __device__ float b(int z, int k, int n) const { return w[z / splits][k * kHidden + n]; }
+  __device__ float a(int z, int m, int k) const { return slot3(in, z / splits)[m * kFlat + k]; }
+  __device__ float b(int z, int k, int n) const { return slot3(w, z / splits)[k * kHidden + n]; }
   __device__ void store(int z, int m, int n, float v) const { part[(z * nb + m) * kHidden + n] = v; }
 };
 

@@ -31,7 +31,7 @@ __device__ __forceinline__ void zero8(float v[8]) {
 // ==========================================================================================
 struct UmmaState {
   // activation planes per net: [hi plane | lo plane], NHWC fp16
-  __half* h16[3][2] = {};     // H1, H2, H3  x  (online, target)
+  __half* h16[3][3] = {};     // H1, H2, H3  x  network slot (online, target, online on the poststates: Double DQN only)
   int64_t h_elems[3] = {};
   __half* dz16[4] = {};       // dZ4, dZ3, dZ2, dZ1 (online)
   int64_t dz_elems[4] = {};
@@ -62,6 +62,8 @@ struct PlanePair {
   int64_t lo_off;   // lo plane = hi + lo_off
 };
 
+// Network slots of a train-step forward (blockIdx z of k_umma2, y of k_conv23_fwd; slot3 / wslot in net_simt.cuh): slot
+// 2 reads slot 1's frames, the online network's weight images and has its own fp16 planes.
 __device__ __forceinline__ void store_f32_and_planes(float* f32, const PlanePair& pl, int64_t i, const float v[8]) {
   if (f32) st8(f32 + i, v);
   umma2::split8_planes(v, pl.hi + i, pl.hi + pl.lo_off + i);
@@ -77,12 +79,12 @@ struct V2Conv1Fwd {
   static constexpr int kAMode = umma2::kReg, kBMode = umma2::kBulk;
   static constexpr bool kStagedEpilogue = true, kDumpA = true, kPrefetch = false;
   uint8_t* im2col;          // online net only: [mtile][H kb][128 x 128 B] A_hi tiles for conv1_wgrad (nullptr = off)
-  const uint8_t* src[2];
+  const uint8_t* src[2];    // frame sources of slots 0 and 1; slot 2 reads slot 1's
   const int32_t* idx[2];
   int shift[2];
   const uint8_t* wimg[2];   // [H kb][hi 32x128 | lo 32x128]
-  float* out[2];
-  PlanePair out16[2];
+  float* out[3];
+  PlanePair out16[3];
   int rows;
   __device__ int M(int) const { return rows * kP1 * kP1; }
   __device__ int N(int) const { return kC1; }
@@ -107,7 +109,7 @@ struct V2Conv1Fwd {
       v[4 + j] = float((raw.y >> (8 * j)) & 0xffu);
     }
   }
-  __device__ const uint8_t* b_tile(int z, int, int kb) const { return (z ? wimg[1] : wimg[0]) + kb * (kC1 * 256); }
+  __device__ const uint8_t* b_tile(int z, int, int kb) const { return wslot(wimg, z) + kb * (kC1 * 256); }
   __device__ uint8_t* a_dump(int z, int mtile, int kb) const {
     return (z == 0 && im2col) ? im2col + (int64_t(mtile) * H + kb) * (128 * 128) : nullptr;
   }
@@ -115,7 +117,7 @@ struct V2Conv1Fwd {
     float o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = fmaxf(v[j] * (1.0f / 255.0f), 0.f);
-    store_f32_and_planes(z ? out[1] : out[0], z ? out16[1] : out16[0], int64_t(m) * kC1 + n0, o);
+    store_f32_and_planes(slot3(out, z), slot3(out16, z), int64_t(m) * kC1 + n0, o);
   }
 };
 
@@ -127,15 +129,15 @@ struct V2ConvFwd {
   static constexpr bool kAExact = false, kARowMajorThreads = true, kBRowMajorThreads = false;
   static constexpr int kAMode = umma2::kAsync, kBMode = umma2::kBulk;
   static constexpr bool kStagedEpilogue = true, kDumpA = false, kPrefetch = false;
-  PlanePair in16[2];
+  PlanePair in16[3];
   const uint8_t* wimg[2];   // [K/64][hi KOx128 | lo KOx128]
-  float* out[2];
-  PlanePair out16[2];
+  float* out[3];
+  PlanePair out16[3];
   int rows;
   __device__ int M(int) const { return rows * P * P; }
   __device__ int N(int) const { return KO; }
   __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = K / 64; }
-  __device__ umma2::Planes a_planes(int z) const { return {z ? in16[1].hi : in16[0].hi, in16[0].lo_off}; }
+  __device__ umma2::Planes a_planes(int z) const { return {slot3(in16, z).hi, in16[0].lo_off}; }
   __device__ umma2::RowCtx a_row(int, int m) const {
     const int n = m / (P * P), pq = m % (P * P), p = pq / P, q = pq % P;
     return {(int64_t(n * H + p * ST) * H + q * ST) * C, 0, 0, m < rows * P * P};
@@ -145,16 +147,16 @@ struct V2ConvFwd {
     off = rc.base + r * (H * C) + sc;
     return true;
   }
-  __device__ const uint8_t* b_tile(int z, int, int kb) const { return (z ? wimg[1] : wimg[0]) + kb * (KO * 256); }
+  __device__ const uint8_t* b_tile(int z, int, int kb) const { return wslot(wimg, z) + kb * (KO * 256); }
   __device__ void store8(int z, int m, int n0, const float v[8]) const {
     float o[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j] = fmaxf(v[j], 0.f);
-    store_f32_and_planes(z ? out[1] : out[0], z ? out16[1] : out16[0], int64_t(m) * KO + n0, o);
+    store_f32_and_planes(slot3(out, z), slot3(out16, z), int64_t(m) * KO + n0, o);
   }
 };
 
-// ---- conv2 + conv3 forward, one CTA per (sample, network) ------------------------------------------
+// ---- conv2 + conv3 forward, one CTA per (sample, network slot) --------------------------------------
 // conv3's receptive field never leaves a sample, so one CTA runs conv2 on its sample (81 live rows of a 128-row tile,
 // the k_umma2 pipeline), keeps H2 in shared memory as fp16 hi/lo rows and runs conv3 on it (49 live rows of one
 // 64-row wgmma tile, one k-block per filter tap): no CTA waits on another, and the conv2 -> conv3 link of the chain
@@ -211,8 +213,8 @@ __global__ void __launch_bounds__(umma2::kThreads2, 1) k_conv23_fwd(const Conv23
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
   uint8_t* h2 = smem_gen + kH2;
-  const uint8_t* wimg2 = z ? p.c2.wimg[1] : p.c2.wimg[0];
-  const uint8_t* wimg3 = z ? p.c3.wimg[1] : p.c3.wimg[0];
+  const uint8_t* wimg2 = wslot(p.c2.wimg, z);
+  const uint8_t* wimg3 = wslot(p.c3.wimg, z);
 
   if (tid == 0) {
 #pragma unroll
@@ -449,9 +451,9 @@ struct V2Fc1Fwd {
   // image of its own and nothing has to be re-packed after the optimizer.
   static constexpr bool kAMnMajor = true;
   static constexpr uint32_t kAMnLoOffset = 128 * 128;   // lo half of a [hi 128x128 B | lo 128x128 B] tile
-  PlanePair in16[2];        // H3 planes [rows][3136]
+  PlanePair in16[3];        // H3 planes [rows][3136]
   const uint8_t* wimg[2];   // [25 flat tiles][8 hidden blocks][hi 128x128 | lo 128x128]
-  float* part;              // [2*splits][rows][512]
+  float* part;              // [nets*splits][rows][512]
   int rows, splits;
   __device__ int M(int) const { return kHidden; }
   __device__ int N(int) const { return rows; }
@@ -462,10 +464,10 @@ struct V2Fc1Fwd {
   }
   // hi sub-tile [64 flat rows x 64 hidden] of hidden block 2*mtile + chunk, flat k-block kb
   __device__ const uint8_t* a_sub(int z, int mtile, int kb, int chunk) const {
-    return ((z / splits) ? wimg[1] : wimg[0]) + (int64_t(kb >> 1) * (kHidden / 64) + 2 * mtile + chunk) * (128 * 256) +
+    return wslot(wimg, z / splits) + (int64_t(kb >> 1) * (kHidden / 64) + 2 * mtile + chunk) * (128 * 256) +
            (kb & 1) * (64 * 128);
   }
-  __device__ umma2::Planes b_planes(int z) const { return {(z / splits) ? in16[1].hi : in16[0].hi, in16[0].lo_off}; }
+  __device__ umma2::Planes b_planes(int z) const { return {slot3(in16, z / splits).hi, in16[0].lo_off}; }
   __device__ umma2::RowCtx b_row(int, int n) const { return {int64_t(n) * kFlat, 0, 0, n < rows}; }
   __device__ bool b_chunk(int, const umma2::RowCtx& rc, int kk, int64_t& off) const {
     off = rc.base + kk;
@@ -1071,11 +1073,23 @@ int umma_net_init(b200dqn_net* n) {
   return B200DQN_OK;
 }
 
+// fp16 planes of network slot 2 (Double DQN), allocated the first time it is switched on
+int umma_double_q_alloc(b200dqn_net* n) {
+  UmmaState* u = ust(n);
+  if (!u) return B200DQN_OK;
+  for (int i = 0; i < 3; ++i) {
+    if (u->h16[i][2]) continue;
+    B2_CHECK_CUDA(cudaMalloc(&u->h16[i][2], 2 * u->h_elems[i] * sizeof(__half)));
+    B2_CHECK_CUDA(cudaMemset(u->h16[i][2], 0, 2 * u->h_elems[i] * sizeof(__half)));
+  }
+  return B200DQN_OK;
+}
+
 void umma_net_destroy(b200dqn_net* n) {
   UmmaState* u = ust(n);
   if (!u) return;
   for (int i = 0; i < 3; ++i) {
-    for (int z = 0; z < 2; ++z) cudaFree(u->h16[i][z]);
+    for (int z = 0; z < 3; ++z) cudaFree(u->h16[i][z]);
     if (i > 0) cudaFree(u->img_dgr[i]);   // [0] aliases img_fwd[0][3]
   }
   for (int i = 0; i < 4; ++i) cudaFree(u->dz16[i]);
@@ -1150,20 +1164,22 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       V2Conv1Fwd<H> p;
       for (int z = 0; z < 2; ++z) {
         p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
-        p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z]; p.out16[z] = planes(0, z);
+        p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z];
       }
+      for (int z = 0; z < 3; ++z) p.out16[z] = planes(0, z);
+      p.out[2] = nullptr;                                                  // slot 2 keeps no fp32 activations
       p.rows = rows;
-      p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
+      p.im2col = (nets >= 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
       return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early);
     });
     if (rc) return rc;
   }
   if (rows <= kConv23MaxRows) {
     Conv23Fwd p{};
-    for (int z = 0; z < 2; ++z) {
-      p.c2.in16[z] = planes(0, z); p.c2.wimg[z] = u->img_fwd[z][1];
-      p.c3.wimg[z] = u->img_fwd[z][2]; p.c3.out16[z] = planes(2, z);
-      p.c3.out[z] = z ? nullptr : n->d_h3[z];   // nothing reads the target network's fp32 activations
+    for (int z = 0; z < 2; ++z) { p.c2.wimg[z] = u->img_fwd[z][1]; p.c3.wimg[z] = u->img_fwd[z][2]; }
+    for (int z = 0; z < 3; ++z) {
+      p.c2.in16[z] = planes(0, z); p.c3.out16[z] = planes(2, z);
+      p.c3.out[z] = z ? nullptr : n->d_h3[z];   // nothing reads the fp32 activations of slots 1 and 2
     }
     p.c2.out[0] = n->d_h2[0]; p.c2.out16[0] = planes(1, 0);   // the kernel stores H2 of the online net only
     p.c2.rows = p.c3.rows = rows;
@@ -1172,9 +1188,10 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     {
       using P = V2ConvFwd<kP1, kC1, 4, 2, kC2>;
       P p;
-      for (int z = 0; z < 2; ++z) {
-        p.in16[z] = planes(0, z); p.wimg[z] = u->img_fwd[z][1]; p.out16[z] = planes(1, z);
-        p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the target network's fp32 activations
+      for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][1];
+      for (int z = 0; z < 3; ++z) {
+        p.in16[z] = planes(0, z); p.out16[z] = planes(1, z);
+        p.out[z] = z ? nullptr : n->d_h2[z];     // nothing reads the fp32 activations of slots 1 and 2
       }
       p.rows = rows;
       if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st, false))) return rc;
@@ -1182,8 +1199,9 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     {
       using P = V2ConvFwd<kP2, kC2, 3, 1, kC3>;
       P p;
-      for (int z = 0; z < 2; ++z) {
-        p.in16[z] = planes(1, z); p.wimg[z] = u->img_fwd[z][2]; p.out16[z] = planes(2, z);
+      for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][2];
+      for (int z = 0; z < 3; ++z) {
+        p.in16[z] = planes(1, z); p.out16[z] = planes(2, z);
         p.out[z] = z ? nullptr : n->d_h3[z];
       }
       p.rows = rows;
@@ -1191,10 +1209,11 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     }
   }
   // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
-  if (nets == 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
+  if (nets >= 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
   {
     V2Fc1Fwd p;
-    for (int z = 0; z < 2; ++z) { p.in16[z] = planes(2, z); p.wimg[z] = u->img_fwd[z][3]; }
+    for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][3];
+    for (int z = 0; z < 3; ++z) p.in16[z] = planes(2, z);
     p.part = n->d_fc1part; p.rows = rows; p.splits = fc1_splits_for(rows);
     if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st, false))) return rc;
   }

@@ -16,6 +16,7 @@ OptArgs make_opt_args(const b200dqn_net* n, int rows);   // net.cu: optimizer co
 // tensor-core engine (net_umma.cu)
 int umma_net_init(b200dqn_net* n);                      // allocate operand images etc. (no-op in SIMT mode)
 void umma_net_destroy(b200dqn_net* n);
+int umma_double_q_alloc(b200dqn_net* n);                // fp16 planes of network slot 2 (Double DQN), once
 int umma_weights_changed(b200dqn_net* n, cudaStream_t st);  // fp32 master weights were overwritten by the host
 int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
 // nframes[z]: frames in the array src[z] points to (the tensor-map TMA gather of conv1 needs the extent)

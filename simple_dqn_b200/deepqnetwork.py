@@ -78,6 +78,10 @@ class DeepQNetwork:
                 w = rng.uniform(-scale, scale, shp).astype(np.float32)
                 self._set_layer(which, layer, w, np.zeros_like(w))
         self.train_iterations = 0
+        # Double DQN target (van Hasselt et al., 2016): a new capability, off unless args.double_dqn is set
+        self.double_dqn = False
+        if _arg(args, "double_dqn", False):
+            self.set_double_dqn(True)
         self.save_weights_prefix = _arg(args, "save_weights_prefix", None)
         self.callback = None
 
@@ -148,6 +152,13 @@ class DeepQNetwork:
         """Make the tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 next to their fp16 planes (tests / debugging)."""
         L.call("b200dqn_net_set_keep_grads", self._h, int(bool(keep)))
 
+    def set_double_dqn(self, on=True):
+        """Switch the Double DQN target on or off: the online network picks the poststate action (first index of the
+        maximum), the target network values it.  Raises NotImplementedError for data-parallel learners and for the
+        B200DQN_CONV1=tma conv1."""
+        L.call("b200dqn_net_set_double_q", self._h, int(bool(on)))
+        self.double_dqn = bool(on)
+
     def get_grads(self):
         out = []
         for layer, shp in enumerate(self.layer_shapes()):
@@ -187,6 +198,10 @@ class DeepQNetwork:
         dz3 = self._read_f32(L.NET_PTR_DZ3, (b, 7, 7, 64)).transpose(0, 3, 1, 2)
         dz4 = self._read_f32(L.NET_PTR_DZ4, (b, 512))
         return dz1, dz2, dz3, dz4
+
+    def last_online_postq(self):
+        """The online network's Q on the poststates of the last Double DQN train() as a (batch, A) array."""
+        return self._read_f32(L.NET_PTR_Q_ONLINE_POST, (self.batch_size, self.num_actions))
 
     def last_deltas(self):
         return self._read_f32(L.NET_PTR_DELTAS, (self.batch_size, self.num_actions))

@@ -11,11 +11,13 @@ replay = 50000
 base, actions, rewards, terminals = synthetic_meta(replay)
 B = int(os.environ.get("BATCH", "32"))
 HIST = int(os.environ.get("HIST", "4"))   # --history_length: frames per state, conv1's input channels
+DOUBLE = os.environ.get("DOUBLE", "0") == "1"   # the Double DQN target (a third forward slot)
 
 
 def args():
     a = make_args(B)
     a.history_length = HIST
+    a.double_dqn = DOUBLE
     return a
 
 
@@ -41,5 +43,5 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("batch %d hist %d period_us min %.2f median %.2f  all %s" % (B, HIST, min(res), float(np.median(res)),
-                                                                  " ".join("%.2f" % r for r in res)))
+print("batch %d hist %d double %d period_us min %.2f median %.2f  all %s" % (B, HIST, DOUBLE, min(res), float(np.median(res)),
+                                                                            " ".join("%.2f" % r for r in res)))
