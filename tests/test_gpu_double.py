@@ -4,6 +4,15 @@ Bars as in test_gpu_net.py: Q rows <= 1e-3 * max, cost rel 1e-3, gradients rel-L
 The device and the oracle compute Q to about 1e-3, so where two online Q values on a poststate are closer than that
 they may pick different actions; the oracle then takes the device's choice (and the test checks that the two values
 really are inside that band).  Bit-exact checks restate the head from the device's own Q rows.
+
+An error in the third network slot alone (the online network on the poststates) would hide inside that 1e-3 band: its
+only output is Q_online_post, which reaches the loss through an argmax.  So the slot is pinned bit for bit instead.
+Every slot of a forward launch runs the same per-CTA code with no atomics, and the head sums the split-K partials in
+slot-independent order, so slot 2 of a Double DQN step must equal slot 1 of a vanilla twin whose target network IS
+the online network, at every batch-size dispatch, history length, engine and fc1 split count.  Where the Double DQN
+target cannot differ from the vanilla one (all-terminal minibatches, one action), the whole step must be the vanilla
+step bit for bit, which pins that the third slot clobbers no buffer the backward pass or the optimizer reads.
+(The float64 bound on every kernel of a Double DQN step is in tests/test_gpu_kernels.py.)
 """
 import os
 import random
@@ -19,6 +28,7 @@ from helpers import make_args, rel_l2
 from oracle import dqn_oracle as O
 from oracle.mt19937 import MT19937
 from oracle.replay_oracle import ReplayOracle, synthetic_ring
+from test_gpu_kernels import SCHEDS, SWEEP
 
 pytestmark = pytest.mark.gpu
 
@@ -205,7 +215,7 @@ def _state(net):
 
 def _assert_same(a, b):
     for x, y in zip(a, b):
-        if isinstance(x, list):
+        if isinstance(x, (list, tuple)):
             _assert_same(x, y)
         else:
             assert (x == y).all()
@@ -256,18 +266,25 @@ def test_double_equals_vanilla_at_target_steps_zero(mode):
     assert (nb.last_online_postq() == nb.last_q()[1]).all()   # one network: Q_online_post is the postq row
 
 
-@pytest.mark.parametrize("mode", ["tcgen05", "fp32"])
-def test_double_fused_ring_equals_host_minibatch(mode):
+FUSED_CASES = ([("tcgen05", 32, 4), ("fp32", 32, 4), ("tcgen05", 65, 4), ("tcgen05", 257, 4)] +
+               [("tcgen05", 32, h) for h in (1, 5, 16)] + [("fp32", 65, 4)])
+
+
+@pytest.mark.parametrize("mode,batch,hist", FUSED_CASES,
+                         ids=[m if (b, h) == (32, 4) else "%s-b%d-h%d" % (m, b, h) for m, b, h in FUSED_CASES])
+def test_double_fused_ring_equals_host_minibatch(mode, batch, hist):
+    """Batches 65 and 257 cross the two-kernel conv forward and the 4-split fc1 with three slots; H = 16 refills
+    conv1's frame ring across three slots of CTAs."""
     from simple_dqn_b200 import ReplayMemory, Stream
-    ring = ReplayOracle(4000, batch_size=32)
+    ring = ReplayOracle(4000, history_length=hist, batch_size=batch)
     synthetic_ring(ring, seed=4, block=200, terminal_p=0.02)
     nets = []
     for fused in (True, False):
         stream = Stream() if fused else None
-        mem = ReplayMemory(4000, make_args(), rng="device", stream=stream)
+        mem = ReplayMemory(4000, make_args(batch_size=batch, history_length=hist), rng="device", stream=stream)
         mem.add_batch(ring.actions, ring.rewards, ring.screens, ring.terminals)
         mem.set_cursor(ring.count, ring.current)
-        net, _ = _paired(4, mode, stream=stream)
+        net, _ = _paired(4, mode, batch=batch, hist=hist, stream=stream)
         random.seed(77)
         mem.seed_device_rng(random)
         if fused:
@@ -339,3 +356,165 @@ def test_double_refused_under_conv1_tma():
     out = subprocess.run([sys.executable, "-s", "-c", code], env=env, capture_output=True, text=True, timeout=600)
     assert out.returncode == 0, out.stderr
     assert "REFUSED" in out.stdout and "B200DQN_CONV1=tma" in out.stdout, out.stdout
+
+
+def _twins(num_actions, mode, batch, hist, sched, **kw):
+    """N (Double DQN, online W, target T != W), V1 (vanilla, W and T) and V2 (vanilla, W and W): all weights set
+    from the host, so every tile image comes from the pack kernels."""
+    n, _ = _paired(num_actions, mode, batch=batch, hist=hist, stream=_stream(sched), **kw)
+    v1, _ = _paired(num_actions, mode, batch=batch, hist=hist, stream=_stream(sched), double=False, **kw)
+    v2, _ = _paired(num_actions, mode, batch=batch, hist=hist, stream=_stream(sched), double=False, **kw)
+    v2.set_weights(v2.get_weights(with_states=False), None, which=1)
+    return n, v1, v2
+
+
+def _assert_slot_identity(mode, batch, hist=4, num_actions=4, sched="branches"):
+    """Slots 0 and 1 of N are V1's; slot 2 of N (Q_online_post) is V2's slot 1, on the same poststates.  Three steps:
+    before steps 2 and 3 V2 is reloaded with N's updated fp32 weights (both of its networks), so N's
+    optimizer-refreshed online tile images must equal a fresh pack of the same weights, in slot 0 and in slot 2."""
+    n, v1, v2 = _twins(num_actions, mode, batch, hist, sched)
+    for step in range(3):
+        mb = _mb(batch, num_actions, 40 + step, hist=hist)
+        assert (mb[0] != mb[3]).any()
+        if step > 0:
+            ws = n.get_weights(with_states=False)
+            v2.set_weights(ws, None)
+            v2.set_weights(ws, None, which=1)
+        n._w5_before = n.get_weights(with_states=False)[4].copy()
+        for net in (n, v1, v2) if step == 0 else (n, v2):
+            net.train(mb, 0)
+        preq, postq = n.last_q()
+        oq = n.last_online_postq()
+        vpre, vpost = v2.last_q()
+        assert (oq == vpost).all(), (step, np.abs(oq - vpost).max())
+        assert (preq == vpre).all(), (step, np.abs(preq - vpre).max())
+        _check_head_bits(n, mb)
+        if step == 0:
+            v1pre, v1post = v1.last_q()
+            assert (preq == v1pre).all() and (postq == v1post).all()
+            for h, hv in zip(n.last_activations(), v1.last_activations()):
+                assert (h == hv).all()
+            if batch >= 32 and num_actions > 1:     # online and target disagree: the slot decides some targets
+                assert (_first_max(oq) != _first_max(postq))[~mb[4]].any()
+
+
+SLOT_CASES = ([("tcgen05", s, b, 4, 4) for s in SCHEDS for b in SWEEP] +
+              [("tcgen05", "branches", b, h, 4) for h in (1, 5, 16) for b in (1, 64, 65)] +
+              [("tcgen05", "branches", 33, 4, a) for a in (1, 18)] +
+              [("fp32", "serial", b, 4, 4) for b in (1, 32, 65)])
+
+
+@pytest.mark.parametrize("mode,sched,batch,hist,num_actions", SLOT_CASES)
+def test_double_third_slot_is_the_online_forward(mode, sched, batch, hist, num_actions):
+    _assert_slot_identity(mode, batch, hist, num_actions, sched)
+
+
+@pytest.mark.parametrize("splits", [1, 4, 14])
+def test_double_third_slot_under_forced_fc1_splits(splits):
+    """B200DQN_FC1_SPLITS is read once per process, so the check runs in a child process."""
+    code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
+            "import test_gpu_double as T\n"
+            "for batch in (33, 257):\n"
+            "    T._assert_slot_identity('tcgen05', batch)\n"
+            "print('SLOTS OK')\n" % (ROOT, os.path.join(ROOT, "tests")))
+    env = dict(os.environ, B200DQN_FC1_SPLITS=str(splits))
+    out = subprocess.run([sys.executable, "-s", "-c", code], env=env, capture_output=True, text=True, timeout=900)
+    assert out.returncode == 0, out.stderr[-4000:]
+    assert "SLOTS OK" in out.stdout
+
+
+VANILLA_CASES = ([(m, s, b, "all_terminal") for m in ("tcgen05", "fp32") for s in SCHEDS for b in SWEEP] +
+                 [("tcgen05", "branches", 33, "adam"), ("fp32", "branches", 33, "adam")] +
+                 [("tcgen05", "branches", b, "one_action") for b in (1, 33, 65, 257)] +
+                 [("fp32", "serial", b, "one_action") for b in (1, 33)])
+
+
+@pytest.mark.parametrize("mode,sched,batch,case", VANILLA_CASES)
+def test_double_step_is_vanilla_where_the_target_cannot_differ(mode, sched, batch, case):
+    """All-terminal minibatches (the target ignores Q) and A = 1 (a* = 0 is the maximum), with T != W: two Double DQN
+    steps equal two vanilla steps bit for bit (costs, deltas, gradients, online and target weights, every optimizer
+    state plane), although the Double DQN step runs the third slot in every forward launch."""
+    num_actions, terminal_p = (1, 0.0) if case == "one_action" else (4, 1.0)
+    optimizer = "adam" if case == "adam" else "rmsprop"
+    runs = []
+    for double in (False, True):
+        net, _ = _paired(num_actions, mode, batch=batch, stream=_stream(sched), optimizer=optimizer, double=double)
+        steps = []
+        for i in range(2):
+            net.train(_mb(batch, num_actions, 50 + i, terminal_p=terminal_p), 0)
+            steps.append((net.last_deltas(), net.get_grads()))
+        runs.append((net.last_costs(2), steps, _state(net)))
+        if double:      # the third slot really ran, with the online weights
+            assert (net.last_online_postq() != net.last_q()[1]).any()
+    (ca, sa, wa), (cb, sb, wb) = runs
+    assert (ca == cb).all(), (ca, cb)
+    _assert_same(sa, sb)
+    _assert_same(wa, wb)
+
+
+def _live_net(ring, mode, double_at_creation):
+    from simple_dqn_b200 import ReplayMemory, StateBuffer, Stream
+    stream = Stream()
+    mem = ReplayMemory(ring.size, make_args(), rng="device", stream=stream)
+    mem.add_batch(ring.actions, ring.rewards, ring.screens, ring.terminals)
+    mem.set_cursor(ring.count, ring.current)
+    net, _ = _paired(6, mode, stream=stream, double=double_at_creation)
+    if double_at_creation:
+        net.set_double_dqn(False)       # the third slot's buffers exist; the steps below start vanilla
+    random.seed(21)
+    mem.seed_device_rng(random)
+    return net, mem, StateBuffer(make_args(), stream=stream)
+
+
+@pytest.mark.parametrize("mode", ["tcgen05", "fp32"])
+def test_double_switched_on_live_equals_switched_on_at_creation(mode):
+    """A is created vanilla, runs fused-step graphs and the state-window predict graph, then switches Double DQN on,
+    which reallocates the fc1 partials those graphs hold; B allocated the third slot at creation.  Every cost, weight,
+    optimizer state and fast-path Q row must agree, also across A switching off and on again, toggling keep_grads and
+    a target sync in the middle of the run; the fast-path Q equals host predict on the same window."""
+    ring = ReplayOracle(3000, batch_size=32)
+    synthetic_ring(ring, seed=12, block=150, terminal_p=0.02)
+    frames = np.random.RandomState(0).randint(0, 256, (8, 84, 84)).astype(np.uint8)
+    nets = [_live_net(ring, mode, at_creation) for at_creation in (False, True)]
+    n_frames = [0]
+
+    def predict_both():
+        qs = []
+        for net, _, buf in nets:
+            for i in range(n_frames[0], n_frames[0] + 2):
+                buf.add(frames[i])
+            states = buf.getStateMinibatch()
+            q = net.predict(states)             # the captured predict graph
+            host = net.predict(np.asarray(states))
+            assert (q[0] == host[0]).all() and not q[1:].any()
+            qs.append(q)
+        n_frames[0] += 2
+        assert (qs[0] == qs[1]).all()
+
+    def train_both(k, total):
+        for net, mem, _ in nets:
+            net.train_fused(mem, k)
+        (a, _, _), (b, _, _) = nets
+        assert (a.last_costs(total) == b.last_costs(total)).all()
+        _assert_same(_state(a), _state(b))
+
+    (a, _, _), (b, _, _) = nets
+    train_both(2, 2)
+    predict_both()
+    for net in (a, b):
+        net.set_double_dqn(True)
+    train_both(2, 4)
+    predict_both()
+    assert (a.last_online_postq() == b.last_online_postq()).all()
+    a.set_double_dqn(False)
+    a.set_double_dqn(True)
+    train_both(1, 5)
+    a.keep_grads(False)
+    train_both(1, 6)
+    a.keep_grads(True)
+    for net in (a, b):
+        net.update_target_network()
+    train_both(2, 8)
+    predict_both()
+    assert (a.last_online_postq() == b.last_online_postq()).all()
+    assert (a.last_online_postq() != a.last_q()[1]).any()      # still a Double DQN step: T != W after the sync

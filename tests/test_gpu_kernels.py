@@ -7,6 +7,9 @@ skipped k-block or a wrong tile tail exceeds it, and tests/test_kernel_ref.py sh
 
 The head is restated bit for bit: the deltas from the device's preq/postq, dZ4 = δ·W5 under the H4 mask.
 
+The test_double_* cases run the same checks on Double DQN steps, where every forward launch carries a third network
+slot (the online net on the poststates) and the deltas and cost follow the Double DQN target (head_restated).
+
 Batch sweep of the tensor-core engine (A = 4, H = 4) and what each size runs (kernel_ref.dispatch):
 
     batch                 1    2    3   16   33   63   64   65  128  129  256  257  512  4096 (forward only)
@@ -25,6 +28,7 @@ import numpy as np
 import pytest
 
 import kernel_ref as K
+from double_oracle import head_restated
 from helpers import make_args, rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -33,20 +37,22 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SWEEP = [1, 2, 3, 16, 33, 63, 64, 65, 128, 129, 256, 257, 512]
 SCHEDS = ["serial", "branches"]
 F32 = np.float32
-WORST = {}          # kernel -> largest ratio of error to bound seen in this module
+WORST = {}          # kernel -> largest ratio of error to bound seen in this module (vanilla steps and predicts)
+WORST_DOUBLE = {}   # the same for the Double DQN steps
 
 
-def _note(ratios):
+def _note(ratios, double=False):
+    worst = WORST_DOUBLE if double else WORST
     for k, v in ratios.items():
-        WORST[k] = max(WORST.get(k, 0.0), v)
+        worst[k] = max(worst.get(k, 0.0), v)
 
 
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     yield
-    print("\nlargest |error| / bound per kernel:")
-    for k in sorted(WORST):
-        print("  %-12s %.3g" % (k, WORST[k]))
+    print("\nlargest |error| / bound per kernel:  vanilla   double")
+    for k in sorted(set(WORST) | set(WORST_DOUBLE)):
+        print("  %-20s %11s %8s" % (k, *("%.3g" % w[k] if k in w else "-" for w in (WORST, WORST_DOUBLE))))
 
 
 def minibatch(n, hist, num_actions, seed, terminal_p=0.3, rewards=(-3, 4), states=None):
@@ -58,11 +64,13 @@ def minibatch(n, hist, num_actions, seed, terminal_p=0.3, rewards=(-3, 4), state
 
 
 def make_net(batch, engine="tcgen05", hist=4, num_actions=4, sched="branches", seed=3, w5_scale=3.0, keep=True,
-             **kw):
+             double=False, **kw):
     """A net with Xavier weights, fc1 × 3 and fc2 × w5_scale (Q of order 1, like a trained net), small RMSProp
-    state and a freshly synced target."""
+    state and a freshly synced target.  double: the Double DQN target, with target weights perturbed away from the
+    online ones (by 0.3·max|W| of noise per layer), so that the two networks prefer different poststate actions."""
     from simple_dqn_b200 import DeepQNetwork, Stream
-    net = DeepQNetwork(num_actions, make_args(batch_size=batch, history_length=hist, random_seed=seed, **kw),
+    net = DeepQNetwork(num_actions, make_args(batch_size=batch, history_length=hist, random_seed=seed,
+                                              double_dqn=double, **kw),
                        math_mode=engine, stream=Stream() if sched == "branches" else None)
     ws, _ = net.get_weights()
     ws[3] = ws[3] * F32(3.0)
@@ -70,6 +78,9 @@ def make_net(batch, engine="tcgen05", hist=4, num_actions=4, sched="branches", s
     rs = np.random.RandomState(seed)
     net.set_weights(ws, [np.abs(rs.randn(*w.shape)).astype(F32) * F32(1e-4) for w in ws])
     net.update_target_network()
+    if double:
+        net.set_weights([(w + rs.randn(*w.shape).astype(F32) * F32(0.3) * np.abs(w).max()).astype(F32) for w in ws],
+                        None, which=1)
     net.keep_grads(keep)
     return net
 
@@ -139,8 +150,13 @@ def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward
     pre = mb[0]
     preq, postq = net.last_q()
     acts = net.last_activations()
-    raw, clipped = K.head_td(preq, postq, mb[1], mb[2], mb[4], clip=clip, min_reward=min_reward,
-                             max_reward=max_reward)
+    if net.double_dqn:      # the target values the action the online network picks on the poststates
+        oq = net.last_online_postq()
+        raw, clipped = (head_restated(preq, postq, oq, mb[1], mb[2], mb[4], min_reward=min_reward,
+                                      max_reward=max_reward, clip=c)[0] for c in (0, clip))
+    else:
+        raw, clipped = K.head_td(preq, postq, mb[1], mb[2], mb[4], clip=clip, min_reward=min_reward,
+                                 max_reward=max_reward)
     deltas = net.last_deltas()
     assert (deltas == clipped).all(), np.abs(deltas - clipped).max()
     cost = float(net.last_costs(1)[0])
@@ -154,7 +170,7 @@ def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward
     q = net.predict(fresh)
     r.update({k + "@updated": v for k, v in
               forward_ratios(engine, fresh, ws1, net.last_activations(), q, fc1_forced).items()})
-    _note(r)
+    _note(r, net.double_dqn)
     bad = {k: v for k, v in r.items() if not v <= 1.0}
     assert not bad, bad
     return r, step
@@ -165,6 +181,17 @@ def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward
 def test_train_step_kernels(batch, sched):
     net = make_net(batch, sched=sched)
     train_and_check(net, minibatch(batch, 4, 4, 2))
+
+
+@pytest.mark.parametrize("sched", SCHEDS)
+@pytest.mark.parametrize("batch", SWEEP)
+def test_double_train_step_kernels(batch, sched):
+    """Double DQN: every forward launch runs a third network slot (the online net on the poststates)."""
+    net = make_net(batch, sched=sched, double=True)
+    mb = minibatch(batch, 4, 4, 2)
+    train_and_check(net, mb)
+    if batch >= 33:         # the two networks disagree on some poststates: the Double DQN target is really in play
+        assert (net.last_online_postq().argmax(1) != net.last_q()[1].argmax(1))[~mb[4]].any()
 
 
 def test_forward_kernels_at_4096():
@@ -179,6 +206,13 @@ def test_forward_kernels_at_4096():
 @pytest.mark.parametrize("batch", [1, 64, 65])
 def test_history_lengths(hist, batch):
     net = make_net(batch, hist=hist)
+    train_and_check(net, minibatch(batch, hist, 4, 3))
+
+
+@pytest.mark.parametrize("hist", [1, 5, 16])
+@pytest.mark.parametrize("batch", [1, 64, 65])
+def test_double_history_lengths(hist, batch):
+    net = make_net(batch, hist=hist, double=True)
     train_and_check(net, minibatch(batch, hist, 4, 3))
 
 
@@ -277,20 +311,26 @@ def test_simt_engine_kernels(batch):
     train_and_check(net, minibatch(batch, 4, 4, 19))
 
 
-def _child(env, cases):
+@pytest.mark.parametrize("batch", [1, 32, 65])
+def test_double_simt_engine_kernels(batch):
+    net = make_net(batch, engine="fp32", sched="serial", double=True)
+    train_and_check(net, minibatch(batch, 4, 4, 19))
+
+
+def _child(env, cases, double=False):
     """Run train_and_check in a child process: the B200DQN_* switches are read once per process."""
     code = ("import json, sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
             "import test_gpu_kernels as T\n"
             "out = []\n"
             "for batch, kw in %r:\n"
-            "    out.append(T.train_and_check(T.make_net(batch), T.minibatch(batch, 4, 4, 21), **kw)[0])\n"
-            "print('RATIOS', json.dumps(out))\n" % (ROOT, os.path.join(ROOT, "tests"), cases))
+            "    out.append(T.train_and_check(T.make_net(batch, double=%r), T.minibatch(batch, 4, 4, 21), **kw)[0])\n"
+            "print('RATIOS', json.dumps(out))\n" % (ROOT, os.path.join(ROOT, "tests"), cases, double))
     out = subprocess.run([sys.executable, "-s", "-c", code], env=dict(os.environ, **env), capture_output=True,
                          text=True, timeout=900)
     assert out.returncode == 0, out.stderr[-4000:]
     line = [l for l in out.stdout.splitlines() if l.startswith("RATIOS ")][0]
     for r in json.loads(line[len("RATIOS "):]):
-        _note(r)
+        _note(r, double)
 
 
 def test_conv1_tma_twin():
@@ -300,3 +340,9 @@ def test_conv1_tma_twin():
 @pytest.mark.parametrize("splits", [1, 4, 14])
 def test_fc1_forced_splits(splits):
     _child({"B200DQN_FC1_SPLITS": str(splits)}, [(b, {"fc1_forced": splits}) for b in (33, 257)])
+
+
+@pytest.mark.parametrize("splits", [1, 4, 14])
+def test_double_fc1_forced_splits(splits):
+    """Three slots of split-K partials: 14 forced splits fill the whole partial buffer."""
+    _child({"B200DQN_FC1_SPLITS": str(splits)}, [(b, {"fc1_forced": splits}) for b in (33, 257)], double=True)
