@@ -150,9 +150,34 @@ int b200dqn_replay_read_minibatch(b200dqn_replay* r, uint8_t* host_pre, uint8_t*
 enum {
   B200DQN_PTR_SCREENS = 0, B200DQN_PTR_ACTIONS, B200DQN_PTR_REWARDS, B200DQN_PTR_TERMINALS,
   B200DQN_PTR_PRESTATES, B200DQN_PTR_POSTSTATES, B200DQN_PTR_MB_ACTIONS, B200DQN_PTR_MB_REWARDS,
-  B200DQN_PTR_MB_TERMINALS, B200DQN_PTR_INDEXES, B200DQN_PTR_WORDS_CONSUMED, B200DQN_PTR_MT_STATE
+  B200DQN_PTR_MB_TERMINALS, B200DQN_PTR_INDEXES, B200DQN_PTR_WORDS_CONSUMED, B200DQN_PTR_MT_STATE,
+  /* Prioritized replay (b200dqn_replay_set_prioritized); NULL with 0 bytes until it is first switched on.
+   * PRIORITIES: f64[size], the stored priority p^alpha of every slot.  SUM_TREE: f64, the 32-ary sum tree level by
+   * level from the leaves (level l has n_l = ceil(n_{l-1} / 32) nodes, n_0 = size, and starts at a multiple of 32
+   * entries; the padding is 0).  Leaf i is PRIORITIES[i] if getMinibatch would accept slot i, else 0.  IS_WEIGHTS:
+   * f32[batch] of the last draw or set_indexes.  MAX_PRIORITY: f64[1] (not raised to alpha).  MIN_TREE: f64, levels
+   * 1.. of the min tree in the same layout (a leaf's min value is itself if positive, else +inf). */
+  B200DQN_PTR_PRIORITIES, B200DQN_PTR_SUM_TREE, B200DQN_PTR_IS_WEIGHTS, B200DQN_PTR_MAX_PRIORITY, B200DQN_PTR_MIN_TREE
 };
 int b200dqn_replay_device_ptr(b200dqn_replay* r, int which, void** dev_ptr, size_t* bytes);
+
+/* Proportional prioritized experience replay (Schaul et al., 2016; the variant of OpenAI baselines'
+ * PrioritizedReplayBuffer; new capability, no reference counterpart), off by default.  While it is on:
+ *   - the index draw (b200dqn_replay_sample, the fused step) is stratified over the sum tree: sample i takes
+ *     mass = random.random() * (total / batch) + i * (total / batch) and descends to the leaf holding it, so a draw
+ *     consumes exactly 2 * batch MT19937 words and never draws a slot getMinibatch would reject;
+ *   - importance weights w_i = (N P_i)^-beta / (N P_min)^-beta, N = count, beta = beta0 + (1 - beta0) *
+ *     min(1, k / beta_steps), k = samplings done, scale each sample's clipped delta and its cost in the train step;
+ *   - after a train step on the ring, each sampled slot gets (|delta_i| + eps)^alpha, delta_i the TD error before the
+ *     clip (the last occurrence wins for a repeated slot), and max_priority = max(max_priority, |delta_i| + eps);
+ *   - slots written by add / add_batch / step_host get max_priority^alpha.
+ * Switching on sets every stored priority and max_priority to 1 and builds the trees from the ring as it stands
+ * (the first switch-on allocates them).  Either switch rebuilds the captured step graphs of the nets that train from
+ * r.  A draw from a ring with no drawable slot reports ESTATE at the next result poll.  Train steps from a
+ * prioritized ring return ENOTIMPL for data-parallel learners and, on the tensor-core engine, under
+ * B200DQN_CONV1=tma.  Synchronises. */
+int b200dqn_replay_set_prioritized(b200dqn_replay* r, int on, double alpha, double beta0, double beta_steps,
+                                   double eps);
 
 /* ------------------------------------------------------------------ state window -------- */
 
@@ -289,7 +314,10 @@ enum {
   /* The online network's Q on the poststates of the last Double DQN train step, (batch,A) f32: the row whose first
    * maximum picks the action the target network values.  With target_steps = 0 it is the Q_TARGET buffer (the two
    * networks are one). */
-  B200DQN_NET_PTR_Q_ONLINE_POST
+  B200DQN_NET_PTR_Q_ONLINE_POST,
+  /* (batch,) f32: the TD error delta_i = preq[a_i] - target_i before the clip, of the last train step on a
+   * prioritized ring (the quantity its priority update uses).  EINVAL before the first such step. */
+  B200DQN_NET_PTR_TD_ERRORS
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

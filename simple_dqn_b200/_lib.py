@@ -11,10 +11,11 @@ MATH_FP32_SIMT, MATH_TCGEN05 = 0, 1
 OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
 
 (PTR_SCREENS, PTR_ACTIONS, PTR_REWARDS, PTR_TERMINALS, PTR_PRESTATES, PTR_POSTSTATES, PTR_MB_ACTIONS,
- PTR_MB_REWARDS, PTR_MB_TERMINALS, PTR_INDEXES, PTR_WORDS_CONSUMED, PTR_MT_STATE) = range(12)
+ PTR_MB_REWARDS, PTR_MB_TERMINALS, PTR_INDEXES, PTR_WORDS_CONSUMED, PTR_MT_STATE, PTR_PRIORITIES, PTR_SUM_TREE,
+ PTR_IS_WEIGHTS, PTR_MAX_PRIORITY, PTR_MIN_TREE) = range(17)
 (NET_PTR_Q_ONLINE, NET_PTR_Q_TARGET, NET_PTR_DELTAS, NET_PTR_GRADS, NET_PTR_WEIGHTS, NET_PTR_COST, NET_PTR_H1,
  NET_PTR_H2, NET_PTR_H3, NET_PTR_H4, NET_PTR_DZ4, NET_PTR_DZ3, NET_PTR_DZ2, NET_PTR_DZ1,
- NET_PTR_Q_ONLINE_POST) = range(15)
+ NET_PTR_Q_ONLINE_POST, NET_PTR_TD_ERRORS) = range(16)
 
 
 class B200DQNError(RuntimeError):
@@ -68,6 +69,7 @@ SIGNATURES = {
     "b200dqn_replay_gather": [_P, _P],
     "b200dqn_replay_read_minibatch": [_P, _P, _P, _P, _P, _P, _P, _P, _P],
     "b200dqn_replay_device_ptr": [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_size_t)],
+    "b200dqn_replay_set_prioritized": [_P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double],
     "b200dqn_statebuf_create": [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)],
     "b200dqn_statebuf_destroy": [_P],
     "b200dqn_statebuf_add": [_P, _P, _P],

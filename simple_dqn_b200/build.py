@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200dqn.so")
 # nvcc from PATH, else from the CUDA toolkit (CUDA_HOME, default /usr/local/cuda)
 NVCC = shutil.which("nvcc") or os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
-SOURCES = ["capi.cu", "replay.cu", "net.cu", "net_umma.cu", "comm.cu"]
+SOURCES = ["capi.cu", "replay.cu", "per.cu", "net.cu", "net_umma.cu", "comm.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17",
                 "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

@@ -482,6 +482,9 @@ extern "C" int b200dqn_net_comm_init(b200dqn_net* n, const void* id128, int rank
   // the data-parallel schedules exchange and gather the two-slot forward's tensors only
   B2_REQUIRE(!n->double_q, B200DQN_ENOTIMPL,
              "net_comm_init: the Double DQN target is implemented for a single learner only (switch double Q off first)");
+  B2_REQUIRE(!n->d_td_err, B200DQN_ENOTIMPL,
+             "net_comm_init: prioritized replay is implemented for a single learner only (this net has trained from a "
+             "prioritized ring)");
   int rc = nccl_load();
   if (rc) return rc;
   DeviceGuard g(n->device);

@@ -46,6 +46,10 @@ struct HeadTrainArgs {
   int num_actions;    // actions[] >= num_actions would index q / W5 out of bounds: flagged in err, clamped
   uint32_t* err;
   HeadPush push;      // data-parallel gather schedule: this CTA's dZ4 row goes straight to every rank (world = 0: off)
+  // prioritized replay (nullptr: off, today's step): the sample's importance weight scales its cost and its clipped
+  // delta; the TD error before the clip goes to td_err for the priority update
+  const float* isw;
+  float* td_err;
 };
 
 template <int kSlots>
@@ -136,8 +140,16 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
     const double y = td_term ? double(r) : double(r) + td.discount * double(maxq);          // :140-143
     const float target = static_cast<float>(y);
     float d = s_q[0][a] - target;                                                         // SumSquared grad (:149)
-    td.row_cost[b] = 0.5f * d * d;                                                        // :154, before the clip
-    if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);                            // :158-159
+    if (td.isw) {                                                                         // prioritized replay
+      const float wb = td.isw[b];
+      td.td_err[b] = d;
+      td.row_cost[b] = wb * (0.5f * d * d);
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+      d = d * wb;
+    } else {
+      td.row_cost[b] = 0.5f * d * d;                                                      // :154, before the clip
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);                          // :158-159
+    }
     for (int j = 0; j < A; ++j) td.delta[b * A + j] = (j == a) ? d : 0.f;
     s_d = d;
     s_a = a;
@@ -213,6 +225,7 @@ k_cost_finish(const float* __restrict__ row_cost, int rows, float* cost_ring, ui
       if (sampler_words) {         // this step's index draw: words consumed, for the host's lock-step `random`
         host_words[1] = sampler_words[0];
         host_words[2] = sampler_words[1];
+        host_words[3] = sampler_words[3];   // sticky error of the prioritized sampler
       }
       __threadfence_system();
       if (sampler_words) host_words[0] = sampler_words[2];
@@ -493,6 +506,8 @@ static int cost_finish_on(b200dqn_net* n, int rows, cudaStream_t s) {
                            n->h_res, (const uint32_t*)(r ? r->d_words : nullptr),
                            (volatile uint32_t*)(r ? r->h_words : nullptr), ktrace_slot("cost")));
   B2_PROF("cost", s);
+  if (r && r->per_on)   // priorities of the sampled slots, after the head (td_err) on the same off-chain branch
+    return launch_per_update(r, r->d_idx + n->rank * n->nb, n->d_td_err, rows, s);
   return B200DQN_OK;
 }
 
@@ -843,6 +858,10 @@ static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* acti
                    reinterpret_cast<uint32_t*>(n->d_cost + kCostRing + 1), HeadPush{}};
   umma_dz4_planes(n, &td.dz4_hi, &td.dz4_lo_off);
   comm_head_push(n, st, &td.push);
+  if (n->step_replay && n->step_replay->per_on) {   // a prioritized ring: weighted step, TD errors for the update
+    td.isw = n->step_replay->d_isw + n->rank * n->nb;
+    td.td_err = n->d_td_err;
+  }
   // Double DQN adds the online network on the poststates as a third slot of the same launches.  With target_steps = 0
   // the target network IS the online network, so slot 1 already holds that forward and a* = argmax of the same row:
   // the vanilla step is the Double DQN step, bit for bit.
@@ -1053,6 +1072,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_fc1part); cudaFree(n->d_delta); cudaFree(n->d_dz4); cudaFree(n->d_dz3); cudaFree(n->d_dz2);
   cudaFree(n->d_dz1); cudaFree(n->d_cost); cudaFree(n->d_step); cudaFree(n->d_rowcost); cudaFree(n->d_pre); cudaFree(n->d_post);
   cudaFree(n->d_act); cudaFree(n->d_term); cudaFree(n->d_rew); cudaFree(n->d_iota1); cudaFree(n->d_iota4);
+  cudaFree(n->d_td_err);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -1286,6 +1306,17 @@ static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
              kFrameH, kFrameW, n->cfg.history_length);
   B2_REQUIRE(r->batch == n->nb * n->world, B200DQN_EINVAL,
              "train_fused: replay batch (%d) must equal the global minibatch %d x %d", r->batch, n->nb, n->world);
+  if (r->per_on) {
+    B2_REQUIRE(n->world == 1 && !n->nccl_comm, B200DQN_ENOTIMPL,
+               "prioritized replay is implemented for a single learner only (comm_init has run)");
+    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
+               "prioritized replay: the B200DQN_CONV1=tma conv1 is not supported");
+    if (!n->d_td_err) {   // the first step on a prioritized ring (before any graph capture)
+      DeviceGuard g(n->device);
+      B2_CHECK_CUDA(cudaMalloc(&n->d_td_err, n->nb * sizeof(float)));
+      B2_CHECK_CUDA(cudaMemset(n->d_td_err, 0, n->nb * sizeof(float)));
+    }
+  }
   return B200DQN_OK;
 }
 
@@ -1305,7 +1336,7 @@ static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t 
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (!use_graph) return train_on_ring(n, r, st);
   if (!n->graph_train_exec || n->graph_train_replay != r || n->graph_train_stream != st ||
-      n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen) {
+      n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen || n->graph_train_per_gen != r->per_gen) {
     if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
     cudaGraph_t graph = nullptr;
     B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
@@ -1317,6 +1348,7 @@ static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t 
     cudaGraphDestroy(graph);
     n->graph_train_replay = r; n->graph_train_stream = st; n->graph_train_world = n->world;
     n->graph_train_gen = g_ktrace_gen;
+    n->graph_train_per_gen = r->per_gen;
   }
   B2_CHECK_CUDA(cudaGraphLaunch(n->graph_train_exec, st));
   return B200DQN_OK;
@@ -1367,9 +1399,10 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (use_graph) {
     if (n->graph_replay != r || n->graph_stream != st || n->graph_world != n->world ||
-        n->graph_trace_gen != g_ktrace_gen) {
+        n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen) {
       destroy_step_graphs(n);
       n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
+      n->graph_per_gen = r->per_gen;
     }
     if (!n->graph_exec) {
       cudaGraph_t graph = nullptr;
@@ -1494,6 +1527,11 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_Q_ONLINE_POST:   // target_steps = 0: the target forward is the online one (train_step)
       p = n->d_tw == n->d_w ? n->d_q[1] : n->d_q[2];
       b = size_t(n->nb) * n->A * 4;
+      break;
+    case B200DQN_NET_PTR_TD_ERRORS:
+      B2_REQUIRE(n->d_td_err, B200DQN_EINVAL, "net_device_ptr: no train step on a prioritized ring has run");
+      p = n->d_td_err;
+      b = size_t(n->nb) * 4;
       break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }

@@ -97,6 +97,8 @@ struct b200dqn_net {
   b200dqn_replay* graph_train_replay = nullptr;
   cudaStream_t graph_train_stream = nullptr;
   int graph_train_world = 0, graph_train_gen = 0;
+  uint32_t graph_per_gen = 0, graph_train_per_gen = 0;   // b200dqn_replay::per_gen the step graphs were captured at
+  float* d_td_err = nullptr;   // [nb] TD errors before the clip (prioritized replay; allocated at its first step)
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

@@ -111,6 +111,10 @@ int replay_flush(b200dqn_replay* r, cudaStream_t st) {
                                      r->bank_actions(b), r->bank_rewards(b), r->bank_terminals(b), r->count,
                                      r->current);
   B2_LAUNCH_CHECK();
+  if (r->per_on) {
+    int rc = per_after_add(r, pos0, n, st);
+    if (rc) return rc;
+  }
   B2_CHECK_CUDA(cudaEventRecord(r->bank_done[b], st));
   r->bank ^= 1;
   r->npend = 0;
@@ -120,7 +124,11 @@ int replay_flush(b200dqn_replay* r, cudaStream_t st) {
 
 // wait (polling host-mapped memory) until every sampler launched so far has published its word count
 int replay_wait_words(b200dqn_replay* r, cudaStream_t st) {
-  return poll_mapped_seq(r->h_words, r->samples_launched, st, "sampler result");
+  const int rc = poll_mapped_seq(r->h_words, r->samples_launched, st, "sampler result");
+  if (rc) return rc;
+  B2_REQUIRE(r->h_words[3] == 0, B200DQN_ESTATE,
+             "prioritized getMinibatch: the ring has no slot the sampler may draw (every leaf of the sum tree is 0)");
+  return B200DQN_OK;
 }
 
 int replay_set_rng_async(b200dqn_replay* r, const uint32_t* key624, uint32_t pos, cudaStream_t st) {
@@ -140,6 +148,7 @@ int replay_set_rng_async(b200dqn_replay* r, const uint32_t* key624, uint32_t pos
 int launch_sample(b200dqn_replay* r, cudaStream_t st) {
   int frc = replay_flush(r, st);
   if (frc) return frc;
+  if (r->per_on) return launch_sample_per(r, st);
   B2_CHECK_CUDA(launch_pdl(k_sample, dim3(1), dim3(kSampleThreads), 0, st, r->d_mt, (const uint8_t*)r->d_terminals,
                            (const int64_t*)r->d_cursor, r->hist, r->batch, r->d_idx, r->d_words, ktrace_slot("sample")));
   B2_PROF("sample", st);
@@ -279,6 +288,7 @@ extern "C" int b200dqn_replay_destroy(b200dqn_replay* r) {
   cudaFree(r->d_cursor); cudaFree(r->d_mt); cudaFree(r->d_idx); cudaFree(r->d_words);
   cudaFree(r->d_pre); cudaFree(r->d_post); cudaFree(r->d_mb_actions); cudaFree(r->d_mb_rewards);
   cudaFree(r->d_mb_terminals);
+  per_free(r);
   cudaFreeHost(r->h_stage);
   cudaFreeHost(const_cast<uint32_t*>(r->h_words));
   cudaFreeHost(r->h_mt);
@@ -315,6 +325,7 @@ extern "C" int b200dqn_replay_add_batch(b200dqn_replay* r, int64_t n, const uint
   DeviceGuard g(r->device);
   cudaStream_t st = as_stream(stream);
   { int frc = replay_flush(r, st); if (frc) return frc; }
+  const int64_t pos_first = r->current;
   int64_t done = 0;
   while (done < n) {
     const int64_t pos = r->current;
@@ -331,6 +342,10 @@ extern "C" int b200dqn_replay_add_batch(b200dqn_replay* r, int64_t n, const uint
   }
   k_set_cursor<<<1, 1, 0, st>>>(r->d_cursor, r->count, r->current);
   B2_LAUNCH_CHECK();
+  if (r->per_on) {   // the written slots get max_priority^alpha; every leaf and node is re-derived
+    int rc = per_rebuild(r, pos_first, n, false, st);
+    if (rc) return rc;
+  }
   B2_CHECK_CUDA(cudaStreamSynchronize(st));  // host arrays may be reused by the caller
   return B200DQN_OK;
 }
@@ -351,6 +366,10 @@ extern "C" int b200dqn_replay_set_cursor(b200dqn_replay* r, int64_t count, int64
   r->current = current;
   k_set_cursor<<<1, 1>>>(r->d_cursor, count, current);
   B2_LAUNCH_CHECK();
+  if (r->per_on) {   // the drawable set follows the cursor
+    int rc = per_rebuild(r, 0, 0, false, nullptr);
+    if (rc) return rc;
+  }
   B2_CHECK_CUDA(cudaDeviceSynchronize());
   return B200DQN_OK;
 }
@@ -434,6 +453,11 @@ extern "C" int b200dqn_replay_set_indexes(b200dqn_replay* r, const int32_t* host
   DeviceGuard g(r->device);
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemcpyAsync(r->d_idx, host_indexes, r->batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (r->per_on) {   // a prioritized ring trains these indexes exactly as if they had been drawn
+    { int frc = replay_flush(r, st); if (frc) return frc; }
+    int rc = per_weights_of_indexes(r, st);
+    if (rc) return rc;
+  }
   B2_CHECK_CUDA(cudaStreamSynchronize(st));
   return B200DQN_OK;
 }
@@ -493,6 +517,14 @@ extern "C" int b200dqn_replay_device_ptr(b200dqn_replay* r, int which, void** de
     case B200DQN_PTR_INDEXES: p = r->d_idx; b = r->batch * sizeof(int32_t); break;
     case B200DQN_PTR_WORDS_CONSUMED: p = r->d_words; b = 2 * sizeof(uint32_t); break;
     case B200DQN_PTR_MT_STATE: p = r->mt_slot_ptr(); b = 625 * sizeof(uint32_t); break;
+    case B200DQN_PTR_PRIORITIES: p = r->d_prio; b = r->d_prio ? r->size * sizeof(double) : 0; break;
+    case B200DQN_PTR_SUM_TREE: p = r->d_sum; b = r->d_sum ? r->per_off[r->per_nlev] * sizeof(double) : 0; break;
+    case B200DQN_PTR_IS_WEIGHTS: p = r->d_isw; b = r->d_isw ? r->batch * sizeof(float) : 0; break;
+    case B200DQN_PTR_MAX_PRIORITY: p = r->d_maxp; b = r->d_maxp ? sizeof(double) : 0; break;
+    case B200DQN_PTR_MIN_TREE:
+      p = r->d_min;
+      b = r->d_min ? (r->per_off[r->per_nlev] - r->per_off[1]) * sizeof(double) : 0;
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "replay_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;

@@ -56,6 +56,24 @@ struct b200dqn_replay {
   int64_t* bank_rewards(int b) const { return reinterpret_cast<int64_t*>(h_bank[b] + size_t(kPend) * frame_bytes); }
   uint8_t* bank_actions(int b) const { return reinterpret_cast<uint8_t*>(bank_rewards(b) + kPend); }
   uint8_t* bank_terminals(int b) const { return bank_actions(b) + kPend; }
+
+  // Proportional prioritized replay (per.cu; Schaul et al. 2016), off by default.  Allocated the first time it is
+  // switched on.  The 32-ary fp64 sum tree holds the leaves (level 0: stored priority of a drawable slot, else 0) and
+  // every level above them; the min tree holds levels 1.. (a leaf's min value is itself if positive, else +inf).
+  // Each level starts on a 32-node boundary; the padding stays zero.
+  static constexpr int kPerMaxLevels = 8;
+  bool per_on = false;
+  uint32_t per_gen = 0;               // bumped by every switch: step graphs that sample from this ring are stale
+  double per_alpha = 0.6, per_beta0 = 0.4, per_beta_steps = 1.0, per_eps = 1e-6;
+  int per_nlev = 0;                   // levels including the leaves; the root is level per_nlev - 1
+  int64_t per_n[kPerMaxLevels] = {};  // nodes per level
+  int64_t per_off[kPerMaxLevels + 1] = {};
+  double* d_prio = nullptr;           // [size] stored priorities p^alpha
+  double* d_sum = nullptr;            // [per_off[nlev]]
+  double* d_min = nullptr;            // [per_off[nlev] - per_off[1]]
+  double* d_maxp = nullptr;           // [1] max_priority (not raised to alpha)
+  float* d_isw = nullptr;             // [batch] importance weights of the last draw / set_indexes
+  uint32_t* d_per_ticket = nullptr;   // [1] CTA arrival counter of the prioritized sampler
 };
 
 struct b200dqn_statebuf {
@@ -98,6 +116,26 @@ __device__ __forceinline__ uint32_t mt_temper(uint32_t y) {
   y ^= (y >> 18);
   return y;
 }
+// genrand_uint32's regeneration of the whole 624-word key in shared memory, CTA-wide (every thread calls it; the
+// caller has synchronised since the last read of the old key).  Three dependency-free segments, then word 623.  Word i
+// of a segment reads the OLD word i + 1, which another warp's thread rewrites in the same segment: every thread reads
+// its operands, the CTA synchronises, and only then are the new words stored.
+__device__ __forceinline__ void mt_regenerate(uint32_t* mt, int tid, int nthreads) {
+#pragma unroll 1
+  for (int seg = 0; seg < 3; ++seg) {
+    const int lo = seg * 227, hi = seg == 2 ? 623 : lo + 227, far = seg == 0 ? kMtM : -227;
+    for (int base = lo; base < hi; base += nthreads) {   // one pass when nthreads >= 227
+      const int i = base + tid;
+      const uint32_t v = i < hi ? mt_mix(mt[i], mt[i + 1], mt[i + far]) : 0u;
+      __syncthreads();
+      if (i < hi) mt[i] = v;
+      __syncthreads();
+    }
+  }
+  if (tid == 0) mt[623] = mt_mix(mt[623], mt[0], mt[396]);
+  __syncthreads();
+}
+
 // Every thread of the CTA calls this (nthreads = blockDim.x, a multiple of 32, <= 384; __syncthreads inside).  sh.mt
 // holds the state on entry and the advanced state (position in [624]) on return; accepted indexes go to idx_out
 // (shared or global), in acceptance order.  Returns the number of 32-bit words consumed.
@@ -113,14 +151,7 @@ __device__ __forceinline__ uint32_t sample_block(SampleShared& sh, const uint8_t
   uint32_t words = 0;
   while (accepted < batch) {
     if (pos >= kMtN) {  // genrand_uint32: regenerate the whole key, position 0
-      for (int i = tid; i < 227; i += nthreads) mt[i] = mt_mix(mt[i], mt[i + 1], mt[i + kMtM]);
-      __syncthreads();
-      for (int i = 227 + tid; i < 454; i += nthreads) mt[i] = mt_mix(mt[i], mt[i + 1], mt[i - 227]);
-      __syncthreads();
-      for (int i = 454 + tid; i < 623; i += nthreads) mt[i] = mt_mix(mt[i], mt[i + 1], mt[i - 227]);
-      __syncthreads();
-      if (tid == 0) mt[623] = mt_mix(mt[623], mt[0], mt[396]);
-      __syncthreads();
+      mt_regenerate(mt, tid, nthreads);
       pos = 0;
     }
     const int avail = min(kMtN - pos, nthreads);
@@ -170,14 +201,28 @@ __device__ __forceinline__ uint32_t sample_block(SampleShared& sh, const uint8_t
   return words;
 }
 
-// [0] samplings completed (published last), [1] words of the last one, [2] running total
+// [0] samplings completed (published last), [1] words of the last one, [2] running total, [3] sticky error of the
+// prioritized sampler (a draw from a ring with no drawable slot)
 __device__ __forceinline__ void publish_words(const uint32_t* __restrict__ words, volatile uint32_t* host_words) {
   host_words[1] = words[0];
   host_words[2] = words[1];
+  host_words[3] = words[3];
   __threadfence_system();
   host_words[0] = words[2];
 }
 #endif
 // adopt a host MT19937 state (624 key words + position) without synchronising the stream
 int replay_set_rng_async(b200dqn_replay* r, const uint32_t* key624, uint32_t pos, cudaStream_t st);
+
+// ---- prioritized replay (per.cu)
+int launch_sample_per(b200dqn_replay* r, cudaStream_t st);
+// leaves and ancestors of the slots written by a flush of n deferred add()s starting at pos0
+int per_after_add(b200dqn_replay* r, int64_t pos0, int64_t n, cudaStream_t st);
+// every leaf and node from the stored priorities (fill_from/fill_n: slots that get max_priority^alpha first)
+int per_rebuild(b200dqn_replay* r, int64_t fill_from, int64_t fill_n, bool init, cudaStream_t st);
+// importance weights of the indexes in d_idx (set_indexes on a prioritized ring)
+int per_weights_of_indexes(b200dqn_replay* r, cudaStream_t st);
+// priority update after a train step: td_err[rows] of the indexes idx[rows]
+int launch_per_update(b200dqn_replay* r, const int32_t* idx, const float* td_err, int rows, cudaStream_t st);
+void per_free(b200dqn_replay* r);
 }  // namespace b200

@@ -203,6 +203,10 @@ class DeepQNetwork:
         """The online network's Q on the poststates of the last Double DQN train() as a (batch, A) array."""
         return self._read_f32(L.NET_PTR_Q_ONLINE_POST, (self.batch_size, self.num_actions))
 
+    def last_td_errors(self):
+        """TD errors before the clip of the last train() on a prioritized ring, (batch,) float32."""
+        return self._read_f32(L.NET_PTR_TD_ERRORS, (self.batch_size,))
+
     def last_deltas(self):
         return self._read_f32(L.NET_PTR_DELTAS, (self.batch_size, self.num_actions))
 
@@ -211,8 +215,10 @@ class DeepQNetwork:
         L.call("b200dqn_net_sync_target", self._h, self._stream)        # :102-105
 
     def train(self, minibatch, epoch=0):
-        """deepqnetwork.py:107-172.  A pristine DeviceMinibatch is trained in place from the ring."""
-        if isinstance(minibatch, DeviceMinibatch) and not minibatch.materialised:
+        """deepqnetwork.py:107-172.  A pristine DeviceMinibatch is trained in place from the ring, and so is one from a
+        prioritized ring even once it has been looked at (the importance weights and the priority update live there).
+        A host tuple is always the uniform, unweighted step."""
+        if isinstance(minibatch, DeviceMinibatch) and (not minibatch.materialised or minibatch._mem.prioritized):
             minibatch._check_current()
             mem = minibatch._mem
             cost = C.c_float()

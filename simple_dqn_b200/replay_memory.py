@@ -138,6 +138,19 @@ class ReplayMemory:
         self.last_indexes = None
         self.last_words_consumed = None
         logger.info("Replay memory size: %d" % self.size)
+        # proportional prioritized replay (Schaul et al., 2016), parameters named as in OpenAI baselines: a new
+        # capability, off unless args.prioritized_replay is set.  beta is annealed to 1 over beta_steps samplings,
+        # by default the number of train steps the reference's main loop runs.
+        self.prioritized = False
+        self.alpha = getattr(args, "alpha", 0.6)
+        self.beta0 = getattr(args, "beta0", 0.4)
+        self.eps = getattr(args, "eps", 1e-6)
+        self.beta_steps = getattr(args, "beta_steps", None)
+        if self.beta_steps is None:
+            self.beta_steps = (getattr(args, "epochs", 200) * getattr(args, "train_steps", 250000) //
+                               getattr(args, "train_frequency", 4) * getattr(args, "train_repeat", 1))
+        if getattr(args, "prioritized_replay", False):
+            self.set_prioritized(True)
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -189,6 +202,39 @@ class ReplayMemory:
     @property
     def screens(self):
         return self._download(L.PTR_SCREENS, np.uint8, (self.size,) + self.dims)
+
+    # ---- prioritized replay
+    def set_prioritized(self, on=True, alpha=None, beta0=None, beta_steps=None, eps=None):
+        """Switch proportional prioritized replay on or off (include/b200dqn.h, b200dqn_replay_set_prioritized).
+        Switching on resets every stored priority and max_priority to 1.  Parameters left None keep their values."""
+        self.alpha = self.alpha if alpha is None else alpha
+        self.beta0 = self.beta0 if beta0 is None else beta0
+        self.beta_steps = self.beta_steps if beta_steps is None else beta_steps
+        self.eps = self.eps if eps is None else eps
+        L.call("b200dqn_replay_set_prioritized", self._h, int(bool(on)), float(self.alpha), float(self.beta0),
+               float(self.beta_steps), float(self.eps))
+        self.prioritized = bool(on)
+
+    @property
+    def priorities(self):
+        """Host copy of the stored priorities p^alpha, float64 (size,)."""
+        assert self.prioritized or self._has_per_buffers(), "prioritized replay was never switched on"
+        return self._download(L.PTR_PRIORITIES, np.float64, (self.size,))
+
+    @property
+    def last_weights(self):
+        """Importance weights of the last prioritized draw (or set_indexes), float32 (batch,)."""
+        assert self.prioritized or self._has_per_buffers(), "prioritized replay was never switched on"
+        return self._download(L.PTR_IS_WEIGHTS, np.float32, (self.batch_size,))
+
+    @property
+    def max_priority(self):
+        return float(self._download(L.PTR_MAX_PRIORITY, np.float64, (1,))[0])
+
+    def _has_per_buffers(self):
+        p, b = C.c_void_p(), C.c_size_t()
+        L.call("b200dqn_replay_device_ptr", self._h, L.PTR_PRIORITIES, C.byref(p), C.byref(b))
+        return b.value > 0
 
     # ---- reference methods
     def add(self, action, reward, screen, terminal):
@@ -302,7 +348,7 @@ class ReplayMemory:
 
     def getMinibatch(self):
         # replay_memory.py:50-79
-        if self.device_minibatch:
+        if self.device_minibatch or self.prioritized:   # a prioritized minibatch must train from the ring
             # agent.py:112-114 is `mb = mem.getMinibatch(); net.train(mb, epoch)` with nothing in between: hand out
             # a handle and let the draw ride in train()'s graph (one launch, one wait per step).  Anything else that
             # looks at the handle (statistics.py:85) triggers the draw on the spot.
