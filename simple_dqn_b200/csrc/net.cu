@@ -1335,8 +1335,9 @@ static int train_on_ring(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
 static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (!use_graph) return train_on_ring(n, r, st);
-  if (!n->graph_train_exec || n->graph_train_replay != r || n->graph_train_stream != st ||
-      n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen || n->graph_train_per_gen != r->per_gen) {
+  if (!n->graph_train_exec || n->graph_train_replay != r || n->graph_train_replay_serial != r->serial ||
+      n->graph_train_stream != st || n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen ||
+      n->graph_train_per_gen != r->per_gen) {
     if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
     cudaGraph_t graph = nullptr;
     B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
@@ -1347,6 +1348,7 @@ static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t 
     B2_CHECK_CUDA(cudaGraphInstantiate(&n->graph_train_exec, graph, 0));
     cudaGraphDestroy(graph);
     n->graph_train_replay = r; n->graph_train_stream = st; n->graph_train_world = n->world;
+    n->graph_train_replay_serial = r->serial;
     n->graph_train_gen = g_ktrace_gen;
     n->graph_train_per_gen = r->per_gen;
   }
@@ -1398,10 +1400,11 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
   // and replayed: one graph launch per step instead of ~17 stream operations.
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (use_graph) {
-    if (n->graph_replay != r || n->graph_stream != st || n->graph_world != n->world ||
-        n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen) {
+    if (n->graph_replay != r || n->graph_replay_serial != r->serial || n->graph_stream != st ||
+        n->graph_world != n->world || n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen) {
       destroy_step_graphs(n);
       n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
+      n->graph_replay_serial = r->serial;
       n->graph_per_gen = r->per_gen;
     }
     if (!n->graph_exec) {

@@ -98,6 +98,8 @@ struct b200dqn_net {
   cudaStream_t graph_train_stream = nullptr;
   int graph_train_world = 0, graph_train_gen = 0;
   uint32_t graph_per_gen = 0, graph_train_per_gen = 0;   // b200dqn_replay::per_gen the step graphs were captured at
+  // b200dqn_replay::serial of the ring the step graphs were captured on: the pointer alone can name a newer ring
+  uint64_t graph_replay_serial = 0, graph_train_replay_serial = 0;
   float* d_td_err = nullptr;   // [nb] TD errors before the clip (prioritized replay; allocated at its first step)
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)

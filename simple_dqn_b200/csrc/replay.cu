@@ -1,6 +1,7 @@
 // replay.cu — replay ring in HBM: add / getState / device MT19937 sampler / TMA-bulk gather,
 // and the device-side StateBuffer.  Replaces src/replay_memory.py and src/state_buffer.py of
 // the reference (file:line cited per function in include/b200dqn.h).
+#include <atomic>
 #include <new>
 
 #include "replay.cuh"
@@ -216,6 +217,9 @@ __global__ void k_statebuf_shift(T* __restrict__ row0, const T* __restrict__ fre
 
 using namespace b200;
 
+// b200dqn_replay::serial of the next ring created in this process (0 names no ring)
+static std::atomic<uint64_t> g_replay_serial{1};
+
 // ============================================================================ C ABI: replay
 extern "C" int b200dqn_replay_create(int device, int64_t size, int screen_h, int screen_w, int history_length,
                                      int batch_size, b200dqn_replay** out) {
@@ -274,8 +278,18 @@ extern "C" int b200dqn_replay_create(int device, int64_t size, int screen_h, int
   }
   for (int i = 0; i < b200dqn_replay::kSlots; ++i)
     B2_CHECK_CUDA(cudaEventCreateWithFlags(&r->slot_done[i], cudaEventDisableTiming));
-  B2_CHECK_CUDA(cudaFuncSetAttribute(k_gather, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     int(r->frame_bytes + 128)));
+  // k_gather stages one frame in dynamic shared memory.  Its limit is raised to all that one block may opt into, the
+  // same for every ring on the device, so that creating a ring of smaller frames never lowers it under another
+  // ring's; frames larger than that take the byte loop (b200dqn_replay_gather).
+  {
+    int optin = 0;
+    cudaFuncAttributes fa{};
+    B2_CHECK_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+    B2_CHECK_CUDA(cudaFuncGetAttributes(&fa, k_gather));
+    r->gather_smem = optin - int(fa.sharedSizeBytes);
+    B2_CHECK_CUDA(cudaFuncSetAttribute(k_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, r->gather_smem));
+  }
+  r->serial = g_replay_serial.fetch_add(1, std::memory_order_relaxed);
   *out = r;
   return B200DQN_OK;
 }
@@ -466,7 +480,7 @@ extern "C" int b200dqn_replay_gather(b200dqn_replay* r, void* stream) {
   B2_REQUIRE(r, B200DQN_EINVAL, "null replay");
   DeviceGuard g(r->device);
   { int frc = replay_flush(r, as_stream(stream)); if (frc) return frc; }
-  const int use_tma = (r->frame_bytes % 16 == 0) ? 1 : 0;
+  const int use_tma = (r->frame_bytes % 16 == 0 && r->frame_bytes <= r->gather_smem) ? 1 : 0;
   dim3 grid(r->batch, r->hist + 1);
   k_gather<<<grid, 128, use_tma ? r->frame_bytes : 0, as_stream(stream)>>>(
       r->d_screens, r->d_actions, r->d_rewards, r->d_terminals, r->d_idx, r->hist, uint32_t(r->frame_bytes),

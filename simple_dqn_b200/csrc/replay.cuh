@@ -3,10 +3,14 @@
 #include "common.cuh"
 
 struct b200dqn_replay {
+  // process-wide creation number, never reused (a ring created after another is destroyed may get its address):
+  // what a net's cached step graphs, which bake in this ring's buffers and shape, are keyed by
+  uint64_t serial = 0;
   int device = 0;
   int64_t size = 0;
   int h = 0, w = 0, hist = 0, batch = 0;
   int64_t frame_bytes = 0;
+  int gather_smem = 0;   // dynamic shared memory k_gather may use on this device: larger frames take its byte loop
   // host mirror of the cursor (src/replay_memory.py:17-18)
   int64_t count = 0, current = 0;
 
