@@ -206,8 +206,9 @@ typedef struct b200dqn_net_config {
   double learning_rate;  /* :51  RMSProp                                                  */
   double decay_rate;     /* :52                                                           */
   double clip_error;     /* :23  (0 disables the clip, as `if self.clip_error:` does)     */
-  int min_reward;        /* :24  */
-  int max_reward;        /* :25  */
+  double min_reward;     /* :24  main.py:43-44 declare both bounds type=float; the reward is clipped  */
+  double max_reward;     /* :25  as np.clip(r, min, max) clips: min(max(r, min), max), so max wins if  */
+                         /*      the bounds cross                                                     */
   int target_steps;      /* :65  0 ⇒ the target network aliases the online network (:72-73) */
   int math_mode;         /* B200DQN_MATH_*                                                */
   int optimizer;         /* B200DQN_OPT_*  (:50-61; args.optimizer, main.py:40)           */
@@ -317,7 +318,10 @@ enum {
   B200DQN_NET_PTR_Q_ONLINE_POST,
   /* (batch,) f32: the TD error delta_i = preq[a_i] - target_i before the clip, of the last train step on a
    * prioritized ring (the quantity its priority update uses).  EINVAL before the first such step. */
-  B200DQN_NET_PTR_TD_ERRORS
+  B200DQN_NET_PTR_TD_ERRORS,
+  /* (batch,) f32: the per-sample cost 0.5*delta^2 before the clip (times the importance weight on a prioritized ring)
+   * of the last train step, whose mean in row order is the step's cost. */
+  B200DQN_NET_PTR_ROW_COSTS
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

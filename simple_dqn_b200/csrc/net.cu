@@ -32,7 +32,7 @@ struct HeadTrainArgs {
   const uint8_t* terminals;
   const int32_t* midx;
   double discount;
-  int min_reward, max_reward;
+  double min_reward, max_reward;
   float clip;
   float* delta;       // [rows][A]
   const uint32_t* step;   // completed train steps (k_cost_finish increments it)
@@ -125,8 +125,9 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
   __syncthreads();
   if (t == 0) {
     const int a = td_a;
-    int64_t r = td_r;
-    r = r < td.min_reward ? td.min_reward : (r > td.max_reward ? td.max_reward : r);     // np.clip (:136)
+    // np.clip (:136) with float bounds (main.py:43-44): maximum with the lower bound, then minimum with the upper
+    // one, so crossed bounds give the upper bound.  For bounds that are exact doubles this is numpy's int64 clamp.
+    const double rr = fmin(fmax(double(td_r), td.min_reward), td.max_reward);
     float maxq;
     if constexpr (kSlots == 3) {   // Double DQN: a* = argmax_a Q_online(s', a), valued by the target network
       int best = 0;
@@ -137,7 +138,7 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
       maxq = s_q[1][0];
       for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);                          // be.max(postq) (:124)
     }
-    const double y = td_term ? double(r) : double(r) + td.discount * double(maxq);          // :140-143
+    const double y = td_term ? rr : rr + td.discount * double(maxq);                        // :140-143
     const float target = static_cast<float>(y);
     float d = s_q[0][a] - target;                                                         // SumSquared grad (:149)
     if (td.isw) {                                                                         // prioritized replay
@@ -1536,6 +1537,7 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       p = n->d_td_err;
       b = size_t(n->nb) * 4;
       break;
+    case B200DQN_NET_PTR_ROW_COSTS: p = n->d_rowcost; b = size_t(n->nb) * 4; break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;

@@ -43,6 +43,9 @@ class DeepQNetwork:
             raise NotImplementedError("only --datatype float32 is implemented in this library")
         if _arg(args, "stochastic_round", False):
             raise NotImplementedError("--stochastic_round is not implemented in this library")
+        if self.clip_error is not None and self.clip_error < 0:
+            # the reference hands Neon's be.clip a lower bound above its upper bound (:159), whose result is unpinned
+            raise NotImplementedError("--clip_error < 0 is not implemented in this library")
         self.device = _arg(args, "device_id", 0) if device is None else device
         self._stream_obj = stream            # keep the stream alive as long as this object uses it
         self._stream = L.stream_ptr(stream)
@@ -56,8 +59,8 @@ class DeepQNetwork:
         cfg.learning_rate = args.learning_rate
         cfg.decay_rate = args.decay_rate
         cfg.clip_error = float(args.clip_error or 0)
-        cfg.min_reward = int(args.min_reward)
-        cfg.max_reward = int(args.max_reward)
+        cfg.min_reward = float(args.min_reward)         # type=float (main.py:43-44)
+        cfg.max_reward = float(args.max_reward)
         cfg.target_steps = int(args.target_steps or 0)
         if math_mode is None:
             math_mode = _arg(args, "math_mode", "fp32")
@@ -206,6 +209,11 @@ class DeepQNetwork:
     def last_td_errors(self):
         """TD errors before the clip of the last train() on a prioritized ring, (batch,) float32."""
         return self._read_f32(L.NET_PTR_TD_ERRORS, (self.batch_size,))
+
+    def last_row_costs(self):
+        """Per-sample costs of the last train() (before the clip, importance-weighted on a prioritized ring), (batch,)
+        float32; the step's cost is their mean, summed in row order."""
+        return self._read_f32(L.NET_PTR_ROW_COSTS, (self.batch_size,))
 
     def last_deltas(self):
         return self._read_f32(L.NET_PTR_DELTAS, (self.batch_size, self.num_actions))

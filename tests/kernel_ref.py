@@ -239,11 +239,12 @@ def wgrad_fp32_chunked(x_cols, dz_rows, per, splits, a_exact=False):
 def head_td(preq, postq, actions, rewards, terminals, discount=0.99, min_reward=-1, max_reward=1, clip=1.0):
     """(unclipped deltas, clipped deltas) as float32 from the device's own preq/postq: the target is formed in
     double from the clipped reward and max(postq) and stored as fp32, delta = preq[a] - target in fp32, and the
-    clip (when clip > 0) follows the cost."""
+    clip (when clip > 0) follows the cost.  The reward is clipped as np.clip does, in double: the maximum with
+    min_reward first, then the minimum with max_reward (crossed bounds give max_reward)."""
     preq, postq = np.asarray(preq, np.float32), np.asarray(postq, np.float32)
     raw = np.zeros_like(preq)
     for i, a in enumerate(actions):
-        r = float(min(max(int(rewards[i]), min_reward), max_reward))
+        r = min(max(float(rewards[i]), float(min_reward)), float(max_reward))
         y = r if terminals[i] else r + float(discount) * float(postq[i].max())
         raw[i, a] = np.float32(preq[i, a]) - np.float32(y)
     clipped = np.clip(raw, np.float32(-clip), np.float32(clip)) if clip > 0 else raw.copy()

@@ -53,6 +53,10 @@ def test_config_default_matches_reference_flags(lib):
     assert (cfg.batch_size, cfg.history_length, cfg.screen_h, cfg.screen_w) == (32, 4, 84, 84)
     assert (cfg.discount_rate, cfg.learning_rate, cfg.decay_rate, cfg.clip_error) == (0.99, 0.00025, 0.95, 1.0)
     assert (cfg.min_reward, cfg.max_reward, cfg.target_steps) == (-1, 1, 10000)
+    # the reward bounds are floats (main.py:43-44): a fractional bound crosses the boundary unchanged
+    fields = dict(L.NetConfig._fields_)
+    assert fields["min_reward"] is C.c_double and fields["max_reward"] is C.c_double
+    assert "double min_reward;" in open(os.path.join(ROOT, "include", "b200dqn.h")).read()
 
 
 def test_binary_is_hopper_native():

@@ -159,9 +159,12 @@ def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward
                                  max_reward=max_reward)
     deltas = net.last_deltas()
     assert (deltas == clipped).all(), np.abs(deltas - clipped).max()
-    cost = float(net.last_costs(1)[0])
-    ref_cost = float(np.mean(0.5 * np.square(raw.astype(np.float64)).sum(axis=1)))
-    assert abs(cost - ref_cost) <= 1e-6 * abs(ref_cost) or cost == ref_cost == 0.0, (cost, ref_cost)
+    row_cost = (F32(0.5) * raw * raw).sum(axis=1)          # one non-zero delta per row
+    assert (net.last_row_costs() == row_cost).all()
+    tot = F32(0)
+    for c in row_cost:                                      # k_cost_finish: fp32, row order, then / rows
+        tot = F32(tot + c)
+    assert net.last_costs(1)[0] == F32(tot / F32(len(row_cost))), (net.last_costs(1)[0], tot)
     r = forward_ratios(engine, pre, ws0, acts, preq, fc1_forced)
     step = dict(acts=acts, dz=net.last_dz(), grads=net.get_grads())
     r.update(backward_ratios(engine, pre, ws0, acts, step["dz"], step["grads"], deltas, conv1_tma))
