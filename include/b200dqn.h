@@ -179,6 +179,21 @@ int b200dqn_replay_device_ptr(b200dqn_replay* r, int which, void** dev_ptr, size
 int b200dqn_replay_set_prioritized(b200dqn_replay* r, int on, double alpha, double beta0, double beta_steps,
                                    double eps);
 
+/* n-step returns (Hessel et al., 2018; new capability, no reference counterpart), N = n_step, default 1.  With N > 1:
+ *   - the draw is randint(hist, count - N) (one MT19937 word per trial, as at N = 1) and rejects a sample whose
+ *     window [index - hist, index + N - 1] holds the write pointer (index + N - 1 >= current and index - hist <
+ *     current) or whose terminals[index - hist .. index - 1] has a set flag; it needs count >= hist + N;
+ *   - the poststate is getState(index + N - 1); b200dqn_replay_gather / read_minibatch stage rewards and terminals
+ *     of index .. index + N - 1 as (batch, N) arrays (B200DQN_PTR_MB_REWARDS / _MB_TERMINALS grow to match);
+ *   - a train step on the ring forms y = R if a terminal lies in index .. index + N - 1, else R + gamma^N Q^(post),
+ *     R = sum_{k<m} gamma^k clip(rewards[index + k]), m the first terminal (or N), in fp64 without contraction;
+ *   - the prioritized sum tree masks the same slots.
+ * Host-supplied minibatches (b200dqn_net_train / _train_device) stay one-step.  Train steps from a ring with N > 1
+ * return ENOTIMPL for data-parallel learners and, on the tensor-core engine, under B200DQN_CONV1=tma; so does
+ * b200dqn_net_comm_init on a net whose last train step used such a ring.  Switching rebuilds the captured step graphs
+ * of the nets that train from r.  EINVAL unless 1 <= n and hist + n <= size.  Synchronises. */
+int b200dqn_replay_set_n_step(b200dqn_replay* r, int n);
+
 /* ------------------------------------------------------------------ state window -------- */
 
 /* StateBuffer(args) — src/state_buffer.py:9-13: (batch,hist,h,w) u8 zeros on the device. */

@@ -70,6 +70,7 @@ SIGNATURES = {
     "b200dqn_replay_read_minibatch": [_P, _P, _P, _P, _P, _P, _P, _P, _P],
     "b200dqn_replay_device_ptr": [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_size_t)],
     "b200dqn_replay_set_prioritized": [_P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double],
+    "b200dqn_replay_set_n_step": [_P, C.c_int],
     "b200dqn_statebuf_create": [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(_P)],
     "b200dqn_statebuf_destroy": [_P],
     "b200dqn_statebuf_add": [_P, _P, _P],

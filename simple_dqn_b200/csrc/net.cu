@@ -50,14 +50,18 @@ struct HeadTrainArgs {
   // delta; the TD error before the clip goes to td_err for the priority update
   const float* isw;
   float* td_err;
+  // n-step returns (Hessel et al. 2018): N > 1 forms y = sum_{k<m} gamma^k clip(r[i+k]) (+ gamma^N Q^ when no terminal
+  // in rewards/terminals[i .. i+N-1], m the first terminal) in fp64 without contraction; N <= 1 is today's one-step y
+  int nstep;
 };
 
-template <int kSlots>
+template <int kSlots, bool kNstep>
 __global__ void __launch_bounds__(kHidden)
 k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4_online, float* h4_target,
        const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
        float* q_target, float* q_online_post, int A, const HeadTrainArgs td, const KTrace kt) {
   static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  // kNstep (td.nstep > 1): the n-step target; the one-step instantiation is today's kernel unchanged
   __shared__ float red[kSlots][kHidden / 32][kMaxActions];
   __shared__ float s_q[kSlots][kMaxActions];
   __shared__ float s_d;
@@ -77,6 +81,39 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
     if (td_a >= td.num_actions) {   // the reference would raise IndexError (deepqnetwork.py:141); here: sticky flag
       atomicExch(td.err, 1u);
       td_a = td.num_actions - 1;
+    }
+  }
+  // n-step: lane k of warp 0 loads reward and terminal k (32 at a time), and every lane reduces them in k order through
+  // shuffles: g = 1; for k: R = R + g c_k; stop at a terminal; g = g gamma.  Thread 0 keeps R, g and the flag.
+  double td_ret = 0.0, td_g = 1.0;
+  if (kNstep && td.enable && t < 32) {
+    const int64_t mi = td.midx[b];
+    double R = 0.0, g = 1.0;
+    bool term = false;
+    for (int base = 0; base < td.nstep && !term; base += 32) {
+      const int k = base + t;
+      double c = 0.0;
+      int tk = 0;
+      if (k < td.nstep) {
+        c = fmin(fmax(double(td.rewards[mi + k]), td.min_reward), td.max_reward);
+        tk = td.terminals[mi + k];
+      }
+      const int m = min(32, td.nstep - base);
+      for (int j = 0; j < m; ++j) {
+        const double cj = __shfl_sync(0xffffffffu, c, j);
+        const int tj = __shfl_sync(0xffffffffu, tk, j);
+        R = __dadd_rn(R, __dmul_rn(g, cj));
+        if (tj) {
+          term = true;
+          break;
+        }
+        g = __dmul_rn(g, td.discount);
+      }
+    }
+    if (t == 0) {
+      td_ret = R;
+      td_g = g;
+      td_term = term ? 1 : 0;
     }
   }
   if (td.enable && td.adam_l && b == 0 && t == 32) {
@@ -138,7 +175,9 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
       maxq = s_q[1][0];
       for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);                          // be.max(postq) (:124)
     }
-    const double y = td_term ? rr : rr + td.discount * double(maxq);                        // :140-143
+    double y;
+    if constexpr (kNstep) y = td_term ? td_ret : __dadd_rn(td_ret, __dmul_rn(td_g, double(maxq)));
+    else y = td_term ? rr : rr + td.discount * double(maxq);                                // :140-143
     const float target = static_cast<float>(y);
     float d = s_q[0][a] - target;                                                         // SumSquared grad (:149)
     if (td.isw) {                                                                         // prioritized replay
@@ -408,7 +447,10 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     }
   }
   const int fc1_splits = n->cfg.math_mode == B200DQN_MATH_TCGEN05 ? umma_fc1_splits(rows) : kFc1Splits;
-  B2_CHECK_CUDA(launch_pdl(nets == 3 ? k_head<3> : k_head<2>, dim3(rows), dim3(kHidden), 0, st,
+  const bool nstep = td.enable && td.nstep > 1;
+  B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head<3, true> : k_head<3, false>)
+                                     : (nstep ? k_head<2, true> : k_head<2, false>),
+                           dim3(rows), dim3(kHidden), 0, st,
                            (const float*)n->d_fc1part, fc1_splits, rows, nets, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
                            w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, td, ktrace_slot("head")));
   B2_PROF(td.enable ? "head(fc2+td+fc2_bwd)" : "fc2_fwd", st);
@@ -863,6 +905,7 @@ static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* acti
     td.isw = n->step_replay->d_isw + n->rank * n->nb;
     td.td_err = n->d_td_err;
   }
+  td.nstep = n->step_replay ? n->step_replay->nstep : 1;   // host-staged minibatches are one-step
   // Double DQN adds the online network on the poststates as a third slot of the same launches.  With target_steps = 0
   // the target network IS the online network, so slot 1 already holds that forward and a* = argmax of the same row:
   // the vanilla step is the Double DQN step, bit for bit.
@@ -1318,14 +1361,21 @@ static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
       B2_CHECK_CUDA(cudaMemset(n->d_td_err, 0, n->nb * sizeof(float)));
     }
   }
+  if (r->nstep > 1) {
+    B2_REQUIRE(n->world == 1 && !n->nccl_comm, B200DQN_ENOTIMPL,
+               "n-step returns are implemented for a single learner only (comm_init has run)");
+    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
+               "n-step returns: the B200DQN_CONV1=tma conv1 draws its own 4-frame windows and is not supported");
+  }
+  n->ring_nstep = r->nstep;
   return B200DQN_OK;
 }
 
 static int train_on_ring(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   const int32_t* my_idx = r->d_idx + n->rank * n->nb;  // this rank's slice of the global minibatch
-  // prestates = frames index-H .. index-1, poststates = index-H+1 .. index (src/replay_memory.py:71-72)
+  // prestates = frames index-H .. index-1, poststates = index-H+N .. index+N-1 (src/replay_memory.py:71-72 at N = 1)
   const int hist = n->cfg.history_length;
-  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-hist, -hist + 1}, {r->size, r->size}};
+  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-hist, -hist + r->nstep}, {r->size, r->size}};
   n->step_replay = r;
   const int rc = train_step(n, fs, r->d_actions, r->d_rewards, r->d_terminals, my_idx, st);
   n->step_replay = nullptr;
@@ -1338,7 +1388,7 @@ static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t 
   if (!use_graph) return train_on_ring(n, r, st);
   if (!n->graph_train_exec || n->graph_train_replay != r || n->graph_train_replay_serial != r->serial ||
       n->graph_train_stream != st || n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen ||
-      n->graph_train_per_gen != r->per_gen) {
+      n->graph_train_per_gen != r->per_gen || n->graph_train_nstep != r->nstep) {
     if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
     cudaGraph_t graph = nullptr;
     B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
@@ -1352,6 +1402,7 @@ static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t 
     n->graph_train_replay_serial = r->serial;
     n->graph_train_gen = g_ktrace_gen;
     n->graph_train_per_gen = r->per_gen;
+    n->graph_train_nstep = r->nstep;
   }
   B2_CHECK_CUDA(cudaGraphLaunch(n->graph_train_exec, st));
   return B200DQN_OK;
@@ -1392,7 +1443,8 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
   B2_REQUIRE(n && r && nsteps >= 1, B200DQN_EINVAL, "net_train_fused: bad argument");
   int rc = check_fusable(n, r);
   if (rc) return rc;
-  B2_REQUIRE(r->count > r->hist, B200DQN_ESTATE, "getMinibatch: count must exceed history_length");
+  B2_REQUIRE(r->count >= r->hist + r->nstep, B200DQN_ESTATE,
+             "getMinibatch: count must be at least history_length + n_step");
   B2_REQUIRE(r->rng_set, B200DQN_ESTATE, "net_train_fused: call b200dqn_replay_set_rng first");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
@@ -1402,11 +1454,13 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (use_graph) {
     if (n->graph_replay != r || n->graph_replay_serial != r->serial || n->graph_stream != st ||
-        n->graph_world != n->world || n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen) {
+        n->graph_world != n->world || n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen ||
+        n->graph_nstep != r->nstep) {
       destroy_step_graphs(n);
       n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
       n->graph_replay_serial = r->serial;
       n->graph_per_gen = r->per_gen;
+      n->graph_nstep = r->nstep;
     }
     if (!n->graph_exec) {
       cudaGraph_t graph = nullptr;

@@ -100,6 +100,8 @@ struct b200dqn_net {
   uint32_t graph_per_gen = 0, graph_train_per_gen = 0;   // b200dqn_replay::per_gen the step graphs were captured at
   // b200dqn_replay::serial of the ring the step graphs were captured on: the pointer alone can name a newer ring
   uint64_t graph_replay_serial = 0, graph_train_replay_serial = 0;
+  int graph_nstep = 1, graph_train_nstep = 1;   // b200dqn_replay::nstep the step graphs were captured at
+  int ring_nstep = 1;   // n-step length of the ring this net last trained from (comm_init refuses N > 1)
   float* d_td_err = nullptr;   // [nb] TD errors before the clip (prioritized replay; allocated at its first step)
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)

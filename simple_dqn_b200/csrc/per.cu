@@ -23,7 +23,7 @@ struct PerView {
   const int64_t* cursor;      // {count, current}
   int64_t off[b200dqn_replay::kPerMaxLevels + 1];
   int64_t n[b200dqn_replay::kPerMaxLevels];
-  int nlev, hist;
+  int nlev, hist, nstep;
   int64_t size;
 };
 
@@ -33,14 +33,15 @@ static PerView per_view(const b200dqn_replay* r) {
   v.terminals = r->d_terminals; v.cursor = r->d_cursor;
   for (int l = 0; l <= b200dqn_replay::kPerMaxLevels; ++l) v.off[l] = r->per_off[l];
   for (int l = 0; l < b200dqn_replay::kPerMaxLevels; ++l) v.n[l] = r->per_n[l];
-  v.nlev = r->per_nlev; v.hist = r->hist; v.size = r->size;
+  v.nlev = r->per_nlev; v.hist = r->hist; v.nstep = r->nstep; v.size = r->size;
   return v;
 }
 
-// the acceptance test of getMinibatch (src/replay_memory.py:59-65) for slot i
+// the acceptance test of getMinibatch (src/replay_memory.py:59-65) for slot i, with the window of n-step returns
+// [i - hist, i + nstep - 1] (sample_block)
 __device__ __forceinline__ bool per_valid(const PerView& v, int64_t i, int64_t count, int64_t current) {
-  if (i < v.hist || i > count - 1) return false;
-  if (i >= current && i - v.hist < current) return false;
+  if (i < v.hist || i > count - v.nstep) return false;
+  if (i + v.nstep - 1 >= current && i - v.hist < current) return false;
   unsigned any = 0;
   for (int j = 1; j <= v.hist; ++j) any |= v.terminals[i - j];
   return any == 0;
@@ -104,22 +105,25 @@ __global__ void k_per_level(const PerView v, int l) {
   if (j < v.n[l]) per_node(v, l, j, threadIdx.x & 31);
 }
 
-// A flush of n deferred add()s at pos0: those slots get max_priority^alpha, and the leaves of [pos0, pos0 + n + hist)
-// (mod size) are re-derived: the written slots, and the slots that entered the [current, current + hist) window.  No
-// other slot's acceptance can change.  Then their ancestors, level by level.  One CTA.
+// A flush of n deferred add()s at pos0: those slots get max_priority^alpha, and the leaves of
+// [pos0 - (nstep - 1), pos0 + n + hist) (mod size) are re-derived: the written slots, the slots whose window
+// [i - hist, i + nstep - 1] held the old write pointer or holds the new one, and the slots that became drawable as
+// count grew past i + nstep - 1.  No other slot's acceptance can change.  Then their ancestors, level by level.  One
+// CTA.
 constexpr int kPerAddThreads = 256;
 __global__ void __launch_bounds__(kPerAddThreads) k_per_add(const PerView v, const double* maxp, double alpha,
                                                             int64_t pos0, int n) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int touched = n + v.hist;
+  const int64_t touched = min(int64_t(n) + v.hist + v.nstep - 1, v.size);
+  const int64_t first = pos0 - (v.nstep - 1) + v.size;   // + size: the leaves before pos0 may lie across the wrap
   const int64_t count = v.cursor[0], current = v.cursor[1];
   const double p = pow(*maxp, alpha);
   for (int t = tid; t < n; t += kPerAddThreads) v.prio[(pos0 + t) % v.size] = p;
   __syncthreads();
-  for (int t = tid; t < touched; t += kPerAddThreads) per_set_leaf(v, (pos0 + t) % v.size, count, current);
+  for (int64_t t = tid; t < touched; t += kPerAddThreads) per_set_leaf(v, (first + t) % v.size, count, current);
   __syncthreads();
   for (int l = 1; l < v.nlev; ++l) {
-    for (int t = warp; t < touched; t += kPerAddThreads / 32) per_node(v, l, ((pos0 + t) % v.size) >> (5 * l), lane);
+    for (int64_t t = warp; t < touched; t += kPerAddThreads / 32) per_node(v, l, ((first + t) % v.size) >> (5 * l), lane);
     __syncthreads();
   }
 }

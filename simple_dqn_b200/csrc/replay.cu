@@ -63,7 +63,7 @@ constexpr int kSampleThreads = 256;
 
 __global__ void __launch_bounds__(kSampleThreads, 1)
 k_sample(uint32_t* __restrict__ mt_state, const uint8_t* __restrict__ terminals,
-         const int64_t* __restrict__ cursor, int hist, int batch, int32_t* __restrict__ idx_out,
+         const int64_t* __restrict__ cursor, int hist, int nstep, int batch, int32_t* __restrict__ idx_out,
          uint32_t* __restrict__ words_out, const KTrace kt) {
   __shared__ SampleShared sh;
   const int tid = threadIdx.x;
@@ -75,7 +75,8 @@ k_sample(uint32_t* __restrict__ mt_state, const uint8_t* __restrict__ terminals,
   uint32_t* nxt = mt_state + ((k + 1u) & 1u) * kMtSlot;
   for (int i = tid; i < kMtN + 1; i += kSampleThreads) sh.mt[i] = cur[i];
   __syncthreads();
-  const uint32_t words = sample_block(sh, terminals, cursor[0], cursor[1], hist, batch, idx_out, tid, kSampleThreads);
+  const uint32_t words =
+      sample_block(sh, terminals, cursor[0], cursor[1], hist, nstep, batch, idx_out, tid, kSampleThreads);
   for (int i = tid; i < kMtN + 1; i += kSampleThreads) nxt[i] = sh.mt[i];
   if (tid == 0) {
     words_out[0] = words;
@@ -151,7 +152,8 @@ int launch_sample(b200dqn_replay* r, cudaStream_t st) {
   if (frc) return frc;
   if (r->per_on) return launch_sample_per(r, st);
   B2_CHECK_CUDA(launch_pdl(k_sample, dim3(1), dim3(kSampleThreads), 0, st, r->d_mt, (const uint8_t*)r->d_terminals,
-                           (const int64_t*)r->d_cursor, r->hist, r->batch, r->d_idx, r->d_words, ktrace_slot("sample")));
+                           (const int64_t*)r->d_cursor, r->hist, r->nstep, r->batch, r->d_idx, r->d_words,
+                           ktrace_slot("sample")));
   B2_PROF("sample", st);
   return B200DQN_OK;
 }
@@ -162,11 +164,14 @@ int launch_sample(b200dqn_replay* r, cudaStream_t st) {
 // into shared memory with one TMA bulk copy (UBLKCP) and pushes it back out with bulk stores to
 // the prestates slot f (f < hist) and the poststates slot f-1 (f >= 1): each ring byte is read
 // from HBM exactly once.  Frame sizes that are not a multiple of 16 B take the byte-loop path.
+// n-step returns (nstep = N): the span is index-hist .. index+N-1 (hist+N frames), frame f goes to the prestates if
+// f < hist and to poststate slot f-N if f >= N, and the rewards and terminals of index .. index+N-1 are staged as
+// [batch][N].  A CTA whose frame is in neither state (hist <= f < N) has nothing to copy.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(128)
 k_gather(const uint8_t* __restrict__ screens, const uint8_t* __restrict__ actions,
          const int64_t* __restrict__ rewards, const uint8_t* __restrict__ terminals,
-         const int32_t* __restrict__ idx, int hist, uint32_t frame_bytes, uint8_t* __restrict__ pre,
+         const int32_t* __restrict__ idx, int hist, int nstep, uint32_t frame_bytes, uint8_t* __restrict__ pre,
          uint8_t* __restrict__ post, uint8_t* __restrict__ mb_actions, int64_t* __restrict__ mb_rewards,
          uint8_t* __restrict__ mb_terminals, int use_tma) {
   extern __shared__ __align__(128) uint8_t s_frame[];
@@ -175,13 +180,17 @@ k_gather(const uint8_t* __restrict__ screens, const uint8_t* __restrict__ action
   const int64_t index = idx[k];
   const uint8_t* src = screens + (index - hist + f) * static_cast<int64_t>(frame_bytes);
   uint8_t* dst_pre = pre + (static_cast<int64_t>(k) * hist + f) * frame_bytes;
-  uint8_t* dst_post = post + (static_cast<int64_t>(k) * hist + (f - 1)) * frame_bytes;
+  uint8_t* dst_post = post + (static_cast<int64_t>(k) * hist + (f - nstep)) * frame_bytes;
 
-  if (f == 0 && threadIdx.x == 32) {
-    mb_actions[k] = actions[index];
-    mb_rewards[k] = rewards[index];
-    mb_terminals[k] = terminals[index];
+  if (f == 0 && threadIdx.x == 32) mb_actions[k] = actions[index];
+  if (f == 0 && threadIdx.x >= 32 && threadIdx.x < 64) {
+    for (int j = threadIdx.x - 32; j < nstep; j += 32) {
+      mb_rewards[int64_t(k) * nstep + j] = rewards[index + j];
+      mb_terminals[int64_t(k) * nstep + j] = terminals[index + j];
+    }
   }
+  const bool to_pre = f < hist, to_post = f >= nstep;
+  if (!to_pre && !to_post) return;
   if (use_tma) {
     if (threadIdx.x == 0) {
       mbar_init(&bar, 1);
@@ -189,16 +198,16 @@ k_gather(const uint8_t* __restrict__ screens, const uint8_t* __restrict__ action
       mbar_arrive_expect_tx(&bar, frame_bytes);
       tma_bulk_g2s(s_frame, src, frame_bytes, &bar);
       mbar_wait(&bar, 0);
-      if (f < hist) tma_bulk_s2g(dst_pre, s_frame, frame_bytes);
-      if (f >= 1) tma_bulk_s2g(dst_post, s_frame, frame_bytes);
+      if (to_pre) tma_bulk_s2g(dst_pre, s_frame, frame_bytes);
+      if (to_post) tma_bulk_s2g(dst_post, s_frame, frame_bytes);
       tma_bulk_commit();
       tma_bulk_wait_read_all();  // smem may be released once the reads are done
     }
   } else {
     for (uint32_t i = threadIdx.x; i < frame_bytes; i += blockDim.x) {
       const uint8_t v = src[i];
-      if (f < hist) dst_pre[i] = v;
-      if (f >= 1) dst_post[i] = v;
+      if (to_pre) dst_pre[i] = v;
+      if (to_post) dst_post[i] = v;
     }
   }
 }
@@ -439,8 +448,9 @@ extern "C" int b200dqn_replay_get_rng(b200dqn_replay* r, uint32_t host_mt625[625
 
 extern "C" int b200dqn_replay_sample(b200dqn_replay* r, void* stream) {
   B2_REQUIRE(r, B200DQN_EINVAL, "null replay");
-  B2_REQUIRE(r->count > r->hist, B200DQN_ESTATE, "getMinibatch: count (%lld) must exceed history_length (%d)",
-             (long long)r->count, r->hist);  // :52
+  B2_REQUIRE(r->count >= r->hist + r->nstep, B200DQN_ESTATE,
+             "getMinibatch: count (%lld) must be at least history_length (%d) + n_step (%d)", (long long)r->count,
+             r->hist, r->nstep);  // :52 at n_step 1
   B2_REQUIRE(r->rng_set, B200DQN_ESTATE, "replay_sample: call b200dqn_replay_set_rng first");
   DeviceGuard g(r->device);
   int rc = launch_sample(r, as_stream(stream));
@@ -462,8 +472,8 @@ extern "C" int b200dqn_replay_sample_sync(b200dqn_replay* r, uint32_t* host_word
 extern "C" int b200dqn_replay_set_indexes(b200dqn_replay* r, const int32_t* host_indexes, void* stream) {
   B2_REQUIRE(r && host_indexes, B200DQN_EINVAL, "replay_set_indexes: null argument");
   for (int i = 0; i < r->batch; ++i)
-    B2_REQUIRE(host_indexes[i] >= r->hist && host_indexes[i] < r->size, B200DQN_EINVAL,
-               "replay_set_indexes: index %d out of [hist, size)", host_indexes[i]);
+    B2_REQUIRE(host_indexes[i] >= r->hist && host_indexes[i] <= r->size - r->nstep, B200DQN_EINVAL,
+               "replay_set_indexes: index %d out of [hist, size - n_step]", host_indexes[i]);
   DeviceGuard g(r->device);
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemcpyAsync(r->d_idx, host_indexes, r->batch * sizeof(int32_t), cudaMemcpyHostToDevice, st));
@@ -481,9 +491,9 @@ extern "C" int b200dqn_replay_gather(b200dqn_replay* r, void* stream) {
   DeviceGuard g(r->device);
   { int frc = replay_flush(r, as_stream(stream)); if (frc) return frc; }
   const int use_tma = (r->frame_bytes % 16 == 0 && r->frame_bytes <= r->gather_smem) ? 1 : 0;
-  dim3 grid(r->batch, r->hist + 1);
+  dim3 grid(r->batch, r->hist + r->nstep);
   k_gather<<<grid, 128, use_tma ? r->frame_bytes : 0, as_stream(stream)>>>(
-      r->d_screens, r->d_actions, r->d_rewards, r->d_terminals, r->d_idx, r->hist, uint32_t(r->frame_bytes),
+      r->d_screens, r->d_actions, r->d_rewards, r->d_terminals, r->d_idx, r->hist, r->nstep, uint32_t(r->frame_bytes),
       r->d_pre, r->d_post, r->d_mb_actions, r->d_mb_rewards, r->d_mb_terminals, use_tma);
   B2_LAUNCH_CHECK();
   B2_PROF("gather", as_stream(stream));
@@ -500,15 +510,44 @@ extern "C" int b200dqn_replay_read_minibatch(b200dqn_replay* r, uint8_t* host_pr
   if (host_pre) B2_CHECK_CUDA(cudaMemcpyAsync(host_pre, r->d_pre, state_bytes, cudaMemcpyDeviceToHost, st));
   if (host_post) B2_CHECK_CUDA(cudaMemcpyAsync(host_post, r->d_post, state_bytes, cudaMemcpyDeviceToHost, st));
   if (host_actions) B2_CHECK_CUDA(cudaMemcpyAsync(host_actions, r->d_mb_actions, r->batch, cudaMemcpyDeviceToHost, st));
+  const size_t nmb = size_t(r->batch) * r->nstep;   // (batch, n_step) rewards and terminals
   if (host_rewards)
-    B2_CHECK_CUDA(cudaMemcpyAsync(host_rewards, r->d_mb_rewards, r->batch * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    B2_CHECK_CUDA(cudaMemcpyAsync(host_rewards, r->d_mb_rewards, nmb * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   if (host_terminals)
-    B2_CHECK_CUDA(cudaMemcpyAsync(host_terminals, r->d_mb_terminals, r->batch, cudaMemcpyDeviceToHost, st));
+    B2_CHECK_CUDA(cudaMemcpyAsync(host_terminals, r->d_mb_terminals, nmb, cudaMemcpyDeviceToHost, st));
   if (host_indexes)
     B2_CHECK_CUDA(cudaMemcpyAsync(host_indexes, r->d_idx, r->batch * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (host_words_consumed)
     B2_CHECK_CUDA(cudaMemcpyAsync(host_words_consumed, r->d_words, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   B2_CHECK_CUDA(cudaStreamSynchronize(st));
+  return B200DQN_OK;
+}
+
+extern "C" int b200dqn_replay_set_n_step(b200dqn_replay* r, int n) {
+  B2_REQUIRE(r, B200DQN_EINVAL, "null replay");
+  B2_REQUIRE(n >= 1 && int64_t(r->hist) + n <= r->size, B200DQN_EINVAL,
+             "replay_set_n_step: need 1 <= n_step and history_length (%d) + n_step (%d) <= size (%lld)", r->hist, n,
+             (long long)r->size);
+  if (n == r->nstep) return B200DQN_OK;
+  DeviceGuard g(r->device);
+  B2_CHECK_CUDA(cudaDeviceSynchronize());   // nothing in flight reads the staged rewards and terminals
+  { int frc = replay_flush(r, nullptr); if (frc) return frc; }
+  int64_t* rew = nullptr;
+  uint8_t* term = nullptr;
+  B2_CHECK_CUDA(cudaMalloc(&rew, size_t(r->batch) * n * sizeof(int64_t)));
+  B2_CHECK_CUDA(cudaMalloc(&term, size_t(r->batch) * n));
+  B2_CHECK_CUDA(cudaMemset(rew, 0, size_t(r->batch) * n * sizeof(int64_t)));
+  B2_CHECK_CUDA(cudaMemset(term, 0, size_t(r->batch) * n));
+  cudaFree(r->d_mb_rewards);
+  cudaFree(r->d_mb_terminals);
+  r->d_mb_rewards = rew;
+  r->d_mb_terminals = term;
+  r->nstep = n;   // the nets' step graphs compare it
+  if (r->per_on) {   // the drawable set follows the window
+    int rc = per_rebuild(r, 0, 0, false, nullptr);
+    if (rc) return rc;
+  }
+  B2_CHECK_CUDA(cudaDeviceSynchronize());
   return B200DQN_OK;
 }
 
@@ -526,8 +565,8 @@ extern "C" int b200dqn_replay_device_ptr(b200dqn_replay* r, int which, void** de
     case B200DQN_PTR_PRESTATES: p = r->d_pre; b = state_bytes; break;
     case B200DQN_PTR_POSTSTATES: p = r->d_post; b = state_bytes; break;
     case B200DQN_PTR_MB_ACTIONS: p = r->d_mb_actions; b = r->batch; break;
-    case B200DQN_PTR_MB_REWARDS: p = r->d_mb_rewards; b = r->batch * sizeof(int64_t); break;
-    case B200DQN_PTR_MB_TERMINALS: p = r->d_mb_terminals; b = r->batch; break;
+    case B200DQN_PTR_MB_REWARDS: p = r->d_mb_rewards; b = size_t(r->batch) * r->nstep * sizeof(int64_t); break;
+    case B200DQN_PTR_MB_TERMINALS: p = r->d_mb_terminals; b = size_t(r->batch) * r->nstep; break;
     case B200DQN_PTR_INDEXES: p = r->d_idx; b = r->batch * sizeof(int32_t); break;
     case B200DQN_PTR_WORDS_CONSUMED: p = r->d_words; b = 2 * sizeof(uint32_t); break;
     case B200DQN_PTR_MT_STATE: p = r->mt_slot_ptr(); b = 625 * sizeof(uint32_t); break;

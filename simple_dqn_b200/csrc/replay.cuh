@@ -39,8 +39,11 @@ struct b200dqn_replay {
   uint8_t* d_pre = nullptr;        // [batch][hist][h][w]
   uint8_t* d_post = nullptr;       // [batch][hist][h][w]
   uint8_t* d_mb_actions = nullptr;
-  int64_t* d_mb_rewards = nullptr;
-  uint8_t* d_mb_terminals = nullptr;
+  int64_t* d_mb_rewards = nullptr;   // [batch][nstep]: rewards[index .. index + nstep - 1]
+  uint8_t* d_mb_terminals = nullptr; // [batch][nstep]
+  // n-step returns (b200dqn_replay_set_n_step): a sample is the window [index - hist, index + nstep - 1]; the
+  // poststate is getState(index + nstep - 1).  Step graphs capture it (shifts, head), so they compare it.
+  int nstep = 1;
 
   // pinned staging slots (small host<->device landing pads)
   static constexpr int kSlots = 16;
@@ -143,12 +146,14 @@ __device__ __forceinline__ void mt_regenerate(uint32_t* mt, int tid, int nthread
 // Every thread of the CTA calls this (nthreads = blockDim.x, a multiple of 32, <= 384; __syncthreads inside).  sh.mt
 // holds the state on entry and the advanced state (position in [624]) on return; accepted indexes go to idx_out
 // (shared or global), in acceptance order.  Returns the number of 32-bit words consumed.
+// n-step returns (nstep = N >= 1; count >= hist + N): the trial is randint(hist, count - N), and a sample is rejected
+// when its window [index - hist, index + N - 1] straddles the write pointer; at N = 1 this is :59 and :61 exactly.
 __device__ __forceinline__ uint32_t sample_block(SampleShared& sh, const uint8_t* __restrict__ terminals, int64_t count,
-                                                 int64_t current, int hist, int batch, int32_t* idx_out, int tid,
-                                                 int nthreads) {
+                                                 int64_t current, int hist, int nstep, int batch, int32_t* idx_out,
+                                                 int tid, int nthreads) {
   const int lane = tid & 31, wid = tid >> 5, nwarps = nthreads >> 5;
   uint32_t* mt = sh.mt;
-  const uint32_t n = static_cast<uint32_t>(count - hist);  // width of randrange(hist, count)
+  const uint32_t n = static_cast<uint32_t>(count - hist - nstep + 1);  // width of randrange(hist, count - N + 1)
   const int kbits = 32 - __clz(n);                         // n.bit_length(), n >= 1
   int pos = static_cast<int>(mt[kMtN]);
   int accepted = 0;
@@ -165,7 +170,7 @@ __device__ __forceinline__ uint32_t sample_block(SampleShared& sh, const uint8_t
       const uint32_t r = mt_temper(mt[pos + tid]) >> (32 - kbits);
       if (r < n) {
         index = hist + static_cast<int>(r);
-        ok = !(index >= current && index - hist < current);  // :61 wraps over the write pointer
+        ok = !(index + nstep - 1 >= current && index - hist < current);  // :61 wraps over the write pointer
         // :65 episode end — all `hist` bytes are requested at once (no short-circuit: one memory latency, not four)
         unsigned any = 0;
         for (int j = 1; j <= hist; ++j) any |= terminals[index - j];

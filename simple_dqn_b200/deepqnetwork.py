@@ -224,9 +224,10 @@ class DeepQNetwork:
 
     def train(self, minibatch, epoch=0):
         """deepqnetwork.py:107-172.  A pristine DeviceMinibatch is trained in place from the ring, and so is one from a
-        prioritized ring even once it has been looked at (the importance weights and the priority update live there).
-        A host tuple is always the uniform, unweighted step."""
-        if isinstance(minibatch, DeviceMinibatch) and (not minibatch.materialised or minibatch._mem.prioritized):
+        prioritized or n-step ring even once it has been looked at (the importance weights, the priority update and
+        the n-step window live there).  A host tuple is always the uniform, unweighted one-step step."""
+        if isinstance(minibatch, DeviceMinibatch) and (not minibatch.materialised or minibatch._mem.prioritized or
+                                                       minibatch._mem.n_step > 1):
             minibatch._check_current()
             mem = minibatch._mem
             cost = C.c_float()

@@ -151,6 +151,10 @@ class ReplayMemory:
                                getattr(args, "train_frequency", 4) * getattr(args, "train_repeat", 1))
         if getattr(args, "prioritized_replay", False):
             self.set_prioritized(True)
+        # n-step returns (Hessel et al., 2018): a new capability, one-step (the reference) unless args.n_step > 1
+        self.n_step = 1
+        if getattr(args, "n_step", 1) != 1:
+            self.set_n_step(args.n_step)
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -235,6 +239,16 @@ class ReplayMemory:
         p, b = C.c_void_p(), C.c_size_t()
         L.call("b200dqn_replay_device_ptr", self._h, L.PTR_PRIORITIES, C.byref(p), C.byref(b))
         return b.value > 0
+
+    # ---- n-step returns
+    def set_n_step(self, n):
+        """Train on n-step returns (include/b200dqn.h, b200dqn_replay_set_n_step): a sample's poststate is
+        getState(index + n - 1) and its target sums the discounted rewards of index .. index + n - 1, cut at the first
+        terminal.  n = 1 is the reference's step.  Raises AssertionError unless 1 <= n and history_length + n <= size.
+        A minibatch handed out before the switch can no longer be trained."""
+        L.call("b200dqn_replay_set_n_step", self._h, int(n))
+        self.n_step = int(n)
+        self._sample_ticket += 1
 
     # ---- reference methods
     def add(self, action, reward, screen, terminal):
@@ -322,7 +336,7 @@ class ReplayMemory:
         """The index draw of getMinibatch (:55-69) on the device.  rng="python": in lock-step with the process-global
         stream — its state is uploaded only if somebody else drew from `random` since our last sample, and the host
         is advanced by exactly the number of 32-bit words the device consumed."""
-        assert self.count > self.history_length                        # :52
+        assert self.count >= self.history_length + self.n_step         # :52 at n_step 1
         self._sample_now()
         self._sample_ticket += 1
 
@@ -333,10 +347,13 @@ class ReplayMemory:
         self._sample_ticket += 1
 
     def _gather_to_host(self):
+        """The reference's 5-tuple; with n_step > 1 rewards and terminals are (batch, n_step) windows starting at the
+        index, and the poststates are getState(index + n_step - 1)."""
         L.call("b200dqn_replay_gather", self._h, self._stream)
+        mb = (self.batch_size,) if self.n_step == 1 else (self.batch_size, self.n_step)
         actions = np.empty(self.batch_size, dtype=np.uint8)
-        rewards = np.empty(self.batch_size, dtype=np.int64)
-        terminals = np.empty(self.batch_size, dtype=np.uint8)
+        rewards = np.empty(mb, dtype=np.int64)
+        terminals = np.empty(mb, dtype=np.uint8)
         indexes = np.empty(self.batch_size, dtype=np.int32)
         words = np.zeros(1, dtype=np.uint32)
         L.call("b200dqn_replay_read_minibatch", self._h, L.np_ptr(self.prestates), L.np_ptr(actions),
@@ -348,11 +365,12 @@ class ReplayMemory:
 
     def getMinibatch(self):
         # replay_memory.py:50-79
-        if self.device_minibatch or self.prioritized:   # a prioritized minibatch must train from the ring
+        # a prioritized or n-step minibatch must train from the ring
+        if self.device_minibatch or self.prioritized or self.n_step > 1:
             # agent.py:112-114 is `mb = mem.getMinibatch(); net.train(mb, epoch)` with nothing in between: hand out
             # a handle and let the draw ride in train()'s graph (one launch, one wait per step).  Anything else that
             # looks at the handle (statistics.py:85) triggers the draw on the spot.
-            assert self.count > self.history_length                    # :52
+            assert self.count >= self.history_length + self.n_step     # :52 at n_step 1
             self._sample_ticket += 1
             return DeviceMinibatch(self, sampled=False)
         self.sample()

@@ -13,6 +13,7 @@ B = int(os.environ.get("BATCH", "32"))
 HIST = int(os.environ.get("HIST", "4"))   # --history_length: frames per state, conv1's input channels
 DOUBLE = os.environ.get("DOUBLE", "0") == "1"   # the Double DQN target (a third forward slot)
 PER = os.environ.get("PER", "0") == "1"         # prioritized replay (tree-descent sampler + priority update)
+NSTEP = int(os.environ.get("NSTEP", "1"))       # n-step returns (poststates N frames on, discounted reward sum)
 
 
 def args():
@@ -20,6 +21,7 @@ def args():
     a.history_length = HIST
     a.double_dqn = DOUBLE
     a.prioritized_replay = PER
+    a.n_step = NSTEP
     return a
 
 
@@ -45,5 +47,5 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("batch %d hist %d double %d per %d period_us min %.2f median %.2f  all %s" % (
-    B, HIST, DOUBLE, PER, min(res), float(np.median(res)), " ".join("%.2f" % r for r in res)))
+print("batch %d hist %d double %d per %d nstep %d period_us min %.2f median %.2f  all %s" % (
+    B, HIST, DOUBLE, PER, NSTEP, min(res), float(np.median(res)), " ".join("%.2f" % r for r in res)))
