@@ -174,8 +174,7 @@ int b200dqn_replay_device_ptr(b200dqn_replay* r, int which, void** dev_ptr, size
  * Switching on sets every stored priority and max_priority to 1 and builds the trees from the ring as it stands
  * (the first switch-on allocates them).  Either switch rebuilds the captured step graphs of the nets that train from
  * r.  A draw from a ring with no drawable slot reports ESTATE at the next result poll.  Train steps from a
- * prioritized ring return ENOTIMPL for data-parallel learners and, on the tensor-core engine, under
- * B200DQN_CONV1=tma.  Synchronises. */
+ * prioritized ring return ENOTIMPL for data-parallel learners.  Synchronises. */
 int b200dqn_replay_set_prioritized(b200dqn_replay* r, int on, double alpha, double beta0, double beta_steps,
                                    double eps);
 
@@ -189,8 +188,8 @@ int b200dqn_replay_set_prioritized(b200dqn_replay* r, int on, double alpha, doub
  *     R = sum_{k<m} gamma^k clip(rewards[index + k]), m the first terminal (or N), in fp64 without contraction;
  *   - the prioritized sum tree masks the same slots.
  * Host-supplied minibatches (b200dqn_net_train / _train_device) stay one-step.  Train steps from a ring with N > 1
- * return ENOTIMPL for data-parallel learners and, on the tensor-core engine, under B200DQN_CONV1=tma; so does
- * b200dqn_net_comm_init on a net whose last train step used such a ring.  Switching rebuilds the captured step graphs
+ * return ENOTIMPL for data-parallel learners; so does b200dqn_net_comm_init on a net whose last train step used such
+ * a ring.  Switching rebuilds the captured step graphs
  * of the nets that train from r.  EINVAL unless 1 <= n and hist + n <= size.  Synchronises. */
 int b200dqn_replay_set_n_step(b200dqn_replay* r, int n);
 
@@ -347,8 +346,8 @@ int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
  * in place of max_a Q_target(s'_i, a) (deepqnetwork.py:124,140-143); terminals, reward and error clipping, the cost,
  * the backward and the optimizers are unchanged, and predict is not affected.  The train-step forward runs the online
  * network on the poststates as a third slot of its launches.  The first switch-on allocates that slot's buffers
- * (synchronises the device).  Captured step graphs are rebuilt.  ENOTIMPL once b200dqn_net_comm_init has run and, on
- * the tensor-core engine, under B200DQN_CONV1=tma; b200dqn_net_comm_init returns ENOTIMPL while it is on. */
+ * (synchronises the device).  Captured step graphs are rebuilt.  ENOTIMPL once b200dqn_net_comm_init has run;
+ * b200dqn_net_comm_init returns ENOTIMPL while it is on. */
 int b200dqn_net_set_double_q(b200dqn_net* n, int on);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
 int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream);

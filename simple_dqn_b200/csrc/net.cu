@@ -399,7 +399,6 @@ struct FrameSource {
   const uint8_t* src[2];
   const int32_t* idx[2];
   int shift[2];
-  int64_t nframes[2];   // frames in each source array
 };
 
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
@@ -411,7 +410,7 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
   int rc;
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
     // one GPU: the forward launches are links of the critical chain (umma_forward picks the ones that release early)
-    rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.nframes, nets, rows, st, n->world == 1);
+    rc = umma_forward(n, fs.src, fs.idx, fs.shift, nets, rows, st, n->world == 1);
     if (rc) return rc;
   } else {
     {
@@ -980,9 +979,6 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
              "net_create: unknown math_mode %d", cfg->math_mode);
   B2_REQUIRE(cfg->optimizer >= B200DQN_OPT_RMSPROP && cfg->optimizer <= B200DQN_OPT_ADADELTA, B200DQN_EINVAL,
              "net_create: unknown optimizer %d", cfg->optimizer);   // deepqnetwork.py:61 `assert false, "Unknown optimizer"`
-  B2_REQUIRE(cfg->math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma() || cfg->history_length == kHist,
-             B200DQN_ENOTIMPL, "net_create: the B200DQN_CONV1=tma conv1 gathers %d-frame windows only (history_length %d)",
-             kHist, cfg->history_length);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -1209,8 +1205,7 @@ extern "C" int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_sta
              "net_predict_device: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
-  const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
-  FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
+  FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}};
   HeadTrainArgs no_td{};
   int rc = forward(n, fs, 1, live_rows, st, no_td);
   if (rc) return rc;
@@ -1258,8 +1253,7 @@ extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* de
     if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }
     cudaGraph_t graph = nullptr;
     B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
-    FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
+    FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}};
     HeadTrainArgs no_td{};
     int rc = forward(n, fs, 1, live_rows, st, no_td);
     if (!rc) {
@@ -1307,8 +1301,7 @@ extern "C" int b200dqn_net_train_device(b200dqn_net* n, const uint8_t* dev_pre, 
   B2_REQUIRE(n && dev_pre && dev_actions && dev_rewards && dev_post && dev_terminals, B200DQN_EINVAL,
              "net_train_device: null argument");
   DeviceGuard g(n->device);
-  const int64_t state_frames = int64_t(n->nb) * n->cfg.history_length;
-  FrameSource fs{{dev_pre, dev_post}, {n->d_iota4, n->d_iota4}, {0, 0}, {state_frames, state_frames}};
+  FrameSource fs{{dev_pre, dev_post}, {n->d_iota4, n->d_iota4}, {0, 0}};
   B2_TRY(train_step(n, fs, dev_actions, dev_rewards, dev_terminals, n->d_iota1, as_stream(stream)));
   n->train_iterations += 1;
   return B200DQN_OK;
@@ -1353,8 +1346,6 @@ static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
   if (r->per_on) {
     B2_REQUIRE(n->world == 1 && !n->nccl_comm, B200DQN_ENOTIMPL,
                "prioritized replay is implemented for a single learner only (comm_init has run)");
-    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
-               "prioritized replay: the B200DQN_CONV1=tma conv1 is not supported");
     if (!n->d_td_err) {   // the first step on a prioritized ring (before any graph capture)
       DeviceGuard g(n->device);
       B2_CHECK_CUDA(cudaMalloc(&n->d_td_err, n->nb * sizeof(float)));
@@ -1364,8 +1355,6 @@ static int check_fusable(b200dqn_net* n, b200dqn_replay* r) {
   if (r->nstep > 1) {
     B2_REQUIRE(n->world == 1 && !n->nccl_comm, B200DQN_ENOTIMPL,
                "n-step returns are implemented for a single learner only (comm_init has run)");
-    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
-               "n-step returns: the B200DQN_CONV1=tma conv1 draws its own 4-frame windows and is not supported");
   }
   n->ring_nstep = r->nstep;
   return B200DQN_OK;
@@ -1375,7 +1364,7 @@ static int train_on_ring(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   const int32_t* my_idx = r->d_idx + n->rank * n->nb;  // this rank's slice of the global minibatch
   // prestates = frames index-H .. index-1, poststates = index-H+N .. index+N-1 (src/replay_memory.py:71-72 at N = 1)
   const int hist = n->cfg.history_length;
-  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-hist, -hist + r->nstep}, {r->size, r->size}};
+  FrameSource fs{{r->d_screens, r->d_screens}, {my_idx, my_idx}, {-hist, -hist + r->nstep}};
   n->step_replay = r;
   const int rc = train_step(n, fs, r->d_actions, r->d_rewards, r->d_terminals, my_idx, st);
   n->step_replay = nullptr;
@@ -1640,8 +1629,6 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   if (on) {
     B2_REQUIRE(!n->nccl_comm, B200DQN_ENOTIMPL,
                "net_set_double_q: the Double DQN target is implemented for a single learner only (comm_init has run)");
-    B2_REQUIRE(n->cfg.math_mode != B200DQN_MATH_TCGEN05 || !umma_conv1_tma(), B200DQN_ENOTIMPL,
-               "net_set_double_q: the B200DQN_CONV1=tma conv1 has no Double DQN slot");
     B2_TRY(double_q_alloc(n));
   }
   n->double_q = on != 0;

@@ -8,7 +8,6 @@
 #include "umma.cuh"
 #include "umma2.cuh"
 #include "umma_mn.cuh"
-#include "conv1_tma.cuh"
 
 namespace b200 {
 
@@ -620,23 +619,15 @@ struct WConv1Wgrad {
   PlanePair dz16;          // dZ1 [rows][20][20][32]
   float* part;             // [splits][64 H][32]
   int rows, kb_per_split;
-  int tile_rows;           // live rows per 128-row im2col tile: 128 (dense tiling) or 100 (conv1_tma.cuh: 4 tiles/sample)
   __device__ int M(int) const { return 64 * H; }
   __device__ int N(int) const { return kC1; }
-  __device__ int total_kb() const {
-    return tile_rows == 128 ? (rows * kP1 * kP1 + 63) / 64 : rows * conv1tma::kTilesPerSample * 2;
-  }
   __device__ void krange(int z, int& kb, int& ke) const {
-    const int total = total_kb();
+    const int total = (rows * kP1 * kP1 + 63) / 64;
     kb = min(z * kb_per_split, total);
     ke = min(kb + kb_per_split, total);
   }
-  // kpix indexes the padded im2col rows; n = the real pixel (row of dZ1)
-  __device__ umma_mn::PixCtx pix(int, int kpix) const {
-    if (tile_rows == 128) return {kpix, 0, 0, kpix < rows * kP1 * kP1};
-    const int tile = kpix >> 7, local = kpix & 127;
-    return {tile * tile_rows + local, 0, 0, local < tile_rows && tile < rows * conv1tma::kTilesPerSample};
-  }
+  // kpix = the im2col row = the output pixel (row of dZ1); the last 128-row tile is padded
+  __device__ umma_mn::PixCtx pix(int, int kpix) const { return {kpix, 0, 0, kpix < rows * kP1 * kP1}; }
   __device__ const uint8_t* a_sub(int, int c, int kb) const {   // kb = global 64-pixel block; nullptr: c >= H
     if (c >= H) return nullptr;
     return im2col + (int64_t(kb >> 1) * H + c) * (128 * 128) + (kb & 1) * (64 * 128);
@@ -1005,19 +996,10 @@ static inline int fc1_splits_for(int rows) {
 }
 constexpr int kUWgradKb = 4;      // minimum k-blocks (of 64 pixels) per wgrad split
 
-// conv1 gathers its frames on the register path of umma2.cuh (V2Conv1Fwd, plain loads) unless B200DQN_CONV1=tma selects
-// the tensor-map TMA twin (conv1_tma.cuh).  On an H100 80GB HBM3 the register path made the step 3 % (700 W) to 5 %
-// (400 W) faster at batch 32 and 5-6 % faster at batch 256.
-static const bool g_conv1_tma = getenv("B200DQN_CONV1") && strcmp(getenv("B200DQN_CONV1"), "tma") == 0;
-// rows of conv1's im2col image (= conv1_wgrad's reduction length): dense 128-row tiles on the register path, 4 tiles
-// of 100 live rows per sample on the TMA path
-static inline int conv1_pixels_padded(int rows) { return g_conv1_tma ? rows * conv1tma::kTilesPerSample * 128 : rows * kP1 * kP1; }
-bool umma_conv1_tma() { return g_conv1_tma; }
-
 // k-blocks (of 64 pixels) per wgrad split: at least kUWgradKb, and few enough splits (<= 48) for the
 // one-pass reduction of k_opt_conv
 int umma_wgrad_kb(int layer, int rows) {
-  const int kred = layer == 0 ? conv1_pixels_padded(rows) : layer == 1 ? rows * kP2 * kP2 : rows * kP3 * kP3;
+  const int kred = layer == 0 ? rows * kP1 * kP1 : layer == 1 ? rows * kP2 * kP2 : rows * kP3 * kP3;
   const int kbs = (kred + 63) / 64;
   int per = (kbs + 47) / 48;
   // conv1: at least 8 k-blocks per split (25 splits at batch 32).  On an H100 80GB HBM3 (400 W) the batch-32 step took
@@ -1027,7 +1009,7 @@ int umma_wgrad_kb(int layer, int rows) {
   return per > kUWgradKb ? per : kUWgradKb;
 }
 int umma_wgrad_splits(int layer, int rows) {
-  const int kred = layer == 0 ? conv1_pixels_padded(rows) : layer == 1 ? rows * kP2 * kP2 : rows * kP3 * kP3;
+  const int kred = layer == 0 ? rows * kP1 * kP1 : layer == 1 ? rows * kP2 * kP2 : rows * kP3 * kP3;
   const int kbs = (kred + 63) / 64, per = umma_wgrad_kb(layer, rows);
   return (kbs + per - 1) / per;
 }
@@ -1063,7 +1045,7 @@ int umma_net_init(b200dqn_net* n) {
     }
   }
   B2_CHECK_CUDA(cudaMalloc(&u->im2col1,
-                           int64_t((conv1_pixels_padded(nb) + 127) / 128) * n->cfg.history_length * 128 * 128));
+                           int64_t((nb * kP1 * kP1 + 127) / 128) * n->cfg.history_length * 128 * 128));
   u->img_dgr[0] = u->img_fwd[0][3];   // fc1: ONE row-oriented image serves the dgrad (K-major) and the forward (MN-major)
   const int64_t dgr_bytes[3] = {0, int64_t(kK3 / 64) * kC2 * 256, int64_t(4) * (256 / 64) * kC1 * 256};
   for (int i = 1; i < 3; ++i) {
@@ -1124,56 +1106,26 @@ void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
 }
 
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 const int64_t nframes[2], int nets, int rows, cudaStream_t st, bool release_early) {
+                 int nets, int rows, cudaStream_t st, bool release_early) {
   // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
   // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.  conv23_fwd keeps
   // its own release point.
   UmmaState* u = ust(n);
-  int rc;
   auto planes = [&](int i, int z) { return PlanePair{u->h16[i][z], u->h_elems[i]}; };
-  if (g_conv1_tma) {
-    // frames by tensor-map TMA.  Ring case (both states out of one frame array, poststates one frame later): ONE
-    // 5-frame window per CTA serves both networks.
-    conv1tma::Params p{};
-    const bool shared5 = nets == 2 && src[0] == src[1] && idx[0] == idx[1] && shift[1] == shift[0] + 1;
+  int rc = with_hist(n->cfg.history_length, [&](auto h) {
+    constexpr int H = decltype(h)::value;
+    V2Conv1Fwd<H> p;
     for (int z = 0; z < 2; ++z) {
-      p.idx[z] = idx[z]; p.shift[z] = shift[z];
-      p.wimg[z] = u->img_fwd[z][0]; p.out16[z] = u->h16[0][z];
+      p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
+      p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z];
     }
-    p.out[0] = n->d_h1[0];
-    p.out[1] = nullptr;                       // nothing reads the target network's fp32 H1
-    p.shared5 = shared5 ? 1 : 0; p.nets = nets; p.rows = rows; p.lo_off = u->h_elems[0];
-    p.im2col = (nets == 2 && rows == n->nb) ? u->im2col1 : nullptr;
-    CUtensorMap m0, m1;
-    const int64_t nframes0 = nframes[0], nframes1 = nframes[1];
-    if ((rc = conv1tma::make_frame_map(&m0, src[0], nframes0, shared5 ? kHist + 1 : kHist))) return rc;
-    if ((rc = conv1tma::make_frame_map(&m1, src[nets == 2 ? 1 : 0], nets == 2 ? nframes1 : nframes0, kHist))) return rc;
-    static bool configured = false;
-    if (!configured) {
-      B2_CHECK_CUDA(cudaFuncSetAttribute(conv1tma::k_conv1_tma, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         int(conv1tma::smem_bytes(2))));
-      configured = true;
-    }
-    const uint32_t smem = conv1tma::smem_bytes((nets == 2 && !shared5) ? 2 : 1);
-    B2_CHECK_CUDA(launch_pdl(conv1tma::k_conv1_tma, dim3(rows * conv1tma::kTilesPerSample), dim3(umma2::kThreads2),
-                             smem, st, m0, m1, p, ktrace_slot("conv1_fwd")));
-    B2_PROF("conv1_fwd", st);
-  } else {
-    rc = with_hist(n->cfg.history_length, [&](auto h) {
-      constexpr int H = decltype(h)::value;
-      V2Conv1Fwd<H> p;
-      for (int z = 0; z < 2; ++z) {
-        p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
-        p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z];
-      }
-      for (int z = 0; z < 3; ++z) p.out16[z] = planes(0, z);
-      p.out[2] = nullptr;                                                  // slot 2 keeps no fp32 activations
-      p.rows = rows;
-      p.im2col = (nets >= 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
-      return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early);
-    });
-    if (rc) return rc;
-  }
+    for (int z = 0; z < 3; ++z) p.out16[z] = planes(0, z);
+    p.out[2] = nullptr;                                                  // slot 2 keeps no fp32 activations
+    p.rows = rows;
+    p.im2col = (nets >= 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
+    return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early);
+  });
+  if (rc) return rc;
   if (rows <= kConv23MaxRows) {
     Conv23Fwd p{};
     for (int z = 0; z < 2; ++z) { p.c2.wimg[z] = u->img_fwd[z][1]; p.c3.wimg[z] = u->img_fwd[z][2]; }
@@ -1283,7 +1235,7 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
       return with_hist(n->cfg.history_length, [&](auto h) {
         constexpr int H = decltype(h)::value;
         WConv1Wgrad<H> p{u->im2col1, PlanePair{u->dz16[3], u->dz_elems[3]}, n->d_part + lt.part_off[0], rows,
-                           umma_wgrad_kb(0, rows), g_conv1_tma ? conv1tma::kTileRows : 128};
+                           umma_wgrad_kb(0, rows)};
         return umma_mn::launch_umma_mn("conv1_wgrad", p, 64 * H, kC1, lt.splits[0], st, release_early);
       });
     }

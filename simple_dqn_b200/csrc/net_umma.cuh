@@ -19,11 +19,10 @@ void umma_net_destroy(b200dqn_net* n);
 int umma_double_q_alloc(b200dqn_net* n);                // fp16 planes of network slot 2 (Double DQN), once
 int umma_weights_changed(b200dqn_net* n, cudaStream_t st);  // fp32 master weights were overwritten by the host
 int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
-// nframes[z]: frames in the array src[z] points to (the tensor-map TMA gather of conv1 needs the extent)
 // release_early: the launches are links of the single-GPU critical chain; the kernels that gain from it let their
-// successor pre-launch right after their own dependency wait (conv1's TMA twin keeps its own release point)
+// successor pre-launch right after their own dependency wait
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 const int64_t nframes[2], int nets, int rows, cudaStream_t st, bool release_early);
+                 int nets, int rows, cudaStream_t st, bool release_early);
 int umma_fc1_splits(int rows);
 // RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel
 int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false);
@@ -35,7 +34,6 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
 // fp16 hi plane of dZ4 and the offset of its lo plane (nullptr when math_mode != TCGEN05)
 void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
 int umma_wgrad_splits(int layer, int rows);   // split-K factor of the conv wgrad of `layer` (0..2)
-bool umma_conv1_tma();   // B200DQN_CONV1=tma: conv1 runs the tensor-map TMA twin (4-frame windows only)
 // op: 0 fc1_wgrad, 1 fc1_dgrad, 2 conv3_wgrad, 3 conv3_dgrad, 4 conv2_wgrad, 5 conv2_dgrad, 6 conv1_wgrad
 // release_early: as for umma_forward
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,

@@ -22,7 +22,8 @@ struct b200dqn_replay {
   int64_t* d_cursor = nullptr;     // {count, current} — read by the sampler, graph-safe
   // MT19937 state: 624 key words + position (CPython random.getstate()[1]), DOUBLE-BUFFERED: sampling number k
   // (0-based count of samplings done) reads slot k & 1 and leaves the advanced state in slot (k + 1) & 1, so that
-  // the many CTAs of the fused conv1 kernel can all read the state while one of them writes its successor
+  // the many CTAs of the prioritized sampler (per.cu::k_sample_per) can all read the state while one of them writes
+  // its successor
   uint32_t* d_mt = nullptr;        // [2][kMtSlot]
   uint32_t* mt_slot_ptr() const { return d_mt + (samples_launched & 1u) * 640; }   // host view: current slot
   int32_t* d_idx = nullptr;        // [batch] accepted indexes, acceptance order
@@ -102,10 +103,9 @@ int replay_flush(b200dqn_replay* r, cudaStream_t st);
 int replay_wait_words(b200dqn_replay* r, cudaStream_t st);
 int replay_publish_words(b200dqn_replay* r, cudaStream_t st);   // device counters -> host-mapped mirror (tiny kernel)
 #ifdef __CUDACC__
-// ---- the sampling loop of getMinibatch (src/replay_memory.py:55-69) as a CTA-wide device function, shared by the
-// stand-alone sampler kernel (replay.cu::k_sample) and the first conv layer, which draws its own indexes
-// (conv1_tma.cuh).  See k_sample for the formulation (one MT19937 word per trial; accepted indexes = the first
-// `batch` stream words passing all three tests, in stream order).
+// ---- the sampling loop of getMinibatch (src/replay_memory.py:55-69) as a CTA-wide device function, run by the
+// sampler kernel (replay.cu::k_sample).  See k_sample for the formulation (one MT19937 word per trial; accepted
+// indexes = the first `batch` stream words passing all three tests, in stream order).
 constexpr int kMtN = 624, kMtM = 397, kMtSlot = 640;
 struct SampleShared {
   uint32_t mt[kMtN + 1];

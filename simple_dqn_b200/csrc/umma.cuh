@@ -1,5 +1,5 @@
 // umma.cuh — Hopper (sm_90a) warpgroup-MMA building blocks shared by the kernels of umma2.cuh (K-major
-// operands: forward, dgrad), umma_mn.cuh (MN-major operands: wgrad) and conv1_tma.cuh.
+// operands: forward, dgrad) and umma_mn.cuh (MN-major operands: wgrad).
 //
 //   D[128 x BN] (fp32, registers) = A[128 x K] * B[BN x K]^T        A, B: fp16 in SWIZZLE_128B shared memory
 //

@@ -157,8 +157,7 @@ class DeepQNetwork:
 
     def set_double_dqn(self, on=True):
         """Switch the Double DQN target on or off: the online network picks the poststate action (first index of the
-        maximum), the target network values it.  Raises NotImplementedError for data-parallel learners and for the
-        B200DQN_CONV1=tma conv1."""
+        maximum), the target network values it.  Raises NotImplementedError for data-parallel learners."""
         L.call("b200dqn_net_set_double_q", self._h, int(bool(on)))
         self.double_dqn = bool(on)
 

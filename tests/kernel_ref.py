@@ -115,9 +115,9 @@ def fc1_splits(rows, forced=0):
     return forced if 1 <= forced <= 14 else (7 if rows <= 256 else 4)
 
 
-def wgrad_split(layer, rows, conv1_tma=False):
+def wgrad_split(layer, rows):
     """(k-blocks per split, splits) of conv layer `layer`'s weight gradient (umma_wgrad_kb / umma_wgrad_splits)."""
-    kred = (rows * 4 * 128 if conv1_tma else rows * 400) if layer == 0 else rows * (81 if layer == 1 else 49)
+    kred = rows * (400, 81, 49)[layer]
     kbs = (kred + 63) // 64
     per = (kbs + 47) // 48
     if layer == 0:
@@ -126,7 +126,7 @@ def wgrad_split(layer, rows, conv1_tma=False):
     return per, (kbs + per - 1) // per
 
 
-def chain(kernel, rows, hist=4, fc1_forced=0, conv1_tma=False):
+def chain(kernel, rows, hist=4, fc1_forced=0):
     """Longest serial fp32 accumulation chain of one output of `kernel` at `rows` samples."""
     fixed = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_dgrad": 512, "conv3_dgrad": 576,
              "conv2_dgrad": 256}
@@ -138,7 +138,7 @@ def chain(kernel, rows, hist=4, fc1_forced=0, conv1_tma=False):
     if kernel == "fc1_wgrad":
         return -(-rows // 64) * 64
     layer = {"conv1_wgrad": 0, "conv2_wgrad": 1, "conv3_wgrad": 2}[kernel]
-    per, sp = wgrad_split(layer, rows, conv1_tma)
+    per, sp = wgrad_split(layer, rows)
     return min(per * 64, rows * (400, 81, 49)[layer]) + sp
 
 

@@ -61,7 +61,8 @@ def test_config_default_matches_reference_flags(lib):
 
 def test_binary_is_hopper_native():
     """The shipped cubin targets sm_90a (and nothing else), the GEMM-shaped kernels run on warpgroup MMAs, conv1
-    gathers its frames by tensor-map TMA, and the replay gather uses the TMA bulk-copy engine."""
+    loads its frames from the ring inside its warpgroup-MMA kernel and fetches its weight tiles by TMA bulk copy, and
+    the replay gather uses the TMA bulk-copy engine."""
     from simple_dqn_b200.build import NVCC
     cuobjdump = shutil.which("cuobjdump") or os.path.join(os.path.dirname(NVCC), "cuobjdump")
     if not os.path.exists(cuobjdump):
@@ -73,7 +74,10 @@ def test_binary_is_hopper_native():
     sass = subprocess.check_output([cuobjdump, "-sass", L.LIB_PATH], text=True, stderr=subprocess.STDOUT)
     for shape in ("64x32x16", "64x64x16", "64x128x16"):
         assert "HGMMA.%s.F32" % shape in sass, shape
-    assert "UTMALDG.3D" in sass
+    conv1 = sass[sass.index("k_umma2INS_10V2Conv1FwdILi4E"):]
+    conv1 = conv1[:conv1.index("Function :")] if "Function :" in conv1 else conv1
+    for op in ("HGMMA.64x64x16.F32", "LDG.E", "UBLKCP"):
+        assert op in conv1, op
     gather = sass[sass.index("k_gather"):]
     gather = gather[:gather.index(".....", 200) if "....." in gather[200:] else len(gather)]
     assert "UBLKCP" in gather

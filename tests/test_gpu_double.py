@@ -342,22 +342,6 @@ def test_double_comm_init_refused():
     assert not net.double_dqn
 
 
-def test_double_refused_under_conv1_tma():
-    """B200DQN_CONV1 is read once per process, so the check runs in a child process."""
-    code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-            "from helpers import make_args\n"
-            "from simple_dqn_b200 import DeepQNetwork\n"
-            "DeepQNetwork(4, make_args(double_dqn=True), math_mode='fp32')\n"
-            "try:\n"
-            "    DeepQNetwork(4, make_args(double_dqn=True), math_mode='tcgen05')\n"
-            "except NotImplementedError as e:\n"
-            "    print('REFUSED', e)\n" % (ROOT, os.path.join(ROOT, "tests")))
-    env = dict(os.environ, B200DQN_CONV1="tma")
-    out = subprocess.run([sys.executable, "-s", "-c", code], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr
-    assert "REFUSED" in out.stdout and "B200DQN_CONV1=tma" in out.stdout, out.stdout
-
-
 def _twins(num_actions, mode, batch, hist, sched, **kw):
     """N (Double DQN, online W, target T != W), V1 (vanilla, W and T) and V2 (vanilla, W and W): all weights set
     from the host, so every tile image comes from the pack kernels."""

@@ -5,11 +5,8 @@ keeps its shape.  Bars as in tests/test_gpu_net.py.
 H runs over 1, 2, 3, 5 and 8: odd and even, below, at and above the tensor-core engine's 4-stage operand ring, and an
 odd number of 64-row m chunks in conv1's weight gradient.  H = 16, the largest implemented, is in the predict and
 train-step sweeps."""
-import os
 import pickle
 import random
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -21,7 +18,6 @@ from oracle.replay_oracle import ReplayOracle, synthetic_ring
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODES = ["fp32", "tcgen05"]
 SCHEDS = ["serial", "branches"]
 HISTS = [1, 2, 3, 5, 8]
@@ -299,19 +295,3 @@ def test_comm_init_needs_four_frames(hist):
     net = _net(hist, "tcgen05")
     with pytest.raises(NotImplementedError, match="history_length"):
         net.comm_init(bytes(128), 0, 2)
-
-
-def test_conv1_tma_switch_is_four_frames_only():
-    """B200DQN_CONV1 is read once per process, so the check runs in a child process."""
-    code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-            "from helpers import make_args\n"
-            "from simple_dqn_b200 import DeepQNetwork\n"
-            "DeepQNetwork(4, make_args(history_length=4), math_mode='tcgen05')\n"
-            "try:\n"
-            "    DeepQNetwork(4, make_args(history_length=2), math_mode='tcgen05')\n"
-            "except NotImplementedError as e:\n"
-            "    print('REFUSED', e)\n" % (ROOT, os.path.join(ROOT, "tests")))
-    env = dict(os.environ, B200DQN_CONV1="tma")
-    out = subprocess.run([sys.executable, "-s", "-c", code], env=env, capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0, out.stderr
-    assert "REFUSED" in out.stdout and "B200DQN_CONV1=tma" in out.stdout, out.stdout

@@ -85,9 +85,9 @@ def make_net(batch, engine="tcgen05", hist=4, num_actions=4, sched="branches", s
     return net
 
 
-def _chain(engine, kernel, rows, hist, fc1_forced=0, conv1_tma=False):
+def _chain(engine, kernel, rows, hist, fc1_forced=0):
     if engine == "tcgen05":
-        return K.chain(kernel, rows, hist, fc1_forced, conv1_tma)
+        return K.chain(kernel, rows, hist, fc1_forced)
     full = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_fwd": K.FLAT, "fc1_dgrad": K.HIDDEN,
             "conv3_dgrad": 576, "conv2_dgrad": 1024, "fc1_wgrad": rows, "conv3_wgrad": rows * 49,
             "conv2_wgrad": rows * 81, "conv1_wgrad": rows * 400}
@@ -119,11 +119,11 @@ def forward_ratios(engine, states, ws, acts, q, fc1_forced=0):
     return r
 
 
-def backward_ratios(engine, states, ws, acts, dz, grads, deltas, conv1_tma=False):
+def backward_ratios(engine, states, ws, acts, dz, grads, deltas):
     rows, hist = states.shape[0], states.shape[1]
     h1, h2, h3, h4 = acts
     dz1, dz2, dz3, dz4 = dz
-    c = lambda k: _chain(engine, k, rows, hist, conv1_tma=conv1_tma)
+    c = lambda k: _chain(engine, k, rows, hist)
     # dZ4 = δ·W5 under the H4 mask: one fp32 product per element (k_head / the SIMT head alike)
     ref4 = (deltas.astype(F32) @ ws[4]) * (h4 > 0)
     assert (dz4 == ref4).all(), np.abs(dz4 - ref4).max()
@@ -141,7 +141,7 @@ def backward_ratios(engine, states, ws, acts, dz, grads, deltas, conv1_tma=False
     return r
 
 
-def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward=-1, max_reward=1):
+def train_and_check(net, mb, fc1_forced=0, clip=1.0, min_reward=-1, max_reward=1):
     """One train step, every kernel of it held to its bound; then predict on fresh states with the updated weights
     (the refreshed tile images, lo halves included).  Returns the ratios and the train step's device tensors."""
     engine = net.math_mode
@@ -167,7 +167,7 @@ def train_and_check(net, mb, fc1_forced=0, conv1_tma=False, clip=1.0, min_reward
     assert net.last_costs(1)[0] == F32(tot / F32(len(row_cost))), (net.last_costs(1)[0], tot)
     r = forward_ratios(engine, pre, ws0, acts, preq, fc1_forced)
     step = dict(acts=acts, dz=net.last_dz(), grads=net.get_grads())
-    r.update(backward_ratios(engine, pre, ws0, acts, step["dz"], step["grads"], deltas, conv1_tma))
+    r.update(backward_ratios(engine, pre, ws0, acts, step["dz"], step["grads"], deltas))
     ws1 = net.get_weights(with_states=False)
     fresh = minibatch(len(pre), pre.shape[1], net.num_actions, 1234)[0]
     q = net.predict(fresh)
@@ -334,10 +334,6 @@ def _child(env, cases, double=False):
     line = [l for l in out.stdout.splitlines() if l.startswith("RATIOS ")][0]
     for r in json.loads(line[len("RATIOS "):]):
         _note(r, double)
-
-
-def test_conv1_tma_twin():
-    _child({"B200DQN_CONV1": "tma"}, [(b, {"conv1_tma": True}) for b in (1, 32, 65, 256)])
 
 
 @pytest.mark.parametrize("splits", [1, 4, 14])
