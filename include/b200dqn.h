@@ -226,6 +226,21 @@ typedef struct b200dqn_net_config {
   int target_steps;      /* :65  0 ⇒ the target network aliases the online network (:72-73) */
   int math_mode;         /* B200DQN_MATH_*                                                */
   int optimizer;         /* B200DQN_OPT_*  (:50-61; args.optimizer, main.py:40)           */
+  /* Distributional value head (C51, Bellemare, Dabney and Munos, 2017; new capability, no reference counterpart),
+   * off when num_atoms = 0 (the default).  Otherwise 2..64 atoms on the fixed support z_i = v_min + i dz,
+   * dz = (v_max - v_min) / (num_atoms - 1) (fp64), with v_min < v_max both finite (EINVAL otherwise):
+   *   - fc2 grows to A * num_atoms outputs (Neon shape (A * num_atoms, 512), row a * num_atoms + i);
+   *   - p[a] = softmax(logits[a]) (fp32, row maximum subtracted), Q[a] = sum_i float(z_i) p[a][i] in i order: every
+   *     Q output (predict, Q rows) carries these expected values;
+   *   - the train step projects the target network's distribution at a* (argmax of its Q, or of the online network's
+   *     with Double DQN) onto the support in fp64: T_j = clamp(R + g z_j, v_min, v_max), b_j = (T_j - v_min) / dz,
+   *     m_i = float(sum_j q_j max(0, 1 - |b_j - i|)), R the clipped (or n-step) return, g = gamma^N (0 at a terminal);
+   *   - the cost is the cross-entropy -sum_i m_i log p[a][i] at the taken action (times the importance weight on a
+   *     prioritized ring, whose priority update gets the unweighted loss); clip_error is not applied;
+   *   - the logit gradient is (p[a][i] - m_i) w at the taken action and 0 elsewhere.
+   * b200dqn_net_comm_init returns ENOTIMPL on such a net. */
+  int num_atoms;
+  double v_min, v_max;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -257,8 +272,9 @@ int b200dqn_net_sync_target(b200dqn_net* n, void* stream);
  * host_q (batch,A) f32 (already transposed as `qvalues.T`).  H2D + forward + D2H; synchronises. */
 int b200dqn_net_predict(b200dqn_net* n, const uint8_t* host_states, float* host_q, void* stream);
 /* Same on device memory; rows >= live_rows must be all-zero frames (the StateBuffer case,
- * agent.py:55-58): they are not computed — with no biases Q(0) = 0 exactly — and dev_q rows
- * >= live_rows are written as 0.  live_rows = batch computes everything.  Asynchronous. */
+ * agent.py:55-58): they are padding, not computed, and dev_q rows >= live_rows are written as
+ * exact zeros (not the network's value there, which a distributional head makes mean(z)).
+ * live_rows = batch computes everything.  Asynchronous. */
 int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_states, int live_rows, float* dev_q,
                                void* stream);
 
@@ -334,8 +350,18 @@ enum {
    * prioritized ring (the quantity its priority update uses).  EINVAL before the first such step. */
   B200DQN_NET_PTR_TD_ERRORS,
   /* (batch,) f32: the per-sample cost 0.5*delta^2 before the clip (times the importance weight on a prioritized ring)
-   * of the last train step, whose mean in row order is the step's cost. */
-  B200DQN_NET_PTR_ROW_COSTS
+   * of the last train step, whose mean in row order is the step's cost.  Distributional head: the cross-entropy. */
+  B200DQN_NET_PTR_ROW_COSTS,
+  /* Distributional head only (num_atoms > 0; EINVAL otherwise).  DELTAS is EINVAL on such a net: there is no scalar
+   * delta.  Slots as in the forward: 0 online on the prestates, 1 target on the poststates, 2 online on the
+   * poststates (Double DQN). */
+  B200DQN_NET_PTR_LOGITS,       /* (3, batch, A * num_atoms) f32 fc2 outputs of the last forward         */
+  B200DQN_NET_PTR_PROBS,        /* (3, batch, A, num_atoms) f32 softmax of each action's logits           */
+  B200DQN_NET_PTR_TARGET_DIST,  /* (batch, num_atoms) f32 projected target distribution m                 */
+  B200DQN_NET_PTR_LOGIT_GRADS,  /* (batch, num_atoms) f32 gradient on the taken action's logits           */
+  /* Tensor-core engine only (EINVAL on the SIMT engine): the fp16 planes of DZ4 the tensor-core dgrad reads, hi then
+   * lo (scaled by 2048), each (batch, 512) row-major; the lo plane starts bytes / 2 - batch * 512 elements after hi. */
+  B200DQN_NET_PTR_DZ4_PLANES
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

@@ -2,6 +2,7 @@
 // (src/deepqnetwork.py:15-192 of the reference; per-entry citations in include/b200dqn.h).
 #include <stdlib.h>
 
+#include <cmath>
 #include <new>
 #include <vector>
 
@@ -55,24 +56,14 @@ struct HeadTrainArgs {
   int nstep;
 };
 
-template <int kSlots, bool kNstep>
-__global__ void __launch_bounds__(kHidden)
-k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4_online, float* h4_target,
-       const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
-       float* q_target, float* q_online_post, int A, const HeadTrainArgs td, const KTrace kt) {
-  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
-  // kNstep (td.nstep > 1): the n-step target; the one-step instantiation is today's kernel unchanged
-  __shared__ float red[kSlots][kHidden / 32][kMaxActions];
-  __shared__ float s_q[kSlots][kMaxActions];
-  __shared__ float s_d;
-  __shared__ int s_a;
-  __shared__ __align__(16) __half s_row[2][kHidden];   // hi / lo of this sample's dZ4 row (peer push)
-  const int b = blockIdx.x, t = threadIdx.x;
-  kt_begin(kt);
-  // The TD scalars of this sample depend only on the sampler (several kernels upstream, complete by now):
-  // fetch them before the dependency wait, off the tail of the kernel.
-  int td_a = 0, td_term = 0;
-  int64_t td_r = 0;
+// The TD scalars of sample b, shared by both heads.  They depend only on the sampler (several kernels upstream,
+// complete by now), so the heads fetch them before the dependency wait, off the tail of the kernel.  Thread 0 gets the
+// taken action a (clamped, out-of-range actions flagged in td.err), the reward r and the terminal flag; with kNstep it
+// also gets the n-step return R, g = gamma^m and the flag "a terminal cut the window".  Thread 32 of CTA 0 writes
+// Adam's step scalar.
+template <bool kNstep>
+__device__ __forceinline__ void head_td_scalars(const HeadTrainArgs& td, int b, int t, int& td_a, int64_t& td_r,
+                                                int& td_term, double& td_ret, double& td_g) {
   if (td.enable && t == 0) {
     const int64_t mi = td.midx[b];
     td_a = td.actions[mi];
@@ -85,7 +76,6 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
   }
   // n-step: lane k of warp 0 loads reward and terminal k (32 at a time), and every lane reduces them in k order through
   // shuffles: g = 1; for k: R = R + g c_k; stop at a terminal; g = g gamma.  Thread 0 keeps R, g and the flag.
-  double td_ret = 0.0, td_g = 1.0;
   if (kNstep && td.enable && t < 32) {
     const int64_t mi = td.midx[b];
     double R = 0.0, g = 1.0;
@@ -122,6 +112,26 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
     const float a = float(1.0 - pow(0.999, tt)), c = float(1.0 - pow(0.9, tt));
     *td.adam_l = __fdiv_rn(__fmul_rn(td.adam_lr, __fsqrt_rn(a)), c);
   }
+}
+
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4_online, float* h4_target,
+       const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
+       float* q_target, float* q_online_post, int A, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  // kNstep (td.nstep > 1): the n-step target; the one-step instantiation is today's kernel unchanged
+  __shared__ float red[kSlots][kHidden / 32][kMaxActions];
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_d;
+  __shared__ int s_a;
+  __shared__ __align__(16) __half s_row[2][kHidden];   // hi / lo of this sample's dZ4 row (peer push)
+  const int b = blockIdx.x, t = threadIdx.x;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
   pdl_wait();
   pdl_launch_dependents();
   float h[kSlots] = {};
@@ -311,6 +321,246 @@ k_opt_small(const float* __restrict__ part, int splits, int64_t size, float* __r
 }
 
 // ------------------------------------------------------------------------------------------
+// Distributional head (C51, Bellemare, Dabney and Munos 2017; b200dqn.h has the rules).  Three kernels:
+//   k_fc2_dist       fc1 finish + fc2 for every slot: l[z][b][c] = sum_k H4[z][b][k] W5[k][c], c = a * atoms + i
+//   k_head_dist      one CTA per sample: softmax, Q, a*, projection, cross-entropy, logit gradient, dZ4 (+ fp16
+//                    planes) and the compact dW5 row partial [512][atoms] of the taken action
+//   k_opt_fc2_dist   fc2's gradient from those partials (rows with the action, row order) + the configured update
+// ------------------------------------------------------------------------------------------
+struct DistArgs {
+  int atoms;
+  double v_min, v_max, dz;
+  float* probs;      // [3][ld][A][atoms]
+  float* tdist;      // [ld][atoms]
+  float* lgrad;      // [ld][atoms]
+  int32_t* act_rows; // [ld]
+};
+
+constexpr int kDistTB = 16, kDistTN = 64;   // k_fc2_dist tile: samples x output columns, 256 threads
+
+// grid (sample tiles, column tiles, slots).  Each CTA finishes fc1 for its 16 samples (split-K partials summed in
+// k_head's order, then Rectlin: H4 is bit-identical to the scalar head's) into shared memory, and then reads its W5
+// column slice once for all of them.  Thread (c, group) accumulates 4 samples of column c in k order, fp32, without
+// contraction.  The CTAs of column tile 0 store H4 of slots 0 and 1.
+__global__ void __launch_bounds__(256)
+k_fc2_dist(const float* __restrict__ part, int splits, int rows, int ld, float* h4_online, float* h4_target,
+           const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* __restrict__ logits,
+           int ncols, const KTrace kt) {
+  __shared__ float s_h[kDistTB][kHidden];
+  const int z = blockIdx.z, b0 = blockIdx.x * kDistTB, t = threadIdx.x;
+  const int c = blockIdx.y * kDistTN + t % kDistTN, g0 = (t / kDistTN) * 4;
+  const int nrow = min(kDistTB, rows - b0);
+  const float* w5 = (z == 1 ? w5_target : w5_online) + c;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  for (int e = t; e < kDistTB * kHidden; e += 256) {
+    const int r = e / kHidden, k = e % kHidden;
+    float h = 0.f;
+    if (r < nrow) {
+      float acc = 0.f;
+      for (int s = 0; s < splits; ++s) acc += part[((z * splits + s) * rows + b0 + r) * kHidden + k];
+      h = fmaxf(acc, 0.f);
+      if (z < 2 && blockIdx.y == 0) (z ? h4_target : h4_online)[(b0 + r) * kHidden + k] = h;
+    }
+    s_h[r][k] = h;
+  }
+  __syncthreads();
+  if (c < ncols) {
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll 8
+    for (int k = 0; k < kHidden; ++k) {
+      const float w = w5[int64_t(k) * ncols];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[j] = __fadd_rn(acc[j], __fmul_rn(s_h[g0 + j][k], w));
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (g0 + j < nrow) logits[(int64_t(z) * ld + b0 + g0 + j) * ncols + c] = acc[j];
+  }
+  kt_end(kt);
+}
+
+// One CTA (512 threads) per sample b.  Thread r < nets * A owns row (slot z, action a): max, e_i = expf(l_i - max),
+// s = sum_i e_i, p_i = e_i / s, Q = sum_i zf_i p_i, all sequential in i.  With td.enable the rest of the step follows
+// (b200dqn.h): a* = first maximum of slot 1's Q (slot 2's with kSlots = 3), the fp64 projection of p[1][a*] (one
+// thread per atom, j order, no contraction), the loss, gl, dZ4 and the dW5 row partial dw[b][k][i] = H4[k] gl_i.
+// The TD scalars and Adam's step scalar come from head_td_scalars, before the dependency wait.
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_dist(const float* __restrict__ logits, int ld, int nets, const float* __restrict__ h4_online,
+            const float* __restrict__ w5_online, float* q_online, float* q_target, float* q_online_post, int A,
+            const DistArgs da, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 1 || kSlots == 2 || kSlots == 3, "predict, online + target, or Double DQN's three slots");
+  __shared__ float s_p[kSlots][kMaxActions * kMaxAtoms];
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_mx[kMaxActions], s_ls[kMaxActions];   // slot 0: row maximum and log of the sum
+  __shared__ double s_b[kMaxAtoms], s_qd[kMaxAtoms];
+  __shared__ float s_zf[kMaxAtoms], s_m[kMaxAtoms], s_g[kMaxAtoms], s_h4[kHidden];
+  __shared__ double s_ret, s_gam;
+  __shared__ int s_a, s_astar;
+  const int b = blockIdx.x, t = threadIdx.x, atoms = da.atoms, ncols = A * atoms;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  if (t < atoms) s_zf[t] = float(__dadd_rn(da.v_min, __dmul_rn(double(t), da.dz)));
+  pdl_wait();
+  pdl_launch_dependents();
+  if (td.enable) s_h4[t] = h4_online[b * kHidden + t];
+  __syncthreads();
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float* l = logits + (int64_t(z) * ld + b) * ncols + a * atoms;
+    float* p = s_p[z] + a * atoms;
+    float mx = l[0];
+    for (int i = 1; i < atoms; ++i) mx = fmaxf(mx, l[i]);
+    float s = 0.f;
+    for (int i = 0; i < atoms; ++i) {
+      p[i] = expf(__fsub_rn(l[i], mx));
+      s = __fadd_rn(s, p[i]);
+    }
+    float q = 0.f;
+    float* gp = da.probs + ((int64_t(z) * ld + b) * A + a) * atoms;
+    for (int i = 0; i < atoms; ++i) {
+      p[i] = __fdiv_rn(p[i], s);
+      gp[i] = p[i];
+      q = __fadd_rn(q, __fmul_rn(s_zf[i], p[i]));
+    }
+    s_q[z][a] = q;
+    (z == 0 ? q_online : z == 2 ? q_online_post : q_target)[b * A + a] = q;
+    if (z == 0) {
+      s_mx[a] = mx;
+      s_ls[a] = logf(s);
+    }
+  }
+  if constexpr (kSlots > 1) {
+    if (!td.enable) {
+      kt_end(kt);
+      return;
+    }
+    __syncthreads();
+    if (t == 0) {
+      const float* qs = s_q[kSlots == 3 ? 2 : 1];
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (qs[j] > qs[best]) best = j;
+      double R, g;
+      if constexpr (kNstep) {
+        R = td_ret;
+        g = td_term ? 0.0 : td_g;
+      } else {
+        R = fmin(fmax(double(td_r), td.min_reward), td.max_reward);   // np.clip as the scalar head
+        g = td_term ? 0.0 : td.discount;
+      }
+      s_ret = R;
+      s_gam = g;
+      s_a = td_a;
+      s_astar = best;
+      da.act_rows[b] = td_a;
+    }
+    __syncthreads();
+    const int a = s_a;
+    if (t < atoms) {   // T_j = clamp(R + g z_j), b_j = (T_j - v_min) / dz; q_j = target network's p[a*][j]
+      const double zj = __dadd_rn(da.v_min, __dmul_rn(double(t), da.dz));
+      const double T = fmin(fmax(__dadd_rn(s_ret, __dmul_rn(s_gam, zj)), da.v_min), da.v_max);
+      s_b[t] = __ddiv_rn(__dsub_rn(T, da.v_min), da.dz);
+      s_qd[t] = double(s_p[1][s_astar * atoms + t]);
+    }
+    __syncthreads();
+    if (t < atoms) {   // m_i = sum_j q_j max(0, 1 - |b_j - i|): the floor/ceil split in gather form
+      double acc = 0.0;
+      for (int j = 0; j < atoms; ++j) {
+        const double hat = fmax(0.0, __dsub_rn(1.0, fabs(__dsub_rn(s_b[j], double(t)))));
+        acc = __dadd_rn(acc, __dmul_rn(s_qd[j], hat));
+      }
+      const float m = float(acc);
+      float gl = __fsub_rn(s_p[0][a * atoms + t], m);
+      if (td.isw) gl = __fmul_rn(gl, td.isw[b]);
+      s_m[t] = m;
+      s_g[t] = gl;
+      da.tdist[b * atoms + t] = m;
+      da.lgrad[b * atoms + t] = gl;
+    }
+    __syncthreads();
+    if (t == 0) {   // cross-entropy at the taken action: -sum_i m_i (l_i - max - log s), i order
+      const float* l = logits + int64_t(b) * ncols + a * atoms;
+      float acc = 0.f;
+      for (int i = 0; i < atoms; ++i) acc = __fadd_rn(acc, __fmul_rn(s_m[i], __fsub_rn(__fsub_rn(l[i], s_mx[a]), s_ls[a])));
+      const float loss = -acc;
+      if (td.isw) {
+        td.td_err[b] = loss;
+        td.row_cost[b] = __fmul_rn(td.isw[b], loss);
+      } else {
+        td.row_cost[b] = loss;
+      }
+    }
+    {
+      const float hv = s_h4[t];
+      const float* w = w5_online + int64_t(t) * ncols + a * atoms;
+      float o = 0.f;
+      if (hv > 0.f)
+        for (int i = 0; i < atoms; ++i) o = __fadd_rn(o, __fmul_rn(w[i], s_g[i]));
+      td.dz4[b * kHidden + t] = o;
+      if (td.dz4_hi) {
+        const __half hh = __float2half_rn(o);
+        const __half ll = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+        td.dz4_hi[b * kHidden + t] = hh;
+        td.dz4_hi[td.dz4_lo_off + b * kHidden + t] = ll;
+      }
+    }
+    float* dw = td.dw5_rows + int64_t(b) * kHidden * atoms;
+    for (int e = t; e < kHidden * atoms; e += kHidden) dw[e] = __fmul_rn(s_h4[e / atoms], s_g[e % atoms]);
+  }
+  kt_end(kt);
+}
+
+// fc2's gradient and update on a distributional net.  grid (cdiv(512 * atoms, 256), A): CTA (x, a) lists, in row
+// order, the rows whose taken action is a (warp 0, by ballot), then thread e sums dw[row][e] over that list (0 for an
+// action no row took) for parameter (k, a * atoms + i), e = k * atoms + i.  mode bit1: write the sum to g (d_g,
+// internal layout); bit2: apply the configured update.
+__global__ void __launch_bounds__(256)
+k_opt_fc2_dist(const float* __restrict__ part, const int32_t* __restrict__ act_rows, int rows, int A, int atoms,
+               float* __restrict__ g_out, float* __restrict__ w, float* __restrict__ sst, int mode, const OptArgs opt,
+               const KTrace kt) {
+  __shared__ int s_list[4096];
+  __shared__ int s_n;
+  const int a = blockIdx.y, t = threadIdx.x, e = blockIdx.x * 256 + t;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (t < 32) {
+    int cnt = 0;
+    for (int base = 0; base < rows; base += 32) {
+      const int r = base + t;
+      const bool hit = r < rows && act_rows[r] == a;
+      const unsigned m = __ballot_sync(0xffffffffu, hit);
+      if (hit) s_list[cnt + __popc(m & ((1u << t) - 1u))] = r;
+      cnt += __popc(m);
+    }
+    if (t == 0) s_n = cnt;
+  }
+  __syncthreads();
+  if (e < kHidden * atoms) {
+    const int64_t stride = int64_t(kHidden) * atoms;
+    float g = 0.f;
+    for (int j = 0; j < s_n; ++j) g = __fadd_rn(g, part[s_list[j] * stride + e]);
+    const int64_t wi = int64_t(e / atoms) * A * atoms + a * atoms + e % atoms;
+    if (mode & 2) g_out[wi] = g;
+    if (mode & 4) {
+      float s[3] = {0.f, 0.f, 0.f};
+      for (int k = 0; k < opt.nstates; ++k) s[k] = sst[k * opt.plane + wi];
+      float wv = w[wi];
+      opt_update1(opt, opt_step_scalar(opt), g, wv, s[0], s[1], s[2]);
+      w[wi] = wv;
+      for (int k = 0; k < opt.nstates; ++k) sst[k * opt.plane + wi] = s[k];
+    }
+  }
+  kt_end(kt);
+}
+
+// ------------------------------------------------------------------------------------------
 // K6: gradient reduction + the configured Neon optimizer (src/deepqnetwork.py:50-61,165; rules in optim.cuh).
 // RMSProp:  g = dW / bsz;  s = decay*s + g*g*(1-decay);  W = W - (g*lr) / (sqrt(s + eps) + eps)
 // The split-K partials of every layer are summed here in fixed order (deterministic), so the
@@ -447,6 +697,22 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
   }
   const int fc1_splits = n->cfg.math_mode == B200DQN_MATH_TCGEN05 ? umma_fc1_splits(rows) : kFc1Splits;
   const bool nstep = td.enable && td.nstep > 1;
+  if (n->atoms) {
+    const int ncols = n->fc2_cols();
+    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
+                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
+                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_logits, ncols, ktrace_slot("fc2_dist")));
+    B2_PROF("fc2_dist", st);
+    const DistArgs da{n->atoms, n->cfg.v_min, n->cfg.v_max, n->dz, n->d_probs, n->d_tdist, n->d_lgrad, n->d_act_rows};
+    auto* kern = nets == 1 ? k_head_dist<1, false>
+               : nets == 3 ? (nstep ? k_head_dist<3, true> : k_head_dist<3, false>)
+                           : (nstep ? k_head_dist<2, true> : k_head_dist<2, false>);
+    B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_logits, n->nb, nets,
+                             (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, da, td,
+                             ktrace_slot("head_dist")));
+    B2_PROF(td.enable ? "head_dist(td+fc2_bwd)" : "head_dist", st);
+    return B200DQN_OK;
+  }
   B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head<3, true> : k_head<3, false>)
                                      : (nstep ? k_head<2, true> : k_head<2, false>),
                            dim3(rows), dim3(kHidden), 0, st,
@@ -553,8 +819,31 @@ static int cost_finish_on(b200dqn_net* n, int rows, cudaStream_t s) {
   return B200DQN_OK;
 }
 
+// fc2 of a distributional net from the head's compact row partials; mode bits as k_opt_fc2_dist's
+static int opt_fc2_dist(b200dqn_net* n, int rows, int mode, cudaStream_t s, const char* label) {
+  const LayerTable& lt = n->lt;
+  B2_CHECK_CUDA(launch_pdl(k_opt_fc2_dist, dim3(cdiv(int64_t(kHidden) * n->atoms, 256), n->A), dim3(256), 0, s,
+                           (const float*)n->d_part + lt.part_off[4], (const int32_t*)n->d_act_rows, rows, n->A, n->atoms,
+                           n->d_g + lt.off[4], n->d_w + lt.off[4], n->d_s + lt.off[4], mode, make_opt_args(n, rows),
+                           ktrace_slot(label)));
+  B2_PROF(label, s);
+  return B200DQN_OK;
+}
+
+// The update over layers [l0, l1] of the single-learner schedules (mode 1 | 4): fc2 of a distributional net goes
+// through opt_fc2_dist, every other layer through optimizer_range.
+static int update_range(b200dqn_net* n, int l0, int l1, int rows, cudaStream_t st, const char* label) {
+  if (!n->atoms || l1 < 4) return optimizer_range(n, l0, l1, 1 | 4, rows, st, label);
+  if (l0 < 4) {
+    const int rc = optimizer_range(n, l0, 3, 1 | 4, rows, st, label);
+    if (rc) return rc;
+  }
+  return opt_fc2_dist(n, rows, 4, st, "opt_fc2_dist");
+}
+
 // fc2 update from the head's per-row partials (single-GPU schedules): 8-lane reduction, no image
 static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
+  if (n->atoms) return opt_fc2_dist(n, rows, 4, s, "opt_fc2_dist");
   const LayerTable& lt = n->lt;
   const int64_t size = lt.off[5] - lt.off[4];
   B2_CHECK_CUDA(launch_pdl(k_opt_small, dim3(cdiv(size / 4, 32)), dim3(256), 0, s, (const float*)n->d_part + lt.part_off[4],
@@ -828,7 +1117,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
       B2_PROF("allreduce", st);
       B2_TRY(optimizer_range(n, 0, kLayers - 1, 4, rows, st, "optimizer"));
     } else {
-      B2_TRY(optimizer_range(n, 0, kLayers - 1, 1 | 4, rows, st, "optimizer"));
+      B2_TRY(update_range(n, 0, kLayers - 1, rows, st, "optimizer"));
     }
     return B200DQN_OK;
   }
@@ -843,9 +1132,9 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     NoPdlScope side;
     B2_TRY(bwd_op(n, fs, rows, kFc1Wgrad, sA));             // overlaps fc1_dgrad (few CTAs)
     // fourth branch: the scalar cost and the 512 x A layer — nothing later in the step reads W5, and nothing here
-    // sits in front of the fc1 optimizer any more
+    // sits in front of the fc1 optimizer any more (the SIMT engine's scalar fc2 rides with fc1 in opt_fc)
     B2_TRY(cost_finish_on(n, rows, sN));
-    if (tc) B2_TRY(opt_fc2_small(n, rows, sN));
+    if (tc || n->atoms) B2_TRY(opt_fc2_small(n, rows, sN));
   }
   B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
@@ -853,7 +1142,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   {
     NoPdlScope side;
     if (tc) B2_TRY(umma_opt_fc1(n, rows, sA));               // smem-free: co-resides with the dgrad chain
-    else B2_TRY(optimizer_range(n, 3, 4, 1 | 4, rows, sA, "opt_fc"));
+    else B2_TRY(optimizer_range(n, 3, n->atoms ? 3 : 4, 1 | 4, rows, sA, "opt_fc"));
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
@@ -961,6 +1250,9 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->target_steps = 10000;     // main.py:63
   cfg->math_mode = B200DQN_MATH_FP32_SIMT;
   cfg->optimizer = B200DQN_OPT_RMSPROP;   // main.py:40
+  cfg->num_atoms = 0;            // scalar head; the distributional head's support defaults to [-10, 10]
+  cfg->v_min = -10.0;
+  cfg->v_max = 10.0;
   return B200DQN_OK;
 }
 
@@ -979,6 +1271,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
              "net_create: unknown math_mode %d", cfg->math_mode);
   B2_REQUIRE(cfg->optimizer >= B200DQN_OPT_RMSPROP && cfg->optimizer <= B200DQN_OPT_ADADELTA, B200DQN_EINVAL,
              "net_create: unknown optimizer %d", cfg->optimizer);   // deepqnetwork.py:61 `assert false, "Unknown optimizer"`
+  B2_REQUIRE(cfg->num_atoms == 0 || (cfg->num_atoms >= 2 && cfg->num_atoms <= kMaxAtoms), B200DQN_EINVAL,
+             "net_create: num_atoms %d is neither 0 (scalar head) nor in [2,%d]", cfg->num_atoms, kMaxAtoms);
+  B2_REQUIRE(cfg->num_atoms == 0 || (std::isfinite(cfg->v_min) && std::isfinite(cfg->v_max) && cfg->v_min < cfg->v_max),
+             B200DQN_EINVAL, "net_create: the support needs finite v_min < v_max (got %g, %g)", cfg->v_min, cfg->v_max);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -988,10 +1284,12 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->cfg = *cfg;
   n->nb = cfg->batch_size;
   n->A = cfg->num_actions;
+  n->atoms = cfg->num_atoms;
+  if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
   const int nb = n->nb, A = n->A, hist = cfg->history_length;
   LayerTable& lt = n->lt;
   const int rows_[kLayers] = {64 * hist, kK2, kK3, kFlat, kHidden};   // conv1: one 64-tap k-block per frame
-  const int cols_[kLayers] = {kC1, kC2, kC3, kHidden, A};
+  const int cols_[kLayers] = {kC1, kC2, kC3, kHidden, n->fc2_cols()};
   lt.off[0] = 0;
   for (int l = 0; l < kLayers; ++l) {
     lt.rows[l] = rows_[l];
@@ -1011,7 +1309,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     else
       lt.splits[l] = l < 3 ? int(cdiv(kred[l], wgrad_chunk(kred[l], base[l]))) : 1;
     lt.part_off[l] = po;
-    po += int64_t(lt.splits[l]) * (lt.off[l + 1] - lt.off[l]);
+    if (l == 4 && n->atoms)   // distributional head: the taken action's [512][atoms] block per sample
+      po += int64_t(nb) * kHidden * n->atoms;
+    else
+      po += int64_t(lt.splits[l]) * (lt.off[l + 1] - lt.off[l]);
   }
   n->part_elems = po;
 
@@ -1057,6 +1358,15 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   B2_CHECK_CUDA(cudaMalloc(&n->d_step, sizeof(uint32_t)));
   B2_CHECK_CUDA(cudaMemset(n->d_step, 0, sizeof(uint32_t)));
   B2_CHECK_CUDA(fmalloc(&n->d_rowcost, nb));
+  if (n->atoms) {
+    const size_t dist = size_t(nb) * A * n->atoms;
+    B2_CHECK_CUDA(fmalloc(&n->d_logits, 3 * dist));
+    B2_CHECK_CUDA(fmalloc(&n->d_probs, 3 * dist));
+    B2_CHECK_CUDA(fmalloc(&n->d_tdist, size_t(nb) * n->atoms));
+    B2_CHECK_CUDA(fmalloc(&n->d_lgrad, size_t(nb) * n->atoms));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
+    B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
+  }
   const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
   B2_CHECK_CUDA(cudaMalloc(&n->d_pre, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_post, state_bytes + 256));
@@ -1113,6 +1423,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_dz1); cudaFree(n->d_cost); cudaFree(n->d_step); cudaFree(n->d_rowcost); cudaFree(n->d_pre); cudaFree(n->d_post);
   cudaFree(n->d_act); cudaFree(n->d_term); cudaFree(n->d_rew); cudaFree(n->d_iota1); cudaFree(n->d_iota4);
   cudaFree(n->d_td_err);
+  cudaFree(n->d_logits); cudaFree(n->d_probs); cudaFree(n->d_tdist); cudaFree(n->d_lgrad); cudaFree(n->d_act_rows);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -1122,7 +1433,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
 extern "C" int b200dqn_net_layer_shape(const b200dqn_net* n, int layer, int* rows, int* cols) {
   B2_REQUIRE(n && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_layer_shape: bad layer");
   // NEON shapes: conv (C*R*S, K); linear (nout, nin)
-  const int r[kLayers] = {n->lt.rows[0], kK2, kK3, kHidden, n->A};
+  const int r[kLayers] = {n->lt.rows[0], kK2, kK3, kHidden, n->fc2_cols()};
   const int c[kLayers] = {kC1, kC2, kC3, kFlat, kHidden};
   if (rows) *rows = r[layer];
   if (cols) *cols = c[layer];
@@ -1133,13 +1444,13 @@ static int xfer_params(b200dqn_net* n, float* dev_base, int layer, float* host, 
   const int64_t off = n->lt.off[layer], cnt = n->lt.off[layer + 1] - off;
   std::vector<float> tmp(cnt);
   if (to_device) {
-    for (int64_t i = 0; i < cnt; ++i) tmp[neon_to_internal(layer, i, n->A)] = host[i];
+    for (int64_t i = 0; i < cnt; ++i) tmp[neon_to_internal(layer, i, n->fc2_cols())] = host[i];
     B2_CHECK_CUDA(cudaMemcpyAsync(dev_base + off, tmp.data(), cnt * sizeof(float), cudaMemcpyHostToDevice, st));
     B2_CHECK_CUDA(cudaStreamSynchronize(st));
   } else {
     B2_CHECK_CUDA(cudaMemcpyAsync(tmp.data(), dev_base + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
     B2_CHECK_CUDA(cudaStreamSynchronize(st));
-    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[neon_to_internal(layer, i, n->A)];
+    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[neon_to_internal(layer, i, n->fc2_cols())];
   }
   return B200DQN_OK;
 }
@@ -1233,7 +1544,7 @@ __global__ void k_publish_q_counter(const float* __restrict__ q, int count, vola
 
 // agent.py:55-61 on a device-resident state window (StateBuffer): the forward pass for the live rows, captured once
 // into a CUDA graph (one launch per env step), Q rows back through host-mapped memory (no memcpy, polled).
-// host_q receives (batch, A); rows >= live_rows are exact zeros (no biases: Q(0) = 0).
+// host_q receives (batch, A); rows >= live_rows are padding and come back as exact zeros.
 extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* dev_states, int live_rows, float* host_q,
                                                void* stream) {
   B2_REQUIRE(n && dev_states && host_q && live_rows >= 1 && live_rows <= n->nb, B200DQN_EINVAL,
@@ -1559,7 +1870,11 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
   switch (which) {
     case B200DQN_NET_PTR_Q_ONLINE: p = n->d_q[0]; b = size_t(n->nb) * n->A * 4; break;
     case B200DQN_NET_PTR_Q_TARGET: p = n->d_q[1]; b = size_t(n->nb) * n->A * 4; break;
-    case B200DQN_NET_PTR_DELTAS: p = n->d_delta; b = size_t(n->nb) * n->A * 4; break;
+    case B200DQN_NET_PTR_DELTAS:
+      B2_REQUIRE(!n->atoms, B200DQN_EINVAL, "net_device_ptr: a distributional head has no scalar delta");
+      p = n->d_delta;
+      b = size_t(n->nb) * n->A * 4;
+      break;
     case B200DQN_NET_PTR_GRADS: p = n->d_g; b = n->n_params * 4; break;
     case B200DQN_NET_PTR_WEIGHTS: p = n->d_w; b = n->n_params * 4; break;
     case B200DQN_NET_PTR_COST: p = n->d_cost; b = kCostRing * 4; break;
@@ -1581,6 +1896,25 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       b = size_t(n->nb) * 4;
       break;
     case B200DQN_NET_PTR_ROW_COSTS: p = n->d_rowcost; b = size_t(n->nb) * 4; break;
+    case B200DQN_NET_PTR_LOGITS:
+    case B200DQN_NET_PTR_PROBS:
+    case B200DQN_NET_PTR_TARGET_DIST:
+    case B200DQN_NET_PTR_LOGIT_GRADS:
+      B2_REQUIRE(n->atoms, B200DQN_EINVAL, "net_device_ptr: selector %d needs a distributional head", which);
+      p = which == B200DQN_NET_PTR_LOGITS ? n->d_logits : which == B200DQN_NET_PTR_PROBS ? n->d_probs
+        : which == B200DQN_NET_PTR_TARGET_DIST ? n->d_tdist : n->d_lgrad;
+      b = (which <= B200DQN_NET_PTR_PROBS ? size_t(3) * n->nb * n->A : size_t(n->nb)) * n->atoms * 4;
+      break;
+    case B200DQN_NET_PTR_DZ4_PLANES: {
+      __half* hi = nullptr;
+      int64_t lo_off = 0;
+      umma_dz4_planes(n, &hi, &lo_off);
+      B2_REQUIRE(n->cfg.math_mode == B200DQN_MATH_TCGEN05 && hi, B200DQN_EINVAL,
+                 "net_device_ptr: the dZ4 planes exist on the tensor-core engine only");
+      p = hi;
+      b = size_t(lo_off + int64_t(n->nb) * kHidden) * 2;
+      break;
+    }
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -1643,9 +1977,14 @@ extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, 
   cudaStream_t st = as_stream(stream);
   const int64_t n4 = n->n_params / 4;
   if (n->world == 1) {  // partials of the last step are still in scratch; sum them into d_g
-    k_optimizer<<<cdiv(n4, 256), 256, 0, st>>>(n->lt, n->d_part, n->d_g, n->d_w, n->d_s, 0, n4, 1 | 2, OptArgs{},
+    const int64_t e4 = n->atoms ? n->lt.off[4] / 4 : n4;   // a distributional fc2 is summed by its own kernel
+    k_optimizer<<<cdiv(e4, 256), 256, 0, st>>>(n->lt, n->d_part, n->d_g, n->d_w, n->d_s, 0, e4, 1 | 2, OptArgs{},
                                                KTrace{nullptr, 0});
     B2_LAUNCH_CHECK();
+    if (n->atoms) {
+      NoPdlScope plain;
+      B2_TRY(opt_fc2_dist(n, n->nb, 2, st, "grads_fc2_dist"));
+    }
   } else if (n->xchg_ok && n->xchg_sched == 2 && n->d_xbuf && layer == 3) {
     // gather schedule: fc1's global gradient was computed locally and never passed through d_g
     const int64_t b4 = n->lt.off[3] / 4, e4 = n->lt.off[4] / 4;
@@ -1664,7 +2003,8 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     *launches = n->graph_launches;
   } else {
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
-    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4));
+    // a distributional head adds k_fc2_dist, and on the SIMT engine fc2's own update
+    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->atoms ? (tc ? 1 : 2) : 0);
   }
   return B200DQN_OK;
 }

@@ -11,6 +11,7 @@ namespace b200 {
 
 constexpr int kLayers = 5;
 constexpr int kMaxActions = 32;
+constexpr int kMaxAtoms = 64;             // distributional head: atoms per action
 constexpr int kCostRing = 1024;
 constexpr int kHostCosts = 60;            // per-step costs mirrored in host-mapped memory
 constexpr int kHostQ = 64, kHostQFloats = 960;   // word offset / capacity of the Q rows in the host-mapped block
@@ -103,6 +104,17 @@ struct b200dqn_net {
   int graph_nstep = 1, graph_train_nstep = 1;   // b200dqn_replay::nstep the step graphs were captured at
   int ring_nstep = 1;   // n-step length of the ring this net last trained from (comm_init refuses N > 1)
   float* d_td_err = nullptr;   // [nb] TD errors before the clip (prioritized replay; allocated at its first step)
+
+  // distributional head (cfg.num_atoms > 0; nothing below is allocated otherwise).  fc2 has A * atoms outputs, and its
+  // per-row gradient partials in d_part are compact: [nb][512][atoms], the taken action's block only.
+  int atoms = 0;
+  double dz = 0.0;               // (v_max - v_min) / (atoms - 1)
+  float* d_logits = nullptr;     // [3][nb][A * atoms]
+  float* d_probs = nullptr;      // [3][nb][A][atoms]
+  float* d_tdist = nullptr;      // [nb][atoms] projected target distribution
+  float* d_lgrad = nullptr;      // [nb][atoms] gradient on the taken action's logits
+  int32_t* d_act_rows = nullptr; // [nb] taken action of each row of the last train step (selects the dW5 block)
+  int fc2_cols() const { return atoms ? A * atoms : A; }
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

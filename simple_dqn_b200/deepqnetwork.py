@@ -67,9 +67,21 @@ class DeepQNetwork:
         cfg.math_mode = {"fp32": L.MATH_FP32_SIMT, "tcgen05": L.MATH_TCGEN05}[math_mode]
         cfg.optimizer, self.num_states = _OPTIMIZERS[self.optimizer]
         self.math_mode = math_mode
+        # distributional value head (C51, Bellemare et al., 2017): a new capability, off unless args.distributional is
+        # set; it fixes fc2's shape, so it is chosen here and not switchable later
+        self.distributional = bool(_arg(args, "distributional", False))
+        self.num_atoms, self.support = 0, None
+        if self.distributional:
+            cfg.num_atoms = int(_arg(args, "num_atoms", 51))
+            cfg.v_min = float(_arg(args, "v_min", -10.0))
+            cfg.v_max = float(_arg(args, "v_max", 10.0))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
+        if self.distributional:
+            self.num_atoms, self.v_min, self.v_max = cfg.num_atoms, cfg.v_min, cfg.v_max
+            dz = (cfg.v_max - cfg.v_min) / (cfg.num_atoms - 1)         # z_i = v_min + i dz in fp64, as the device
+            self.support = np.array([cfg.v_min + i * dz for i in range(cfg.num_atoms)], dtype=np.float64)
 
         # model.initialize (:49, :70): Xavier draws from one numpy RandomState(random_seed) —
         # online layers first, then the separately-initialised target model.
@@ -201,6 +213,16 @@ class DeepQNetwork:
         dz4 = self._read_f32(L.NET_PTR_DZ4, (b, 512))
         return dz1, dz2, dz3, dz4
 
+    def last_dz4_planes(self):
+        """(hi, lo) float16 planes of dZ4 the tensor-core dgrad reads, each (batch, 512); lo is scaled by 2048."""
+        p, b = C.c_void_p(), C.c_size_t()
+        L.call("b200dqn_net_device_ptr", self._h, L.NET_PTR_DZ4_PLANES, C.byref(p), C.byref(b))
+        n = self.batch_size * 512
+        lo_off = b.value // 2 - n
+        hi = L.download(self.device, p.value, (self.batch_size, 512), np.float16, self._stream)
+        lo = L.download(self.device, p.value + 2 * lo_off, (self.batch_size, 512), np.float16, self._stream)
+        return hi, lo
+
     def last_online_postq(self):
         """The online network's Q on the poststates of the last Double DQN train() as a (batch, A) array."""
         return self._read_f32(L.NET_PTR_Q_ONLINE_POST, (self.batch_size, self.num_actions))
@@ -216,6 +238,24 @@ class DeepQNetwork:
 
     def last_deltas(self):
         return self._read_f32(L.NET_PTR_DELTAS, (self.batch_size, self.num_actions))
+
+    # ---- distributional head (num_atoms > 0): slot 0 online on the prestates, 1 target on the poststates, 2 online on
+    # the poststates (Double DQN)
+    def last_logits(self):
+        """fc2's outputs of the last forward, (3, batch, A, num_atoms) float32."""
+        return self._read_f32(L.NET_PTR_LOGITS, (3, self.batch_size, self.num_actions, self.num_atoms))
+
+    def last_distributions(self):
+        """Softmax of each action's logits of the last forward, (3, batch, A, num_atoms) float32."""
+        return self._read_f32(L.NET_PTR_PROBS, (3, self.batch_size, self.num_actions, self.num_atoms))
+
+    def last_target_distribution(self):
+        """The projected target distribution m of the last train(), (batch, num_atoms) float32."""
+        return self._read_f32(L.NET_PTR_TARGET_DIST, (self.batch_size, self.num_atoms))
+
+    def last_logit_grads(self):
+        """The gradient on the taken action's logits of the last train(), (batch, num_atoms) float32."""
+        return self._read_f32(L.NET_PTR_LOGIT_GRADS, (self.batch_size, self.num_atoms))
 
     # ---- reference methods
     def update_target_network(self):

@@ -14,6 +14,8 @@ HIST = int(os.environ.get("HIST", "4"))   # --history_length: frames per state, 
 DOUBLE = os.environ.get("DOUBLE", "0") == "1"   # the Double DQN target (a third forward slot)
 PER = os.environ.get("PER", "0") == "1"         # prioritized replay (tree-descent sampler + priority update)
 NSTEP = int(os.environ.get("NSTEP", "1"))       # n-step returns (poststates N frames on, discounted reward sum)
+ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with this many atoms; 0: the scalar head
+NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
 
 
 def args():
@@ -22,6 +24,8 @@ def args():
     a.double_dqn = DOUBLE
     a.prioritized_replay = PER
     a.n_step = NSTEP
+    a.distributional = ATOMS > 0
+    a.num_atoms = ATOMS
     return a
 
 
@@ -29,7 +33,7 @@ mem = ReplayMemory(replay, args(), stream=st, rng="device")
 for s in range(0, replay, 10000):
     mem.add_batch(actions[s:s + 10000], rewards[s:s + 10000], base, terminals[s:s + 10000])
 mem.set_cursor(replay, 1234)
-net = DeepQNetwork(NUM_ACTIONS, args(), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
+net = DeepQNetwork(NACT, args(), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
 net.update_target_network()
 random.seed(1); mem.seed_device_rng(random)
 net.train_fused(mem, 300); st.synchronize()
@@ -47,5 +51,5 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("batch %d hist %d double %d per %d nstep %d period_us min %.2f median %.2f  all %s" % (
-    B, HIST, DOUBLE, PER, NSTEP, min(res), float(np.median(res)), " ".join("%.2f" % r for r in res)))
+print("batch %d hist %d double %d per %d nstep %d actions %d atoms %d period_us min %.2f median %.2f  all %s" % (
+    B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, min(res), float(np.median(res)), " ".join("%.2f" % r for r in res)))

@@ -8,11 +8,21 @@ st = Stream()
 replay = 50000
 base, actions, rewards, terminals = synthetic_meta(replay)
 B = int(os.environ.get("BATCH", "32"))
+ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with this many atoms; 0: the scalar head
+NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
+
+
+def net_args():
+    a = make_args(B)
+    a.distributional, a.num_atoms = ATOMS > 0, ATOMS
+    return a
+
+
 mem = ReplayMemory(replay, make_args(B), stream=st, rng="device")
 for s in range(0, replay, 10000):
     mem.add_batch(actions[s:s + 10000], rewards[s:s + 10000], base, terminals[s:s + 10000])
 mem.set_cursor(replay, 1234)
-net = DeepQNetwork(NUM_ACTIONS, make_args(B), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
+net = DeepQNetwork(NACT, net_args(), stream=st, math_mode=os.environ.get("MATH", "tcgen05"))
 net.update_target_network()
 random.seed(1); mem.seed_device_rng(random)
 net.train_fused(mem, 50); st.synchronize()
