@@ -116,10 +116,12 @@ def test_save_weights_structure_matches_reference_layout(tmp_path, layout):
 
 
 @pytest.mark.parametrize("layout,actions", [("pre-1.0", 4), ("neon-1.3.0", 18), ("neon-1.3.0", 3),
-                                            ("neon-1.3.0", 6)])
+                                            ("neon-1.3.0", 6), ("neon-1.3.0", 1), ("neon-1.3.0", 2),
+                                            ("neon-1.3.0", 17), ("neon-1.3.0", 32)])
 def test_rebuilt_snapshots_of_every_action_count(tmp_path, layout, actions):
     """Checkpoint files in both layouts for the four action counts of the reference's snapshots (Breakout 4,
-    Seaquest 18, Pong 3, Space Invaders 6) through load_weights, against the oracle on what the file holds."""
+    Seaquest 18, Pong 3, Space Invaders 6) and for 1, 2, 17 and 32 (kMaxActions) actions through load_weights, against
+    the oracle on what the file holds."""
     from simple_dqn_b200 import DeepQNetwork
     path = str(tmp_path / "snap.pkl")
     _write_checkpoint(path, layout, *_snapshot_weights(actions, seed=100 + actions))

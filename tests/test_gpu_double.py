@@ -100,7 +100,7 @@ def _follow_device(dev_online_postq):
     return pick
 
 
-CASES = [(4, 4), (18, 4), (4, 1), (4, 5)]   # (num_actions, history_length)
+CASES = [(4, 4), (18, 4), (32, 4), (4, 1), (4, 5)]   # (num_actions, history_length)
 
 
 @pytest.mark.parametrize("mode,sched,batch", [("tcgen05", s, b) for s in ("serial", "branches") for b in (1, 32, 40, 256)] +

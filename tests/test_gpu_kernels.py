@@ -221,6 +221,7 @@ def test_double_history_lengths(hist, batch):
 
 HEAD_CASES = {
     "A18": dict(num_actions=18),
+    "A32": dict(num_actions=32),
     "rewards_asym": dict(min_reward=-2, max_reward=3, rewards=(-6, 7)),
     "all_terminal": dict(terminal_p=1.1),
     "no_terminal": dict(terminal_p=-0.1),
