@@ -241,6 +241,20 @@ typedef struct b200dqn_net_config {
    * b200dqn_net_comm_init returns ENOTIMPL on such a net. */
   int num_atoms;
   double v_min, v_max;
+  /* Dueling network (Wang et al., 2016; new capability, no reference counterpart), off when dueling = 0 (the default;
+   * values other than 0 and 1 are EINVAL).  With dueling = 1:
+   *   - fc1 has 1024 Rectlin units, Neon shape (1024, 3136): rows 0..511 are the advantage stream, rows 512..1023 the
+   *     value stream.  fc2 has Neon shape (A + 1, 512): rows 0..A-1 weigh the advantage units into A_a, row A weighs
+   *     the value units into V;
+   *   - A_a and V are each formed as the scalar head forms Q (fp32 products, the warp's xor butterfly, the 16 warp
+   *     sums in warp order), m = (sum_j A_j in j order) / A, Q_a = V + (A_a - m), every operation rounded on its own.
+   *     Every Q output (predict, the Q rows, the TD target, the Double DQN choice) carries this Q;
+   *   - the TD step (delta, clip, cost, prioritized and n-step targets) is the scalar head's; backward: g = delta / A,
+   *     dA_j = (j == a ? delta - g : -g), dV = delta, dZ4 = (sum_j dA_j W5[j][k], j order) on advantage unit k and
+   *     delta W5[A][k] on value unit k, under the H4 mask.  The paper's 1/sqrt(2) rescale of the gradient entering the
+   *     convolutions and its gradient-norm clipping are not applied.
+   * Both engines.  ENOTIMPL with num_atoms > 0; b200dqn_net_comm_init returns ENOTIMPL on such a net. */
+  int dueling;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -334,11 +348,11 @@ enum {
   B200DQN_NET_PTR_H1,           /* online activations of the last forward, NHWC fp32: (batch,20,20,32) */
   B200DQN_NET_PTR_H2,           /* (batch,9,9,64)                                                      */
   B200DQN_NET_PTR_H3,           /* (batch,7,7,64)                                                      */
-  B200DQN_NET_PTR_H4,           /* (batch,512)                                                         */
+  B200DQN_NET_PTR_H4,           /* (batch,512); (batch,1024) on a dueling net                           */
   /* Online-network gradients at each layer's pre-activation (Rectlin mask applied) of the last train step, NHWC
    * fp32.  DZ4 is always written.  DZ3..DZ1 are always written by the FP32_SIMT engine; the tensor-core engine writes
    * them only while b200dqn_net_set_keep_grads is on, otherwise they hold whatever was there before. */
-  B200DQN_NET_PTR_DZ4,          /* (batch,512)                                                         */
+  B200DQN_NET_PTR_DZ4,          /* (batch,512); (batch,1024) on a dueling net                           */
   B200DQN_NET_PTR_DZ3,          /* (batch,7,7,64)                                                      */
   B200DQN_NET_PTR_DZ2,          /* (batch,9,9,64)                                                      */
   B200DQN_NET_PTR_DZ1,          /* (batch,20,20,32)                                                    */
@@ -360,8 +374,13 @@ enum {
   B200DQN_NET_PTR_TARGET_DIST,  /* (batch, num_atoms) f32 projected target distribution m                 */
   B200DQN_NET_PTR_LOGIT_GRADS,  /* (batch, num_atoms) f32 gradient on the taken action's logits           */
   /* Tensor-core engine only (EINVAL on the SIMT engine): the fp16 planes of DZ4 the tensor-core dgrad reads, hi then
-   * lo (scaled by 2048), each (batch, 512) row-major; the lo plane starts bytes / 2 - batch * 512 elements after hi. */
-  B200DQN_NET_PTR_DZ4_PLANES
+   * lo (scaled by 2048), each (batch, 512) row-major, (batch, 1024) on a dueling net; the lo plane starts
+   * bytes / 2 - batch * width elements after hi. */
+  B200DQN_NET_PTR_DZ4_PLANES,
+  /* Dueling net only (EINVAL otherwise): (3, batch, A + 1) f32, the advantages A_0..A_{A-1} and then V of each row of
+   * the last forward, slots as for the distributional head (slot 2 is written by Double DQN steps with a separate
+   * target network only). */
+  B200DQN_NET_PTR_DUELING_VA
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

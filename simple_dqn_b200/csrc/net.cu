@@ -245,6 +245,147 @@ k_head(const float* __restrict__ part, int splits, int rows, int nets, float* h4
   kt_end(kt);
 }
 
+// ------------------------------------------------------------------------------------------
+// Dueling head (Wang et al. 2016; b200dqn.h has the rules): k_head's job on a dueling net.  One CTA of 1024 threads per
+// sample, thread t = fc1 unit t: warps 0..15 hold the advantage units, warps 16..31 the value units.  Per slot,
+// A_a = fc2 column a over the advantage units and V = column A over the value units, each as k_head forms Q (fp32
+// products, xor butterfly, the 16 warp sums in warp order); m = (sum_j A_j in j order) / A; Q_a = V + (A_a - m).  With
+// td.enable the TD step of k_head follows on these Q, then the backward: g = delta / A, dA_j = (j == a ? delta - g :
+// -g), dV = delta; dZ4 = (sum_j dA_j W5[k][j], j order) on advantage unit k and delta W5[k][A] on value unit k, both
+// under the H4 mask; the dW5 row partial is H4[k] dA_j (column j < A) and H4[512 + k] delta (column A).  Every
+// operation is rounded on its own (explicit _rn intrinsics).
+// ------------------------------------------------------------------------------------------
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kDuelHidden)
+k_head_duel(const float* __restrict__ part, int splits, int rows, int nets, int ld, float* h4_online, float* h4_target,
+            const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
+            float* q_target, float* q_online_post, float* va, int A, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  constexpr int kWarps = kHidden / 32;   // warps per stream
+  __shared__ float red[kSlots][2][kWarps][kMaxActions];   // [stream 0: advantages, 1: value][warp][column]
+  __shared__ float s_va[kSlots][kMaxActions + 1];
+  __shared__ float s_m[kSlots];
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_d;
+  __shared__ int s_a;
+  const int b = blockIdx.x, t = threadIdx.x, C = A + 1;
+  const bool value = t >= kHidden;
+  const int k = value ? t - kHidden : t, w = k >> 5;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  pdl_wait();
+  pdl_launch_dependents();
+  float h[kSlots] = {};
+#pragma unroll
+  for (int z = 0; z < kSlots; ++z) {
+    if (z < nets) {
+      float acc = 0.f;
+      for (int s = 0; s < splits; ++s) acc = __fadd_rn(acc, part[((z * splits + s) * rows + b) * kDuelHidden + t]);
+      h[z] = fmaxf(acc, 0.f);
+      if (z < 2) (z ? h4_target : h4_online)[b * kDuelHidden + t] = h[z];
+    }
+  }
+#pragma unroll
+  for (int z = 0; z < kSlots; ++z) {
+    if (z < nets) {
+      const float* w5 = (z == 1 ? w5_target : w5_online) + k * C;
+      for (int a = value ? A : 0; a < (value ? C : A); ++a) {   // warp-uniform: a whole warp is one stream
+        float v = __fmul_rn(h[z], w5[a]);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, o));
+        if ((t & 31) == 0) red[z][value][w][value ? 0 : a] = v;
+      }
+    }
+  }
+  __syncthreads();
+  if (t < nets * C) {
+    const int z = t / C, a = t % C, sv = a == A;
+    float v = 0.f;
+#pragma unroll
+    for (int wI = 0; wI < kWarps; ++wI) v = __fadd_rn(v, red[z][sv][wI][sv ? 0 : a]);
+    s_va[z][a] = v;
+    va[(int64_t(z) * ld + b) * C + a] = v;
+  }
+  __syncthreads();
+  if (t < nets) {
+    float s = 0.f;
+    for (int j = 0; j < A; ++j) s = __fadd_rn(s, s_va[t][j]);
+    s_m[t] = __fdiv_rn(s, float(A));
+  }
+  __syncthreads();
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float q = __fadd_rn(s_va[z][A], __fsub_rn(s_va[z][a], s_m[z]));
+    (z == 0 ? q_online : (kSlots == 3 && z == 2) ? q_online_post : q_target)[b * A + a] = q;
+    s_q[z][a] = q;
+  }
+  if (!td.enable) {
+    kt_end(kt);
+    return;
+  }
+  __syncthreads();
+  if (t == 0) {   // k_head's TD step, line for line, on the dueling Q (a shared helper changed k_head<3, false>'s SASS)
+    const int a = td_a;
+    const double rr = fmin(fmax(double(td_r), td.min_reward), td.max_reward);
+    float maxq;
+    if constexpr (kSlots == 3) {
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (s_q[2][j] > s_q[2][best]) best = j;
+      maxq = s_q[1][best];
+    } else {
+      maxq = s_q[1][0];
+      for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);
+    }
+    double y;
+    if constexpr (kNstep) y = td_term ? td_ret : __dadd_rn(td_ret, __dmul_rn(td_g, double(maxq)));
+    else y = td_term ? rr : rr + td.discount * double(maxq);
+    const float target = static_cast<float>(y);
+    float d = s_q[0][a] - target;
+    if (td.isw) {
+      const float wb = td.isw[b];
+      td.td_err[b] = d;
+      td.row_cost[b] = wb * (0.5f * d * d);
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+      d = d * wb;
+    } else {
+      td.row_cost[b] = 0.5f * d * d;
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+    }
+    for (int j = 0; j < A; ++j) td.delta[b * A + j] = (j == a) ? d : 0.f;
+    s_d = d;
+    s_a = a;
+  }
+  __syncthreads();
+  const float d = s_d, g = __fdiv_rn(d, float(A)), hv = h[0];
+  const int a = s_a;
+  const float* w5 = w5_online + k * C;
+  float* dw = td.dw5_rows + (int64_t(b) * kHidden + k) * C;   // per-row partial, summed by the optimizer
+  float o;
+  if (value) {
+    o = __fmul_rn(d, w5[A]);
+    dw[A] = __fmul_rn(hv, d);
+  } else {
+    o = 0.f;
+    for (int j = 0; j < A; ++j) {
+      const float dA = j == a ? __fsub_rn(d, g) : -g;
+      o = __fadd_rn(o, __fmul_rn(dA, w5[j]));
+      dw[j] = __fmul_rn(hv, dA);
+    }
+  }
+  o = hv > 0.f ? o : 0.f;
+  td.dz4[b * kDuelHidden + t] = o;
+  if (td.dz4_hi) {   // the tensor-core dgrad / wgrad operand: hi and scaled lo fp16 planes, as k_head writes them
+    const __half hh = __float2half_rn(o);
+    td.dz4_hi[b * kDuelHidden + t] = hh;
+    td.dz4_hi[td.dz4_lo_off + b * kDuelHidden + t] = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+  }
+  kt_end(kt);
+}
+
 // cost = mean over the batch of the per-sample costs (GeneralizedCost.get_cost, src/deepqnetwork.py:154), summed in
 // row order by one thread (deterministic); advances the cost ring and the step counter.  Runs off the critical
 // chain (the stream of the fc2 optimizer): nothing on the device waits for the scalar.
@@ -651,6 +792,15 @@ struct FrameSource {
   int shift[2];
 };
 
+// fc1's forward on the SIMT engine at width W (kHidden, or kDuelHidden on a dueling net)
+template <int W>
+static int fc1_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int rows, cudaStream_t st) {
+  Fc1Fwd<W> p;
+  for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h3[z]; p.w[z] = w[z] + n->lt.off[3]; }
+  p.part = n->d_fc1part; p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+  return launch_gemm<Fc1Fwd<W>, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, W, nets * kFc1Splits, st);
+}
+
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
 // for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
@@ -688,15 +838,20 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
       p.nb = rows;
       if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
     }
-    {
-      Fc1Fwd p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h3[z]; p.w[z] = w[z] + lt.off[3]; }
-      p.part = n->d_fc1part; p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
-      if ((rc = launch_gemm<Fc1Fwd, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, kHidden, nets * kFc1Splits, st))) return rc;
-    }
+    if ((rc = n->dueling ? fc1_fwd_simt<kDuelHidden>(n, w, nets, rows, st) : fc1_fwd_simt<kHidden>(n, w, nets, rows, st)))
+      return rc;
   }
   const int fc1_splits = n->cfg.math_mode == B200DQN_MATH_TCGEN05 ? umma_fc1_splits(rows) : kFc1Splits;
   const bool nstep = td.enable && td.nstep > 1;
+  if (n->dueling) {
+    B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head_duel<3, true> : k_head_duel<3, false>)
+                                       : (nstep ? k_head_duel<2, true> : k_head_duel<2, false>),
+                             dim3(rows), dim3(kDuelHidden), 0, st, (const float*)n->d_fc1part, fc1_splits, rows, nets,
+                             n->nb, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1],
+                             n->d_q[2], n->d_va, n->A, td, ktrace_slot("head_duel")));
+    B2_PROF(td.enable ? "head_duel(td+fc2_bwd)" : "head_duel", st);
+    return B200DQN_OK;
+  }
   if (n->atoms) {
     const int ncols = n->fc2_cols();
     B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
@@ -728,6 +883,18 @@ static int wgrad_chunk(int kred, int base) {
   return round_up(c, 16);
 }
 
+template <int W>
+static int fc1_wgrad_simt(b200dqn_net* n, int rows, cudaStream_t st) {
+  Fc1Wgrad<W> p{n->d_h3[0], n->d_dz4, n->d_part + n->lt.part_off[3], rows};
+  return launch_gemm<Fc1Wgrad<W>, 64, 64, 16, 4, 4>("fc1_wgrad", p, kFlat, W, 1, st);
+}
+
+template <int W>
+static int fc1_dgrad_simt(b200dqn_net* n, int rows, cudaStream_t st) {
+  Fc1Dgrad<W> p{n->d_dz4, n->d_w + n->lt.off[3], n->d_h3[0], n->d_dz3, rows};
+  return launch_gemm<Fc1Dgrad<W>, 32, 32, 16, 2, 2>("fc1_dgrad", p, rows, kFlat, 1, st);
+}
+
 enum BwdOp { kFc1Wgrad, kFc1Dgrad, kConv3Wgrad, kConv3Dgrad, kConv2Wgrad, kConv2Dgrad, kConv1Wgrad };
 
 // One GEMM-shaped backward op on stream `st`, on whichever engine math_mode selects.  release_early (tensor-core
@@ -740,14 +907,10 @@ static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cud
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
     return umma_backward_op(n, int(op), fs.src[0], fs.idx[0], fs.shift[0], rows, st, release_early);
   switch (op) {
-    case kFc1Wgrad: {
-      Fc1Wgrad p{n->d_h3[0], n->d_dz4, n->d_part + lt.part_off[3], rows};
-      return launch_gemm<Fc1Wgrad, 64, 64, 16, 4, 4>("fc1_wgrad", p, kFlat, kHidden, 1, st);
-    }
-    case kFc1Dgrad: {
-      Fc1Dgrad p{n->d_dz4, w + lt.off[3], n->d_h3[0], n->d_dz3, rows};
-      return launch_gemm<Fc1Dgrad, 32, 32, 16, 2, 2>("fc1_dgrad", p, rows, kFlat, 1, st);
-    }
+    case kFc1Wgrad:
+      return n->dueling ? fc1_wgrad_simt<kDuelHidden>(n, rows, st) : fc1_wgrad_simt<kHidden>(n, rows, st);
+    case kFc1Dgrad:
+      return n->dueling ? fc1_dgrad_simt<kDuelHidden>(n, rows, st) : fc1_dgrad_simt<kHidden>(n, rows, st);
     case kConv3Wgrad: {
       using P = ConvWgrad<kP2, kC2, 3, 1, kC3>;
       P p{n->d_h2[0], n->d_dz3, n->d_part + lt.part_off[2], rows, wgrad_chunk(rows * kP3 * kP3, 112)};
@@ -1204,7 +1367,7 @@ static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* acti
 
 // ---------------------------------------------------------------- layout conversion (host)
 // Neon layout <-> internal layout index map for one layer; returns internal linear index.
-static inline int64_t neon_to_internal(int layer, int64_t i, int A) {
+static inline int64_t neon_to_internal(int layer, int64_t i, int A, int hidden) {
   switch (layer) {
     case 0: return i;  // (c,r,s) x K: identical
     case 1: {          // neon rows (c,r,s), C=32,R=4 -> internal rows (r,s,c)
@@ -1217,12 +1380,12 @@ static inline int64_t neon_to_internal(int layer, int64_t i, int A) {
       const int c = int(row / 9), r = int(row / 3) % 3, s = int(row % 3);
       return ((int64_t(r) * 3 + s) * kC2 + c) * kC3 + k;
     }
-    case 3: {          // neon W[n][(c,p,q)] -> internal W[(p,q,c)][n]
+    case 3: {          // neon W[n][(c,p,q)] -> internal W[(p,q,c)][n], n < hidden
       const int64_t nn = i / kFlat, col = i % kFlat;
       const int c = int(col / 49), p = int(col / 7) % 7, q = int(col % 7);
-      return ((int64_t(p) * 7 + q) * kC3 + c) * kHidden + nn;
+      return ((int64_t(p) * 7 + q) * kC3 + c) * hidden + nn;
     }
-    default: {         // neon W[a][k] -> internal W[k][a]
+    default: {         // neon W[a][k] -> internal W[k][a] (dueling: a = A is the value row)
       const int64_t a = i / kHidden, k = i % kHidden;
       return k * A + a;
     }
@@ -1253,6 +1416,7 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->num_atoms = 0;            // scalar head; the distributional head's support defaults to [-10, 10]
   cfg->v_min = -10.0;
   cfg->v_max = 10.0;
+  cfg->dueling = 0;              // one value stream
   return B200DQN_OK;
 }
 
@@ -1275,6 +1439,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
              "net_create: num_atoms %d is neither 0 (scalar head) nor in [2,%d]", cfg->num_atoms, kMaxAtoms);
   B2_REQUIRE(cfg->num_atoms == 0 || (std::isfinite(cfg->v_min) && std::isfinite(cfg->v_max) && cfg->v_min < cfg->v_max),
              B200DQN_EINVAL, "net_create: the support needs finite v_min < v_max (got %g, %g)", cfg->v_min, cfg->v_max);
+  B2_REQUIRE(cfg->dueling == 0 || cfg->dueling == 1, B200DQN_EINVAL, "net_create: dueling %d is neither 0 nor 1",
+             cfg->dueling);
+  B2_REQUIRE(!(cfg->dueling && cfg->num_atoms), B200DQN_ENOTIMPL,
+             "net_create: a dueling net with a distributional head is not implemented");
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -1285,11 +1453,13 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->nb = cfg->batch_size;
   n->A = cfg->num_actions;
   n->atoms = cfg->num_atoms;
+  n->dueling = cfg->dueling != 0;
+  n->hidden = n->dueling ? kDuelHidden : kHidden;
   if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
   const int nb = n->nb, A = n->A, hist = cfg->history_length;
   LayerTable& lt = n->lt;
   const int rows_[kLayers] = {64 * hist, kK2, kK3, kFlat, kHidden};   // conv1: one 64-tap k-block per frame
-  const int cols_[kLayers] = {kC1, kC2, kC3, kHidden, n->fc2_cols()};
+  const int cols_[kLayers] = {kC1, kC2, kC3, n->hidden, n->fc2_cols()};
   lt.off[0] = 0;
   for (int l = 0; l < kLayers; ++l) {
     lt.rows[l] = rows_[l];
@@ -1345,12 +1515,12 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(fmalloc(&n->d_h1[z], size_t(nb) * kP1 * kP1 * kC1));
     B2_CHECK_CUDA(fmalloc(&n->d_h2[z], size_t(nb) * kP2 * kP2 * kC2));
     B2_CHECK_CUDA(fmalloc(&n->d_h3[z], size_t(nb) * kFlat));
-    B2_CHECK_CUDA(fmalloc(&n->d_h4[z], size_t(nb) * kHidden));
+    B2_CHECK_CUDA(fmalloc(&n->d_h4[z], size_t(nb) * n->hidden));
   }
   for (int z = 0; z < 3; ++z) B2_CHECK_CUDA(fmalloc(&n->d_q[z], size_t(nb) * A));
-  B2_CHECK_CUDA(fmalloc(&n->d_fc1part, size_t(2) * kFc1Splits * nb * kHidden));
+  B2_CHECK_CUDA(fmalloc(&n->d_fc1part, size_t(2) * kFc1Splits * nb * n->hidden));
   B2_CHECK_CUDA(fmalloc(&n->d_delta, size_t(nb) * A));
-  B2_CHECK_CUDA(fmalloc(&n->d_dz4, size_t(nb) * kHidden));
+  B2_CHECK_CUDA(fmalloc(&n->d_dz4, size_t(nb) * n->hidden));
   B2_CHECK_CUDA(fmalloc(&n->d_dz3, size_t(nb) * kFlat));
   B2_CHECK_CUDA(fmalloc(&n->d_dz2, size_t(nb) * kP2 * kP2 * kC2));
   B2_CHECK_CUDA(fmalloc(&n->d_dz1, size_t(nb) * kP1 * kP1 * kC1));
@@ -1367,6 +1537,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
     B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
   }
+  if (n->dueling) B2_CHECK_CUDA(fmalloc(&n->d_va, size_t(3) * nb * (A + 1)));
   const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
   B2_CHECK_CUDA(cudaMalloc(&n->d_pre, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_post, state_bytes + 256));
@@ -1424,6 +1595,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_act); cudaFree(n->d_term); cudaFree(n->d_rew); cudaFree(n->d_iota1); cudaFree(n->d_iota4);
   cudaFree(n->d_td_err);
   cudaFree(n->d_logits); cudaFree(n->d_probs); cudaFree(n->d_tdist); cudaFree(n->d_lgrad); cudaFree(n->d_act_rows);
+  cudaFree(n->d_va);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -1433,7 +1605,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
 extern "C" int b200dqn_net_layer_shape(const b200dqn_net* n, int layer, int* rows, int* cols) {
   B2_REQUIRE(n && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_layer_shape: bad layer");
   // NEON shapes: conv (C*R*S, K); linear (nout, nin)
-  const int r[kLayers] = {n->lt.rows[0], kK2, kK3, kHidden, n->fc2_cols()};
+  const int r[kLayers] = {n->lt.rows[0], kK2, kK3, n->hidden, n->fc2_cols()};
   const int c[kLayers] = {kC1, kC2, kC3, kFlat, kHidden};
   if (rows) *rows = r[layer];
   if (cols) *cols = c[layer];
@@ -1444,13 +1616,13 @@ static int xfer_params(b200dqn_net* n, float* dev_base, int layer, float* host, 
   const int64_t off = n->lt.off[layer], cnt = n->lt.off[layer + 1] - off;
   std::vector<float> tmp(cnt);
   if (to_device) {
-    for (int64_t i = 0; i < cnt; ++i) tmp[neon_to_internal(layer, i, n->fc2_cols())] = host[i];
+    for (int64_t i = 0; i < cnt; ++i) tmp[neon_to_internal(layer, i, n->fc2_cols(), n->hidden)] = host[i];
     B2_CHECK_CUDA(cudaMemcpyAsync(dev_base + off, tmp.data(), cnt * sizeof(float), cudaMemcpyHostToDevice, st));
     B2_CHECK_CUDA(cudaStreamSynchronize(st));
   } else {
     B2_CHECK_CUDA(cudaMemcpyAsync(tmp.data(), dev_base + off, cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
     B2_CHECK_CUDA(cudaStreamSynchronize(st));
-    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[neon_to_internal(layer, i, n->fc2_cols())];
+    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[neon_to_internal(layer, i, n->fc2_cols(), n->hidden)];
   }
   return B200DQN_OK;
 }
@@ -1881,8 +2053,8 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_H1: p = n->d_h1[0]; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
     case B200DQN_NET_PTR_H2: p = n->d_h2[0]; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_H3: p = n->d_h3[0]; b = size_t(n->nb) * kFlat * 4; break;
-    case B200DQN_NET_PTR_H4: p = n->d_h4[0]; b = size_t(n->nb) * kHidden * 4; break;
-    case B200DQN_NET_PTR_DZ4: p = n->d_dz4; b = size_t(n->nb) * kHidden * 4; break;
+    case B200DQN_NET_PTR_H4: p = n->d_h4[0]; b = size_t(n->nb) * n->hidden * 4; break;
+    case B200DQN_NET_PTR_DZ4: p = n->d_dz4; b = size_t(n->nb) * n->hidden * 4; break;
     case B200DQN_NET_PTR_DZ3: p = n->d_dz3; b = size_t(n->nb) * kFlat * 4; break;
     case B200DQN_NET_PTR_DZ2: p = n->d_dz2; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_DZ1: p = n->d_dz1; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
@@ -1912,9 +2084,14 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       B2_REQUIRE(n->cfg.math_mode == B200DQN_MATH_TCGEN05 && hi, B200DQN_EINVAL,
                  "net_device_ptr: the dZ4 planes exist on the tensor-core engine only");
       p = hi;
-      b = size_t(lo_off + int64_t(n->nb) * kHidden) * 2;
+      b = size_t(lo_off + int64_t(n->nb) * n->hidden) * 2;
       break;
     }
+    case B200DQN_NET_PTR_DUELING_VA:
+      B2_REQUIRE(n->dueling, B200DQN_EINVAL, "net_device_ptr: selector %d needs a dueling net", which);
+      p = n->d_va;
+      b = size_t(3) * n->nb * (n->A + 1) * 4;
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -1938,8 +2115,8 @@ static int double_q_alloc(b200dqn_net* n) {
   B2_CHECK_CUDA(cudaDeviceSynchronize());   // no step or predict in flight still reads the old partial buffer
   const size_t nb = size_t(n->nb);
   float* part = nullptr;
-  B2_CHECK_CUDA(cudaMalloc(&part, size_t(3) * kFc1Splits * nb * kHidden * sizeof(float)));
-  B2_CHECK_CUDA(cudaMemset(part, 0, size_t(3) * kFc1Splits * nb * kHidden * sizeof(float)));
+  B2_CHECK_CUDA(cudaMalloc(&part, size_t(3) * kFc1Splits * nb * n->hidden * sizeof(float)));
+  B2_CHECK_CUDA(cudaMemset(part, 0, size_t(3) * kFc1Splits * nb * n->hidden * sizeof(float)));
   cudaFree(n->d_fc1part);
   n->d_fc1part = part;
   if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }

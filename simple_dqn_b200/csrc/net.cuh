@@ -52,7 +52,7 @@ struct b200dqn_net {
   // activations: [0] online, [1] target, [2] online on the poststates (Double DQN; SIMT engine only, allocated
   // when double Q is first switched on)
   float* d_h1[3] = {}, *d_h2[3] = {}, *d_h3[3] = {}, *d_h4[2] = {};
-  float* d_fc1part = nullptr;  // [2*splits][nb][512], [3*splits][nb][512] once double Q has been switched on
+  float* d_fc1part = nullptr;  // [2*splits][nb][hidden], [3*splits][nb][hidden] once double Q has been switched on
   float* d_q[3] = {};          // [nb][A]: preq, postq, Q_online_post (Double DQN)
   float* d_delta = nullptr;    // [nb][A] clipped
   float* d_dz4 = nullptr, *d_dz3 = nullptr, *d_dz2 = nullptr, *d_dz1 = nullptr;
@@ -114,7 +114,13 @@ struct b200dqn_net {
   float* d_tdist = nullptr;      // [nb][atoms] projected target distribution
   float* d_lgrad = nullptr;      // [nb][atoms] gradient on the taken action's logits
   int32_t* d_act_rows = nullptr; // [nb] taken action of each row of the last train step (selects the dW5 block)
-  int fc2_cols() const { return atoms ? A * atoms : A; }
+  int fc2_cols() const { return atoms ? A * atoms : dueling ? A + 1 : A; }
+
+  // dueling network (cfg.dueling): fc1 is kDuelHidden wide (advantage units [0, 512), value units [512, 1024)) and
+  // fc2 is block-structured [512][A + 1]: column a < A reads the advantage units, column A the value units
+  bool dueling = false;
+  int hidden = b200::kHidden;    // fc1's width: H4, dZ4 and the fc1 partials are [.][hidden]
+  float* d_va = nullptr;         // [3][nb][A + 1]: the advantages, then V, of every slot of the last forward
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

@@ -7,6 +7,7 @@
 //
 // Geometry is the reference's (src/deepqnetwork.py:77-92): 84x84xH u8 (H = history_length frames as input
 // channels) -> conv 8x8x32 s4 -> conv 4x4x64 s2 -> conv 3x3x64 s1 -> fc 512 -> fc A; no bias, no padding.
+// A dueling net (b200dqn_net_config::dueling) has fc 1024 -> fc A + 1 in place of the last two.
 //
 // Internal layouts (HBM):
 //   activations  NHWC fp32:  H1[n][20][20][32]  H2[n][9][9][64]  H3[n][7][7][64]  H4[n][512]
@@ -27,6 +28,7 @@ constexpr int kP2 = 9, kC2 = 64;                // conv2 output
 constexpr int kP3 = 7, kC3 = 64;                // conv3 output
 constexpr int kFlat = kP3 * kP3 * kC3;          // 3136
 constexpr int kHidden = 512;
+constexpr int kDuelHidden = 2 * kHidden;      // dueling fc1: advantage units [0, 512), value units [512, 1024)
 constexpr int kK2 = 4 * 4 * kC1;                // 512
 constexpr int kK3 = 3 * 3 * kC2;                // 576
 
@@ -154,22 +156,23 @@ struct ConvFwd {
 };
 
 // fc1 forward with split-K: z = net * splits + split; partial[z][m][n].  ReLU is applied by the
-// consumer (k_fc2_fwd) after it sums the splits.
+// consumer (the head) after it sums the splits.  W = fc1's width: kHidden, or kDuelHidden on a dueling net.
+template <int W>
 struct Fc1Fwd {
   const float* in[3];   // H3 flat [nb][3136]
-  const float* w[3];    // W4 [3136][512]
-  float* part;          // [nets*splits][nb][512]
+  const float* w[3];    // W4 [3136][W]
+  float* part;          // [nets*splits][nb][W]
   int nb, splits, kchunk;
   static constexpr bool kAKContig = true, kBKContig = false;
   __device__ int M(int) const { return nb; }
-  __device__ int N(int) const { return kHidden; }
+  __device__ int N(int) const { return W; }
   __device__ void krange(int z, int& kb, int& ke) const {
     kb = (z % splits) * kchunk;
     ke = min(kb + kchunk, kFlat);
   }
   __device__ float a(int z, int m, int k) const { return slot3(in, z / splits)[m * kFlat + k]; }
-  __device__ float b(int z, int k, int n) const { return slot3(w, z / splits)[k * kHidden + n]; }
-  __device__ void store(int z, int m, int n, float v) const { part[(z * nb + m) * kHidden + n] = v; }
+  __device__ float b(int z, int k, int n) const { return slot3(w, z / splits)[k * W + n]; }
+  __device__ void store(int z, int m, int n, float v) const { part[(z * nb + m) * W + n] = v; }
 };
 
 // ------------------------------------------------------------------------------------------
@@ -178,18 +181,19 @@ struct Fc1Fwd {
 // ------------------------------------------------------------------------------------------
 
 // fc1 dgrad: dZ3[b][k] = (sum_n dZ4[b][n] * W4[k][n]) * (H3[b][k] > 0)
+template <int W>
 struct Fc1Dgrad {
-  const float* dz4;  // [nb][512]
-  const float* w4;   // [3136][512]
+  const float* dz4;  // [nb][W]
+  const float* w4;   // [3136][W]
   const float* h3;   // [nb][3136]
   float* dz3;        // [nb][3136]
   int nb;
   static constexpr bool kAKContig = true, kBKContig = true;
   __device__ int M(int) const { return nb; }
   __device__ int N(int) const { return kFlat; }
-  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = kHidden; }
-  __device__ float a(int, int m, int k) const { return dz4[m * kHidden + k]; }
-  __device__ float b(int, int k, int n) const { return w4[n * kHidden + k]; }
+  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = W; }
+  __device__ float a(int, int m, int k) const { return dz4[m * W + k]; }
+  __device__ float b(int, int k, int n) const { return w4[n * W + k]; }
   __device__ void store(int, int m, int n, float v) const {
     const int i = m * kFlat + n;
     dz3[i] = h3[i] > 0.f ? v : 0.f;
@@ -197,18 +201,19 @@ struct Fc1Dgrad {
 };
 
 // fc1 wgrad: dW4[k][n] = sum_b H3[b][k] * dZ4[b][n]   (reduction dim = batch, no split)
+template <int W>
 struct Fc1Wgrad {
   const float* h3;
   const float* dz4;
-  float* dw4;  // [3136][512]
+  float* dw4;  // [3136][W]
   int nb;
   static constexpr bool kAKContig = false, kBKContig = false;
   __device__ int M(int) const { return kFlat; }
-  __device__ int N(int) const { return kHidden; }
+  __device__ int N(int) const { return W; }
   __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = nb; }
   __device__ float a(int, int m, int k) const { return h3[k * kFlat + m]; }
-  __device__ float b(int, int k, int n) const { return dz4[k * kHidden + n]; }
-  __device__ void store(int, int m, int n, float v) const { dw4[m * kHidden + n] = v; }
+  __device__ float b(int, int k, int n) const { return dz4[k * W + n]; }
+  __device__ void store(int, int m, int n, float v) const { dw4[m * W + n] = v; }
 };
 
 // conv dgrad (input gradient of a stride-ST RxR conv, NHWC), decomposed by output-parity class

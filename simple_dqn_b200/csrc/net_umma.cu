@@ -440,6 +440,8 @@ static int launch_conv23(const Conv23Fwd& p, int rows, int nets, cudaStream_t st
   return B200DQN_OK;
 }
 
+// W = fc1's width (kHidden, or kDuelHidden on a dueling net) in the fc1 problems, image and update below.
+template <int W>
 struct V2Fc1Fwd {
   static constexpr int kBN = 32;
   static constexpr bool kAExact = false, kARowMajorThreads = false, kBRowMajorThreads = true;
@@ -451,10 +453,10 @@ struct V2Fc1Fwd {
   static constexpr bool kAMnMajor = true;
   static constexpr uint32_t kAMnLoOffset = 128 * 128;   // lo half of a [hi 128x128 B | lo 128x128 B] tile
   PlanePair in16[3];        // H3 planes [rows][3136]
-  const uint8_t* wimg[2];   // [25 flat tiles][8 hidden blocks][hi 128x128 | lo 128x128]
-  float* part;              // [nets*splits][rows][512]
+  const uint8_t* wimg[2];   // [25 flat tiles][W / 64 hidden blocks][hi 128x128 | lo 128x128]
+  float* part;              // [nets*splits][rows][W]
   int rows, splits;
-  __device__ int M(int) const { return kHidden; }
+  __device__ int M(int) const { return W; }
   __device__ int N(int) const { return rows; }
   __device__ void krange(int z, int& kb, int& ke) const {
     const int per = (kFlat / 64 + splits - 1) / splits;
@@ -463,7 +465,7 @@ struct V2Fc1Fwd {
   }
   // hi sub-tile [64 flat rows x 64 hidden] of hidden block 2*mtile + chunk, flat k-block kb
   __device__ const uint8_t* a_sub(int z, int mtile, int kb, int chunk) const {
-    return wslot(wimg, z / splits) + (int64_t(kb >> 1) * (kHidden / 64) + 2 * mtile + chunk) * (128 * 256) +
+    return wslot(wimg, z / splits) + (int64_t(kb >> 1) * (W / 64) + 2 * mtile + chunk) * (128 * 256) +
            (kb & 1) * (64 * 128);
   }
   __device__ umma2::Planes b_planes(int z) const { return {slot3(in16, z / splits).hi, in16[0].lo_off}; }
@@ -475,30 +477,31 @@ struct V2Fc1Fwd {
   __device__ void store8(int z, int m, int n0, const float v[8]) const {
 #pragma unroll
     for (int j = 0; j < 8; ++j)
-      if (n0 + j < rows) part[(z * rows + n0 + j) * kHidden + m] = v[j];
+      if (n0 + j < rows) part[(z * rows + n0 + j) * W + m] = v[j];
   }
 };
 
 // ---- dgrad -------------------------------------------------------------------------------
+template <int W>
 struct V2Fc1Dgrad {
   static constexpr int kBN = 32;
   static constexpr bool kAExact = false, kARowMajorThreads = true, kBRowMajorThreads = true;
   static constexpr int kAMode = umma2::kBulk, kBMode = umma2::kAsync;
   static constexpr bool kStagedEpilogue = false, kDumpA = false, kPrefetch = true;
-  const uint8_t* wimg;   // [25 mtiles][8 kb][hi | lo]   rows m = flat index (p,q,c), K = hidden unit
-  PlanePair dz4;         // [rows][512]
+  const uint8_t* wimg;   // [25 mtiles][W / 64 kb][hi | lo]   rows m = flat index (p,q,c), K = hidden unit
+  PlanePair dz4;         // [rows][W]
   const float* h3;       // [rows][3136] (mask)
   float* dz3;
   PlanePair dz3_16;
   int rows;
   __device__ int M(int) const { return kFlat; }
   __device__ int N(int) const { return rows; }
-  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = kHidden / 64; }
+  __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = W / 64; }
   __device__ const uint8_t* a_tile(int, int mtile, int kb) const {
-    return wimg + (int64_t(mtile) * (kHidden / 64) + kb) * (128 * 256);
+    return wimg + (int64_t(mtile) * (W / 64) + kb) * (128 * 256);
   }
   __device__ umma2::Planes b_planes(int) const { return {dz4.hi, dz4.lo_off}; }
-  __device__ umma2::RowCtx b_row(int, int n) const { return {int64_t(n) * kHidden, 0, 0, n < rows}; }
+  __device__ umma2::RowCtx b_row(int, int n) const { return {int64_t(n) * W, 0, 0, n < rows}; }
   __device__ bool b_chunk(int, const umma2::RowCtx& rc, int kk, int64_t& off) const {
     off = rc.base + kk;
     return true;
@@ -643,15 +646,16 @@ struct WConv1Wgrad {
 };
 
 // fc1: dW4[m][n] = sum_b H3[b][m] * dZ4[b][n]; the reduction rows are the batch samples.
+template <int W>
 struct WFc1Wgrad {
   static constexpr int kBN = 64, kStages = 2;
   static constexpr bool kAExact = false, kABulk = false;
   PlanePair h3_16;   // [rows][3136]
-  PlanePair dz4_16;  // [rows][512]
-  float* dw4;        // [3136][512]
+  PlanePair dz4_16;  // [rows][W]
+  float* dw4;        // [3136][W]
   int rows;
   __device__ int M(int) const { return kFlat; }
-  __device__ int N(int) const { return kHidden; }
+  __device__ int N(int) const { return W; }
   __device__ void krange(int, int& kb, int& ke) const { kb = 0; ke = (rows + 63) / 64; }
   __device__ umma_mn::PixCtx pix(int, int b) const { return {b, 0, 0, b < rows}; }
   __device__ umma2::Planes a_planes(int) const { return {h3_16.hi, h3_16.lo_off}; }
@@ -660,8 +664,8 @@ struct WFc1Wgrad {
     return mchunk * 64 < kFlat;
   }
   __device__ umma2::Planes b_planes(int) const { return {dz4_16.hi, dz4_16.lo_off}; }
-  __device__ int64_t b_off(int, const umma_mn::PixCtx& px) const { return int64_t(px.n) * kHidden; }
-  __device__ void store8(int, int m, int n0, const float v[8]) const { st8(dw4 + int64_t(m) * kHidden + n0, v); }
+  __device__ int64_t b_off(int, const umma_mn::PixCtx& px) const { return int64_t(px.n) * W; }
+  __device__ void store8(int, int m, int n0, const float v[8]) const { st8(dw4 + int64_t(m) * W + n0, v); }
 };
 
 // Data-parallel variant: the rows are ALL learners' samples, read from the gather areas that every rank's
@@ -702,16 +706,17 @@ struct PackFwdConv {   // B operand of a forward conv: rows = output channel n, 
     for (int j = 0; j < 8; ++j) v[j] = w[(k0 + j) * N + r];
   }
 };
+template <int W>
 struct PackFc1Dgrad {  // the fc1 image: rows = flat index m, 64 hidden units per row (dgrad: K-major A; forward: MN-major A)
   static constexpr bool kRowMajorThreads = true;
   const float* w;
   __host__ __device__ int tiles() const { return (kFlat + 127) / 128; }
   __host__ __device__ int rows() const { return 128; }
-  __host__ __device__ int kblocks() const { return kHidden / 64; }
+  __host__ __device__ int kblocks() const { return W / 64; }
   __device__ void src8(int tile, int r, int k0, float v[8]) const {
     const int m = tile * 128 + r;
     if (m >= kFlat) { zero8(v); return; }
-    ld8(w + m * kHidden + k0, v);
+    ld8(w + m * W + k0, v);
   }
 };
 template <int H, int C, int R, int ST, int KO>
@@ -839,23 +844,24 @@ k_opt_conv(const float* __restrict__ part, int splits, float* __restrict__ w, fl
 // column-oriented (forward) image is rebuilt by k_pack_image right after.  Both kernels are smem-free,
 // light on registers and launched on a CAPPED grid (2 CTAs per SM, grid-stride loop) so that they
 // co-reside with the tensor-core kernels of the critical chain instead of locking them out of the SMs.
+template <int W>
 __global__ void __launch_bounds__(256)
 k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
           const OptArgs opt, const KTrace kt) {
   kt_begin(kt);
   pdl_wait();
   pdl_launch_dependents();
-  constexpr int kNB = kHidden / 8;
+  constexpr int kNB = W / 8;
   const float l_step = opt_step_scalar(opt);
   for (int id = blockIdx.x * blockDim.x + threadIdx.x; id < kFlat * kNB; id += gridDim.x * blockDim.x) {
     const int m = id / kNB, n0 = (id % kNB) * 8;
-    const int64_t i = int64_t(m) * kHidden + n0;
+    const int64_t i = int64_t(m) * W + n0;
     float g[8], wv[8];
     ld8(dw + i, g);
     opt_update_vec<8>(opt, l_step, g, wv, w + i, sst + i);   // the configured Neon optimizer (optim.cuh)
     uint4 hi, lo;
     umma::split8(wv, hi, lo);
-    uint8_t* base = img_dgr + (int64_t(m / 128) * (kHidden / 64) + n0 / 64) * (128 * 256) +
+    uint8_t* base = img_dgr + (int64_t(m / 128) * (W / 64) + n0 / 64) * (128 * 256) +
                     umma::sw128_off(m % 128, (n0 % 64) / 8);
     *reinterpret_cast<uint4*>(base) = hi;
     *reinterpret_cast<uint4*>(base + 128 * 128) = lo;
@@ -872,7 +878,8 @@ int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g) {
   // 6.4 MB written per step, 5 us at the end of the fc1 branch) are gone.
   // capped grid (2 CTAs per SM, grid-stride): the kernel shares the SMs — and the L2 — with the dgrad chain
   const int ctas = 2 * n->sm_count;
-  B2_CHECK_CUDA(launch_pdl(k_opt_fc1, dim3(ctas), dim3(256), 0, st, dw, n->d_w + lt.off[3],
+  B2_CHECK_CUDA(launch_pdl(n->dueling ? k_opt_fc1<kDuelHidden> : k_opt_fc1<kHidden>, dim3(ctas), dim3(256), 0, st, dw,
+                           n->d_w + lt.off[3],
                            n->d_s + lt.off[3], u->img_dgr[0], make_opt_args(n, rows), ktrace_slot("opt_fc1")));
   B2_PROF("opt_fc1", st);
   return B200DQN_OK;
@@ -942,12 +949,12 @@ int umma_opt_conv_xll(b200dqn_net* n, int l, int rows, cudaStream_t st, const ch
   return B200DQN_OK;
 }
 
-static int64_t fwd_image_bytes(int layer, int hist) {
+static int64_t fwd_image_bytes(int layer, int hist, int hidden) {
   switch (layer) {
     case 0: return int64_t(hist) * kC1 * 256;
     case 1: return int64_t(kK2 / 64) * kC2 * 256;
     case 2: return int64_t(kK3 / 64) * kC3 * 256;
-    default: return int64_t((kFlat + 127) / 128) * (kHidden / 64) * 128 * 256;   // fc1: the row-oriented image
+    default: return int64_t((kFlat + 127) / 128) * (hidden / 64) * 128 * 256;   // fc1: the row-oriented image
   }
 }
 
@@ -977,7 +984,8 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
           rc = umma2::launch_pack("pack_c3d", PackConvDgrad<kP2, kC2, 3, 1, kC3>{w + lt.off[2]}, u->img_dgr[1], st);
         break;
       case 3:
-        rc = umma2::launch_pack("pack_fc1", PackFc1Dgrad{w + lt.off[3]}, u->img_fwd[which][3], st);
+        rc = n->dueling ? umma2::launch_pack("pack_fc1", PackFc1Dgrad<kDuelHidden>{w + lt.off[3]}, u->img_fwd[which][3], st)
+                        : umma2::launch_pack("pack_fc1", PackFc1Dgrad<kHidden>{w + lt.off[3]}, u->img_fwd[which][3], st);
         break;
       default: break;  // fc2 runs on CUDA cores (N = A <= 18)
     }
@@ -1022,7 +1030,7 @@ int umma_net_init(b200dqn_net* n) {
   u->h_elems[0] = int64_t(nb) * kP1 * kP1 * kC1;
   u->h_elems[1] = int64_t(nb) * kP2 * kP2 * kC2;
   u->h_elems[2] = int64_t(nb) * kFlat;
-  u->dz_elems[0] = int64_t(nb) * kHidden;
+  u->dz_elems[0] = int64_t(nb) * n->hidden;
   u->dz_elems[1] = int64_t(nb) * kFlat;
   u->dz_elems[2] = int64_t(nb) * kP2 * kP2 * kC2;
   u->dz_elems[3] = int64_t(nb) * kP1 * kP1 * kC1;
@@ -1037,7 +1045,7 @@ int umma_net_init(b200dqn_net* n) {
     B2_CHECK_CUDA(cudaMemset(u->dz16[i], 0, 2 * u->dz_elems[i] * sizeof(__half)));
   }
   for (int l = 0; l < 4; ++l) {
-    u->img_fwd_bytes[l] = fwd_image_bytes(l, n->cfg.history_length);
+    u->img_fwd_bytes[l] = fwd_image_bytes(l, n->cfg.history_length, n->hidden);
     for (int z = 0; z < 2; ++z) {
       if (z == 1 && n->d_tw == n->d_w) { u->img_fwd[1][l] = u->img_fwd[0][l]; continue; }
       B2_CHECK_CUDA(cudaMalloc(&u->img_fwd[z][l], u->img_fwd_bytes[l]));
@@ -1105,6 +1113,16 @@ void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
   *lo_off = u ? u->dz_elems[0] : 0;
 }
 
+template <int W>
+static int fc1_fwd_umma(b200dqn_net* n, const PlanePair h3[3], int nets, int rows, cudaStream_t st) {
+  UmmaState* u = ust(n);
+  V2Fc1Fwd<W> p;
+  for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][3];
+  for (int z = 0; z < 3; ++z) p.in16[z] = h3[z];
+  p.part = n->d_fc1part; p.rows = rows; p.splits = fc1_splits_for(rows);
+  return umma2::launch_umma2("fc1_fwd", p, W, rows, nets * p.splits, st, false);
+}
+
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
                  int nets, int rows, cudaStream_t st, bool release_early) {
   // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
@@ -1162,14 +1180,25 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
   }
   // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
   if (nets >= 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
-  {
-    V2Fc1Fwd p;
-    for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][3];
-    for (int z = 0; z < 3; ++z) p.in16[z] = planes(2, z);
-    p.part = n->d_fc1part; p.rows = rows; p.splits = fc1_splits_for(rows);
-    if ((rc = umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * p.splits, st, false))) return rc;
-  }
-  return B200DQN_OK;
+  const PlanePair h3[3] = {planes(2, 0), planes(2, 1), planes(2, 2)};
+  return n->dueling ? fc1_fwd_umma<kDuelHidden>(n, h3, nets, rows, st) : fc1_fwd_umma<kHidden>(n, h3, nets, rows, st);
+}
+
+template <int W>
+static int fc1_wgrad_umma(b200dqn_net* n, int rows, cudaStream_t st, bool release_early) {
+  UmmaState* u = ust(n);
+  WFc1Wgrad<W> p{PlanePair{u->h16[2][0], u->h_elems[2]}, PlanePair{u->dz16[0], u->dz_elems[0]},
+                 n->d_part + n->lt.part_off[3], rows};
+  return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, W, 1, st, release_early);
+}
+
+template <int W>
+static int fc1_dgrad_umma(b200dqn_net* n, int rows, cudaStream_t st, bool release_early) {
+  UmmaState* u = ust(n);
+  // the fp32 copies of dZ3/dZ2/dZ1 have no reader in this engine (wgrads and dgrads take the fp16 planes)
+  V2Fc1Dgrad<W> p{u->img_dgr[0], PlanePair{u->dz16[0], u->dz_elems[0]}, n->d_h3[0], n->keep_grads ? n->d_dz3 : nullptr,
+                  PlanePair{u->dz16[1], u->dz_elems[1]}, rows};
+  return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows, 1, st, release_early);
 }
 
 int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* idx, int shift, int rows,
@@ -1177,19 +1206,12 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
   const LayerTable& lt = n->lt;
   const float* w = n->d_w;
   switch (op) {
-    case 0: {
-      UmmaState* u = ust(n);
-      WFc1Wgrad p{PlanePair{u->h16[2][0], u->h_elems[2]}, PlanePair{u->dz16[0], u->dz_elems[0]},
-                  n->d_part + lt.part_off[3], rows};
-      return umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st, release_early);
-    }
-    case 1: {
-      UmmaState* u = ust(n);
-      // the fp32 copies of dZ3/dZ2/dZ1 have no reader in this engine (wgrads and dgrads take the fp16 planes)
-      V2Fc1Dgrad p{u->img_dgr[0], PlanePair{u->dz16[0], u->dz_elems[0]}, n->d_h3[0], n->keep_grads ? n->d_dz3 : nullptr,
-                   PlanePair{u->dz16[1], u->dz_elems[1]}, rows};
-      return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows, 1, st, release_early);
-    }
+    case 0:
+      return n->dueling ? fc1_wgrad_umma<kDuelHidden>(n, rows, st, release_early)
+                        : fc1_wgrad_umma<kHidden>(n, rows, st, release_early);
+    case 1:
+      return n->dueling ? fc1_dgrad_umma<kDuelHidden>(n, rows, st, release_early)
+                        : fc1_dgrad_umma<kHidden>(n, rows, st, release_early);
     case 2: {
       UmmaState* u = ust(n);
       using P = WConvWgrad<kP2, kC2, 3, 1, kC3>;

@@ -75,6 +75,10 @@ class DeepQNetwork:
             cfg.num_atoms = int(_arg(args, "num_atoms", 51))
             cfg.v_min = float(_arg(args, "v_min", -10.0))
             cfg.v_max = float(_arg(args, "v_max", 10.0))
+        # dueling network (Wang et al., 2016): a new capability, off unless args.dueling is set; it fixes fc1's and fc2's
+        # shapes, so it is chosen here and not switchable later
+        self.dueling = bool(_arg(args, "dueling", False))
+        cfg.dueling = int(self.dueling)
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -200,7 +204,7 @@ class DeepQNetwork:
         h1 = self._read_f32(L.NET_PTR_H1, (b, 20, 20, 32)).transpose(0, 3, 1, 2)
         h2 = self._read_f32(L.NET_PTR_H2, (b, 9, 9, 64)).transpose(0, 3, 1, 2)
         h3 = self._read_f32(L.NET_PTR_H3, (b, 7, 7, 64)).transpose(0, 3, 1, 2)
-        h4 = self._read_f32(L.NET_PTR_H4, (b, 512))
+        h4 = self._read_f32(L.NET_PTR_H4, (b, self._hidden()))
         return h1, h2, h3, h4
 
     def last_dz(self):
@@ -210,17 +214,21 @@ class DeepQNetwork:
         dz1 = self._read_f32(L.NET_PTR_DZ1, (b, 20, 20, 32)).transpose(0, 3, 1, 2)
         dz2 = self._read_f32(L.NET_PTR_DZ2, (b, 9, 9, 64)).transpose(0, 3, 1, 2)
         dz3 = self._read_f32(L.NET_PTR_DZ3, (b, 7, 7, 64)).transpose(0, 3, 1, 2)
-        dz4 = self._read_f32(L.NET_PTR_DZ4, (b, 512))
+        dz4 = self._read_f32(L.NET_PTR_DZ4, (b, self._hidden()))
         return dz1, dz2, dz3, dz4
 
+    def _hidden(self):
+        return self.layer_shapes()[3][0]                                # fc1's width: 512, or 1024 on a dueling net
+
     def last_dz4_planes(self):
-        """(hi, lo) float16 planes of dZ4 the tensor-core dgrad reads, each (batch, 512); lo is scaled by 2048."""
+        """(hi, lo) float16 planes of dZ4 the tensor-core dgrad reads, each (batch, 512), or (batch, 1024) on a dueling
+        net; lo is scaled by 2048."""
         p, b = C.c_void_p(), C.c_size_t()
         L.call("b200dqn_net_device_ptr", self._h, L.NET_PTR_DZ4_PLANES, C.byref(p), C.byref(b))
-        n = self.batch_size * 512
-        lo_off = b.value // 2 - n
-        hi = L.download(self.device, p.value, (self.batch_size, 512), np.float16, self._stream)
-        lo = L.download(self.device, p.value + 2 * lo_off, (self.batch_size, 512), np.float16, self._stream)
+        shape = (self.batch_size, self._hidden())
+        lo_off = b.value // 2 - shape[0] * shape[1]
+        hi = L.download(self.device, p.value, shape, np.float16, self._stream)
+        lo = L.download(self.device, p.value + 2 * lo_off, shape, np.float16, self._stream)
         return hi, lo
 
     def last_online_postq(self):
@@ -256,6 +264,15 @@ class DeepQNetwork:
     def last_logit_grads(self):
         """The gradient on the taken action's logits of the last train(), (batch, num_atoms) float32."""
         return self._read_f32(L.NET_PTR_LOGIT_GRADS, (self.batch_size, self.num_atoms))
+
+    # ---- dueling network: slots as for the distributional head
+    def last_advantages(self):
+        """The advantage stream's outputs A_a of the last forward, (3, batch, A) float32."""
+        return self._read_f32(L.NET_PTR_DUELING_VA, (3, self.batch_size, self.num_actions + 1))[..., :-1]
+
+    def last_values(self):
+        """The value stream's output V of the last forward, (3, batch) float32."""
+        return self._read_f32(L.NET_PTR_DUELING_VA, (3, self.batch_size, self.num_actions + 1))[..., -1]
 
     # ---- reference methods
     def update_target_network(self):

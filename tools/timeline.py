@@ -10,11 +10,13 @@ base, actions, rewards, terminals = synthetic_meta(replay)
 B = int(os.environ.get("BATCH", "32"))
 ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with this many atoms; 0: the scalar head
 NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
+DUELING = os.environ.get("DUELING", "0") == "1"   # dueling network (1024-unit fc1, advantage and value streams)
 
 
 def net_args():
     a = make_args(B)
     a.distributional, a.num_atoms = ATOMS > 0, ATOMS
+    a.dueling = DUELING
     return a
 
 
