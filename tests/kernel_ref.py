@@ -29,7 +29,8 @@ terms, with n = the full reduction length.
 Calibration (tests/test_kernel_ref.py, at every batch of the GPU sweep): the emulated scheme, with f64 sums and, for
 the weight gradients, with fp32 accumulation in k-block and split-K order, stays at least 4× inside the bound.
 A dropped A_lo or B_lo term, lo scaled by 2¹⁰, one skipped k-block, one dropped split-K partial, a zeroed last row
-and a stale lo weight image each exceed it.  A dropped lo term costs ≈ 2⁻¹²·S₂ per output, about 2⁸ times the
+and a stale lo weight image each exceed it; so does, on the dueling net's 1024-wide fc1, one of its two 512-unit
+streams dropped from fc1_fwd's output or from fc1_dgrad's reduction.  A dropped lo term costs ≈ 2⁻¹²·S₂ per output, about 2⁸ times the
 C_REP term; the constants sit between the two with room on both sides.
 """
 import numpy as np
@@ -126,9 +127,10 @@ def wgrad_split(layer, rows):
     return per, (kbs + per - 1) // per
 
 
-def chain(kernel, rows, hist=4, fc1_forced=0):
-    """Longest serial fp32 accumulation chain of one output of `kernel` at `rows` samples."""
-    fixed = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_dgrad": 512, "conv3_dgrad": 576,
+def chain(kernel, rows, hist=4, fc1_forced=0, hidden=HIDDEN):
+    """Longest serial fp32 accumulation chain of one output of `kernel` at `rows` samples.  hidden: fc1's width (512,
+    or 1024 on a dueling net), which fc1_dgrad reduces over."""
+    fixed = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_dgrad": hidden, "conv3_dgrad": 576,
              "conv2_dgrad": 256}
     if kernel in fixed:
         return fixed[kernel]
@@ -142,9 +144,9 @@ def chain(kernel, rows, hist=4, fc1_forced=0):
     return min(per * 64, rows * (400, 81, 49)[layer]) + sp
 
 
-def dispatch(rows, hist=4):
+def dispatch(rows, hist=4, hidden=HIDDEN):
     """What the engine runs at `rows` samples, for test ids and reports."""
-    return dict(conv23=rows <= 64, fc1_splits=fc1_splits(rows),
+    return dict(conv23=rows <= 64, fc1_splits=fc1_splits(rows), fc1_width=hidden,
                 wgrad_splits=tuple(wgrad_split(l, rows)[1] for l in range(3)))
 
 

@@ -436,13 +436,14 @@ def test_double_step_is_vanilla_where_the_target_cannot_differ(mode, sched, batc
     _assert_same(wa, wb)
 
 
-def _live_net(ring, mode, double_at_creation):
+def _live_net(ring, mode, double_at_creation, make=None):
+    """make(stream, double): the net (batch 32, H = 4); by default _paired's with six actions."""
     from simple_dqn_b200 import ReplayMemory, StateBuffer, Stream
     stream = Stream()
     mem = ReplayMemory(ring.size, make_args(), rng="device", stream=stream)
     mem.add_batch(ring.actions, ring.rewards, ring.screens, ring.terminals)
     mem.set_cursor(ring.count, ring.current)
-    net, _ = _paired(6, mode, stream=stream, double=double_at_creation)
+    net = make(stream, double_at_creation) if make else _paired(6, mode, stream=stream, double=double_at_creation)[0]
     if double_at_creation:
         net.set_double_dqn(False)       # the third slot's buffers exist; the steps below start vanilla
     random.seed(21)
@@ -456,10 +457,16 @@ def test_double_switched_on_live_equals_switched_on_at_creation(mode):
     which reallocates the fc1 partials those graphs hold; B allocated the third slot at creation.  Every cost, weight,
     optimizer state and fast-path Q row must agree, also across A switching off and on again, toggling keep_grads and
     a target sync in the middle of the run; the fast-path Q equals host predict on the same window."""
+    assert_switched_on_live_equals_at_creation(mode)
+
+
+def assert_switched_on_live_equals_at_creation(mode, make=None):
+    """The run of test_double_switched_on_live_equals_switched_on_at_creation on the nets make(stream, double)
+    builds (_live_net)."""
     ring = ReplayOracle(3000, batch_size=32)
     synthetic_ring(ring, seed=12, block=150, terminal_p=0.02)
     frames = np.random.RandomState(0).randint(0, 256, (8, 84, 84)).astype(np.uint8)
-    nets = [_live_net(ring, mode, at_creation) for at_creation in (False, True)]
+    nets = [_live_net(ring, mode, at_creation, make) for at_creation in (False, True)]
     n_frames = [0]
 
     def predict_both():

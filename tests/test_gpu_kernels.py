@@ -85,10 +85,11 @@ def make_net(batch, engine="tcgen05", hist=4, num_actions=4, sched="branches", s
     return net
 
 
-def _chain(engine, kernel, rows, hist, fc1_forced=0):
+def _chain(engine, kernel, rows, hist, fc1_forced=0, hidden=K.HIDDEN):
+    """hidden: fc1's width (512, or 1024 on a dueling net), the reduction length of fc1_dgrad."""
     if engine == "tcgen05":
-        return K.chain(kernel, rows, hist, fc1_forced)
-    full = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_fwd": K.FLAT, "fc1_dgrad": K.HIDDEN,
+        return K.chain(kernel, rows, hist, fc1_forced, hidden)
+    full = {"conv1_fwd": 64 * hist, "conv2_fwd": 512, "conv3_fwd": 576, "fc1_fwd": K.FLAT, "fc1_dgrad": hidden,
             "conv3_dgrad": 576, "conv2_dgrad": 1024, "fc1_wgrad": rows, "conv3_wgrad": rows * 49,
             "conv2_wgrad": rows * 81, "conv1_wgrad": rows * 400}
     return full[kernel]
@@ -105,7 +106,9 @@ def _check(name, engine, op, a, b, dev, n, mask=None, post=None, a_exact=False, 
     return {name: K.ratio(dev, y, bnd)}
 
 
-def forward_ratios(engine, states, ws, acts, q, fc1_forced=0):
+def gemm_forward_ratios(engine, states, ws, acts, fc1_forced=0):
+    """conv1..conv3 and fc1 forward, each against its f64 layer on the device's own inputs; fc1 at its width
+    (ws[3]'s rows)."""
     rows, hist = states.shape[0], states.shape[1]
     h1, h2, h3, h4 = acts
     r = {}
@@ -115,29 +118,42 @@ def forward_ratios(engine, states, ws, acts, q, fc1_forced=0):
                                        ("fc1_fwd", K.fc_fwd, h3, ws[3], h4, False)):
         r.update(_check(name, engine, op, a, b, dev, _chain(engine, name, rows, hist, fc1_forced), post=K.relu,
                         a_exact=exact))
-    r.update(_check("fc2_fwd", engine, K.fc_fwd, h4, ws[4], q, K.HIDDEN, split=False))   # the head: fp32 CUDA cores
     return r
 
 
-def backward_ratios(engine, states, ws, acts, dz, grads, deltas):
+def forward_ratios(engine, states, ws, acts, q, fc1_forced=0):
+    r = gemm_forward_ratios(engine, states, ws, acts, fc1_forced)
+    r.update(_check("fc2_fwd", engine, K.fc_fwd, acts[3], ws[4], q, K.HIDDEN, split=False))   # the head: CUDA cores
+    return r
+
+
+def gemm_backward_ratios(engine, states, ws, acts, dz, grads):
+    """The seven GEMM-shaped backward kernels (fc1 and conv dgrads and wgrads), each against its f64 layer on the
+    device's own dZ and activations; fc1_dgrad reduces over fc1's width (ws[3]'s rows)."""
     rows, hist = states.shape[0], states.shape[1]
     h1, h2, h3, h4 = acts
     dz1, dz2, dz3, dz4 = dz
-    c = lambda k: _chain(engine, k, rows, hist)
-    # dZ4 = δ·W5 under the H4 mask: one fp32 product per element (k_head / the SIMT head alike)
-    ref4 = (deltas.astype(F32) @ ws[4]) * (h4 > 0)
-    assert (dz4 == ref4).all(), np.abs(dz4 - ref4).max()
+    c = lambda k: _chain(engine, k, rows, hist, hidden=ws[3].shape[0])
     fc1_dgrad = lambda a, b: K.fc_dgrad(a, b).reshape(len(a), 64, 7, 7)
     r = {}
     r.update(_check("fc1_dgrad", engine, fc1_dgrad, dz4, ws[3], dz3, c("fc1_dgrad"), mask=h3 > 0))
     r.update(_check("conv3_dgrad", engine, K.conv_dgrad(2), dz3, ws[2], dz2, c("conv3_dgrad"), mask=h2 > 0))
     r.update(_check("conv2_dgrad", engine, K.conv_dgrad(1), dz2, ws[1], dz1, c("conv2_dgrad"), mask=h1 > 0))
-    r.update(_check("fc2_wgrad", engine, K.fc_wgrad, h4, deltas, grads[4], rows, split=False))
     r.update(_check("fc1_wgrad", engine, K.fc_wgrad, h3, dz4, grads[3], c("fc1_wgrad")))
     r.update(_check("conv3_wgrad", engine, K.conv_wgrad(2), h2, dz3, grads[2], c("conv3_wgrad")))
     r.update(_check("conv2_wgrad", engine, K.conv_wgrad(1), h1, dz2, grads[1], c("conv2_wgrad")))
     r.update(_check("conv1_wgrad", engine, K.conv_wgrad(0), K.states_f64(states), dz1, grads[0], c("conv1_wgrad"),
                     a_exact=True))
+    return r
+
+
+def backward_ratios(engine, states, ws, acts, dz, grads, deltas):
+    # dZ4 = δ·W5 under the H4 mask: one fp32 product per element (k_head / the SIMT head alike)
+    h4, dz4 = acts[3], dz[3]
+    ref4 = (deltas.astype(F32) @ ws[4]) * (h4 > 0)
+    assert (dz4 == ref4).all(), np.abs(dz4 - ref4).max()
+    r = gemm_backward_ratios(engine, states, ws, acts, dz, grads)
+    r.update(_check("fc2_wgrad", engine, K.fc_wgrad, h4, deltas, grads[4], len(states), split=False))
     return r
 
 

@@ -1,10 +1,11 @@
 """Calibration of tests/kernel_ref.py on the CPU: the f64 layers agree with the oracle, the emulated hi/lo scheme
 stays at least 4× inside the bound at every batch of the GPU sweep, and each way of getting the scheme subtly wrong
-exceeds it.  Run with -s to see the table: per batch and kernel, the scheme's margin (bound / worst error) and the
+exceeds it; for the scalar net and for the dueling net, whose fc1 is 1024 wide.  Run with -s to see the table: per batch and kernel, the scheme's margin (bound / worst error) and the
 worst ratio of error to bound under each mutation ("-" where a kernel has no such part)."""
 import numpy as np
 import pytest
 
+import dueling_oracle as D
 import kernel_ref as K
 from oracle import dqn_oracle as O
 
@@ -12,13 +13,17 @@ SWEEP = [1, 2, 3, 16, 33, 63, 64, 65, 128, 129, 256, 257, 512]
 F32 = np.float32
 MUTATIONS = ["A_lo dropped", "B_lo dropped", "lo x 2^10", "k-block skipped", "split dropped", "last row zeroed",
              "stale lo"]
+# the dueling net's fc1 is two 512-unit streams side by side: fc1_fwd losing m-tiles 4-7 (the value stream's units),
+# fc1_dgrad reducing over only 8 of its 16 k-blocks
+DUELING_MUTATIONS = MUTATIONS + ["one stream dropped"]
 
 
-def _operands(batch, seed=2):
+def _operands(batch, seed=2, dueling=False):
     """The operands each kernel sees in one training step of a Q-of-order-1 network (fc weights × 3, as the GPU
     tests use), with dZ formed in f64 and stored as fp32 like the kernels store it; plus the weights after one
-    RMSProp step from zero state (a stale-lo image is the old weights' lo plane)."""
-    ws = O.xavier_init(4, seed)
+    RMSProp step from zero state (a stale-lo image is the old weights' lo plane).  dueling: the dueling net, fc1
+    (1024, 3136) and fc2 (A + 1, 512), with dZ4 from the dueling head's rule 3 on its deltas."""
+    ws = (D.xavier_init if dueling else O.xavier_init)(4, seed)
     ws[3] = ws[3] * F32(3)
     ws[4] = ws[4] * F32(3)
     rs = np.random.RandomState(seed)
@@ -27,10 +32,14 @@ def _operands(batch, seed=2):
     act = rs.randint(0, 4, batch)
     rew = rs.randint(-3, 4, batch)
     term = rs.rand(batch) < 0.3
-    q, acts = O.forward(ws, pre, keep=True)
-    _, d = K.head_td(q, O.forward(ws, post), act, rew, term)
+    fwd = D.forward if dueling else O.forward
+    q, acts = fwd(ws, pre, keep=True)
+    _, d = K.head_td(q, fwd(ws, post), act, rew, term)
     h1, h2, h3, h4 = acts["h1"], acts["h2"], acts["h3"], acts["h4"]
-    dz4 = ((d @ ws[4]) * (h4 > 0)).astype(F32)
+    if dueling:
+        dz4 = D.dz4(h4, ws[4], *D.stream_grads(d[np.arange(batch), act], act, 4))
+    else:
+        dz4 = ((d @ ws[4]) * (h4 > 0)).astype(F32)
     dz3 = (K.fc_dgrad(dz4, ws[3]).reshape(batch, 64, 7, 7) * (h3 > 0)).astype(F32)
     dz2 = (K.conv_dgrad(2)(dz3, ws[2]) * (h2 > 0)).astype(F32)
     dz1 = (K.conv_dgrad(1)(dz2, ws[1]) * (h1 > 0)).astype(F32)
@@ -52,6 +61,7 @@ def _kernels(o, batch):
     """(name, op, A, B, A exact, weight-operand index or None, k-block skip, split drop, zero last M row).
     The skips zero one operand's slice of the reduction: the last k-block, or the last split's k-blocks."""
     w, n = o["w"], batch
+    hidden = w[3].shape[0]
 
     def pix(t, lo, hi):                  # reduction over output pixels (n, p, q) in order: zero dZ rows [lo, hi)
         flat = np.ascontiguousarray(np.asarray(t).transpose(0, 2, 3, 1)).reshape(-1, t.shape[1])
@@ -83,7 +93,8 @@ def _kernels(o, batch):
     # data gradients: A = dZ, B = weights
     fc1_dgrad = lambda a, b: K.fc_dgrad(a, b).reshape(len(a), 64, 7, 7)
     ks.append(("fc1_dgrad", fc1_dgrad, o["dz4"], w[3], False, 1,
-               lambda: (o["dz4"], _zero(w[3], slice(448, 512))), None, lambda y: _zero(y, (slice(None), 63, 6, 6))))
+               lambda: (o["dz4"], _zero(w[3], slice(hidden - 64, hidden))), None,
+               lambda y: _zero(y, (slice(None), 63, 6, 6))))
     ks.append(("conv3_dgrad", K.conv_dgrad(2), o["dz3"], w[2], False, 1,
                lambda: (o["dz3"], _zero(w[2], np.arange(64) * 9 + 8)), None,
                lambda y: _zero(y, (-1, slice(None), -1, -1))))
@@ -108,12 +119,13 @@ def _kernels(o, batch):
     return ks
 
 
-def _calibrate(batch):
-    o = _operands(batch)
+def _calibrate(batch, dueling=False):
+    o = _operands(batch, dueling=dueling)
+    hidden = o["w"][3].shape[0]
     rows = {}
     for name, op, a, b, exact, widx, skip, drop, zero_row in _kernels(o, batch):
         y = op(np.asarray(a, np.float64), np.asarray(b, np.float64))
-        bnd = K.bound(op, a, b, K.chain(name, batch), y, a_exact=exact)
+        bnd = K.bound(op, a, b, K.chain(name, batch, hidden=hidden), y, a_exact=exact)
         emu = lambda **kw: K.gemm_hilo(op, a, b, a_exact=exact, **kw)
         r = {"scheme": K.ratio(emu(), y, bnd)}
         if name in ("conv1_wgrad", "conv2_wgrad", "conv3_wgrad", "fc1_wgrad"):
@@ -140,24 +152,46 @@ def _calibrate(batch):
                      "conv3_dgrad": 2, "conv2_dgrad": 1}[name]
             wn = o["new"][layer]
             yn = op(np.asarray(a, np.float64), np.asarray(wn, np.float64))
-            bn = K.bound(op, a, wn, K.chain(name, batch), yn, a_exact=exact)
+            bn = K.bound(op, a, wn, K.chain(name, batch, hidden=hidden), yn, a_exact=exact)
             r["stale lo"] = K.ratio(K.gemm_hilo(op, a, wn, a_exact=exact, b_lo_from=b), yn, bn)
+        if not dueling:
+            r["one stream dropped"] = None
+        elif name == "fc1_fwd":       # m-tiles 4-7 (128 units each) never written: the value stream's units read 0
+            r["one stream dropped"] = K.ratio(_zero(emu(), (slice(None), slice(hidden // 2, None))), y, bnd)
+        elif name == "fc1_dgrad":     # k-blocks 8-15 (the value stream's units) left out of the reduction
+            r["one stream dropped"] = K.ratio(K.gemm_hilo(op, a, _zero(b, slice(hidden // 2, None))), y, bnd)
+        else:
+            r["one stream dropped"] = None
         rows[name] = r
     return rows
 
 
-@pytest.mark.parametrize("batch", SWEEP)
-def test_bound_separates_the_scheme_from_its_mutations(batch):
-    rows = _calibrate(batch)
-    print("\nbatch %d  %s" % (batch, K.dispatch(batch)))
-    print("  %-12s %8s  " % ("kernel", "margin") + "  ".join("%15s" % m for m in MUTATIONS))
+def _report_and_assert(batch, rows, mutations, hidden):
+    print("\nbatch %d  %s" % (batch, K.dispatch(batch, hidden=hidden)))
+    print("  %-12s %8s  " % ("kernel", "margin") + "  ".join("%15s" % m for m in mutations))
     for name, r in rows.items():
         print("  %-12s %7.0fx  " % (name, 1 / max(r["scheme"], 1e-30)) +
-              "  ".join("%15s" % ("-" if r[m] is None else "%.3g" % r[m]) for m in MUTATIONS))
+              "  ".join("%15s" % ("-" if r[m] is None else "%.3g" % r[m]) for m in mutations))
     for name, r in rows.items():
         assert r["scheme"] <= 0.25, (name, r["scheme"])
-        for m in MUTATIONS:
+        for m in mutations:
             assert r[m] is None or r[m] > 1.0, (name, m, r[m])
+
+
+@pytest.mark.parametrize("batch", SWEEP)
+def test_bound_separates_the_scheme_from_its_mutations(batch):
+    _report_and_assert(batch, _calibrate(batch), MUTATIONS, K.HIDDEN)
+
+
+@pytest.mark.parametrize("batch", SWEEP)
+def test_bound_separates_the_dueling_scheme_from_its_mutations(batch):
+    """The dueling net: fc1 1024 wide (fc1_dgrad's chain doubles), W5 (A + 1, 512), dZ4 from the dueling head's
+    stream gradients.  Every kernel, the three fc1 kernels at width 1024 among them, stays 4× inside the bound, and
+    each mutation, dropping one of the two streams included, exceeds it."""
+    rows = _calibrate(batch, dueling=True)
+    for name in ("fc1_fwd", "fc1_dgrad"):
+        assert rows[name]["one stream dropped"] is not None
+    _report_and_assert(batch, rows, DUELING_MUTATIONS, 2 * K.HIDDEN)
 
 
 def test_dispatch_of_the_sweep():
