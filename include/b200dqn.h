@@ -255,6 +255,33 @@ typedef struct b200dqn_net_config {
    *     convolutions and its gradient-norm clipping are not applied.
    * Both engines.  ENOTIMPL with num_atoms > 0; b200dqn_net_comm_init returns ENOTIMPL on such a net. */
   int dueling;
+  /* Quantile-regression value head (QR-DQN, Dabney, Rowland, Bellemare and Munos, 2018; new capability, no reference
+   * counterpart), off when num_quantiles = 0 (the default).  Otherwise N = num_quantiles in 1..200 (other values are
+   * EINVAL), and the Huber threshold is kappa = float(clip_error) (1 by default; 0 gives the pure quantile loss; a
+   * non-finite clip_error is EINVAL).  EINVAL with num_atoms > 0 (a net has one head), ENOTIMPL with dueling = 1;
+   * b200dqn_net_comm_init returns ENOTIMPL on such a net.  Every operation below is fp32 with its own rounding (no
+   * contraction) unless marked fp64; a is the taken action, z the slot (0 online on the prestates, 1 target on the
+   * poststates, 2 online on the poststates under Double DQN):
+   *    1. midpoints: tau_i = (2i + 1) / 2N in fp64; wlo_i = float(tau_i) weighs u >= 0, whi_i = float((2N - 2i - 1) / 2N)
+   *       weighs u < 0;
+   *    2. fc2: theta[z][b][a N + i] = sum_k H4[z][b][k] W5[k][a N + i], k = 0..511 in order, as the distributional head's
+   *       logits (Neon shape (A N, 512), row a N + i);
+   *    3. Q[a] = (sum_i theta[a][i] in i order) / float(N).  Every Q output (predict, the Q rows, the TD choice) is this Q;
+   *    4. a* = first index of the maximum of slot 1's Q (slot 2's with Double DQN); q'_j = theta[1][b][a* N + j];
+   *    5. the return R and g as for the distributional head, in fp64 (g = 0 when the window holds a terminal);
+   *       T_j = float(R + g double(q'_j));
+   *    6. u_ij = T_j - theta[0][b][a N + i];
+   *    7. w_ij = u_ij < 0 ? whi_i : wlo_i;
+   *    8. kappa > 0: L = |u| <= kappa ? 0.5 (u u) : kappa (|u| - 0.5 kappa), rho_ij = (w L) / kappa and
+   *       c_ij = (w clamp(u, -kappa, kappa)) / kappa; kappa = 0: rho_ij = w |u|, c_ij = u > 0 ? w : (u < 0 ? -w : 0);
+   *    9. Loss_i = (sum_j rho_ij in j order) / N, the row loss l = sum_i Loss_i in i order; the row cost is l (times the
+   *       importance weight on a prioritized ring, whose priority update gets the unweighted l);
+   *   10. dtheta_i = -((sum_j c_ij in j order) / N), times the importance weight on a prioritized ring; 0 for every other
+   *       action;
+   *   11. dZ4 and its fp16 planes, and fc2's per-row gradient partials, as for the distributional head with the logit
+   *       gradient replaced by dtheta;
+   *   12. fc2's gradient is summed as for the distributional head, then the configured optimizer applies it. */
+  int num_quantiles;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -380,7 +407,12 @@ enum {
   /* Dueling net only (EINVAL otherwise): (3, batch, A + 1) f32, the advantages A_0..A_{A-1} and then V of each row of
    * the last forward, slots as for the distributional head (slot 2 is written by Double DQN steps with a separate
    * target network only). */
-  B200DQN_NET_PTR_DUELING_VA
+  B200DQN_NET_PTR_DUELING_VA,
+  /* Quantile-regression head only (num_quantiles > 0; EINVAL otherwise).  DELTAS is EINVAL on such a net.  Slots as for
+   * the distributional head. */
+  B200DQN_NET_PTR_QUANTILES,        /* (3, batch, A * num_quantiles) f32 fc2 outputs theta of the last forward      */
+  B200DQN_NET_PTR_TARGET_QUANTILES, /* (batch, num_quantiles) f32 target quantiles T_j of the last train step       */
+  B200DQN_NET_PTR_QUANTILE_GRADS    /* (batch, num_quantiles) f32 gradient dtheta on the taken action's quantiles   */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

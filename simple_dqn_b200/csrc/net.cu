@@ -702,6 +702,147 @@ k_opt_fc2_dist(const float* __restrict__ part, const int32_t* __restrict__ act_r
 }
 
 // ------------------------------------------------------------------------------------------
+// Quantile-regression head (QR-DQN, Dabney, Rowland, Bellemare and Munos 2018; b200dqn.h has the rules).  fc2's outputs
+// theta[z][b][a * N + i] come from k_fc2_dist unchanged, and fc2's gradient goes through k_opt_fc2_dist unchanged with N
+// as the block width; k_head_qr does the rest: Q, a*, the target quantiles, the quantile Huber loss and its gradient,
+// dZ4 (+ fp16 planes) and the compact dW5 row partial [512][N] of the taken action.  No expf / logf: every stage is
+// +, -, *, / and comparisons, each rounded on its own.
+// ------------------------------------------------------------------------------------------
+struct QrArgs {
+  int nq;            // N
+  float kappa;       // the Huber threshold (clip_error); 0: the pure quantile loss
+  float* tq;         // [ld][N] target quantiles T_j
+  float* qgrad;      // [ld][N] gradient on the taken action's quantiles
+  int32_t* act_rows; // [ld]
+};
+
+// One CTA (512 threads) per sample b.  Thread r < nets * A owns row (slot z, action a): Q = (sum_i theta_i, i order) / N.
+// With td.enable: thread 0 picks a* (first maximum of slot 1's Q, slot 2's with kSlots = 3) and the fp64 return; thread
+// j < N forms T_j = float(R + g theta[1][a*][j]); thread i < N runs the j loop of the loss and the gradient for quantile
+// i of the taken action; thread 0 sums the row loss; every thread its dZ4 element and a stride of the dW5 row partial.
+// The TD scalars and Adam's step scalar come from head_td_scalars, before the dependency wait.
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_qr(const float* __restrict__ theta, int ld, int nets, const float* __restrict__ h4_online,
+          const float* __restrict__ w5_online, float* q_online, float* q_target, float* q_online_post, int A,
+          const QrArgs qa, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 1 || kSlots == 2 || kSlots == 3, "predict, online + target, or Double DQN's three slots");
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_wlo[kMaxQuantiles], s_whi[kMaxQuantiles], s_t[kMaxQuantiles], s_l[kMaxQuantiles];
+  __shared__ float s_g[kMaxQuantiles], s_h4[kHidden];
+  __shared__ double s_ret, s_gam;
+  __shared__ int s_a, s_astar;
+  const int b = blockIdx.x, t = threadIdx.x, nq = qa.nq, ncols = A * nq;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  if (t < nq) {   // quantile midpoints tau_i = (2i + 1) / 2N in fp64: weight tau_i for u >= 0, 1 - tau_i for u < 0
+    s_wlo[t] = float(__ddiv_rn(double(2 * t + 1), double(2 * nq)));
+    s_whi[t] = float(__ddiv_rn(double(2 * nq - 2 * t - 1), double(2 * nq)));
+  }
+  pdl_wait();
+  pdl_launch_dependents();
+  if (td.enable) s_h4[t] = h4_online[b * kHidden + t];
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float* th = theta + (int64_t(z) * ld + b) * ncols + a * nq;
+    float s = 0.f;
+    for (int i = 0; i < nq; ++i) s = __fadd_rn(s, th[i]);
+    const float q = __fdiv_rn(s, float(nq));
+    s_q[z][a] = q;
+    (z == 0 ? q_online : z == 2 ? q_online_post : q_target)[b * A + a] = q;
+  }
+  if constexpr (kSlots > 1) {
+    if (!td.enable) {
+      kt_end(kt);
+      return;
+    }
+    __syncthreads();
+    if (t == 0) {
+      const float* qs = s_q[kSlots == 3 ? 2 : 1];
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (qs[j] > qs[best]) best = j;
+      double R, g;
+      if constexpr (kNstep) {
+        R = td_ret;
+        g = td_term ? 0.0 : td_g;
+      } else {
+        R = fmin(fmax(double(td_r), td.min_reward), td.max_reward);   // np.clip as the scalar head
+        g = td_term ? 0.0 : td.discount;
+      }
+      s_ret = R;
+      s_gam = g;
+      s_a = td_a;
+      s_astar = best;
+      qa.act_rows[b] = td_a;
+    }
+    __syncthreads();
+    const int a = s_a;
+    if (t < nq) {   // T_j = float(R + g q'_j), q'_j = the target network's theta[a*][j]
+      const float qj = theta[(int64_t(ld) + b) * ncols + s_astar * nq + t];
+      const float T = float(__dadd_rn(s_ret, __dmul_rn(s_gam, double(qj))));
+      s_t[t] = T;
+      qa.tq[b * nq + t] = T;
+    }
+    __syncthreads();
+    if (t < nq) {   // quantile i of the taken action against every target quantile j, j order
+      const float th = theta[int64_t(b) * ncols + a * nq + t];
+      const float wlo = s_wlo[t], whi = s_whi[t], kap = qa.kappa;
+      float rho = 0.f, c = 0.f;
+      for (int j = 0; j < nq; ++j) {
+        const float u = __fsub_rn(s_t[j], th);
+        const float w = u < 0.f ? whi : wlo;
+        const float au = fabsf(u);
+        if (kap > 0.f) {
+          const float L = au <= kap ? __fmul_rn(0.5f, __fmul_rn(u, u)) : __fmul_rn(kap, __fsub_rn(au, __fmul_rn(0.5f, kap)));
+          rho = __fadd_rn(rho, __fdiv_rn(__fmul_rn(w, L), kap));
+          c = __fadd_rn(c, __fdiv_rn(__fmul_rn(w, fminf(fmaxf(u, -kap), kap)), kap));
+        } else {
+          rho = __fadd_rn(rho, __fmul_rn(w, au));
+          c = __fadd_rn(c, u > 0.f ? w : u < 0.f ? -w : 0.f);
+        }
+      }
+      float g = -__fdiv_rn(c, float(nq));
+      if (td.isw) g = __fmul_rn(g, td.isw[b]);
+      s_l[t] = __fdiv_rn(rho, float(nq));
+      s_g[t] = g;
+      qa.qgrad[b * nq + t] = g;
+    }
+    __syncthreads();
+    if (t == 0) {   // the row loss: sum_i Loss_i, i order
+      float l = 0.f;
+      for (int i = 0; i < nq; ++i) l = __fadd_rn(l, s_l[i]);
+      if (td.isw) {
+        td.td_err[b] = l;
+        td.row_cost[b] = __fmul_rn(td.isw[b], l);
+      } else {
+        td.row_cost[b] = l;
+      }
+    }
+    {
+      const float hv = s_h4[t];
+      const float* w = w5_online + int64_t(t) * ncols + a * nq;
+      float o = 0.f;
+      if (hv > 0.f)
+        for (int i = 0; i < nq; ++i) o = __fadd_rn(o, __fmul_rn(w[i], s_g[i]));
+      td.dz4[b * kHidden + t] = o;
+      if (td.dz4_hi) {
+        const __half hh = __float2half_rn(o);
+        const __half ll = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+        td.dz4_hi[b * kHidden + t] = hh;
+        td.dz4_hi[td.dz4_lo_off + b * kHidden + t] = ll;
+      }
+    }
+    float* dw = td.dw5_rows + int64_t(b) * kHidden * nq;
+    for (int e = t; e < kHidden * nq; e += kHidden) dw[e] = __fmul_rn(s_h4[e / nq], s_g[e % nq]);
+  }
+  kt_end(kt);
+}
+
+// ------------------------------------------------------------------------------------------
 // K6: gradient reduction + the configured Neon optimizer (src/deepqnetwork.py:50-61,165; rules in optim.cuh).
 // RMSProp:  g = dW / bsz;  s = decay*s + g*g*(1-decay);  W = W - (g*lr) / (sqrt(s + eps) + eps)
 // The split-K partials of every layer are summed here in fixed order (deterministic), so the
@@ -868,6 +1009,22 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     B2_PROF(td.enable ? "head_dist(td+fc2_bwd)" : "head_dist", st);
     return B200DQN_OK;
   }
+  if (n->quantiles) {
+    const int ncols = n->fc2_cols();
+    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
+                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
+                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_theta, ncols, ktrace_slot("fc2_dist")));
+    B2_PROF("fc2_dist", st);
+    const QrArgs qa{n->quantiles, float(n->cfg.clip_error), n->d_tquant, n->d_qgrad, n->d_act_rows};
+    auto* kern = nets == 1 ? k_head_qr<1, false>
+               : nets == 3 ? (nstep ? k_head_qr<3, true> : k_head_qr<3, false>)
+                           : (nstep ? k_head_qr<2, true> : k_head_qr<2, false>);
+    B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
+                             (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, qa, td,
+                             ktrace_slot("head_qr")));
+    B2_PROF(td.enable ? "head_qr(td+fc2_bwd)" : "head_qr", st);
+    return B200DQN_OK;
+  }
   B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head<3, true> : k_head<3, false>)
                                      : (nstep ? k_head<2, true> : k_head<2, false>),
                            dim3(rows), dim3(kHidden), 0, st,
@@ -982,21 +1139,22 @@ static int cost_finish_on(b200dqn_net* n, int rows, cudaStream_t s) {
   return B200DQN_OK;
 }
 
-// fc2 of a distributional net from the head's compact row partials; mode bits as k_opt_fc2_dist's
+// fc2 of a distributional or quantile net from the head's compact row partials; mode bits as k_opt_fc2_dist's
 static int opt_fc2_dist(b200dqn_net* n, int rows, int mode, cudaStream_t s, const char* label) {
   const LayerTable& lt = n->lt;
-  B2_CHECK_CUDA(launch_pdl(k_opt_fc2_dist, dim3(cdiv(int64_t(kHidden) * n->atoms, 256), n->A), dim3(256), 0, s,
-                           (const float*)n->d_part + lt.part_off[4], (const int32_t*)n->d_act_rows, rows, n->A, n->atoms,
+  const int blk = n->fc2_block();
+  B2_CHECK_CUDA(launch_pdl(k_opt_fc2_dist, dim3(cdiv(int64_t(kHidden) * blk, 256), n->A), dim3(256), 0, s,
+                           (const float*)n->d_part + lt.part_off[4], (const int32_t*)n->d_act_rows, rows, n->A, blk,
                            n->d_g + lt.off[4], n->d_w + lt.off[4], n->d_s + lt.off[4], mode, make_opt_args(n, rows),
                            ktrace_slot(label)));
   B2_PROF(label, s);
   return B200DQN_OK;
 }
 
-// The update over layers [l0, l1] of the single-learner schedules (mode 1 | 4): fc2 of a distributional net goes
-// through opt_fc2_dist, every other layer through optimizer_range.
+// The update over layers [l0, l1] of the single-learner schedules (mode 1 | 4): fc2 of a distributional or quantile
+// net goes through opt_fc2_dist, every other layer through optimizer_range.
 static int update_range(b200dqn_net* n, int l0, int l1, int rows, cudaStream_t st, const char* label) {
-  if (!n->atoms || l1 < 4) return optimizer_range(n, l0, l1, 1 | 4, rows, st, label);
+  if (!n->fc2_block() || l1 < 4) return optimizer_range(n, l0, l1, 1 | 4, rows, st, label);
   if (l0 < 4) {
     const int rc = optimizer_range(n, l0, 3, 1 | 4, rows, st, label);
     if (rc) return rc;
@@ -1006,7 +1164,7 @@ static int update_range(b200dqn_net* n, int l0, int l1, int rows, cudaStream_t s
 
 // fc2 update from the head's per-row partials (single-GPU schedules): 8-lane reduction, no image
 static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
-  if (n->atoms) return opt_fc2_dist(n, rows, 4, s, "opt_fc2_dist");
+  if (n->fc2_block()) return opt_fc2_dist(n, rows, 4, s, "opt_fc2_dist");
   const LayerTable& lt = n->lt;
   const int64_t size = lt.off[5] - lt.off[4];
   B2_CHECK_CUDA(launch_pdl(k_opt_small, dim3(cdiv(size / 4, 32)), dim3(256), 0, s, (const float*)n->d_part + lt.part_off[4],
@@ -1297,7 +1455,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     // fourth branch: the scalar cost and the 512 x A layer — nothing later in the step reads W5, and nothing here
     // sits in front of the fc1 optimizer any more (the SIMT engine's scalar fc2 rides with fc1 in opt_fc)
     B2_TRY(cost_finish_on(n, rows, sN));
-    if (tc || n->atoms) B2_TRY(opt_fc2_small(n, rows, sN));
+    if (tc || n->fc2_block()) B2_TRY(opt_fc2_small(n, rows, sN));
   }
   B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
@@ -1305,7 +1463,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   {
     NoPdlScope side;
     if (tc) B2_TRY(umma_opt_fc1(n, rows, sA));               // smem-free: co-resides with the dgrad chain
-    else B2_TRY(optimizer_range(n, 3, n->atoms ? 3 : 4, 1 | 4, rows, sA, "opt_fc"));
+    else B2_TRY(optimizer_range(n, 3, n->fc2_block() ? 3 : 4, 1 | 4, rows, sA, "opt_fc"));
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
@@ -1417,6 +1575,7 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->v_min = -10.0;
   cfg->v_max = 10.0;
   cfg->dueling = 0;              // one value stream
+  cfg->num_quantiles = 0;        // no quantile-regression head
   return B200DQN_OK;
 }
 
@@ -1443,6 +1602,15 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
              cfg->dueling);
   B2_REQUIRE(!(cfg->dueling && cfg->num_atoms), B200DQN_ENOTIMPL,
              "net_create: a dueling net with a distributional head is not implemented");
+  B2_REQUIRE(cfg->num_quantiles >= 0 && cfg->num_quantiles <= kMaxQuantiles, B200DQN_EINVAL,
+             "net_create: num_quantiles %d is neither 0 (no quantile head) nor in [1,%d]", cfg->num_quantiles,
+             kMaxQuantiles);
+  B2_REQUIRE(!(cfg->num_quantiles && cfg->num_atoms), B200DQN_EINVAL,
+             "net_create: num_quantiles and num_atoms both ask for a head; a net has one");
+  B2_REQUIRE(!cfg->num_quantiles || std::isfinite(cfg->clip_error), B200DQN_EINVAL,
+             "net_create: the quantile Huber threshold clip_error must be finite (got %g)", cfg->clip_error);
+  B2_REQUIRE(!(cfg->dueling && cfg->num_quantiles), B200DQN_ENOTIMPL,
+             "net_create: a dueling net with a quantile-regression head is not implemented");
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -1453,6 +1621,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->nb = cfg->batch_size;
   n->A = cfg->num_actions;
   n->atoms = cfg->num_atoms;
+  n->quantiles = cfg->num_quantiles;
   n->dueling = cfg->dueling != 0;
   n->hidden = n->dueling ? kDuelHidden : kHidden;
   if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
@@ -1479,8 +1648,8 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     else
       lt.splits[l] = l < 3 ? int(cdiv(kred[l], wgrad_chunk(kred[l], base[l]))) : 1;
     lt.part_off[l] = po;
-    if (l == 4 && n->atoms)   // distributional head: the taken action's [512][atoms] block per sample
-      po += int64_t(nb) * kHidden * n->atoms;
+    if (l == 4 && n->fc2_block())   // distributional / quantile head: the taken action's [512][block] per sample
+      po += int64_t(nb) * kHidden * n->fc2_block();
     else
       po += int64_t(lt.splits[l]) * (lt.off[l + 1] - lt.off[l]);
   }
@@ -1534,6 +1703,13 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(fmalloc(&n->d_probs, 3 * dist));
     B2_CHECK_CUDA(fmalloc(&n->d_tdist, size_t(nb) * n->atoms));
     B2_CHECK_CUDA(fmalloc(&n->d_lgrad, size_t(nb) * n->atoms));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
+    B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
+  }
+  if (n->quantiles) {
+    B2_CHECK_CUDA(fmalloc(&n->d_theta, size_t(3) * nb * A * n->quantiles));
+    B2_CHECK_CUDA(fmalloc(&n->d_tquant, size_t(nb) * n->quantiles));
+    B2_CHECK_CUDA(fmalloc(&n->d_qgrad, size_t(nb) * n->quantiles));
     B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
     B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
   }
@@ -1596,6 +1772,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_td_err);
   cudaFree(n->d_logits); cudaFree(n->d_probs); cudaFree(n->d_tdist); cudaFree(n->d_lgrad); cudaFree(n->d_act_rows);
   cudaFree(n->d_va);
+  cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -2044,6 +2221,7 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_Q_TARGET: p = n->d_q[1]; b = size_t(n->nb) * n->A * 4; break;
     case B200DQN_NET_PTR_DELTAS:
       B2_REQUIRE(!n->atoms, B200DQN_EINVAL, "net_device_ptr: a distributional head has no scalar delta");
+      B2_REQUIRE(!n->quantiles, B200DQN_EINVAL, "net_device_ptr: a quantile-regression head has no scalar delta");
       p = n->d_delta;
       b = size_t(n->nb) * n->A * 4;
       break;
@@ -2091,6 +2269,14 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       B2_REQUIRE(n->dueling, B200DQN_EINVAL, "net_device_ptr: selector %d needs a dueling net", which);
       p = n->d_va;
       b = size_t(3) * n->nb * (n->A + 1) * 4;
+      break;
+    case B200DQN_NET_PTR_QUANTILES:
+    case B200DQN_NET_PTR_TARGET_QUANTILES:
+    case B200DQN_NET_PTR_QUANTILE_GRADS:
+      B2_REQUIRE(n->quantiles, B200DQN_EINVAL, "net_device_ptr: selector %d needs a quantile-regression head", which);
+      p = which == B200DQN_NET_PTR_QUANTILES ? n->d_theta : which == B200DQN_NET_PTR_TARGET_QUANTILES ? n->d_tquant
+                                                                                                       : n->d_qgrad;
+      b = (which == B200DQN_NET_PTR_QUANTILES ? size_t(3) * n->nb * n->A : size_t(n->nb)) * n->quantiles * 4;
       break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
@@ -2154,11 +2340,12 @@ extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, 
   cudaStream_t st = as_stream(stream);
   const int64_t n4 = n->n_params / 4;
   if (n->world == 1) {  // partials of the last step are still in scratch; sum them into d_g
-    const int64_t e4 = n->atoms ? n->lt.off[4] / 4 : n4;   // a distributional fc2 is summed by its own kernel
+    // a distributional or quantile fc2 is summed by its own kernel
+    const int64_t e4 = n->fc2_block() ? n->lt.off[4] / 4 : n4;
     k_optimizer<<<cdiv(e4, 256), 256, 0, st>>>(n->lt, n->d_part, n->d_g, n->d_w, n->d_s, 0, e4, 1 | 2, OptArgs{},
                                                KTrace{nullptr, 0});
     B2_LAUNCH_CHECK();
-    if (n->atoms) {
+    if (n->fc2_block()) {
       NoPdlScope plain;
       B2_TRY(opt_fc2_dist(n, n->nb, 2, st, "grads_fc2_dist"));
     }
@@ -2180,8 +2367,8 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     *launches = n->graph_launches;
   } else {
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
-    // a distributional head adds k_fc2_dist, and on the SIMT engine fc2's own update
-    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->atoms ? (tc ? 1 : 2) : 0);
+    // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update
+    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0);
   }
   return B200DQN_OK;
 }

@@ -12,6 +12,7 @@ namespace b200 {
 constexpr int kLayers = 5;
 constexpr int kMaxActions = 32;
 constexpr int kMaxAtoms = 64;             // distributional head: atoms per action
+constexpr int kMaxQuantiles = 200;        // quantile-regression head: quantiles per action
 constexpr int kCostRing = 1024;
 constexpr int kHostCosts = 60;            // per-step costs mirrored in host-mapped memory
 constexpr int kHostQ = 64, kHostQFloats = 960;   // word offset / capacity of the Q rows in the host-mapped block
@@ -114,7 +115,17 @@ struct b200dqn_net {
   float* d_tdist = nullptr;      // [nb][atoms] projected target distribution
   float* d_lgrad = nullptr;      // [nb][atoms] gradient on the taken action's logits
   int32_t* d_act_rows = nullptr; // [nb] taken action of each row of the last train step (selects the dW5 block)
-  int fc2_cols() const { return atoms ? A * atoms : dueling ? A + 1 : A; }
+
+  // quantile-regression head (cfg.num_quantiles > 0; nothing below is allocated otherwise).  fc2 has A * quantiles
+  // outputs and shares the distributional head's compact dW5 partials, d_act_rows and fc2 kernels.
+  int quantiles = 0;
+  float* d_theta = nullptr;      // [3][nb][A * quantiles]
+  float* d_tquant = nullptr;     // [nb][quantiles] target quantiles
+  float* d_qgrad = nullptr;      // [nb][quantiles] gradient on the taken action's quantiles
+  // fc2 outputs per action of a per-action head (C51 atoms or QR quantiles), 0 on the scalar and dueling heads: such
+  // an fc2 is summed and updated by k_opt_fc2_dist from the compact [nb][512][block] partials
+  int fc2_block() const { return atoms ? atoms : quantiles; }
+  int fc2_cols() const { return fc2_block() ? A * fc2_block() : dueling ? A + 1 : A; }
 
   // dueling network (cfg.dueling): fc1 is kDuelHidden wide (advantage units [0, 512), value units [512, 1024)) and
   // fc2 is block-structured [512][A + 1]: column a < A reads the advantage units, column A the value units

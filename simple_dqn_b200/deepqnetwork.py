@@ -79,6 +79,13 @@ class DeepQNetwork:
         # shapes, so it is chosen here and not switchable later
         self.dueling = bool(_arg(args, "dueling", False))
         cfg.dueling = int(self.dueling)
+        # quantile-regression value head (QR-DQN, Dabney et al., 2018): a new capability, off unless
+        # args.quantile_regression is set; its Huber threshold is clip_error.  Fixed here, like the other heads.
+        self.quantile_regression = bool(_arg(args, "quantile_regression", False))
+        self.num_quantiles, self.taus = 0, None
+        if self.quantile_regression:
+            cfg.num_quantiles = int(_arg(args, "num_quantiles", 200))
+            assert cfg.num_quantiles >= 1, "num_quantiles %d: the quantile head needs 1..200" % cfg.num_quantiles
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -86,6 +93,9 @@ class DeepQNetwork:
             self.num_atoms, self.v_min, self.v_max = cfg.num_atoms, cfg.v_min, cfg.v_max
             dz = (cfg.v_max - cfg.v_min) / (cfg.num_atoms - 1)         # z_i = v_min + i dz in fp64, as the device
             self.support = np.array([cfg.v_min + i * dz for i in range(cfg.num_atoms)], dtype=np.float64)
+        if self.quantile_regression:
+            self.num_quantiles = n = cfg.num_quantiles                 # tau_i = (2i + 1) / 2N in fp64, as the device
+            self.taus = np.array([(2 * i + 1) / (2 * n) for i in range(n)], dtype=np.float64).astype(np.float32)
 
         # model.initialize (:49, :70): Xavier draws from one numpy RandomState(random_seed) —
         # online layers first, then the separately-initialised target model.
@@ -264,6 +274,19 @@ class DeepQNetwork:
     def last_logit_grads(self):
         """The gradient on the taken action's logits of the last train(), (batch, num_atoms) float32."""
         return self._read_f32(L.NET_PTR_LOGIT_GRADS, (self.batch_size, self.num_atoms))
+
+    # ---- quantile-regression head (num_quantiles > 0): slots as for the distributional head
+    def last_quantiles(self):
+        """fc2's outputs theta of the last forward, (3, batch, A, num_quantiles) float32."""
+        return self._read_f32(L.NET_PTR_QUANTILES, (3, self.batch_size, self.num_actions, self.num_quantiles))
+
+    def last_target_quantiles(self):
+        """The target quantiles T_j of the last train(), (batch, num_quantiles) float32."""
+        return self._read_f32(L.NET_PTR_TARGET_QUANTILES, (self.batch_size, self.num_quantiles))
+
+    def last_quantile_grads(self):
+        """The gradient on the taken action's quantiles of the last train(), (batch, num_quantiles) float32."""
+        return self._read_f32(L.NET_PTR_QUANTILE_GRADS, (self.batch_size, self.num_quantiles))
 
     # ---- dueling network: slots as for the distributional head
     def last_advantages(self):

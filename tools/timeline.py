@@ -11,12 +11,14 @@ B = int(os.environ.get("BATCH", "32"))
 ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with this many atoms; 0: the scalar head
 NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
 DUELING = os.environ.get("DUELING", "0") == "1"   # dueling network (1024-unit fc1, advantage and value streams)
+QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (QR-DQN) with this many quantiles; 0: off
 
 
 def net_args():
     a = make_args(B)
     a.distributional, a.num_atoms = ATOMS > 0, ATOMS
     a.dueling = DUELING
+    a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
     return a
 
 
