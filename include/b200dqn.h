@@ -282,6 +282,31 @@ typedef struct b200dqn_net_config {
    *       gradient replaced by dtheta;
    *   12. fc2's gradient is summed as for the distributional head, then the configured optimizer applies it. */
   int num_quantiles;
+  /* Munchausen DQN target (M-DQN, Vieillard, Pietquin and Geist, 2020; new capability, no reference counterpart), off
+   * when munchausen = 0 (the default; values other than 0 and 1 are EINVAL).  With pi = softmax(q / tau) over a Q row
+   * of the target network, the scalar head's target becomes
+   *   y = R + alpha clamp(tau ln pi(a | s), l0, 0) + g sum_a' pi(a' | s') (q(s', a') - tau ln pi(a' | s')),
+   * R the clipped (or n-step) return and g = gamma^N, 0 when the window holds a terminal (the bonus still applies).
+   * alpha = munchausen_alpha (finite, >= 0; default 0.9), tau = munchausen_tau (finite, > 0; default 0.03) and
+   * l0 = munchausen_clip (finite, <= 0; default -1); anything else is EINVAL.  ENOTIMPL with dueling, num_atoms or
+   * num_quantiles; b200dqn_net_set_double_q(n, 1) is EINVAL (the target makes no greedy choice) and
+   * b200dqn_net_comm_init returns ENOTIMPL on such a net.  The train step runs the target network on the prestates
+   * as one more forward pass (no pass with target_steps = 0: the online Q row of the prestates is that row).  Every
+   * fp64 operation below is rounded on its own except exp and log, which are the device's fp64 functions (not
+   * bit-identical to numpy's); a is the taken action:
+   *    1. per sample, two fp32 rows x: the target network's Q on the poststates, and its Q on the prestates.  For each
+   *       row: m = max_j x_j; e_j = exp((double(x_j) - m) / tau); s = sum_j e_j in j order; lse = m + tau log(s);
+   *       tau ln pi_j = double(x_j) - lse; pi_j = e_j / s;
+   *    2. bonus = alpha fmin(fmax(tau ln pi_pre[a], l0), 0);
+   *    3. next = sum_j pi_post,j (x_post,j - tau ln pi_post,j) in j order;
+   *    4. y = (R + bonus) + g next, the last operation formed as the scalar head forms its one-step (contracted) and
+   *       n-step (separately rounded) targets, so that with one action y is the scalar head's y bit for bit;
+   *    5. target = float(y); delta, the clip, the importance weight, the cost, the TD error, dZ4 and fc2's gradient
+   *       are the scalar head's. */
+  int munchausen;
+  double munchausen_alpha;
+  double munchausen_tau;
+  double munchausen_clip;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -412,7 +437,11 @@ enum {
    * the distributional head. */
   B200DQN_NET_PTR_QUANTILES,        /* (3, batch, A * num_quantiles) f32 fc2 outputs theta of the last forward      */
   B200DQN_NET_PTR_TARGET_QUANTILES, /* (batch, num_quantiles) f32 target quantiles T_j of the last train step       */
-  B200DQN_NET_PTR_QUANTILE_GRADS    /* (batch, num_quantiles) f32 gradient dtheta on the taken action's quantiles   */
+  B200DQN_NET_PTR_QUANTILE_GRADS,   /* (batch, num_quantiles) f32 gradient dtheta on the taken action's quantiles   */
+  /* Munchausen target only (munchausen = 1; EINVAL otherwise). */
+  B200DQN_NET_PTR_Q_TARGET_PRE,     /* (batch, A) f32 the target network's Q on the prestates of the last train step;
+                                     * with target_steps = 0 it is the Q_ONLINE buffer (the two networks are one)   */
+  B200DQN_NET_PTR_TD_TARGETS        /* (batch,) f32 the targets float(y) of the last train step                     */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well
@@ -424,7 +453,7 @@ int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
  * the backward and the optimizers are unchanged, and predict is not affected.  The train-step forward runs the online
  * network on the poststates as a third slot of its launches.  The first switch-on allocates that slot's buffers
  * (synchronises the device).  Captured step graphs are rebuilt.  ENOTIMPL once b200dqn_net_comm_init has run;
- * b200dqn_net_comm_init returns ENOTIMPL while it is on. */
+ * b200dqn_net_comm_init returns ENOTIMPL while it is on.  EINVAL on a net with the Munchausen target. */
 int b200dqn_net_set_double_q(b200dqn_net* n, int on);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
 int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream);

@@ -386,6 +386,140 @@ k_head_duel(const float* __restrict__ part, int splits, int rows, int nets, int 
   kt_end(kt);
 }
 
+// ------------------------------------------------------------------------------------------
+// Munchausen head (M-DQN, Vieillard, Pietquin and Geist 2020; b200dqn.h has the rules): k_head's job with the Munchausen
+// target.  kSlots = 3: slot 2 is the target network on the prestates, whose fc1 partials the one-slot pass of
+// train_step wrote; its fc2 takes the target W5 and its Q row goes to q_target_pre.  kSlots = 2 (target_steps = 0):
+// slot 0's Q row is the prestate row of the policy.  Lane j < A of warp 0 forms e_j of both rows; every lane of the warp
+// then forms the j-order sums and the logs (shuffles in j order: the operations of one serial loop, done redundantly),
+// lane j the term of action j, and the j-order sum of the terms; thread 0 forms y and runs k_head's TD step and backward
+// from target = float(y) on, line for line (a shared helper changed pinned SASS in the earlier heads).
+// ------------------------------------------------------------------------------------------
+struct MdqnArgs {
+  double alpha, tau, clip;   // alpha, tau and l0 of b200dqn.h
+  float* q_target_pre;       // [rows][A] Q row of slot 2 (kSlots = 3)
+  float* targets;            // [rows] float(y)
+};
+
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_mdqn(const float* __restrict__ part, int splits, int rows, float* h4_online, float* h4_target,
+            const float* __restrict__ w5_online, const float* __restrict__ w5_target, float* q_online,
+            float* q_target, int A, const MdqnArgs ma, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, and the target network on the prestates");
+  __shared__ float red[kSlots][kHidden / 32][kMaxActions];
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_d;
+  __shared__ int s_a;
+  const int b = blockIdx.x, t = threadIdx.x;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  pdl_wait();
+  pdl_launch_dependents();
+  float h[kSlots] = {};
+#pragma unroll
+  for (int z = 0; z < kSlots; ++z) {
+    float acc = 0.f;
+    for (int s = 0; s < splits; ++s) acc += part[((z * splits + s) * rows + b) * kHidden + t];
+    h[z] = fmaxf(acc, 0.f);
+    if (z < 2) (z ? h4_target : h4_online)[b * kHidden + t] = h[z];   // slot 2's H4 has no reader
+  }
+#pragma unroll
+  for (int z = 0; z < kSlots; ++z) {
+    const float* w5 = z == 0 ? w5_online : w5_target;
+    for (int a = 0; a < A; ++a) {
+      float v = h[z] * w5[t * A + a];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if ((t & 31) == 0) red[z][t >> 5][a] = v;
+    }
+  }
+  __syncthreads();
+  if (t < kSlots * A) {
+    const int z = t / A, a = t % A;
+    float v = 0.f;
+#pragma unroll
+    for (int wI = 0; wI < kHidden / 32; ++wI) v += red[z][wI][a];
+    (z == 0 ? q_online : z == 2 ? ma.q_target_pre : q_target)[b * A + a] = v;
+    s_q[z][a] = v;
+  }
+  __syncthreads();
+  if (t < 32) {
+    const float* qpre = s_q[kSlots == 3 ? 2 : 0];
+    const bool live = t < A;
+    const float xo = live ? s_q[1][t] : -INFINITY, xp = live ? qpre[t] : -INFINITY;   // poststate / prestate rows
+    float mo = xo, mp = xp;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      mo = fmaxf(mo, __shfl_xor_sync(0xffffffffu, mo, o));
+      mp = fmaxf(mp, __shfl_xor_sync(0xffffffffu, mp, o));
+    }
+    const double tau = ma.tau;
+    const double eo = live ? exp(__ddiv_rn(__dsub_rn(double(xo), double(mo)), tau)) : 0.0;
+    const double ep = live ? exp(__ddiv_rn(__dsub_rn(double(xp), double(mp)), tau)) : 0.0;
+    double so = 0.0, sp = 0.0;
+    for (int j = 0; j < A; ++j) {
+      so = __dadd_rn(so, __shfl_sync(0xffffffffu, eo, j));
+      sp = __dadd_rn(sp, __shfl_sync(0xffffffffu, ep, j));
+    }
+    const double lseo = __dadd_rn(double(mo), __dmul_rn(tau, log(so)));
+    const double lsep = __dadd_rn(double(mp), __dmul_rn(tau, log(sp)));
+    // lane j: pi_post,j (x_post,j - tau ln pi_post,j)
+    const double term = live ? __dmul_rn(__ddiv_rn(eo, so), __dsub_rn(double(xo), __dsub_rn(double(xo), lseo))) : 0.0;
+    double next = 0.0;
+    for (int j = 0; j < A; ++j) next = __dadd_rn(next, __shfl_sync(0xffffffffu, term, j));
+    if (t == 0) {
+      const int a = td_a;
+      const double rr = fmin(fmax(double(td_r), td.min_reward), td.max_reward);
+      const double bonus = __dmul_rn(ma.alpha, fmin(fmax(__dsub_rn(double(qpre[a]), lsep), ma.clip), 0.0));
+      double y;
+      if constexpr (kNstep) {
+        const double rb = __dadd_rn(td_ret, bonus);
+        y = td_term ? rb : __dadd_rn(rb, __dmul_rn(td_g, next));
+      } else {
+        const double rb = __dadd_rn(rr, bonus);
+        y = td_term ? rb : rb + td.discount * next;   // as k_head's one-step target
+      }
+      const float target = static_cast<float>(y);
+      ma.targets[b] = target;
+      float d = s_q[0][a] - target;
+      if (td.isw) {
+        const float wb = td.isw[b];
+        td.td_err[b] = d;
+        td.row_cost[b] = wb * (0.5f * d * d);
+        if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+        d = d * wb;
+      } else {
+        td.row_cost[b] = 0.5f * d * d;
+        if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+      }
+      for (int j = 0; j < A; ++j) td.delta[b * A + j] = (j == a) ? d : 0.f;
+      s_d = d;
+      s_a = a;
+    }
+  }
+  __syncthreads();
+  {
+    const float d = s_d;
+    const int a = s_a;
+    const float hv = h[0];
+    const float o = hv > 0.f ? d * w5_online[t * A + a] : 0.f;
+    td.dz4[b * kHidden + t] = o;
+    if (td.dz4_hi) {
+      const __half hh = __float2half_rn(o);
+      const __half ll = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+      td.dz4_hi[b * kHidden + t] = hh;
+      td.dz4_hi[td.dz4_lo_off + b * kHidden + t] = ll;
+    }
+    float* dw = td.dw5_rows + (int64_t(b) * kHidden + t) * A;
+    for (int j = 0; j < A; ++j) dw[j] = (j == a) ? hv * d : 0.f;
+  }
+  kt_end(kt);
+}
+
 // cost = mean over the batch of the per-sample costs (GeneralizedCost.get_cost, src/deepqnetwork.py:154), summed in
 // row order by one thread (deterministic); advances the cost ring and the step counter.  Runs off the critical
 // chain (the stream of the fc2 optimizer): nothing on the device waits for the scalar.
@@ -944,8 +1078,9 @@ static int fc1_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int r
 
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
 // for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
+// join (Munchausen train step on a stream): the event of the target pass's branch, waited for before the head.
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
-                   const HeadTrainArgs& td) {
+                   const HeadTrainArgs& td, cudaEvent_t join = nullptr) {
   const LayerTable& lt = n->lt;
   const float* w[3] = {n->d_w, n->d_tw, n->d_w};
   int rc;
@@ -1025,6 +1160,25 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     B2_PROF(td.enable ? "head_qr(td+fc2_bwd)" : "head_qr", st);
     return B200DQN_OK;
   }
+  if (n->munchausen && td.enable) {   // predict takes the scalar head below
+    // slot 2, the target network on the prestates, exists with a separate target network only (train_step's pass)
+    const bool pre = n->d_tw != n->d_w;
+    const MdqnArgs ma{n->cfg.munchausen_alpha, n->cfg.munchausen_tau, n->cfg.munchausen_clip, n->d_q[2], n->d_tdtarget};
+    const bool prev = g_pdl_suppressed;
+    if (join) {   // the pass's branch joins here: the head gets ordinary dependencies on both
+      B2_CHECK_CUDA(cudaStreamWaitEvent(st, join, 0));
+      g_pdl_suppressed = true;
+    }
+    const cudaError_t e = launch_pdl(pre ? (nstep ? k_head_mdqn<3, true> : k_head_mdqn<3, false>)
+                                         : (nstep ? k_head_mdqn<2, true> : k_head_mdqn<2, false>),
+                                     dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_fc1part, fc1_splits, rows,
+                                     n->d_h4[0], n->d_h4[1], w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1],
+                                     n->A, ma, td, ktrace_slot("head_mdqn"));
+    g_pdl_suppressed = prev;
+    B2_CHECK_CUDA(e);
+    B2_PROF("head_mdqn(td+fc2_bwd)", st);
+    return B200DQN_OK;
+  }
   B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head<3, true> : k_head<3, false>)
                                      : (nstep ? k_head<2, true> : k_head<2, false>),
                            dim3(rows), dim3(kHidden), 0, st,
@@ -1032,6 +1186,44 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
                            w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, td, ktrace_slot("head")));
   B2_PROF(td.enable ? "head(fc2+td+fc2_bwd)" : "fc2_fwd", st);
   return B200DQN_OK;
+}
+
+// The Munchausen target pass: the target network on slot 0's frames (the prestates) as forward()'s backbone launches
+// with one network slot (nets = 1) and remapped pointers, into the third slot's activations (SIMT) or fp16 planes
+// (tensor cores) and slot 2's region of the three-slot fc1 partials, which k_head_mdqn<3, .> sums.
+static int forward_target_pre(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
+    return umma_forward_target_pre(n, fs.src[0], fs.idx[0], fs.shift[0], rows, st);
+  const LayerTable& lt = n->lt;
+  const float* w = n->d_tw;
+  int rc;
+  {
+    Conv1Fwd p{};
+    p.src[0] = fs.src[0]; p.idx[0] = fs.idx[0]; p.shift[0] = fs.shift[0];
+    p.w[0] = w + lt.off[0]; p.out[0] = n->d_h1[2];
+    p.nb = rows;
+    p.k1 = lt.rows[0];
+    if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st))) return rc;
+  }
+  {
+    using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
+    P p{};
+    p.in[0] = n->d_h1[2]; p.w[0] = w + lt.off[1]; p.out[0] = n->d_h2[2];
+    p.nb = rows;
+    if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, 1, st))) return rc;
+  }
+  {
+    using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
+    P p{};
+    p.in[0] = n->d_h2[2]; p.w[0] = w + lt.off[2]; p.out[0] = n->d_h3[2];
+    p.nb = rows;
+    if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, 1, st))) return rc;
+  }
+  Fc1Fwd<kHidden> p{};   // 512 wide: a Munchausen net is not a dueling one
+  p.in[0] = n->d_h3[2]; p.w[0] = w + lt.off[3];
+  p.part = n->d_fc1part + int64_t(2) * kFc1Splits * rows * kHidden;
+  p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+  return launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, kHidden, kFc1Splits, st);
 }
 
 static int wgrad_chunk(int kred, int base) {
@@ -1519,7 +1711,26 @@ static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* acti
   // the target network IS the online network, so slot 1 already holds that forward and a* = argmax of the same row:
   // the vanilla step is the Double DQN step, bit for bit.
   const int nets = (n->double_q && n->d_tw != n->d_w) ? 3 : 2;
-  B2_TRY(forward(n, fs, nets, rows, st, td));
+  cudaEvent_t join = nullptr;
+  if (n->munchausen && n->d_tw != n->d_w) {
+    // The Munchausen target needs the target network on the prestates.  The pass reads only weights and frames, so on
+    // a stream it forks into its own branch here, after the sampler, overlaps the forward and joins before the head;
+    // on the serial schedule it runs in line, ahead of the forward.
+    if (n->use_branches && st != nullptr && !g_prof_on) {
+      cudaStream_t sP = n->side[0];
+      B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
+      B2_CHECK_CUDA(cudaStreamWaitEvent(sP, n->ev[15], 0));
+      {
+        NoPdlScope side;
+        B2_TRY(forward_target_pre(n, fs, rows, sP));
+      }
+      B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sP));
+      join = n->ev[16];
+    } else {
+      B2_TRY(forward_target_pre(n, fs, rows, st));
+    }
+  }
+  B2_TRY(forward(n, fs, nets, rows, st, td, join));
   return backward_and_update(n, fs, rows, st, true);
 }
 
@@ -1576,8 +1787,14 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->v_max = 10.0;
   cfg->dueling = 0;              // one value stream
   cfg->num_quantiles = 0;        // no quantile-regression head
+  cfg->munchausen = 0;           // the scalar head's target; the Munchausen constants are the paper's
+  cfg->munchausen_alpha = 0.9;
+  cfg->munchausen_tau = 0.03;
+  cfg->munchausen_clip = -1.0;
   return B200DQN_OK;
 }
+
+static int double_q_alloc(b200dqn_net* n);
 
 extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b200dqn_net** out) {
   B2_REQUIRE(cfg && out, B200DQN_EINVAL, "net_create: null argument");
@@ -1611,6 +1828,19 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
              "net_create: the quantile Huber threshold clip_error must be finite (got %g)", cfg->clip_error);
   B2_REQUIRE(!(cfg->dueling && cfg->num_quantiles), B200DQN_ENOTIMPL,
              "net_create: a dueling net with a quantile-regression head is not implemented");
+  B2_REQUIRE(cfg->munchausen == 0 || cfg->munchausen == 1, B200DQN_EINVAL,
+             "net_create: munchausen %d is neither 0 nor 1 (the Munchausen target)", cfg->munchausen);
+  if (cfg->munchausen) {
+    B2_REQUIRE(std::isfinite(cfg->munchausen_alpha) && cfg->munchausen_alpha >= 0, B200DQN_EINVAL,
+               "net_create: the Munchausen alpha must be finite and >= 0 (got %g)", cfg->munchausen_alpha);
+    B2_REQUIRE(std::isfinite(cfg->munchausen_tau) && cfg->munchausen_tau > 0, B200DQN_EINVAL,
+               "net_create: the Munchausen tau must be finite and > 0 (got %g)", cfg->munchausen_tau);
+    B2_REQUIRE(std::isfinite(cfg->munchausen_clip) && cfg->munchausen_clip <= 0, B200DQN_EINVAL,
+               "net_create: the Munchausen clip l0 must be finite and <= 0 (got %g)", cfg->munchausen_clip);
+    B2_REQUIRE(!cfg->dueling && !cfg->num_atoms && !cfg->num_quantiles, B200DQN_ENOTIMPL,
+               "net_create: the Munchausen target with a dueling network, a distributional or a quantile head is not "
+               "implemented");
+  }
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -1623,6 +1853,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->atoms = cfg->num_atoms;
   n->quantiles = cfg->num_quantiles;
   n->dueling = cfg->dueling != 0;
+  n->munchausen = cfg->munchausen != 0;
   n->hidden = n->dueling ? kDuelHidden : kHidden;
   if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
   const int nb = n->nb, A = n->A, hist = cfg->history_length;
@@ -1714,6 +1945,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
   }
   if (n->dueling) B2_CHECK_CUDA(fmalloc(&n->d_va, size_t(3) * nb * (A + 1)));
+  if (n->munchausen) B2_CHECK_CUDA(fmalloc(&n->d_tdtarget, nb));
   const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
   B2_CHECK_CUDA(cudaMalloc(&n->d_pre, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_post, state_bytes + 256));
@@ -1743,6 +1975,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->use_branches = getenv("B200DQN_NO_BRANCHES") == nullptr;
   int rc = umma_net_init(n);
   if (rc) return rc;
+  if (n->munchausen && n->d_tw != n->d_w && (rc = double_q_alloc(n))) return rc;   // the target pass's third slot
   B2_CHECK_CUDA(cudaDeviceSynchronize());
   *out = n;
   return B200DQN_OK;
@@ -1773,6 +2006,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_logits); cudaFree(n->d_probs); cudaFree(n->d_tdist); cudaFree(n->d_lgrad); cudaFree(n->d_act_rows);
   cudaFree(n->d_va);
   cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
+  cudaFree(n->d_tdtarget);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -2278,6 +2512,17 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
                                                                                                        : n->d_qgrad;
       b = (which == B200DQN_NET_PTR_QUANTILES ? size_t(3) * n->nb * n->A : size_t(n->nb)) * n->quantiles * 4;
       break;
+    case B200DQN_NET_PTR_Q_TARGET_PRE:
+    case B200DQN_NET_PTR_TD_TARGETS:
+      B2_REQUIRE(n->munchausen, B200DQN_EINVAL, "net_device_ptr: selector %d needs the Munchausen target", which);
+      if (which == B200DQN_NET_PTR_TD_TARGETS) {
+        p = n->d_tdtarget;
+        b = size_t(n->nb) * 4;
+      } else {   // target_steps = 0: the target network is the online one, and so is its Q row of the prestates
+        p = n->d_tw == n->d_w ? n->d_q[0] : n->d_q[2];
+        b = size_t(n->nb) * n->A * 4;
+      }
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -2324,6 +2569,8 @@ static int double_q_alloc(b200dqn_net* n) {
 extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   B2_REQUIRE(n, B200DQN_EINVAL, "null net");
   if (on) {
+    B2_REQUIRE(!n->munchausen, B200DQN_EINVAL,
+               "net_set_double_q: the Munchausen target makes no greedy choice for Double DQN to change");
     B2_REQUIRE(!n->nccl_comm, B200DQN_ENOTIMPL,
                "net_set_double_q: the Double DQN target is implemented for a single learner only (comm_init has run)");
     B2_TRY(double_q_alloc(n));
@@ -2367,8 +2614,10 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     *launches = n->graph_launches;
   } else {
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
-    // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update
-    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0);
+    // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
+    // target with a separate target network repeats the forward's launches for its pass
+    *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
+                (n->munchausen && n->d_tw != n->d_w ? 4 : 0);
   }
   return B200DQN_OK;
 }

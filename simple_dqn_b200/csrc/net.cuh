@@ -84,7 +84,7 @@ struct b200dqn_net {
   // step scheduling: side streams / events for the independent wgrad + optimizer branches, and the
   // captured CUDA graph of one fused step
   cudaStream_t side[4] = {};   // three wgrad/optimizer branches + the collective stream
-  cudaEvent_t ev[15] = {};
+  cudaEvent_t ev[17] = {};   // [15] / [16]: fork / join of the Munchausen target pass (train_step)
   bool use_graph = true, use_branches = true;
   bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
   bool double_q = false;     // Double DQN target: the online net picks the poststate action, the target net values it
@@ -132,6 +132,12 @@ struct b200dqn_net {
   bool dueling = false;
   int hidden = b200::kHidden;    // fc1's width: H4, dZ4 and the fc1 partials are [.][hidden]
   float* d_va = nullptr;         // [3][nb][A + 1]: the advantages, then V, of every slot of the last forward
+
+  // Munchausen target (cfg.munchausen): with a separate target network the train step runs it on the prestates as a
+  // one-slot forward pass into the third slot's buffers (made at creation; Double DQN, their other user, is refused),
+  // and the head reads its Q row as slot 2 (Q_TARGET_PRE = d_q[2])
+  bool munchausen = false;
+  float* d_tdtarget = nullptr;   // [nb] float(y) of the last train step
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

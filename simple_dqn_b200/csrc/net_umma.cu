@@ -1184,6 +1184,61 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
   return n->dueling ? fc1_fwd_umma<kDuelHidden>(n, h3, nets, rows, st) : fc1_fwd_umma<kHidden>(n, h3, nets, rows, st);
 }
 
+// The Munchausen target pass: umma_forward's launches with one network slot (nets = 1) and remapped pointers.  Device
+// slot 0 reads the target network's weight images and the prestates (slot 0's frames) and writes the third slot's
+// fp16 planes and fc1 partials; no fp32 activation is kept.  The kernels specialise slot 0 in two places: conv1_fwd
+// dumps no im2col tiles (nets < 2), and conv23_fwd stores its H2 planes (here slot 2's) and, with a null `out`, no
+// fp32 H2.
+int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, int rows,
+                            cudaStream_t st) {
+  UmmaState* u = ust(n);
+  auto planes = [&](int i) { return PlanePair{u->h16[i][2], u->h_elems[i]}; };
+  int rc = with_hist(n->cfg.history_length, [&](auto h) {
+    constexpr int H = decltype(h)::value;
+    V2Conv1Fwd<H> p{};
+    p.src[0] = p.src[1] = src; p.idx[0] = p.idx[1] = idx; p.shift[0] = p.shift[1] = shift;
+    p.wimg[0] = p.wimg[1] = u->img_fwd[1][0];
+    p.out16[0] = planes(0);
+    p.rows = rows;
+    p.im2col = nullptr;
+    return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st, false);
+  });
+  if (rc) return rc;
+  if (rows <= kConv23MaxRows) {
+    Conv23Fwd p{};
+    p.c2.wimg[0] = p.c2.wimg[1] = u->img_fwd[1][1];
+    p.c3.wimg[0] = p.c3.wimg[1] = u->img_fwd[1][2];
+    p.c2.in16[0] = planes(0);
+    p.c2.out16[0] = planes(1);
+    p.c3.out16[0] = planes(2);
+    p.c2.rows = p.c3.rows = rows;
+    if ((rc = launch_conv23(p, rows, 1, st))) return rc;
+  } else {
+    {
+      V2ConvFwd<kP1, kC1, 4, 2, kC2> p{};
+      p.wimg[0] = p.wimg[1] = u->img_fwd[1][1];
+      p.in16[0] = planes(0); p.out16[0] = planes(1);
+      p.rows = rows;
+      if ((rc = umma2::launch_umma2("conv2_fwd", p, rows * kP2 * kP2, kC2, 1, st, false))) return rc;
+    }
+    {
+      V2ConvFwd<kP2, kC2, 3, 1, kC3> p{};
+      p.wimg[0] = p.wimg[1] = u->img_fwd[1][2];
+      p.in16[0] = planes(1); p.out16[0] = planes(2);
+      p.rows = rows;
+      if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, 1, st, false))) return rc;
+    }
+  }
+  // fc1 (512 wide: a Munchausen net is not a dueling one) into slot 2's region of the three-slot partial buffer
+  V2Fc1Fwd<kHidden> p{};
+  p.wimg[0] = p.wimg[1] = u->img_fwd[1][3];
+  p.in16[0] = planes(2);
+  p.splits = fc1_splits_for(rows);
+  p.part = n->d_fc1part + int64_t(2) * p.splits * rows * kHidden;
+  p.rows = rows;
+  return umma2::launch_umma2("fc1_fwd", p, kHidden, rows, p.splits, st, false);
+}
+
 template <int W>
 static int fc1_wgrad_umma(b200dqn_net* n, int rows, cudaStream_t st, bool release_early) {
   UmmaState* u = ust(n);

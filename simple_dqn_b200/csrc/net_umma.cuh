@@ -24,6 +24,10 @@ int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
                  int nets, int rows, cudaStream_t st, bool release_early);
 int umma_fc1_splits(int rows);
+// the Munchausen target pass: the target network on the frames src/idx/shift (the prestates), into slot 2's planes and
+// fc1 partials (nets = 1, no fp32 activations)
+int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, int rows,
+                            cudaStream_t st);
 // RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel
 int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false);
 // fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tensor-core path

@@ -86,6 +86,15 @@ class DeepQNetwork:
         if self.quantile_regression:
             cfg.num_quantiles = int(_arg(args, "num_quantiles", 200))
             assert cfg.num_quantiles >= 1, "num_quantiles %d: the quantile head needs 1..200" % cfg.num_quantiles
+        # Munchausen DQN target (Vieillard et al., 2020): a new capability, off unless args.munchausen is set; alpha,
+        # tau and the clip l0 default to the paper's 0.9, 0.03 and -1.  It sizes the train step's buffers, so it is
+        # fixed here; with args.double_dqn it is refused (AssertionError: the target makes no greedy choice)
+        self.munchausen = bool(_arg(args, "munchausen", False))
+        if self.munchausen:
+            cfg.munchausen = 1
+            cfg.munchausen_alpha = float(_arg(args, "munchausen_alpha", 0.9))
+            cfg.munchausen_tau = float(_arg(args, "munchausen_tau", 0.03))
+            cfg.munchausen_clip = float(_arg(args, "munchausen_clip", -1.0))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -287,6 +296,16 @@ class DeepQNetwork:
     def last_quantile_grads(self):
         """The gradient on the taken action's quantiles of the last train(), (batch, num_quantiles) float32."""
         return self._read_f32(L.NET_PTR_QUANTILE_GRADS, (self.batch_size, self.num_quantiles))
+
+    # ---- Munchausen target (munchausen = True)
+    def last_target_q_pre(self):
+        """The target network's Q on the prestates of the last train(), (batch, A) float32: the row whose log-policy
+        at the taken action forms the Munchausen bonus (with target_steps = 0 the online row, last_q()[0])."""
+        return self._read_f32(L.NET_PTR_Q_TARGET_PRE, (self.batch_size, self.num_actions))
+
+    def last_td_targets(self):
+        """The Munchausen targets float(y) of the last train(), (batch,) float32."""
+        return self._read_f32(L.NET_PTR_TD_TARGETS, (self.batch_size,))
 
     # ---- dueling network: slots as for the distributional head
     def last_advantages(self):

@@ -18,6 +18,7 @@ ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with
 NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
 DUELING = os.environ.get("DUELING", "0") == "1"   # dueling network (1024-unit fc1, advantage and value streams)
 QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (QR-DQN) with this many quantiles; 0: off
+MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target (extra target pass on the prestates)
 
 
 def args():
@@ -30,6 +31,7 @@ def args():
     a.num_atoms = ATOMS
     a.dueling = DUELING
     a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
+    a.munchausen = MUNCHAUSEN
     return a
 
 
@@ -55,6 +57,6 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d period_us min %.2f median %.2f  "
-      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, min(res), float(np.median(res)),
+print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d munchausen %d period_us min %.2f median %.2f  "
+      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, MUNCHAUSEN, min(res), float(np.median(res)),
                   " ".join("%.2f" % r for r in res)))

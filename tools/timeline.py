@@ -12,6 +12,7 @@ ATOMS = int(os.environ.get("ATOMS", "0"))       # distributional head (C51) with
 NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed actions stay below 4)
 DUELING = os.environ.get("DUELING", "0") == "1"   # dueling network (1024-unit fc1, advantage and value streams)
 QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (QR-DQN) with this many quantiles; 0: off
+MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target (extra target pass on the prestates)
 
 
 def net_args():
@@ -19,6 +20,7 @@ def net_args():
     a.distributional, a.num_atoms = ATOMS > 0, ATOMS
     a.dueling = DUELING
     a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
+    a.munchausen = MUNCHAUSEN
     return a
 
 
