@@ -307,6 +307,45 @@ typedef struct b200dqn_net_config {
   double munchausen_alpha;
   double munchausen_tau;
   double munchausen_clip;
+  /* Implicit quantile network head (IQN, Dabney, Ostrovski, Silver and Munos, 2018; new capability, no reference
+   * counterpart), off when num_tau_samples = 0 (the default).  Otherwise N = num_tau_samples in 1..64 and
+   * K = num_quantile_samples in 1..64 (default 32), with nb max(N, K) <= 4096 rows (EINVAL otherwise, before any
+   * device work); kappa = float(clip_error) as for the quantile-regression head (non-finite: EINVAL).  EINVAL with
+   * num_atoms or num_quantiles (a net has one head), ENOTIMPL with dueling or munchausen;
+   * b200dqn_net_set_double_q(n, 1) and b200dqn_net_comm_init return ENOTIMPL on such a net.  The embedding is ABI layer
+   * 5, Neon shape (3136, 64) (row n = fc1's input column in Neon's (c, p, q) order), with its own optimizer states; it
+   * belongs to each network (online and target) like every other layer.  b is the sample, a the taken action, z the
+   * slot (0 online on the prestates, 1 target on the poststates); every fp32 operation is rounded on its own:
+   *    1. tau draw: tau = (2m + 1) 2^-24, m = h >> 9 where h is the high 32 bits of
+   *         x = mix(mix(tau_seed + 0x9E3779B97F4A7C15 (ctr + 1)) ^ (z << 32 | b << 8 | j)),
+   *       mix = splitmix64's finaliser (x ^= x >> 30; x *= 0xBF58476D1CE4E5B9; x ^= x >> 27; x *= 0x94D049BB133111EB;
+   *       x ^= x >> 31), all mod 2^64, ctr the device-resident draw counter.  Every forward (train step or predict)
+   *       draws with the counter's value and then advances it by one, on the device, so replayed step and predict
+   *       graphs draw fresh tau; the replay sampler's MT19937 stream is not touched;
+   *    2. rows r = b N + j (train: N online rows on slot 0, N target rows on slot 1), r = b K + k on predict (slot 0);
+   *    3. c[r][i] = float(cos((pi i) tau_r)) for i = 0..63, formed in fp64 with the device's cos (c[r][0] = 1 is the
+   *       embedding's bias);
+   *    4. phi[r][col] = max(0, sum_i c[r][i] We[i][col], i order), We of the slot's network;
+   *    5. X[r] = psi[b] * phi[r], psi = conv3's Rectlin output H3 of the sample; fc1 and fc2 run on X at nb N rows
+   *       (nb K on predict) with the scalar net's kernels;
+   *    6. theta[z][r][a] = sum_k H4[z][r][k] W5[k][a], k = 0..511 in order;
+   *    7. Q[a] = (sum_j theta[b N + j][a], j order) / float(N) per slot (K on predict).  Every Q output is this Q;
+   *    8. a* = first index of the maximum of slot 1's Q (a simplification: the paper draws K separate samples for a*);
+   *    9. T_j = float(R + g double(theta[1][b N + j][a*])), R and g as for the quantile-regression head;
+   *       u_ij = T_j - theta[0][b N + i][a], weight tau_i (slot 0's tau of row b N + i) for u >= 0 and 1 - tau_i for
+   *       u < 0; the loss, the row cost, the importance weight, the priority and dtheta_i then follow rules 8-10 of
+   *       the quantile-regression head over the N x N pairs;
+   *   10. dZ4[r][k] = H4[0][r][k] > 0 ? W5[k][a] dtheta_r : 0; fc2's gradient is sum_r H4[0][r][k] dtheta_r in row
+   *       order at column a, then the configured optimizer (batch size nb) applies it;
+   *   11. dX = fc1's dgrad at nb N rows (masked by X > 0, harmless: X = psi phi >= 0, and where X = 0 both terms of 12
+   *       vanish anyway);
+   *   12. dpsi[b][col] = (sum_j dX[b N + j][col] phi[b N + j][col], j order), 0 unless psi > 0; it is conv3's dZ (the
+   *       DZ3 selector); dphi[r][col] = phi > 0 ? dX[r][col] psi[b][col] : 0;
+   *   13. dWe[i][col] = sum_r c[r][i] dphi[r][col] over slot 0's rows in row order; the configured optimizer (batch size
+   *       nb) applies it. */
+  int num_tau_samples;
+  int num_quantile_samples;
+  uint64_t tau_seed;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -318,7 +357,8 @@ int b200dqn_net_destroy(b200dqn_net* n);
 
 /* Weights cross the boundary in NEON layout: conv W[C*R*S][K], linear W[nout][nin], fp32,
  * C-contiguous (what Model.get_description / the shipped snapshots hold); host_S is the
- * RMSProp state of the same shape (may be NULL).  layer 0..4; which 0 = online, 1 = target.
+ * RMSProp state of the same shape (may be NULL).  layer 0..4 (and 5, the embedding, on an IQN net); which 0 = online,
+ * 1 = target.
  * Replaces Model.load_params / save_params — src/deepqnetwork.py:188-192.  Synchronises. */
 int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, const float* host_W, const float* host_S,
                             void* stream);
@@ -441,7 +481,20 @@ enum {
   /* Munchausen target only (munchausen = 1; EINVAL otherwise). */
   B200DQN_NET_PTR_Q_TARGET_PRE,     /* (batch, A) f32 the target network's Q on the prestates of the last train step;
                                      * with target_steps = 0 it is the Q_ONLINE buffer (the two networks are one)   */
-  B200DQN_NET_PTR_TD_TARGETS        /* (batch,) f32 the targets float(y) of the last train step                     */
+  B200DQN_NET_PTR_TD_TARGETS,       /* (batch,) f32 the targets float(y) of the last train step                     */
+  /* IQN head only (num_tau_samples > 0; EINVAL otherwise).  Rows as in its rules: nb N per slot after a train step, nb K
+   * on slot 0 after a predict; R = nb max(N, K) rows are reserved per slot.  H4 and DZ4 hold R rows on such a net, DZ3
+   * is dpsi, and the quantile-regression selectors and DELTAS are EINVAL. */
+  B200DQN_NET_PTR_IQN_TAUS,         /* (2, R) f32 tau of the last forward                                            */
+  B200DQN_NET_PTR_IQN_COS,          /* (2, R, 64) f32 cosine features c                                              */
+  B200DQN_NET_PTR_IQN_PHI,          /* (2, R, 3136) f32 embedding output phi, fc1's internal (p, q, c) column order  */
+  B200DQN_NET_PTR_IQN_X,            /* (2, R, 3136) f32 fc1's input X = psi * phi, same order                        */
+  B200DQN_NET_PTR_IQN_QUANTILES,    /* (2, R, A) f32 theta                                                           */
+  B200DQN_NET_PTR_IQN_TARGET_QUANTILES, /* (batch, N) f32 T_j of the last train step                                 */
+  B200DQN_NET_PTR_IQN_QUANTILE_GRADS,   /* (batch N,) f32 dtheta of the taken action, per online row                 */
+  B200DQN_NET_PTR_IQN_DX,           /* (R, 3136) f32 fc1's dgrad dX of the last train step                           */
+  B200DQN_NET_PTR_IQN_DPHI,         /* (R, 3136) f32 dphi of the last train step                                     */
+  B200DQN_NET_PTR_IQN_TAU_COUNTER   /* u64 the draw counter (the next forward draws with this value)                 */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

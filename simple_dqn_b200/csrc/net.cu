@@ -977,6 +977,331 @@ k_head_qr(const float* __restrict__ theta, int ld, int nets, const float* __rest
 }
 
 // ------------------------------------------------------------------------------------------
+// Implicit quantile network head (IQN, Dabney, Ostrovski, Silver and Munos 2018; b200dqn.h has the rules).  fc1 and fc2
+// run on the expanded rows r = b * per + j with the scalar net's fc1 kernels and k_fc2_dist (A columns); fc2's gradient
+// goes through k_opt_fc2_dist with block width 1.  The new kernels:
+//   k_iqn_tau      one CTA: tau of every (slot, row) from the stated hash at the draw counter, then the counter + 1
+//   k_iqn_phi      the cosine features c and the embedding phi = max(0, c We), 16 rows per CTA
+//   k_iqn_mod      X = psi * phi, psi = conv3's output H3 of the row's sample
+//   k_head_iqn     one CTA per sample: Q, a*, the target quantiles, the quantile Huber loss and dtheta, dZ4 and fc2's
+//                  per-row partials
+//   k_iqn_mod_bwd  dpsi (conv3's dZ) and dphi from fc1's dgrad dX
+//   k_iqn_we       dWe and the embedding's update
+// Every fp32 operation is rounded on its own (explicit _rn intrinsics).
+// ------------------------------------------------------------------------------------------
+constexpr int kIqnCos = 64;      // cosine features per row
+constexpr int kIqnMaxPer = 64;   // N, K <= 64
+constexpr int kIqnTB = 16;       // k_iqn_phi: rows per CTA
+
+__device__ __forceinline__ unsigned long long iqn_mix(unsigned long long x) {   // splitmix64's finaliser
+  x ^= x >> 30;
+  x *= 0xBF58476D1CE4E5B9ull;
+  x ^= x >> 27;
+  x *= 0x94D049BB133111EBull;
+  x ^= x >> 31;
+  return x;
+}
+
+// tau[z][b * per + j] for z < nets, b < rows, j < per, drawn at the counter's value; thread 0 then advances the counter
+// (every thread has read it by the barrier), so the next forward, or the next replay of a captured graph, draws fresh.
+__global__ void __launch_bounds__(1024)
+k_iqn_tau(unsigned long long* ctr, unsigned long long seed, int nets, int rows, int per, int ld, float* tau,
+          const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const unsigned long long c = *ctr;
+  const unsigned long long base = iqn_mix(seed + 0x9E3779B97F4A7C15ull * (c + 1ull));
+  const int per_slot = rows * per;
+  for (int e = threadIdx.x; e < nets * per_slot; e += blockDim.x) {
+    const int z = e / per_slot, r = e % per_slot, b = r / per, j = r % per;
+    const unsigned long long x = iqn_mix(base ^ ((unsigned long long)z << 32 | (unsigned long long)b << 8 | unsigned(j)));
+    const unsigned m = unsigned(x >> 32) >> 9;   // the top 23 bits of the 32-bit hash
+    tau[int64_t(z) * ld + r] = __fmul_rn(float(2u * m + 1u), 5.9604644775390625e-08f);   // (2m + 1) 2^-24, exact
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *ctr = c + 1ull;
+  kt_end(kt);
+}
+
+// grid (cdiv(rows, 16), nets).  c[r][i] = float(cos((pi i) tau_r)) in fp64, stored for the embedding's gradient; then
+// thread t takes columns t, t + 256, ... and accumulates the CTA's 16 rows of column col in i order.
+__global__ void __launch_bounds__(256)
+k_iqn_phi(const float* __restrict__ tau, int rows, int ld, const float* __restrict__ we_online,
+          const float* __restrict__ we_target, float* __restrict__ cosf, float* __restrict__ phi, const KTrace kt) {
+  __shared__ float s_c[kIqnTB][kIqnCos];
+  const int z = blockIdx.y, r0 = blockIdx.x * kIqnTB, t = threadIdx.x;
+  const int nrow = min(kIqnTB, rows - r0);
+  const float* we = z ? we_target : we_online;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  for (int e = t; e < kIqnTB * kIqnCos; e += 256) {
+    const int r = e / kIqnCos, i = e % kIqnCos;
+    float c = 0.f;
+    if (r < nrow) {
+      c = float(cos(__dmul_rn(__dmul_rn(3.141592653589793, double(i)), double(tau[int64_t(z) * ld + r0 + r]))));
+      cosf[(int64_t(z) * ld + r0 + r) * kIqnCos + i] = c;
+    }
+    s_c[r][i] = c;
+  }
+  __syncthreads();
+  for (int col = t; col < kFlat; col += 256) {
+    float acc[kIqnTB];
+#pragma unroll
+    for (int j = 0; j < kIqnTB; ++j) acc[j] = 0.f;
+    for (int i = 0; i < kIqnCos; ++i) {
+      const float w = we[i * kFlat + col];
+#pragma unroll
+      for (int j = 0; j < kIqnTB; ++j) acc[j] = __fadd_rn(acc[j], __fmul_rn(s_c[j][i], w));
+    }
+#pragma unroll
+    for (int j = 0; j < kIqnTB; ++j)
+      if (j < nrow) phi[(int64_t(z) * ld + r0 + j) * kFlat + col] = fmaxf(acc[j], 0.f);
+  }
+  kt_end(kt);
+}
+
+// X[z][r][col] = H3[z][r / per][col] * phi[z][r][col] over nets slots of `rows` expanded rows (grid-stride), and on the
+// tensor-core engine (x16 != nullptr) its hi / lo fp16 planes
+__global__ void __launch_bounds__(256)
+k_iqn_mod(const float* __restrict__ h3_online, const float* __restrict__ h3_target, const float* __restrict__ phi,
+          float* __restrict__ x, __half* __restrict__ x16, int nets, int rows, int per, int ld, const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const int64_t slot = int64_t(rows) * kFlat, total = nets * slot;
+  for (int64_t e = int64_t(blockIdx.x) * 256 + threadIdx.x; e < total; e += int64_t(gridDim.x) * 256) {
+    const int z = int(e / slot);
+    const int64_t re = e - z * slot;
+    const int r = int(re / kFlat), col = int(re % kFlat);
+    const float psi = (z ? h3_target : h3_online)[int64_t(r / per) * kFlat + col];
+    const int64_t o = int64_t(z) * ld * kFlat + re;
+    const float v = __fmul_rn(psi, phi[o]);
+    x[o] = v;
+    if (x16) {   // tensor-core engine: fc1's operand planes, hi and lo scaled by 2048, slot z at z * 2 * ld * 3136
+      const __half hh = __float2half_rn(v);
+      __half* hp = x16 + 2 * int64_t(z) * ld * kFlat + re;
+      hp[0] = hh;
+      hp[int64_t(ld) * kFlat] = __float2half_rn((v - __half2float(hh)) * 2048.0f);
+    }
+  }
+  kt_end(kt);
+}
+
+struct IqnArgs {
+  int per;            // rows per sample: N (train) or K (predict)
+  int ld;             // slot stride of tau and theta (iqn_rows)
+  float kappa;        // the Huber threshold (clip_error); 0: the pure quantile loss
+  const float* tau;   // [2][ld]
+  float* tq;          // [nb][N] target quantiles T_j
+  float* qgrad;       // [nb N] dtheta of each online row
+  int32_t* act_rows;  // [nb N] taken action of each online row (selects fc2's gradient column)
+};
+
+// One CTA (512 threads) per sample b; its rows are r = b * per + j.  Thread t < nets * A owns (slot z, action a):
+// Q = (sum_j theta[z][r][a], j order) / per.  With td.enable (kSlots = 2): thread 0 picks a* and the fp64 return, thread
+// j < N forms T_j, thread i < N runs k_head_qr's j loop for online row b N + i with the weights tau_i and 1 - tau_i, thread
+// 0 sums the row loss, and thread k writes dZ4 and fc2's row partial of unit k for every online row of the sample.
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ h4_online,
+           const float* __restrict__ w5_online, float* q_online, float* q_target, int A, const IqnArgs ia,
+           const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 1 || kSlots == 2, "predict, or online + target");
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_t[kIqnMaxPer], s_l[kIqnMaxPer], s_g[kIqnMaxPer];
+  __shared__ double s_ret, s_gam;
+  __shared__ int s_a, s_astar;
+  const int b = blockIdx.x, t = threadIdx.x, np = ia.per;
+  const int64_t ld = ia.ld, r0 = int64_t(b) * np;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float* th = theta + (z * ld + r0) * A + a;
+    float s = 0.f;
+    for (int j = 0; j < np; ++j) s = __fadd_rn(s, th[int64_t(j) * A]);
+    const float q = __fdiv_rn(s, float(np));
+    s_q[z][a] = q;
+    (z == 0 ? q_online : q_target)[b * A + a] = q;
+  }
+  if constexpr (kSlots > 1) {
+    if (!td.enable) {
+      kt_end(kt);
+      return;
+    }
+    __syncthreads();
+    if (t == 0) {
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (s_q[1][j] > s_q[1][best]) best = j;
+      double R, g;
+      if constexpr (kNstep) {
+        R = td_ret;
+        g = td_term ? 0.0 : td_g;
+      } else {
+        R = fmin(fmax(double(td_r), td.min_reward), td.max_reward);   // np.clip as the scalar head
+        g = td_term ? 0.0 : td.discount;
+      }
+      s_ret = R;
+      s_gam = g;
+      s_a = td_a;
+      s_astar = best;
+    }
+    __syncthreads();
+    const int a = s_a;
+    if (t < np) {   // T_j = float(R + g q'_j), q'_j = the target network's theta of row b N + j at a*
+      const float qj = theta[(ld + r0 + t) * A + s_astar];
+      const float T = float(__dadd_rn(s_ret, __dmul_rn(s_gam, double(qj))));
+      s_t[t] = T;
+      ia.tq[r0 + t] = T;
+    }
+    __syncthreads();
+    if (t < np) {   // online row b N + i (i = t) against every target sample j, j order
+      const float th = theta[(r0 + t) * A + a];
+      const float wlo = ia.tau[r0 + t], whi = __fsub_rn(1.f, wlo), kap = ia.kappa;
+      float rho = 0.f, c = 0.f;
+      for (int j = 0; j < np; ++j) {
+        const float u = __fsub_rn(s_t[j], th);
+        const float w = u < 0.f ? whi : wlo;
+        const float au = fabsf(u);
+        if (kap > 0.f) {
+          const float L = au <= kap ? __fmul_rn(0.5f, __fmul_rn(u, u)) : __fmul_rn(kap, __fsub_rn(au, __fmul_rn(0.5f, kap)));
+          rho = __fadd_rn(rho, __fdiv_rn(__fmul_rn(w, L), kap));
+          c = __fadd_rn(c, __fdiv_rn(__fmul_rn(w, fminf(fmaxf(u, -kap), kap)), kap));
+        } else {
+          rho = __fadd_rn(rho, __fmul_rn(w, au));
+          c = __fadd_rn(c, u > 0.f ? w : u < 0.f ? -w : 0.f);
+        }
+      }
+      float g = -__fdiv_rn(c, float(np));
+      if (td.isw) g = __fmul_rn(g, td.isw[b]);
+      s_l[t] = __fdiv_rn(rho, float(np));
+      s_g[t] = g;
+      ia.qgrad[r0 + t] = g;
+      ia.act_rows[r0 + t] = a;
+    }
+    __syncthreads();
+    if (t == 0) {   // the row loss: sum_i Loss_i, i order
+      float l = 0.f;
+      for (int i = 0; i < np; ++i) l = __fadd_rn(l, s_l[i]);
+      if (td.isw) {
+        td.td_err[b] = l;
+        td.row_cost[b] = __fmul_rn(td.isw[b], l);
+      } else {
+        td.row_cost[b] = l;
+      }
+    }
+    const float w5a = w5_online[t * A + a];
+    for (int i = 0; i < np; ++i) {
+      const int64_t r = r0 + i;
+      const float hv = h4_online[r * kHidden + t], g = s_g[i];
+      const float o = hv > 0.f ? __fmul_rn(w5a, g) : 0.f;
+      td.dz4[r * kHidden + t] = o;
+      if (td.dz4_hi) {   // the tensor-core fc1 dgrad / wgrad operand
+        const __half hh = __float2half_rn(o);
+        td.dz4_hi[r * kHidden + t] = hh;
+        td.dz4_hi[td.dz4_lo_off + r * kHidden + t] = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+      }
+      td.dw5_rows[r * kHidden + t] = __fmul_rn(hv, g);
+    }
+  }
+  kt_end(kt);
+}
+
+// One thread per (sample b, column col) of `rows` samples: dpsi[b][col] = (sum_j dX[r][col] phi[r][col], j order) under
+// psi's mask (and its fp16 planes on the tensor-core engine), and dphi[r][col] = phi > 0 ? dX[r][col] psi : 0,
+// r = b * per + j.
+__global__ void __launch_bounds__(256)
+k_iqn_mod_bwd(const float* __restrict__ dx, const float* __restrict__ phi, const float* __restrict__ h3,
+              float* __restrict__ dpsi, __half* __restrict__ dpsi16, int64_t dpsi_lo, float* __restrict__ dphi, int rows,
+              int per, const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const int e = blockIdx.x * 256 + threadIdx.x;
+  if (e < rows * kFlat) {
+    const int b = e / kFlat, col = e % kFlat;
+    const float psi = h3[e];
+    float acc = 0.f;
+    for (int j = 0; j < per; ++j) {
+      const int64_t o = (int64_t(b) * per + j) * kFlat + col;
+      const float d = dx[o], p = phi[o];
+      acc = __fadd_rn(acc, __fmul_rn(d, p));
+      dphi[o] = p > 0.f ? __fmul_rn(d, psi) : 0.f;
+    }
+    const float o = psi > 0.f ? acc : 0.f;
+    dpsi[e] = o;
+    if (dpsi16) {   // tensor-core engine: the planes conv3's dgrad and wgrad read
+      const __half hh = __float2half_rn(o);
+      dpsi16[e] = hh;
+      dpsi16[dpsi_lo + e] = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+    }
+  }
+  kt_end(kt);
+}
+
+// dWe[i][col] = sum_r c[r][i] dphi[r][col] over `rows` online rows in row order, then (update) the configured optimizer.
+// grid cdiv(3136, 32): thread (ig, cl) of a CTA owns column blockIdx.x * 32 + cl and features ig * 8 .. ig * 8 + 7; the
+// rows pass through shared memory 32 at a time.
+constexpr int kWeCols = 32, kWeRows = 32;
+__global__ void __launch_bounds__(256)
+k_iqn_we(const float* __restrict__ cosf, const float* __restrict__ dphi, int rows, float* __restrict__ g_out,
+         float* __restrict__ w, float* __restrict__ sst, int update, const OptArgs opt, const KTrace kt) {
+  __shared__ float s_c[kWeRows][kIqnCos];
+  __shared__ float s_d[kWeRows][kWeCols];
+  const int t = threadIdx.x, cl = t % kWeCols, ig = t / kWeCols, c0 = blockIdx.x * kWeCols;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  float acc[8];
+#pragma unroll
+  for (int u = 0; u < 8; ++u) acc[u] = 0.f;
+  for (int rb = 0; rb < rows; rb += kWeRows) {
+    const int nr = min(kWeRows, rows - rb);
+    __syncthreads();
+    for (int e = t; e < kWeRows * kIqnCos; e += 256) {
+      const int r = e / kIqnCos, i = e % kIqnCos;
+      s_c[r][i] = r < nr ? cosf[int64_t(rb + r) * kIqnCos + i] : 0.f;
+    }
+    for (int e = t; e < kWeRows * kWeCols; e += 256) {
+      const int r = e / kWeCols, cc = c0 + e % kWeCols;
+      s_d[r][e % kWeCols] = r < nr && cc < kFlat ? dphi[int64_t(rb + r) * kFlat + cc] : 0.f;
+    }
+    __syncthreads();
+    for (int r = 0; r < nr; ++r) {
+      const float d = s_d[r][cl];
+#pragma unroll
+      for (int u = 0; u < 8; ++u) acc[u] = __fadd_rn(acc[u], __fmul_rn(s_c[r][ig * 8 + u], d));
+    }
+  }
+  const int col = c0 + cl;
+  if (col < kFlat) {
+    const float l = opt_step_scalar(opt);
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int64_t wi = int64_t(ig * 8 + u) * kFlat + col;
+      g_out[wi] = acc[u];
+      if (update) {
+        float s[3] = {0.f, 0.f, 0.f};
+        for (int k = 0; k < opt.nstates; ++k) s[k] = sst[k * opt.plane + wi];
+        float wv = w[wi];
+        opt_update1(opt, l, acc[u], wv, s[0], s[1], s[2]);
+        w[wi] = wv;
+        for (int k = 0; k < opt.nstates; ++k) sst[k * opt.plane + wi] = s[k];
+      }
+    }
+  }
+  kt_end(kt);
+}
+
+// ------------------------------------------------------------------------------------------
 // K6: gradient reduction + the configured Neon optimizer (src/deepqnetwork.py:50-61,165; rules in optim.cuh).
 // RMSProp:  g = dW / bsz;  s = decay*s + g*g*(1-decay);  W = W - (g*lr) / (sqrt(s + eps) + eps)
 // The split-K partials of every layer are summed here in fixed order (deterministic), so the
@@ -1076,11 +1401,134 @@ static int fc1_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int r
   return launch_gemm<Fc1Fwd<W>, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, W, nets * kFc1Splits, st);
 }
 
+// The IQN forward for `nets` slots of `rows` samples: tau and phi, the conv trunk at `rows`, then X = psi
+// phi, fc1, fc2 and the head at rows * per expanded rows.  phi depends only on tau and We, so on a stream the draw and
+// the embedding run on their own branch from the head of the forward and join before the modulation.
+static int forward_iqn(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
+                       const HeadTrainArgs& td) {
+  const LayerTable& lt = n->lt;
+  const float* w[3] = {n->d_w, n->d_tw, n->d_w};
+  const int per = td.enable ? n->iqn_n : n->iqn_k, R = rows * per, ld = n->iqn_rows;
+  const bool branch = n->use_branches && st != nullptr && !g_prof_on;
+  cudaStream_t sP = branch ? n->side[0] : st;
+  const bool prev = g_pdl_suppressed;
+  if (branch) {
+    B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
+    B2_CHECK_CUDA(cudaStreamWaitEvent(sP, n->ev[15], 0));
+    g_pdl_suppressed = true;
+  }
+  cudaError_t e = launch_pdl(k_iqn_tau, dim3(1), dim3(1024), 0, sP, n->d_tau_ctr, (unsigned long long)n->cfg.tau_seed,
+                             nets, rows, per, ld, n->d_tau, ktrace_slot("iqn_tau"));
+  if (e == cudaSuccess)
+    e = launch_pdl(k_iqn_phi, dim3(cdiv(R, kIqnTB), nets), dim3(256), 0, sP, (const float*)n->d_tau, R, ld,
+                   (const float*)n->d_we, (const float*)n->d_twe, n->d_cos, n->d_phi, ktrace_slot("iqn_phi"));
+  g_pdl_suppressed = prev;
+  B2_CHECK_CUDA(e);
+  B2_PROF("iqn_tau+phi", sP);
+  if (branch) B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sP));
+  const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
+  // the tensor-core fc1 picks its split count by row count; it is taken at the full minibatch, so a predict on fewer
+  // live rows sums every row as the full one does
+  const int splits = tc ? umma_fc1_splits(n->nb * per) : kFc1Splits;
+  int rc;
+  if (tc) {
+    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, nets, rows, st, n->world == 1, true))) return rc;
+  } else {
+    {
+      Conv1Fwd p;
+      for (int z = 0; z < 3; ++z) {
+        const int f = z ? 1 : 0;
+        p.src[z] = fs.src[f]; p.idx[z] = fs.idx[f]; p.shift[z] = fs.shift[f];
+        p.w[z] = w[z] + lt.off[0]; p.out[z] = n->d_h1[z];
+      }
+      p.nb = rows;
+      p.k1 = lt.rows[0];
+      if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st))) return rc;
+    }
+    {
+      using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
+      P p;
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
+      p.nb = rows;
+      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
+    }
+    {
+      using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
+      P p;
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
+      p.nb = rows;
+      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
+    }
+  }
+  if (branch) {   // the embedding's branch joins here: the modulation gets ordinary dependencies on both
+    B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[16], 0));
+    g_pdl_suppressed = true;
+  }
+  const int64_t total = int64_t(nets) * R * kFlat;
+  e = launch_pdl(k_iqn_mod, dim3(unsigned(std::min<int64_t>(cdiv(total, 256), int64_t(n->sm_count) * 16))), dim3(256), 0,
+                 st, (const float*)n->d_h3[0], (const float*)n->d_h3[1], (const float*)n->d_phi, n->d_x, n->d_x16, nets,
+                 R, per, ld, ktrace_slot("iqn_mod"));
+  g_pdl_suppressed = prev;
+  B2_CHECK_CUDA(e);
+  B2_PROF("iqn_mod", st);
+  if (tc) {
+    if ((rc = umma_fc1_fwd_iqn(n, nets, R, splits, st))) return rc;
+  } else {
+    Fc1Fwd<kHidden> p;
+    for (int z = 0; z < 3; ++z) {
+      p.in[z] = n->d_x + int64_t(z < 2 ? z : 0) * ld * kFlat;
+      p.w[z] = w[z] + lt.off[3];
+    }
+    p.part = n->d_fc1part; p.nb = R; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+    if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, R, kHidden, nets * kFc1Splits, st))) return rc;
+  }
+  B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(R, kDistTB), cdiv(n->A, kDistTN), nets), dim3(256), 0, st,
+                           (const float*)n->d_fc1part, splits, R, ld, n->d_h4[0],
+                           n->d_h4[1], w[0] + lt.off[4],
+                           w[1] + lt.off[4], n->d_iqn_theta, n->A, ktrace_slot("fc2_dist")));
+  B2_PROF("fc2_dist", st);
+  const IqnArgs ia{per, ld, float(n->cfg.clip_error), n->d_tau, n->d_iqn_tq, n->d_iqn_qgrad, n->d_act_rows};
+  const bool nstep = td.enable && td.nstep > 1;
+  auto* kern = nets == 1 ? k_head_iqn<1, false> : nstep ? k_head_iqn<2, true> : k_head_iqn<2, false>;
+  B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_iqn_theta, nets,
+                           (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->A, ia, td,
+                           ktrace_slot("head_iqn")));
+  B2_PROF(td.enable ? "head_iqn(td+fc2_bwd)" : "head_iqn", st);
+  return B200DQN_OK;
+}
+
+// The IQN backward between fc1's dgrad and conv3's (on st): dpsi into dZ3 and dphi; then dWe and the embedding's update,
+// on side stream sW when given (its own branch: nothing later in the step reads We), else in line.
+static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t sW, bool update) {
+  __half* dpsi16 = nullptr;
+  int64_t dpsi_lo = 0;
+  umma_dz3_planes(n, &dpsi16, &dpsi_lo);
+  B2_CHECK_CUDA(launch_pdl(k_iqn_mod_bwd, dim3(cdiv(int64_t(rows) * kFlat, 256)), dim3(256), 0, st,
+                           (const float*)n->d_dx, (const float*)n->d_phi, (const float*)n->d_h3[0], n->d_dz3, dpsi16,
+                           dpsi_lo, n->d_dphi, rows, n->iqn_n, ktrace_slot("iqn_mod_bwd")));
+  B2_PROF("iqn_mod_bwd", st);
+  cudaStream_t s = st;
+  if (sW) {
+    B2_CHECK_CUDA(cudaEventRecord(n->ev[8], st));
+    B2_CHECK_CUDA(cudaStreamWaitEvent(sW, n->ev[8], 0));
+    s = sW;
+  }
+  NoPdlScope side;
+  OptArgs o = make_opt_args(n, rows);
+  o.plane = int64_t(kIqnCos) * kFlat;
+  B2_CHECK_CUDA(launch_pdl(k_iqn_we, dim3(cdiv(kFlat, kWeCols)), dim3(256), 0, s, (const float*)n->d_cos,
+                           (const float*)n->d_dphi, rows * n->iqn_n, n->d_weg, n->d_we, n->d_wes, update ? 1 : 0, o,
+                           ktrace_slot("iqn_we")));
+  B2_PROF("iqn_we", s);
+  return B200DQN_OK;
+}
+
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
 // for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
 // join (Munchausen train step on a stream): the event of the target pass's branch, waited for before the head.
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
                    const HeadTrainArgs& td, cudaEvent_t join = nullptr) {
+  if (n->iqn_n) return forward_iqn(n, fs, nets, rows, st, td);
   const LayerTable& lt = n->lt;
   const float* w[3] = {n->d_w, n->d_tw, n->d_w};
   int rc;
@@ -1257,8 +1705,16 @@ static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cud
     return umma_backward_op(n, int(op), fs.src[0], fs.idx[0], fs.shift[0], rows, st, release_early);
   switch (op) {
     case kFc1Wgrad:
+      if (n->iqn_n) {   // IQN: fc1 ran on X at rows N expanded rows
+        Fc1Wgrad<kHidden> p{n->d_x, n->d_dz4, n->d_part + lt.part_off[3], rows * n->iqn_n};
+        return launch_gemm<Fc1Wgrad<kHidden>, 64, 64, 16, 4, 4>("fc1_wgrad", p, kFlat, kHidden, 1, st);
+      }
       return n->dueling ? fc1_wgrad_simt<kDuelHidden>(n, rows, st) : fc1_wgrad_simt<kHidden>(n, rows, st);
     case kFc1Dgrad:
+      if (n->iqn_n) {   // dX, masked by X > 0 (harmless: see rule 11 of b200dqn.h)
+        Fc1Dgrad<kHidden> p{n->d_dz4, w + lt.off[3], n->d_x, n->d_dx, rows * n->iqn_n};
+        return launch_gemm<Fc1Dgrad<kHidden>, 32, 32, 16, 2, 2>("fc1_dgrad", p, rows * n->iqn_n, kFlat, 1, st);
+      }
       return n->dueling ? fc1_dgrad_simt<kDuelHidden>(n, rows, st) : fc1_dgrad_simt<kHidden>(n, rows, st);
     case kConv3Wgrad: {
       using P = ConvWgrad<kP2, kC2, 3, 1, kC3>;
@@ -1331,12 +1787,14 @@ static int cost_finish_on(b200dqn_net* n, int rows, cudaStream_t s) {
   return B200DQN_OK;
 }
 
-// fc2 of a distributional or quantile net from the head's compact row partials; mode bits as k_opt_fc2_dist's
+// fc2 of a distributional, quantile or IQN net from the head's compact row partials (an IQN net has one per expanded
+// row; the optimizer's batch size stays `rows`); mode bits as k_opt_fc2_dist's
 static int opt_fc2_dist(b200dqn_net* n, int rows, int mode, cudaStream_t s, const char* label) {
   const LayerTable& lt = n->lt;
   const int blk = n->fc2_block();
   B2_CHECK_CUDA(launch_pdl(k_opt_fc2_dist, dim3(cdiv(int64_t(kHidden) * blk, 256), n->A), dim3(256), 0, s,
-                           (const float*)n->d_part + lt.part_off[4], (const int32_t*)n->d_act_rows, rows, n->A, blk,
+                           (const float*)n->d_part + lt.part_off[4], (const int32_t*)n->d_act_rows,
+                           n->expanded(rows, true), n->A, blk,
                            n->d_g + lt.off[4], n->d_w + lt.off[4], n->d_s + lt.off[4], mode, make_opt_args(n, rows),
                            ktrace_slot(label)));
   B2_PROF(label, s);
@@ -1621,7 +2079,10 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   // Under the event profiler the same kernels run, but every "branch" is the main stream (serialised).
   const bool branches = update && n->world == 1 && n->use_branches && (st != nullptr || g_prof_on);
   if (!branches) {
-    for (int op = kFc1Wgrad; op <= kConv1Wgrad; ++op) B2_TRY(bwd_op(n, fs, rows, BwdOp(op), st));
+    for (int op = kFc1Wgrad; op <= kConv1Wgrad; ++op) {
+      B2_TRY(bwd_op(n, fs, rows, BwdOp(op), st));
+      if (op == kFc1Dgrad && n->iqn_n) B2_TRY(iqn_backward(n, rows, st, nullptr, update));
+    }
     B2_TRY(cost_finish_on(n, rows, st));
     if (!update) return B200DQN_OK;
     if (n->world > 1) {
@@ -1650,11 +2111,17 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     if (tc || n->fc2_block()) B2_TRY(opt_fc2_small(n, rows, sN));
   }
   B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
+  if (n->iqn_n) B2_TRY(iqn_backward(n, rows, st, sN, true));   // dZ3 is dpsi
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
   {
     NoPdlScope side;
-    if (tc) B2_TRY(umma_opt_fc1(n, rows, sA));               // smem-free: co-resides with the dgrad chain
+    if (tc && n->lt.splits[3] > 1) {                           // IQN: sum fc1's wgrad partials first
+      B2_TRY(optimizer_range(n, 3, 3, 1 | 2, rows, sA, "reduce_fc1"));
+      B2_TRY(umma_opt_fc1(n, rows, sA, true));
+    } else if (tc) {
+      B2_TRY(umma_opt_fc1(n, rows, sA));                       // smem-free: co-resides with the dgrad chain
+    }
     else B2_TRY(optimizer_range(n, 3, n->fc2_block() ? 3 : 4, 1 | 4, rows, sA, "opt_fc"));
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
@@ -1791,6 +2258,9 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->munchausen_alpha = 0.9;
   cfg->munchausen_tau = 0.03;
   cfg->munchausen_clip = -1.0;
+  cfg->num_tau_samples = 0;      // no IQN head; Dopamine's K when it is on
+  cfg->num_quantile_samples = 32;
+  cfg->tau_seed = 0;
   return B200DQN_OK;
 }
 
@@ -1841,6 +2311,22 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
                "net_create: the Munchausen target with a dueling network, a distributional or a quantile head is not "
                "implemented");
   }
+  B2_REQUIRE(cfg->num_tau_samples >= 0 && cfg->num_tau_samples <= kIqnMaxPer, B200DQN_EINVAL,
+             "net_create: num_tau_samples %d is neither 0 (no IQN head) nor in [1,%d]", cfg->num_tau_samples, kIqnMaxPer);
+  if (cfg->num_tau_samples) {
+    B2_REQUIRE(cfg->num_quantile_samples >= 1 && cfg->num_quantile_samples <= kIqnMaxPer, B200DQN_EINVAL,
+               "net_create: num_quantile_samples %d not in [1,%d]", cfg->num_quantile_samples, kIqnMaxPer);
+    B2_REQUIRE(!cfg->num_atoms && !cfg->num_quantiles, B200DQN_EINVAL,
+               "net_create: num_tau_samples with num_atoms or num_quantiles asks for two heads; a net has one");
+    B2_REQUIRE(std::isfinite(cfg->clip_error), B200DQN_EINVAL,
+               "net_create: the quantile Huber threshold clip_error must be finite (got %g)", cfg->clip_error);
+    const int64_t xr = int64_t(cfg->batch_size) * std::max(cfg->num_tau_samples, cfg->num_quantile_samples);
+    B2_REQUIRE(xr <= 4096, B200DQN_EINVAL,
+               "net_create: the IQN head runs fc1 on batch_size x max(num_tau_samples, num_quantile_samples) = %lld rows; "
+               "at most 4096 are supported", (long long)xr);
+    B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
+               "net_create: the IQN head with a dueling network or the Munchausen target is not implemented");
+  }
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -1855,8 +2341,14 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->dueling = cfg->dueling != 0;
   n->munchausen = cfg->munchausen != 0;
   n->hidden = n->dueling ? kDuelHidden : kHidden;
+  if (cfg->num_tau_samples) {
+    n->iqn_n = cfg->num_tau_samples;
+    n->iqn_k = cfg->num_quantile_samples;
+    n->iqn_rows = cfg->batch_size * std::max(n->iqn_n, n->iqn_k);
+  }
   if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
   const int nb = n->nb, A = n->A, hist = cfg->history_length;
+  const int xr = n->iqn_n ? n->iqn_rows : nb;   // rows of fc1's and fc2's buffers (IQN: the expanded rows)
   LayerTable& lt = n->lt;
   const int rows_[kLayers] = {64 * hist, kK2, kK3, kFlat, kHidden};   // conv1: one 64-tap k-block per frame
   const int cols_[kLayers] = {kC1, kC2, kC3, n->hidden, n->fc2_cols()};
@@ -1875,12 +2367,12 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     if (l == 4)
       lt.splits[l] = nb;   // the head kernel leaves one dW5 partial per sample
     else if (cfg->math_mode == B200DQN_MATH_TCGEN05)
-      lt.splits[l] = l < 3 ? umma_wgrad_splits(l, nb) : 1;
+      lt.splits[l] = l < 3 ? umma_wgrad_splits(l, nb) : n->iqn_n ? int(cdiv(nb * n->iqn_n, kIqnWgradRows)) : 1;
     else
       lt.splits[l] = l < 3 ? int(cdiv(kred[l], wgrad_chunk(kred[l], base[l]))) : 1;
     lt.part_off[l] = po;
-    if (l == 4 && n->fc2_block())   // distributional / quantile head: the taken action's [512][block] per sample
-      po += int64_t(nb) * kHidden * n->fc2_block();
+    if (l == 4 && n->fc2_block())   // distributional / quantile / IQN head: the taken action's [512][block] per row
+      po += int64_t(n->iqn_n ? n->iqn_rows : nb) * kHidden * n->fc2_block();
     else
       po += int64_t(lt.splits[l]) * (lt.off[l + 1] - lt.off[l]);
   }
@@ -1915,12 +2407,12 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(fmalloc(&n->d_h1[z], size_t(nb) * kP1 * kP1 * kC1));
     B2_CHECK_CUDA(fmalloc(&n->d_h2[z], size_t(nb) * kP2 * kP2 * kC2));
     B2_CHECK_CUDA(fmalloc(&n->d_h3[z], size_t(nb) * kFlat));
-    B2_CHECK_CUDA(fmalloc(&n->d_h4[z], size_t(nb) * n->hidden));
+    B2_CHECK_CUDA(fmalloc(&n->d_h4[z], size_t(xr) * n->hidden));
   }
   for (int z = 0; z < 3; ++z) B2_CHECK_CUDA(fmalloc(&n->d_q[z], size_t(nb) * A));
-  B2_CHECK_CUDA(fmalloc(&n->d_fc1part, size_t(2) * kFc1Splits * nb * n->hidden));
+  B2_CHECK_CUDA(fmalloc(&n->d_fc1part, size_t(2) * kFc1Splits * xr * n->hidden));
   B2_CHECK_CUDA(fmalloc(&n->d_delta, size_t(nb) * A));
-  B2_CHECK_CUDA(fmalloc(&n->d_dz4, size_t(nb) * n->hidden));
+  B2_CHECK_CUDA(fmalloc(&n->d_dz4, size_t(xr) * n->hidden));
   B2_CHECK_CUDA(fmalloc(&n->d_dz3, size_t(nb) * kFlat));
   B2_CHECK_CUDA(fmalloc(&n->d_dz2, size_t(nb) * kP2 * kP2 * kC2));
   B2_CHECK_CUDA(fmalloc(&n->d_dz1, size_t(nb) * kP1 * kP1 * kC1));
@@ -1946,6 +2438,36 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   if (n->dueling) B2_CHECK_CUDA(fmalloc(&n->d_va, size_t(3) * nb * (A + 1)));
   if (n->munchausen) B2_CHECK_CUDA(fmalloc(&n->d_tdtarget, nb));
+  if (n->iqn_n) {
+    const size_t we = size_t(kIqnCos) * kFlat, R = size_t(xr);
+    B2_CHECK_CUDA(fmalloc(&n->d_we, we));
+    B2_CHECK_CUDA(fmalloc(&n->d_wes, we * n->n_states));
+    if (cfg->target_steps) {
+      B2_CHECK_CUDA(fmalloc(&n->d_twe, we));
+      B2_CHECK_CUDA(fmalloc(&n->d_twes, we * n->n_states));
+    } else {
+      n->d_twe = n->d_we;
+      n->d_twes = n->d_wes;
+    }
+    B2_CHECK_CUDA(fmalloc(&n->d_weg, we));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_tau_ctr, sizeof(unsigned long long)));
+    B2_CHECK_CUDA(cudaMemset(n->d_tau_ctr, 0, sizeof(unsigned long long)));
+    B2_CHECK_CUDA(fmalloc(&n->d_tau, 2 * R));
+    B2_CHECK_CUDA(fmalloc(&n->d_cos, 2 * R * kIqnCos));
+    B2_CHECK_CUDA(fmalloc(&n->d_phi, 2 * R * kFlat));
+    B2_CHECK_CUDA(fmalloc(&n->d_x, 2 * R * kFlat));
+    B2_CHECK_CUDA(fmalloc(&n->d_iqn_theta, 2 * R * A));
+    B2_CHECK_CUDA(fmalloc(&n->d_iqn_tq, size_t(nb) * n->iqn_n));
+    B2_CHECK_CUDA(fmalloc(&n->d_iqn_qgrad, size_t(nb) * n->iqn_n));
+    B2_CHECK_CUDA(fmalloc(&n->d_dx, R * kFlat));
+    B2_CHECK_CUDA(fmalloc(&n->d_dphi, R * kFlat));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, R * sizeof(int32_t)));
+    B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, R * sizeof(int32_t)));
+    if (cfg->math_mode == B200DQN_MATH_TCGEN05) {
+      B2_CHECK_CUDA(cudaMalloc(&n->d_x16, 4 * R * kFlat * sizeof(__half)));
+      B2_CHECK_CUDA(cudaMemset(n->d_x16, 0, 4 * R * kFlat * sizeof(__half)));
+    }
+  }
   const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
   B2_CHECK_CUDA(cudaMalloc(&n->d_pre, state_bytes + 256));
   B2_CHECK_CUDA(cudaMalloc(&n->d_post, state_bytes + 256));
@@ -2007,14 +2529,47 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_va);
   cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
   cudaFree(n->d_tdtarget);
+  if (n->d_twe != n->d_we) { cudaFree(n->d_twe); cudaFree(n->d_twes); }
+  cudaFree(n->d_we); cudaFree(n->d_wes); cudaFree(n->d_weg); cudaFree(n->d_tau_ctr); cudaFree(n->d_tau);
+  cudaFree(n->d_cos); cudaFree(n->d_phi); cudaFree(n->d_x); cudaFree(n->d_iqn_theta); cudaFree(n->d_iqn_tq);
+  cudaFree(n->d_iqn_qgrad); cudaFree(n->d_dx); cudaFree(n->d_dphi); cudaFree(n->d_x16);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
   return B200DQN_OK;
 }
 
+// ABI layer 5, the IQN embedding: Neon W[n][i], n = fc1's input column in (c, p, q) order, i < 64 <-> internal
+// We[i][(p, q, c)].  These take over the five-layer entry points' work for it.
+static int xfer_we(b200dqn_net* n, float* dev_base, float* host, bool to_device, cudaStream_t st) {
+  const int64_t cnt = int64_t(kIqnCos) * kFlat;
+  std::vector<float> tmp(cnt);
+  auto at = [](int64_t i) {
+    const int nn = int(i / kIqnCos), f = int(i % kIqnCos);
+    const int c = nn / 49, p = (nn / 7) % 7, q = nn % 7;
+    return int64_t(f) * kFlat + (p * 7 + q) * kC3 + c;
+  };
+  if (to_device) {
+    for (int64_t i = 0; i < cnt; ++i) tmp[at(i)] = host[i];
+    B2_CHECK_CUDA(cudaMemcpyAsync(dev_base, tmp.data(), cnt * sizeof(float), cudaMemcpyHostToDevice, st));
+    B2_CHECK_CUDA(cudaStreamSynchronize(st));
+  } else {
+    B2_CHECK_CUDA(cudaMemcpyAsync(tmp.data(), dev_base, cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CHECK_CUDA(cudaStreamSynchronize(st));
+    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[at(i)];
+  }
+  return B200DQN_OK;
+}
+
+static bool is_we(const b200dqn_net* n, int layer) { return layer == kLayers && n->iqn_n; }
+
 extern "C" int b200dqn_net_layer_shape(const b200dqn_net* n, int layer, int* rows, int* cols) {
-  B2_REQUIRE(n && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_layer_shape: bad layer");
+  B2_REQUIRE(n && layer >= 0 && (layer < kLayers || is_we(n, layer)), B200DQN_EINVAL, "net_layer_shape: bad layer");
+  if (layer == kLayers) {
+    if (rows) *rows = kFlat;
+    if (cols) *cols = kIqnCos;
+    return B200DQN_OK;
+  }
   // NEON shapes: conv (C*R*S, K); linear (nout, nin)
   const int r[kLayers] = {n->lt.rows[0], kK2, kK3, n->hidden, n->fc2_cols()};
   const int c[kLayers] = {kC1, kC2, kC3, kFlat, kHidden};
@@ -2040,10 +2595,15 @@ static int xfer_params(b200dqn_net* n, float* dev_base, int layer, float* host, 
 
 extern "C" int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, const float* host_W,
                                        const float* host_S, void* stream) {
-  B2_REQUIRE(n && host_W && layer >= 0 && layer < kLayers && (which == 0 || which == 1), B200DQN_EINVAL,
-             "net_set_weights: bad argument");
+  B2_REQUIRE(n && host_W && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1),
+             B200DQN_EINVAL, "net_set_weights: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers) {
+    B2_TRY(xfer_we(n, which ? n->d_twe : n->d_we, const_cast<float*>(host_W), true, st));
+    if (host_S) B2_TRY(xfer_we(n, which ? n->d_twes : n->d_wes, const_cast<float*>(host_S), true, st));
+    return B200DQN_OK;
+  }
   int rc = xfer_params(n, which ? n->d_tw : n->d_w, layer, const_cast<float*>(host_W), true, st);
   if (rc) return rc;
   if (host_S && (rc = xfer_params(n, which ? n->d_ts : n->d_s, layer, const_cast<float*>(host_S), true, st))) return rc;
@@ -2052,10 +2612,15 @@ extern "C" int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, con
 
 extern "C" int b200dqn_net_get_weights(b200dqn_net* n, int which, int layer, float* host_W, float* host_S,
                                        void* stream) {
-  B2_REQUIRE(n && layer >= 0 && layer < kLayers && (which == 0 || which == 1), B200DQN_EINVAL,
+  B2_REQUIRE(n && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1), B200DQN_EINVAL,
              "net_get_weights: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers) {
+    if (host_W) B2_TRY(xfer_we(n, which ? n->d_twe : n->d_we, host_W, false, st));
+    if (host_S) B2_TRY(xfer_we(n, which ? n->d_twes : n->d_wes, host_S, false, st));
+    return B200DQN_OK;
+  }
   int rc;
   if (host_W && (rc = xfer_params(n, which ? n->d_tw : n->d_w, layer, host_W, false, st))) return rc;
   if (host_S && (rc = xfer_params(n, which ? n->d_ts : n->d_s, layer, host_S, false, st))) return rc;
@@ -2069,17 +2634,22 @@ extern "C" int b200dqn_net_num_states(const b200dqn_net* n, int* count) {
 }
 
 extern "C" int b200dqn_net_set_state(b200dqn_net* n, int which, int layer, int k, const float* host_S, void* stream) {
-  B2_REQUIRE(n && host_S && layer >= 0 && layer < kLayers && (which == 0 || which == 1) && k >= 0 && k < n->n_states,
-             B200DQN_EINVAL, "net_set_state: bad argument");
+  B2_REQUIRE(n && host_S && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1) && k >= 0 &&
+             k < n->n_states, B200DQN_EINVAL, "net_set_state: bad argument");
   DeviceGuard g(n->device);
+  if (layer == kLayers)
+    return xfer_we(n, (which ? n->d_twes : n->d_wes) + int64_t(k) * kIqnCos * kFlat, const_cast<float*>(host_S), true,
+                   as_stream(stream));
   return xfer_params(n, (which ? n->d_ts : n->d_s) + int64_t(k) * n->n_params, layer, const_cast<float*>(host_S), true,
                      as_stream(stream));
 }
 
 extern "C" int b200dqn_net_get_state(b200dqn_net* n, int which, int layer, int k, float* host_S, void* stream) {
-  B2_REQUIRE(n && host_S && layer >= 0 && layer < kLayers && (which == 0 || which == 1) && k >= 0 && k < n->n_states,
-             B200DQN_EINVAL, "net_get_state: bad argument");
+  B2_REQUIRE(n && host_S && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1) && k >= 0 &&
+             k < n->n_states, B200DQN_EINVAL, "net_get_state: bad argument");
   DeviceGuard g(n->device);
+  if (layer == kLayers)
+    return xfer_we(n, (which ? n->d_twes : n->d_wes) + int64_t(k) * kIqnCos * kFlat, host_S, false, as_stream(stream));
   return xfer_params(n, (which ? n->d_ts : n->d_s) + int64_t(k) * n->n_params, layer, host_S, false, as_stream(stream));
 }
 
@@ -2090,6 +2660,11 @@ extern "C" int b200dqn_net_sync_target(b200dqn_net* n, void* stream) {
   cudaStream_t st = as_stream(stream);
   B2_CHECK_CUDA(cudaMemcpyAsync(n->d_tw, n->d_w, n->n_params * sizeof(float), cudaMemcpyDeviceToDevice, st));
   B2_CHECK_CUDA(cudaMemcpyAsync(n->d_ts, n->d_s, n->n_params * n->n_states * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  if (n->iqn_n) {   // the embedding is a layer of each network
+    const size_t we = size_t(kIqnCos) * kFlat * sizeof(float);
+    B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twe, n->d_we, we, cudaMemcpyDeviceToDevice, st));
+    B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twes, n->d_wes, we * n->n_states, cudaMemcpyDeviceToDevice, st));
+  }
   return umma_target_synced(n, st);
 }
 
@@ -2456,6 +3031,7 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_DELTAS:
       B2_REQUIRE(!n->atoms, B200DQN_EINVAL, "net_device_ptr: a distributional head has no scalar delta");
       B2_REQUIRE(!n->quantiles, B200DQN_EINVAL, "net_device_ptr: a quantile-regression head has no scalar delta");
+      B2_REQUIRE(!n->iqn_n, B200DQN_EINVAL, "net_device_ptr: an IQN head has no scalar delta");
       p = n->d_delta;
       b = size_t(n->nb) * n->A * 4;
       break;
@@ -2465,8 +3041,8 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_H1: p = n->d_h1[0]; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
     case B200DQN_NET_PTR_H2: p = n->d_h2[0]; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_H3: p = n->d_h3[0]; b = size_t(n->nb) * kFlat * 4; break;
-    case B200DQN_NET_PTR_H4: p = n->d_h4[0]; b = size_t(n->nb) * n->hidden * 4; break;
-    case B200DQN_NET_PTR_DZ4: p = n->d_dz4; b = size_t(n->nb) * n->hidden * 4; break;
+    case B200DQN_NET_PTR_H4: p = n->d_h4[0]; b = size_t(n->iqn_n ? n->iqn_rows : n->nb) * n->hidden * 4; break;
+    case B200DQN_NET_PTR_DZ4: p = n->d_dz4; b = size_t(n->iqn_n ? n->iqn_rows : n->nb) * n->hidden * 4; break;
     case B200DQN_NET_PTR_DZ3: p = n->d_dz3; b = size_t(n->nb) * kFlat * 4; break;
     case B200DQN_NET_PTR_DZ2: p = n->d_dz2; b = size_t(n->nb) * kP2 * kP2 * kC2 * 4; break;
     case B200DQN_NET_PTR_DZ1: p = n->d_dz1; b = size_t(n->nb) * kP1 * kP1 * kC1 * 4; break;
@@ -2523,6 +3099,32 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
         b = size_t(n->nb) * n->A * 4;
       }
       break;
+    case B200DQN_NET_PTR_IQN_TAUS:
+    case B200DQN_NET_PTR_IQN_COS:
+    case B200DQN_NET_PTR_IQN_PHI:
+    case B200DQN_NET_PTR_IQN_X:
+    case B200DQN_NET_PTR_IQN_QUANTILES:
+    case B200DQN_NET_PTR_IQN_TARGET_QUANTILES:
+    case B200DQN_NET_PTR_IQN_QUANTILE_GRADS:
+    case B200DQN_NET_PTR_IQN_DX:
+    case B200DQN_NET_PTR_IQN_DPHI:
+    case B200DQN_NET_PTR_IQN_TAU_COUNTER: {
+      B2_REQUIRE(n->iqn_n, B200DQN_EINVAL, "net_device_ptr: selector %d needs an IQN head", which);
+      const size_t R = size_t(n->iqn_rows), nbn = size_t(n->nb) * n->iqn_n;
+      switch (which) {
+        case B200DQN_NET_PTR_IQN_TAUS: p = n->d_tau; b = 2 * R * 4; break;
+        case B200DQN_NET_PTR_IQN_COS: p = n->d_cos; b = 2 * R * kIqnCos * 4; break;
+        case B200DQN_NET_PTR_IQN_PHI: p = n->d_phi; b = 2 * R * kFlat * 4; break;
+        case B200DQN_NET_PTR_IQN_X: p = n->d_x; b = 2 * R * kFlat * 4; break;
+        case B200DQN_NET_PTR_IQN_QUANTILES: p = n->d_iqn_theta; b = 2 * R * n->A * 4; break;
+        case B200DQN_NET_PTR_IQN_TARGET_QUANTILES: p = n->d_iqn_tq; b = nbn * 4; break;
+        case B200DQN_NET_PTR_IQN_QUANTILE_GRADS: p = n->d_iqn_qgrad; b = nbn * 4; break;
+        case B200DQN_NET_PTR_IQN_DX: p = n->d_dx; b = R * kFlat * 4; break;
+        case B200DQN_NET_PTR_IQN_DPHI: p = n->d_dphi; b = R * kFlat * 4; break;
+        default: p = n->d_tau_ctr; b = sizeof(unsigned long long); break;
+      }
+      break;
+    }
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -2571,6 +3173,7 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   if (on) {
     B2_REQUIRE(!n->munchausen, B200DQN_EINVAL,
                "net_set_double_q: the Munchausen target makes no greedy choice for Double DQN to change");
+    B2_REQUIRE(!n->iqn_n, B200DQN_ENOTIMPL, "net_set_double_q: the Double DQN target with the IQN head is not implemented");
     B2_REQUIRE(!n->nccl_comm, B200DQN_ENOTIMPL,
                "net_set_double_q: the Double DQN target is implemented for a single learner only (comm_init has run)");
     B2_TRY(double_q_alloc(n));
@@ -2582,9 +3185,11 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
 }
 
 extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream) {
-  B2_REQUIRE(n && host_dW && layer >= 0 && layer < kLayers, B200DQN_EINVAL, "net_get_grads: bad argument");
+  B2_REQUIRE(n && host_dW && layer >= 0 && (layer < kLayers || is_we(n, layer)), B200DQN_EINVAL,
+             "net_get_grads: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers) return xfer_we(n, n->d_weg, host_dW, false, st);   // written whole by k_iqn_we
   const int64_t n4 = n->n_params / 4;
   if (n->world == 1) {  // partials of the last step are still in scratch; sum them into d_g
     // a distributional or quantile fc2 is summed by its own kernel
@@ -2616,8 +3221,10 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
     // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
     // target with a separate target network repeats the forward's launches for its pass
+    // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
-                (n->munchausen && n->d_tw != n->d_w ? 4 : 0);
+                (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) +
+                (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
   }
   return B200DQN_OK;
 }

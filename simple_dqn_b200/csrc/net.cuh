@@ -1,6 +1,8 @@
 // net.cuh — the Q-network object: fp32 master weights (online + target), RMSProp state,
 // activations, gradient partials, all resident in HBM.
 #pragma once
+#include <cuda_fp16.h>
+
 #include "common.cuh"
 #include "net_simt.cuh"
 #include "replay.cuh"
@@ -18,6 +20,7 @@ constexpr int kHostCosts = 60;            // per-step costs mirrored in host-map
 constexpr int kHostQ = 64, kHostQFloats = 960;   // word offset / capacity of the Q rows in the host-mapped block
 constexpr int kFc1Splits = 14;            // 3136 / 14 = 224 = 14 * 16
 constexpr int kFc1Chunk = kFlat / kFc1Splits;
+constexpr int kIqnWgradRows = 256;        // IQN on the tensor-core engine: expanded rows per fc1 wgrad partial
 
 struct LayerTable {
   int64_t off[kLayers + 1];   // element offsets into the all-layer parameter vector
@@ -124,7 +127,7 @@ struct b200dqn_net {
   float* d_qgrad = nullptr;      // [nb][quantiles] gradient on the taken action's quantiles
   // fc2 outputs per action of a per-action head (C51 atoms or QR quantiles), 0 on the scalar and dueling heads: such
   // an fc2 is summed and updated by k_opt_fc2_dist from the compact [nb][512][block] partials
-  int fc2_block() const { return atoms ? atoms : quantiles; }
+  int fc2_block() const { return atoms ? atoms : quantiles ? quantiles : iqn_n ? 1 : 0; }
   int fc2_cols() const { return fc2_block() ? A * fc2_block() : dueling ? A + 1 : A; }
 
   // dueling network (cfg.dueling): fc1 is kDuelHidden wide (advantage units [0, 512), value units [512, 1024)) and
@@ -138,6 +141,30 @@ struct b200dqn_net {
   // and the head reads its Q row as slot 2 (Q_TARGET_PRE = d_q[2])
   bool munchausen = false;
   float* d_tdtarget = nullptr;   // [nb] float(y) of the last train step
+
+  // implicit quantile network head (cfg.num_tau_samples > 0; nothing below is allocated otherwise).  fc1 and fc2 run
+  // on the expanded rows r = b N + j (b K + k on predict): H4, dZ4, the fc1 partials and fc2's per-row partials (block
+  // width 1, summed by k_opt_fc2_dist) are sized by iqn_rows; the conv trunk runs at nb rows.
+  int iqn_n = 0, iqn_k = 0;      // N, K
+  int iqn_rows = 0;              // nb max(N, K)
+  float* d_we = nullptr;         // online embedding [64][3136] (internal column order); d_wes: its n_states planes
+  float* d_wes = nullptr;
+  float* d_twe = nullptr;        // target embedding and states (== d_we / d_wes when target_steps == 0)
+  float* d_twes = nullptr;
+  float* d_weg = nullptr;        // dWe of the last train step
+  unsigned long long* d_tau_ctr = nullptr;   // the draw counter
+  float* d_tau = nullptr;        // [2][iqn_rows]
+  float* d_cos = nullptr;        // [2][iqn_rows][64]
+  float* d_phi = nullptr;        // [2][iqn_rows][3136]
+  float* d_x = nullptr;          // [2][iqn_rows][3136]
+  float* d_iqn_theta = nullptr;  // [2][iqn_rows][A]
+  float* d_iqn_tq = nullptr;     // [nb][N]
+  float* d_iqn_qgrad = nullptr;  // [nb N]
+  float* d_dx = nullptr;         // [iqn_rows][3136]
+  float* d_dphi = nullptr;       // [iqn_rows][3136]
+  __half* d_x16 = nullptr;       // tensor-core engine: fp16 planes of X, per slot [hi iqn_rows x 3136 | lo]
+  // rows one fc1 / fc2 pass runs at for `rows` samples: rows N in a train step, rows K on predict
+  int expanded(int rows, bool train) const { return iqn_n ? rows * (train ? iqn_n : iqn_k) : rows; }
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

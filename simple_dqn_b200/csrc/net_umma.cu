@@ -1030,7 +1030,7 @@ int umma_net_init(b200dqn_net* n) {
   u->h_elems[0] = int64_t(nb) * kP1 * kP1 * kC1;
   u->h_elems[1] = int64_t(nb) * kP2 * kP2 * kC2;
   u->h_elems[2] = int64_t(nb) * kFlat;
-  u->dz_elems[0] = int64_t(nb) * n->hidden;
+  u->dz_elems[0] = int64_t(n->iqn_n ? n->iqn_rows : nb) * n->hidden;   // IQN: dZ4 of every expanded row
   u->dz_elems[1] = int64_t(nb) * kFlat;
   u->dz_elems[2] = int64_t(nb) * kP2 * kP2 * kC2;
   u->dz_elems[3] = int64_t(nb) * kP1 * kP1 * kC1;
@@ -1113,6 +1113,12 @@ void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
   *lo_off = u ? u->dz_elems[0] : 0;
 }
 
+void umma_dz3_planes(b200dqn_net* n, __half** hi, int64_t* lo_off) {
+  UmmaState* u = ust(n);
+  *hi = u ? u->dz16[1] : nullptr;
+  *lo_off = u ? u->dz_elems[1] : 0;
+}
+
 template <int W>
 static int fc1_fwd_umma(b200dqn_net* n, const PlanePair h3[3], int nets, int rows, cudaStream_t st) {
   UmmaState* u = ust(n);
@@ -1124,7 +1130,7 @@ static int fc1_fwd_umma(b200dqn_net* n, const PlanePair h3[3], int nets, int row
 }
 
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 int nets, int rows, cudaStream_t st, bool release_early) {
+                 int nets, int rows, cudaStream_t st, bool release_early, bool trunk_only) {
   // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
   // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.  conv23_fwd keeps
   // its own release point.
@@ -1151,6 +1157,7 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
       p.c2.in16[z] = planes(0, z); p.c3.out16[z] = planes(2, z);
       p.c3.out[z] = z ? nullptr : n->d_h3[z];   // nothing reads the fp32 activations of slots 1 and 2
     }
+    if (trunk_only) p.c3.out[1] = n->d_h3[1];   // IQN: the target's psi for its modulation
     p.c2.out[0] = n->d_h2[0]; p.c2.out16[0] = planes(1, 0);   // the kernel stores H2 of the online net only
     p.c2.rows = p.c3.rows = rows;
     if ((rc = launch_conv23(p, rows, nets, st))) return rc;
@@ -1174,14 +1181,31 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
         p.in16[z] = planes(1, z); p.out16[z] = planes(2, z);
         p.out[z] = z ? nullptr : n->d_h3[z];
       }
+      if (trunk_only) p.out[1] = n->d_h3[1];
       p.rows = rows;
       if ((rc = umma2::launch_umma2("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st, release_early))) return rc;
     }
   }
+  if (trunk_only) return B200DQN_OK;
   // data-parallel learners: this rank's H3 rows start travelling to every rank's fc1_wgrad now
   if (nets >= 2 && rows == n->nb && comm_gather_active(n, st) && (rc = umma_push_h3(n, st))) return rc;
   const PlanePair h3[3] = {planes(2, 0), planes(2, 1), planes(2, 2)};
   return n->dueling ? fc1_fwd_umma<kDuelHidden>(n, h3, nets, rows, st) : fc1_fwd_umma<kHidden>(n, h3, nets, rows, st);
+}
+
+// X planes of slot z: [hi ld x 3136 | lo ld x 3136] at d_x16 + z * 2 * ld * 3136 (k_iqn_mod writes them)
+static PlanePair iqn_x_planes(b200dqn_net* n, int z) {
+  const int64_t slot = int64_t(n->iqn_rows) * kFlat;
+  return PlanePair{n->d_x16 + 2 * z * slot, slot};
+}
+
+int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_t st) {
+  UmmaState* u = ust(n);
+  V2Fc1Fwd<kHidden> p;   // 512 wide: an IQN net is not a dueling one
+  for (int z = 0; z < 2; ++z) p.wimg[z] = u->img_fwd[z][3];
+  for (int z = 0; z < 3; ++z) p.in16[z] = iqn_x_planes(n, z == 1 ? 1 : 0);
+  p.part = n->d_fc1part; p.rows = rows; p.splits = splits;
+  return umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * splits, st, false);
 }
 
 // The Munchausen target pass: umma_forward's launches with one network slot (nets = 1) and remapped pointers.  Device
@@ -1262,9 +1286,32 @@ int umma_backward_op(b200dqn_net* n, int op, const uint8_t* src, const int32_t* 
   const float* w = n->d_w;
   switch (op) {
     case 0:
+      if (n->iqn_n) {   // IQN: fc1 ran on X at rows N expanded rows, reduced in chunks of kIqnWgradRows rows, one
+        // partial each (lt.splits[3]): one fp32 accumulation chain over 4096 rows exceeded the hi/lo scheme's bound
+        UmmaState* u = ust(n);
+        const int R = rows * n->iqn_n;
+        const PlanePair x = iqn_x_planes(n, 0);
+        const int64_t wsize = lt.off[4] - lt.off[3];
+        for (int s = 0; s < lt.splits[3]; ++s) {
+          const int r0 = s * kIqnWgradRows;
+          WFc1Wgrad<kHidden> p{PlanePair{x.hi + int64_t(r0) * kFlat, x.lo_off},
+                               PlanePair{u->dz16[0] + int64_t(r0) * kHidden, u->dz_elems[0]},
+                               n->d_part + lt.part_off[3] + s * wsize, std::min(kIqnWgradRows, R - r0)};
+          const int rc = umma_mn::launch_umma_mn("fc1_wgrad", p, kFlat, kHidden, 1, st, release_early);
+          if (rc) return rc;
+        }
+        return B200DQN_OK;
+      }
       return n->dueling ? fc1_wgrad_umma<kDuelHidden>(n, rows, st, release_early)
                         : fc1_wgrad_umma<kHidden>(n, rows, st, release_early);
     case 1:
+      if (n->iqn_n) {   // IQN: dX in fp32 (masked by X > 0, harmless: b200dqn.h rule 11); its fp16 planes have no
+        // reader and go to slot 1's X planes, which nothing reads after the forward
+        UmmaState* u = ust(n);
+        V2Fc1Dgrad<kHidden> p{u->img_dgr[0], PlanePair{u->dz16[0], u->dz_elems[0]}, n->d_x, n->d_dx,
+                              iqn_x_planes(n, 1), rows * n->iqn_n};
+        return umma2::launch_umma2("fc1_dgrad", p, kFlat, rows * n->iqn_n, 1, st, release_early);
+      }
       return n->dueling ? fc1_dgrad_umma<kDuelHidden>(n, rows, st, release_early)
                         : fc1_dgrad_umma<kHidden>(n, rows, st, release_early);
     case 2: {

@@ -21,8 +21,11 @@ int umma_weights_changed(b200dqn_net* n, cudaStream_t st);  // fp32 master weigh
 int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
 // release_early: the launches are links of the single-GPU critical chain; the kernels that gain from it let their
 // successor pre-launch right after their own dependency wait
+// trunk_only (IQN head): conv1..conv3 only, with the fp32 H3 of slots 0 and 1 kept for the modulation; no fc1
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 int nets, int rows, cudaStream_t st, bool release_early);
+                 int nets, int rows, cudaStream_t st, bool release_early, bool trunk_only = false);
+// IQN head: fc1's forward on the modulated rows X (n->d_x16 planes) at `rows` expanded rows with `splits` k-splits
+int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_t st);
 int umma_fc1_splits(int rows);
 // the Munchausen target pass: the target network on the frames src/idx/shift (the prestates), into slot 2's planes and
 // fc1 partials (nets = 1, no fp32 activations)
@@ -37,6 +40,8 @@ int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* 
 int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st);
 // fp16 hi plane of dZ4 and the offset of its lo plane (nullptr when math_mode != TCGEN05)
 void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
+// fp16 hi plane of dZ3 (conv3's output gradient) and the offset of its lo plane (nullptr when math_mode != TCGEN05)
+void umma_dz3_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
 int umma_wgrad_splits(int layer, int rows);   // split-K factor of the conv wgrad of `layer` (0..2)
 // op: 0 fc1_wgrad, 1 fc1_dgrad, 2 conv3_wgrad, 3 conv3_dgrad, 4 conv2_wgrad, 5 conv2_dgrad, 6 conv1_wgrad
 // release_early: as for umma_forward

@@ -1,6 +1,7 @@
 """DeepQNetwork with the reference's call surface (/root/reference/src/deepqnetwork.py:15-192):
 the Neon model/train/predict replaced by hand-written sm_90a kernels (csrc/net*.cu)."""
 import ctypes as C
+import os
 import logging
 import pickle
 
@@ -20,6 +21,14 @@ _OPTIMIZERS = {"rmsprop": (L.OPT_RMSPROP, 1), "adam": (L.OPT_ADAM, 2), "adadelta
 
 def _arg(args, name, default):
     return getattr(args, name, default)
+
+
+def tau_seed(random_seed):
+    """The IQN head's uint64 tau_seed for args.random_seed: a fixed odd multiple of the seed (mod 2^64), so equal seeds
+    draw equal taus; a fresh random one when the seed is None."""
+    if random_seed is None:
+        return int.from_bytes(os.urandom(8), "little")
+    return (int(random_seed) * 0x9E3779B97F4A7C15 + 0x632BE59BD9B4E019) % (1 << 64)
 
 
 class DeepQNetwork:
@@ -95,6 +104,17 @@ class DeepQNetwork:
             cfg.munchausen_alpha = float(_arg(args, "munchausen_alpha", 0.9))
             cfg.munchausen_tau = float(_arg(args, "munchausen_tau", 0.03))
             cfg.munchausen_clip = float(_arg(args, "munchausen_clip", -1.0))
+        # implicit quantile network head (IQN, Dabney et al., 2018): a new capability, off unless args.implicit_quantiles
+        # is set; N = num_tau_samples (64) online and target samples per train row, K = num_quantile_samples (32) per
+        # predict row, as Dopamine.  The device draws tau from a hash of tau_seed, derived from random_seed, and a
+        # device-resident counter; its embedding is a sixth layer.  Fixed here, like the other heads.
+        self.implicit_quantiles = bool(_arg(args, "implicit_quantiles", False))
+        self.num_tau_samples = self.num_quantile_samples = 0
+        if self.implicit_quantiles:
+            cfg.num_tau_samples = int(_arg(args, "num_tau_samples", 64))
+            cfg.num_quantile_samples = int(_arg(args, "num_quantile_samples", 32))
+            assert cfg.num_tau_samples >= 1, "num_tau_samples %d: the IQN head needs 1..64" % cfg.num_tau_samples
+            cfg.tau_seed = tau_seed(_arg(args, "random_seed", None))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -102,12 +122,16 @@ class DeepQNetwork:
             self.num_atoms, self.v_min, self.v_max = cfg.num_atoms, cfg.v_min, cfg.v_max
             dz = (cfg.v_max - cfg.v_min) / (cfg.num_atoms - 1)         # z_i = v_min + i dz in fp64, as the device
             self.support = np.array([cfg.v_min + i * dz for i in range(cfg.num_atoms)], dtype=np.float64)
+        if self.implicit_quantiles:
+            self.num_tau_samples, self.num_quantile_samples = cfg.num_tau_samples, cfg.num_quantile_samples
+            self.tau_seed = cfg.tau_seed
         if self.quantile_regression:
             self.num_quantiles = n = cfg.num_quantiles                 # tau_i = (2i + 1) / 2N in fp64, as the device
             self.taus = np.array([(2 * i + 1) / (2 * n) for i in range(n)], dtype=np.float64).astype(np.float32)
 
         # model.initialize (:49, :70): Xavier draws from one numpy RandomState(random_seed) —
-        # online layers first, then the separately-initialised target model.
+        # online layers first, then the separately-initialised target model.  An IQN embedding is drawn after fc2 of
+        # its network, with fan_in 64.
         rng = np.random.RandomState(_arg(args, "random_seed", None))
         for which in ((0, 1) if cfg.target_steps else (0,)):
             for layer, shp in enumerate(self.layer_shapes()):
@@ -134,7 +158,7 @@ class DeepQNetwork:
     # ---- weights in Neon layout
     def layer_shapes(self):
         out = []
-        for layer in range(5):
+        for layer in range(6 if self.implicit_quantiles else 5):
             r, c = C.c_int(), C.c_int()
             L.call("b200dqn_net_layer_shape", self._h, layer, C.byref(r), C.byref(c))
             out.append((r.value, c.value))
@@ -297,6 +321,27 @@ class DeepQNetwork:
         """The gradient on the taken action's quantiles of the last train(), (batch, num_quantiles) float32."""
         return self._read_f32(L.NET_PTR_QUANTILE_GRADS, (self.batch_size, self.num_quantiles))
 
+    # ---- implicit quantile network head (implicit_quantiles = True).  Rows r = b * N + j of the last train(), slot 0
+    # online on the prestates and slot 1 target on the poststates; after a predict, slot 0 holds rows b * K + k.
+    def last_taus(self):
+        """tau of the last forward, (2, batch * max(N, K)) float32."""
+        return self._read_f32(L.NET_PTR_IQN_TAUS, (2, self._iqn_rows()))
+
+    def last_iqn_quantiles(self):
+        """fc2's outputs theta of the last forward, (2, batch * max(N, K), A) float32."""
+        return self._read_f32(L.NET_PTR_IQN_QUANTILES, (2, self._iqn_rows(), self.num_actions))
+
+    def last_iqn_target_quantiles(self):
+        """The target quantiles T_j of the last train(), (batch, N) float32."""
+        return self._read_f32(L.NET_PTR_IQN_TARGET_QUANTILES, (self.batch_size, self.num_tau_samples))
+
+    def last_iqn_quantile_grads(self):
+        """The gradient dtheta on the taken action of each online row of the last train(), (batch, N) float32."""
+        return self._read_f32(L.NET_PTR_IQN_QUANTILE_GRADS, (self.batch_size, self.num_tau_samples))
+
+    def _iqn_rows(self):
+        return self.batch_size * max(self.num_tau_samples, self.num_quantile_samples)
+
     # ---- Munchausen target (munchausen = True)
     def last_target_q_pre(self):
         """The target network's Q on the prestates of the last train(), (batch, A) float32: the row whose log-policy
@@ -446,7 +491,11 @@ class DeepQNetwork:
             ls = d["layer_params_states"]
         else:
             ls = [l for l in d["model"]["config"]["layers"] if "params" in l]
-        assert len(ls) == 5, "checkpoint does not hold the five weight layers of deepqnetwork.py:77-92"
+        if self.implicit_quantiles:
+            assert len(ls) == 6, ("checkpoint holds %d weight layers; an IQN net needs six: the five of "
+                                  "deepqnetwork.py:77-92 and the tau embedding" % len(ls))
+        else:
+            assert len(ls) == 5, "checkpoint does not hold the five weight layers of deepqnetwork.py:77-92"
         ws = [np.asarray(l["params"]["W"], dtype=np.float32) for l in ls]
         for layer, (l, w) in enumerate(zip(ls, ws)):
             assert w.shape == self.layer_shapes()[layer], \

@@ -13,6 +13,8 @@ NACT = int(os.environ.get("NACT", str(NUM_ACTIONS)))   # actions (the replayed a
 DUELING = os.environ.get("DUELING", "0") == "1"   # dueling network (1024-unit fc1, advantage and value streams)
 QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (QR-DQN) with this many quantiles; 0: off
 MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target (extra target pass on the prestates)
+IQN = int(os.environ.get("IQN", "0"))   # IQN head with this many tau samples per train row; 0: off
+IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per predict row
 
 
 def net_args():
@@ -21,6 +23,7 @@ def net_args():
     a.dueling = DUELING
     a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
     a.munchausen = MUNCHAUSEN
+    a.implicit_quantiles, a.num_tau_samples, a.num_quantile_samples = IQN > 0, IQN, IQN_K
     return a
 
 
