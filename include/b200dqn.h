@@ -346,6 +346,24 @@ typedef struct b200dqn_net_config {
   int num_tau_samples;
   int num_quantile_samples;
   uint64_t tau_seed;
+  /* Random-shift augmentation (DrQ, Kostrikov, Yarats and Fergus, 2020; new capability, no reference counterpart), off
+   * when random_shift = 0 (the default).  Otherwise p = random_shift in 1..8 (DrQ uses 4; other values are EINVAL,
+   * before any device work), and every train step trains on shifted states.  b200dqn_net_comm_init returns ENOTIMPL
+   * on such a net.  b is the sample, z the slot (0 the prestates, 1 the poststates):
+   *    1. draw: x = mix(mix(shift_seed + 0x9E3779B97F4A7C15 (ctr + 1)) ^ (z << 32 | b)),
+   *         dy = ((x >> 32) (2p + 1) >> 32) - p,   dx = ((x & 0xffffffff) (2p + 1) >> 32) - p,
+   *       all mod 2^64, mix = the IQN head's splitmix64 finaliser, ctr the device-resident draw counter of the shift
+   *       (not the IQN head's).  Every train step, on every train entry point, draws with the counter's value and then
+   *       advances it by one, on the device, so replayed step graphs draw fresh offsets; predict, its graph and acting
+   *       neither shift nor touch the counter; the replay sampler's MT19937 stream is not touched;
+   *    2. the shifted state's pixel (f, y, x) is frame f's pixel (clamp(y + dy, 0, 83), clamp(x + dx, 0, 83)): one
+   *       (dy, dx) for all history_length frames of a state; this is edge-replicate padding by p followed by the 84x84
+   *       crop at (p + dy, p + dx);
+   *    3. the online network on the prestates (slot 0) and the Munchausen target pass on the prestates read slot 0's
+   *       offsets; the target network on the poststates (slot 1) and Double DQN's online network on the poststates
+   *       read slot 1's.  The stored frames, and what getMinibatch returns, are never shifted. */
+  int random_shift;
+  uint64_t shift_seed;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -494,7 +512,10 @@ enum {
   B200DQN_NET_PTR_IQN_QUANTILE_GRADS,   /* (batch N,) f32 dtheta of the taken action, per online row                 */
   B200DQN_NET_PTR_IQN_DX,           /* (R, 3136) f32 fc1's dgrad dX of the last train step                           */
   B200DQN_NET_PTR_IQN_DPHI,         /* (R, 3136) f32 dphi of the last train step                                     */
-  B200DQN_NET_PTR_IQN_TAU_COUNTER   /* u64 the draw counter (the next forward draws with this value)                 */
+  B200DQN_NET_PTR_IQN_TAU_COUNTER,  /* u64 the draw counter (the next forward draws with this value)                 */
+  /* Random-shift augmentation only (random_shift > 0; EINVAL otherwise). */
+  B200DQN_NET_PTR_SHIFT_OFFSETS,    /* (2, batch, 2) i32 (dy, dx) of the last train step: prestates, then poststates */
+  B200DQN_NET_PTR_SHIFT_DRAWS       /* u64 the shift's draw counter (the next train step draws with this value)      */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

@@ -1024,6 +1024,28 @@ k_iqn_tau(unsigned long long* ctr, unsigned long long seed, int nets, int rows, 
   kt_end(kt);
 }
 
+// Random-shift augmentation (b200dqn.h states the rule): crop[z][b] = (dy, dx) in [-p, p]^2 for slot z (0 prestates,
+// 1 poststates) and sample b, drawn at the counter's value; thread 0 then advances the counter, so every train step,
+// and every replay of a captured step graph, draws fresh offsets.  The hash is k_iqn_tau's, with its own seed and counter.
+__global__ void __launch_bounds__(1024)
+k_shift_draw(unsigned long long* ctr, unsigned long long seed, int pad, int rows, int32_t* crop, const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const unsigned long long c = *ctr;
+  const unsigned long long base = iqn_mix(seed + 0x9E3779B97F4A7C15ull * (c + 1ull));
+  const unsigned long long span = 2ull * unsigned(pad) + 1ull;
+  for (int e = threadIdx.x; e < 2 * rows; e += blockDim.x) {
+    const int z = e / rows, b = e % rows;
+    const unsigned long long x = iqn_mix(base ^ ((unsigned long long)z << 32 | unsigned(b)));
+    crop[2 * e] = int32_t(((x >> 32) * span) >> 32) - pad;
+    crop[2 * e + 1] = int32_t(((x & 0xffffffffull) * span) >> 32) - pad;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) *ctr = c + 1ull;
+  kt_end(kt);
+}
+
 // grid (cdiv(rows, 16), nets).  c[r][i] = float(cos((pi i) tau_r)) in fp64, stored for the embedding's gradient; then
 // thread t takes columns t, t + 256, ... and accumulates the CTA's 16 rows of column col in i order.
 __global__ void __launch_bounds__(256)
@@ -1386,11 +1408,37 @@ static int launch_gemm(const char* label, const P& p, int M, int N, int Z, cudaS
 }
 
 // Where the first conv layer reads its frames: in place from the ring (fused) or from staged states.
+// crop: the random-shift crop offsets of each source ([nb][2] (dy, dx) int32, slot 0's then slot 1's), nullptr when
+// the states are not shifted (augmentation off, predict).
 struct FrameSource {
   const uint8_t* src[2];
   const int32_t* idx[2];
   int shift[2];
+  const int32_t* crop[2] = {};
 };
+
+// conv1's forward on the SIMT engine for `nets` slots: slot 2 (Double DQN) reads slot 1's frames and crop offsets
+static int conv1_fwd_simt(b200dqn_net* n, const FrameSource& fs, const float* const w[3], int nets, int rows,
+                          cudaStream_t st) {
+  auto fill = [&](Conv1Fwd& p) {
+    for (int z = 0; z < 3; ++z) {
+      const int f = z ? 1 : 0;
+      p.src[z] = fs.src[f]; p.idx[z] = fs.idx[f]; p.shift[z] = fs.shift[f];
+      p.w[z] = w[z] + n->lt.off[0]; p.out[z] = n->d_h1[z];
+    }
+    p.nb = rows;
+    p.k1 = n->lt.rows[0];
+  };
+  if (fs.crop[0]) {
+    Conv1FwdCrop p;
+    fill(p);
+    p.crop[0] = fs.crop[0]; p.crop[1] = fs.crop[1]; p.crop[2] = fs.crop[1];
+    return launch_gemm<Conv1FwdCrop, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st);
+  }
+  Conv1Fwd p;
+  fill(p);
+  return launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st);
+}
 
 // fc1's forward on the SIMT engine at width W (kHidden, or kDuelHidden on a dueling net)
 template <int W>
@@ -1432,19 +1480,9 @@ static int forward_iqn(b200dqn_net* n, const FrameSource& fs, int nets, int rows
   const int splits = tc ? umma_fc1_splits(n->nb * per) : kFc1Splits;
   int rc;
   if (tc) {
-    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, nets, rows, st, n->world == 1, true))) return rc;
+    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1, true))) return rc;
   } else {
-    {
-      Conv1Fwd p;
-      for (int z = 0; z < 3; ++z) {
-        const int f = z ? 1 : 0;
-        p.src[z] = fs.src[f]; p.idx[z] = fs.idx[f]; p.shift[z] = fs.shift[f];
-        p.w[z] = w[z] + lt.off[0]; p.out[z] = n->d_h1[z];
-      }
-      p.nb = rows;
-      p.k1 = lt.rows[0];
-      if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st))) return rc;
-    }
+    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
     {
       using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
       P p;
@@ -1534,20 +1572,10 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
   int rc;
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
     // one GPU: the forward launches are links of the critical chain (umma_forward picks the ones that release early)
-    rc = umma_forward(n, fs.src, fs.idx, fs.shift, nets, rows, st, n->world == 1);
+    rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1);
     if (rc) return rc;
   } else {
-    {
-      Conv1Fwd p;
-      for (int z = 0; z < 3; ++z) {
-        const int f = z ? 1 : 0;   // slot 2 reads slot 1's frames
-        p.src[z] = fs.src[f]; p.idx[z] = fs.idx[f]; p.shift[z] = fs.shift[f];
-        p.w[z] = w[z] + lt.off[0]; p.out[z] = n->d_h1[z];
-      }
-      p.nb = rows;
-      p.k1 = lt.rows[0];
-      if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st))) return rc;
-    }
+    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
     {
       using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
       P p;
@@ -1641,17 +1669,28 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
 // (tensor cores) and slot 2's region of the three-slot fc1 partials, which k_head_mdqn<3, .> sums.
 static int forward_target_pre(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
-    return umma_forward_target_pre(n, fs.src[0], fs.idx[0], fs.shift[0], rows, st);
+    return umma_forward_target_pre(n, fs.src[0], fs.idx[0], fs.shift[0], fs.crop[0], rows, st);
   const LayerTable& lt = n->lt;
   const float* w = n->d_tw;
   int rc;
   {
-    Conv1Fwd p{};
-    p.src[0] = fs.src[0]; p.idx[0] = fs.idx[0]; p.shift[0] = fs.shift[0];
-    p.w[0] = w + lt.off[0]; p.out[0] = n->d_h1[2];
-    p.nb = rows;
-    p.k1 = lt.rows[0];
-    if ((rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st))) return rc;
+    auto fill = [&](Conv1Fwd& p) {
+      p.src[0] = fs.src[0]; p.idx[0] = fs.idx[0]; p.shift[0] = fs.shift[0];
+      p.w[0] = w + lt.off[0]; p.out[0] = n->d_h1[2];
+      p.nb = rows;
+      p.k1 = lt.rows[0];
+    };
+    if (fs.crop[0]) {   // the prestates, shifted by slot 0's offsets
+      Conv1FwdCrop p{};
+      fill(p);
+      p.crop[0] = fs.crop[0];
+      rc = launch_gemm<Conv1FwdCrop, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st);
+    } else {
+      Conv1Fwd p{};
+      fill(p);
+      rc = launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st);
+    }
+    if (rc) return rc;
   }
   {
     using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
@@ -1739,6 +1778,10 @@ static int bwd_op(b200dqn_net* n, const FrameSource& fs, int rows, BwdOp op, cud
     default: {
       Conv1Wgrad p{fs.src[0], fs.idx[0], fs.shift[0], n->d_dz1, n->d_part + lt.part_off[0], rows,
                    wgrad_chunk(rows * kP1 * kP1, 512), lt.rows[0]};
+      if (fs.crop[0]) {   // the prestates as slot 0's forward saw them
+        Conv1WgradCrop pc{p, fs.crop[0]};
+        return launch_gemm<Conv1WgradCrop, 64, 32, 16, 4, 2>("conv1_wgrad", pc, lt.rows[0], kC1, lt.splits[0], st);
+      }
       return launch_gemm<Conv1Wgrad, 64, 32, 16, 4, 2>("conv1_wgrad", p, lt.rows[0], kC1, lt.splits[0], st);
     }
   }
@@ -2158,10 +2201,50 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   return B200DQN_OK;
 }
 
+// The random-shift draw of a train step on its own branch from the head of the step (on a stream; the serial schedule
+// draws in line, in shift_join).  It reads only the counter, so it overlaps the sampler.
+static int shift_fork(b200dqn_net* n, cudaStream_t st) {
+  if (!n->crop_pad || n->crop_forked || !n->use_branches || st == nullptr || g_prof_on) return B200DQN_OK;
+  cudaStream_t sD = n->side[1];
+  B2_CHECK_CUDA(cudaEventRecord(n->ev[17], st));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(sD, n->ev[17], 0));
+  {
+    NoPdlScope side;
+    B2_CHECK_CUDA(launch_pdl(k_shift_draw, dim3(1), dim3(1024), 0, sD, n->d_crop_ctr,
+                             (unsigned long long)n->cfg.shift_seed, n->crop_pad, n->nb, n->d_crop,
+                             ktrace_slot("shift_draw")));
+  }
+  B2_PROF("shift_draw", sD);
+  B2_CHECK_CUDA(cudaEventRecord(n->ev[18], sD));
+  n->crop_forked = true;
+  return B200DQN_OK;
+}
+
+// The draw is complete on st from here on: its branch joins, or it runs here, in line.
+static int shift_join(b200dqn_net* n, cudaStream_t st) {
+  if (n->crop_forked) {
+    n->crop_forked = false;
+    B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[18], 0));
+    return B200DQN_OK;
+  }
+  B2_CHECK_CUDA(launch_pdl(k_shift_draw, dim3(1), dim3(1024), 0, st, n->d_crop_ctr,
+                           (unsigned long long)n->cfg.shift_seed, n->crop_pad, n->nb, n->d_crop,
+                           ktrace_slot("shift_draw")));
+  B2_PROF("shift_draw", st);
+  return B200DQN_OK;
+}
+
 // One DeepQNetwork.train on device-resident inputs (the caller counts train_iterations, :168).
-static int train_step(b200dqn_net* n, const FrameSource& fs, const uint8_t* actions, const int64_t* rewards,
+static int train_step(b200dqn_net* n, const FrameSource& fs_in, const uint8_t* actions, const int64_t* rewards,
                       const uint8_t* terminals, const int32_t* midx, cudaStream_t st) {
   const int rows = n->nb;
+  FrameSource fs = fs_in;
+  if (n->crop_pad) {   // random-shift augmentation: fresh crop offsets for the prestates (slot 0) and poststates
+    B2_TRY(shift_fork(n, st));
+    B2_TRY(shift_join(n, st));
+    fs.crop[0] = n->d_crop;
+    fs.crop[1] = n->d_crop + 2 * rows;
+  }
   HeadTrainArgs td{1, actions, rewards, terminals, midx, n->cfg.discount_rate, n->cfg.min_reward, n->cfg.max_reward,
                    float(n->cfg.clip_error), n->d_delta, n->d_step, n->d_rowcost, n->d_dz4,
                    n->d_part + n->lt.part_off[4], nullptr, 0,
@@ -2261,6 +2344,8 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->num_tau_samples = 0;      // no IQN head; Dopamine's K when it is on
   cfg->num_quantile_samples = 32;
   cfg->tau_seed = 0;
+  cfg->random_shift = 0;         // no augmentation; DrQ's pad is 4
+  cfg->shift_seed = 0;
   return B200DQN_OK;
 }
 
@@ -2327,6 +2412,8 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
                "net_create: the IQN head with a dueling network or the Munchausen target is not implemented");
   }
+  B2_REQUIRE(cfg->random_shift >= 0 && cfg->random_shift <= kMaxCropPad, B200DQN_EINVAL,
+             "net_create: random_shift %d is neither 0 (no augmentation) nor in [1,%d]", cfg->random_shift, kMaxCropPad);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -2438,6 +2525,13 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   if (n->dueling) B2_CHECK_CUDA(fmalloc(&n->d_va, size_t(3) * nb * (A + 1)));
   if (n->munchausen) B2_CHECK_CUDA(fmalloc(&n->d_tdtarget, nb));
+  if (cfg->random_shift) {
+    n->crop_pad = cfg->random_shift;
+    B2_CHECK_CUDA(cudaMalloc(&n->d_crop_ctr, sizeof(unsigned long long)));
+    B2_CHECK_CUDA(cudaMemset(n->d_crop_ctr, 0, sizeof(unsigned long long)));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_crop, size_t(nb) * 4 * sizeof(int32_t)));
+    B2_CHECK_CUDA(cudaMemset(n->d_crop, 0, size_t(nb) * 4 * sizeof(int32_t)));
+  }
   if (n->iqn_n) {
     const size_t we = size_t(kIqnCos) * kFlat, R = size_t(xr);
     B2_CHECK_CUDA(fmalloc(&n->d_we, we));
@@ -2530,6 +2624,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
   cudaFree(n->d_tdtarget);
   if (n->d_twe != n->d_we) { cudaFree(n->d_twe); cudaFree(n->d_twes); }
+  cudaFree(n->d_crop_ctr); cudaFree(n->d_crop);
   cudaFree(n->d_we); cudaFree(n->d_wes); cudaFree(n->d_weg); cudaFree(n->d_tau_ctr); cudaFree(n->d_tau);
   cudaFree(n->d_cos); cudaFree(n->d_phi); cudaFree(n->d_x); cudaFree(n->d_iqn_theta); cudaFree(n->d_iqn_tq);
   cudaFree(n->d_iqn_qgrad); cudaFree(n->d_dx); cudaFree(n->d_dphi); cudaFree(n->d_x16);
@@ -2927,10 +3022,12 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
       {
         const bool prev = g_pdl_suppressed;
         if (ktrace_tick(st)) g_pdl_suppressed = true;   // the sampler must not start ahead of the tick
-        rc = launch_sample(r, st);
+        rc = shift_fork(n, st);
+        if (!rc) rc = launch_sample(r, st);
         g_pdl_suppressed = prev;
       }
       if (!rc) rc = train_on_ring(n, r, st);
+      n->crop_forked = false;
       n->graph_launches = int(g_launch_count - launches_before);
       cudaError_t e = cudaStreamEndCapture(st, &graph);
       if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
@@ -2943,9 +3040,10 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
     for (int i = 0; i < nsteps; ++i) {
       const bool prev = g_pdl_suppressed;
       if (ktrace_tick(st)) g_pdl_suppressed = true;
-      rc = launch_sample(r, st);
+      rc = shift_fork(n, st);
+      if (!rc) rc = launch_sample(r, st);
       g_pdl_suppressed = prev;
-      if (rc) return rc;
+      if (rc) { n->crop_forked = false; return rc; }
       if ((rc = train_on_ring(n, r, st))) return rc;
     }
   }
@@ -3125,6 +3223,17 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       }
       break;
     }
+    case B200DQN_NET_PTR_SHIFT_OFFSETS:
+    case B200DQN_NET_PTR_SHIFT_DRAWS:
+      B2_REQUIRE(n->crop_pad, B200DQN_EINVAL, "net_device_ptr: selector %d needs random_shift > 0", which);
+      if (which == B200DQN_NET_PTR_SHIFT_OFFSETS) {
+        p = n->d_crop;
+        b = size_t(n->nb) * 4 * sizeof(int32_t);
+      } else {
+        p = n->d_crop_ctr;
+        b = sizeof(unsigned long long);
+      }
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -3221,9 +3330,10 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
     // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
     // target with a separate target network repeats the forward's launches for its pass
-    // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient
+    // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient;
+    // random-shift augmentation adds its draw
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
-                (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) +
+                (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->crop_pad ? 1 : 0) +
                 (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
   }
   return B200DQN_OK;

@@ -20,7 +20,8 @@ constexpr int kHostCosts = 60;            // per-step costs mirrored in host-map
 constexpr int kHostQ = 64, kHostQFloats = 960;   // word offset / capacity of the Q rows in the host-mapped block
 constexpr int kFc1Splits = 14;            // 3136 / 14 = 224 = 14 * 16
 constexpr int kFc1Chunk = kFlat / kFc1Splits;
-constexpr int kIqnWgradRows = 256;        // IQN on the tensor-core engine: expanded rows per fc1 wgrad partial
+constexpr int kIqnWgradRows = 256;
+constexpr int kMaxCropPad = 8;            // random-shift augmentation: pads 1..8        // IQN on the tensor-core engine: expanded rows per fc1 wgrad partial
 
 struct LayerTable {
   int64_t off[kLayers + 1];   // element offsets into the all-layer parameter vector
@@ -87,7 +88,8 @@ struct b200dqn_net {
   // step scheduling: side streams / events for the independent wgrad + optimizer branches, and the
   // captured CUDA graph of one fused step
   cudaStream_t side[4] = {};   // three wgrad/optimizer branches + the collective stream
-  cudaEvent_t ev[17] = {};   // [15] / [16]: fork / join of the Munchausen target pass (train_step)
+  cudaEvent_t ev[19] = {};   // [15] / [16]: fork / join of the Munchausen target pass (train_step); [17] / [18]: of the
+                             // random-shift draw
   bool use_graph = true, use_branches = true;
   bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
   bool double_q = false;     // Double DQN target: the online net picks the poststate action, the target net values it
@@ -165,6 +167,13 @@ struct b200dqn_net {
   __half* d_x16 = nullptr;       // tensor-core engine: fp16 planes of X, per slot [hi iqn_rows x 3136 | lo]
   // rows one fc1 / fc2 pass runs at for `rows` samples: rows N in a train step, rows K on predict
   int expanded(int rows, bool train) const { return iqn_n ? rows * (train ? iqn_n : iqn_k) : rows; }
+
+  // random-shift augmentation (cfg.random_shift > 0; nothing below is allocated otherwise): every train step draws
+  // crop offsets on the device and conv1 reads its frames through them
+  int crop_pad = 0;                       // p
+  unsigned long long* d_crop_ctr = nullptr;   // the draw counter
+  int32_t* d_crop = nullptr;              // [2][nb][2] (dy, dx) of the last train step: prestates, then poststates
+  bool crop_forked = false;               // the step's draw was launched on its own branch (ev[17] / ev[18])
 
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 

@@ -134,6 +134,26 @@ struct Conv1Fwd {
   }
 };
 
+// Random-shift augmentation (b200dqn_net_config::random_shift): pixel (y, x) of a sample whose crop offsets are
+// (dy, dx) = (crop[2n], crop[2n + 1]) reads frame pixel (clamp(y + dy, 0, 83), clamp(x + dx, 0, 83)): edge-replicate
+// padding followed by a crop, without leaving the 84x84 frame.
+__device__ __forceinline__ int crop_pixel(const int32_t* crop, int n, int y, int x) {
+  const int yy = min(max(y + crop[2 * n], 0), kFrameH - 1), xx = min(max(x + crop[2 * n + 1], 0), kFrameW - 1);
+  return yy * kFrameW + xx;
+}
+
+// conv1 forward on shifted states: crop[z] = the crop offsets of slot z ([nb][2] int32); slot 2 (Double DQN) reads
+// slot 1's frames and therefore slot 1's offsets, which the caller sets explicitly in crop[2].
+struct Conv1FwdCrop : Conv1Fwd {
+  const int32_t* crop[3];
+  __device__ float a(int z, int m, int k) const {
+    const int n = m / (kP1 * kP1), pq = m % (kP1 * kP1), p = pq / kP1, q = pq % kP1;
+    const int c = k >> 6, r = (k >> 3) & 7, s = k & 7;
+    const int64_t f = static_cast<int64_t>(slot3(idx, z)[n]) + slot3(shift, z) + c;
+    return static_cast<float>(slot3(src, z)[f * kFrameBytes + crop_pixel(slot3(crop, z), n, p * 4 + r, q * 4 + s)]);
+  }
+};
+
 // conv2 / conv3: NHWC fp32 input, k = (r, s, c) so one filter row is (S*C) contiguous floats.
 template <int H, int C, int R, int ST, int KO>
 struct ConvFwd {
@@ -307,6 +327,17 @@ struct Conv1Wgrad {
   }
   __device__ float b(int, int k, int n) const { return dz[k * kC1 + n]; }
   __device__ void store(int z, int m, int n, float v) const { part[(z * k1 + m) * kC1 + n] = v * (1.0f / 255.0f); }
+};
+
+// conv1 wgrad on shifted prestates: it re-reads the pixels, so it takes slot 0's crop offsets, as slot 0's forward did.
+struct Conv1WgradCrop : Conv1Wgrad {
+  const int32_t* crop;
+  __device__ float a(int, int m, int k) const {
+    const int n = k / (kP1 * kP1), pq = k % (kP1 * kP1), p = pq / kP1, q = pq % kP1;
+    const int c = m >> 6, r = (m >> 3) & 7, s = m & 7;
+    const int64_t f = static_cast<int64_t>(idx[n]) + shift + c;
+    return static_cast<float>(src[f * kFrameBytes + crop_pixel(crop, n, p * 4 + r, q * 4 + s)]);
+  }
 };
 
 }  // namespace b200

@@ -120,6 +120,47 @@ struct V2Conv1Fwd {
   }
 };
 
+// conv1 forward on shifted states (random_shift > 0; b200dqn.h has the rule): the same kernel with the crop offsets
+// applied in the gather, so the im2col tiles it dumps for conv1_wgrad hold the shifted pixels and the wgrad needs no
+// change.  crop[z] = [nb][2] (dy, dx) of frame source z; slot 2 reads slot 1's frames and offsets.
+struct CropRow {
+  const uint8_t* frame;   // frame 0 of the row's sample (nullptr = padding row)
+  int y0;                 // top filter row before the clamp: p * 4 + dy
+  int wa;                 // first 32-bit word of the clamped columns
+  uint32_t sel;           // byte selectors of the 8 columns (see a_raw8)
+};
+template <int H>
+struct V2Conv1FwdCrop : V2Conv1Fwd<H> {
+  const int32_t* crop[2];
+  // Columns x0 + j (j < 8), x0 = q * 4 + dx, clamp to [0, 83]; relative to word wa they are rel_j in [0, 11], rising
+  // with j.  rel_0..3 lie in words wa, wa + 1 (rel <= 6); rel_4..7 lie either there (rel_4 < 4) or in words wa + 1,
+  // wa + 2.  sel packs the four 4-bit selectors of each output word for __byte_perm.
+  __device__ CropRow a_row_ptr(int z, int m) const {
+    if (m >= this->rows * kP1 * kP1) return CropRow{nullptr, 0, 0, 0u};
+    const int n = m / (kP1 * kP1), pq = m % (kP1 * kP1), p = pq / kP1, q = pq % kP1;
+    const int32_t* c = z ? crop[1] : crop[0];
+    const int64_t f = static_cast<int64_t>((z ? this->idx[1] : this->idx[0])[n]) + (z ? this->shift[1] : this->shift[0]);
+    const int x0 = q * 4 + c[2 * n + 1];
+    const int wa = min(max(x0, 0), kFrameW - 1) >> 2;
+    uint32_t sel = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sel |= uint32_t(min(max(x0 + j, 0), kFrameW - 1) - 4 * wa) << (4 * j);
+    return CropRow{(z ? this->src[1] : this->src[0]) + f * kFrameBytes, p * 4 + c[2 * n], wa, sel};
+  }
+  // Only aligned 32-bit words of the clamped row, and of words 0..20 of it, are read: no byte outside the frame.
+  __device__ uint2 a_raw8(const CropRow& row, int k0) const {
+    if (!row.frame) return make_uint2(0u, 0u);
+    const int c = k0 >> 6, r = (k0 >> 3) & 7;
+    const int y = min(max(row.y0 + r, 0), kFrameH - 1);
+    const uint32_t* line = reinterpret_cast<const uint32_t*>(row.frame + c * kFrameBytes + y * kFrameW);
+    constexpr int kLastWord = kFrameW / 4 - 1;
+    const uint32_t w0 = line[row.wa], w1 = line[min(row.wa + 1, kLastWord)], w2 = line[min(row.wa + 2, kLastWord)];
+    const uint32_t shi = row.sel >> 16;
+    const uint32_t hi = (shi & 0xfu) >= 4u ? __byte_perm(w1, w2, shi - 0x4444u) : __byte_perm(w0, w1, shi);
+    return make_uint2(__byte_perm(w0, w1, row.sel & 0xffffu), hi);
+  }
+};
+
 template <int H, int C, int R, int ST, int KO>
 struct V2ConvFwd {
   static constexpr int P = (H - R) / ST + 1, K = R * R * C;
@@ -1130,15 +1171,13 @@ static int fc1_fwd_umma(b200dqn_net* n, const PlanePair h3[3], int nets, int row
 }
 
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 int nets, int rows, cudaStream_t st, bool release_early, bool trunk_only) {
+                 const int32_t* const crop[2], int nets, int rows, cudaStream_t st, bool release_early, bool trunk_only) {
   // Early release is applied to conv1_fwd and conv3_fwd only: on an H100 80GB HBM3 (400 W) taking it away from either
   // one slowed the batch-32 step by 0.6-1.4 us, while conv2_fwd and fc1_fwd gained nothing from it.  conv23_fwd keeps
   // its own release point.
   UmmaState* u = ust(n);
   auto planes = [&](int i, int z) { return PlanePair{u->h16[i][z], u->h_elems[i]}; };
-  int rc = with_hist(n->cfg.history_length, [&](auto h) {
-    constexpr int H = decltype(h)::value;
-    V2Conv1Fwd<H> p;
+  auto conv1 = [&](auto& p) {
     for (int z = 0; z < 2; ++z) {
       p.src[z] = src[z]; p.idx[z] = idx[z]; p.shift[z] = shift[z];
       p.wimg[z] = u->img_fwd[z][0]; p.out[z] = n->d_h1[z];
@@ -1148,6 +1187,16 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
     p.rows = rows;
     p.im2col = (nets >= 2 && rows == n->nb) ? u->im2col1 : nullptr;   // only a train step feeds conv1_wgrad
     return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st, release_early);
+  };
+  int rc = with_hist(n->cfg.history_length, [&](auto h) {
+    constexpr int H = decltype(h)::value;
+    if (crop[0]) {
+      V2Conv1FwdCrop<H> p;
+      p.crop[0] = crop[0]; p.crop[1] = crop[1];
+      return conv1(p);
+    }
+    V2Conv1Fwd<H> p;
+    return conv1(p);
   });
   if (rc) return rc;
   if (rows <= kConv23MaxRows) {
@@ -1213,19 +1262,27 @@ int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_
 // fp16 planes and fc1 partials; no fp32 activation is kept.  The kernels specialise slot 0 in two places: conv1_fwd
 // dumps no im2col tiles (nets < 2), and conv23_fwd stores its H2 planes (here slot 2's) and, with a null `out`, no
 // fp32 H2.
-int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, int rows,
-                            cudaStream_t st) {
+int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, const int32_t* crop,
+                            int rows, cudaStream_t st) {
   UmmaState* u = ust(n);
   auto planes = [&](int i) { return PlanePair{u->h16[i][2], u->h_elems[i]}; };
-  int rc = with_hist(n->cfg.history_length, [&](auto h) {
-    constexpr int H = decltype(h)::value;
-    V2Conv1Fwd<H> p{};
+  auto conv1 = [&](auto& p) {
     p.src[0] = p.src[1] = src; p.idx[0] = p.idx[1] = idx; p.shift[0] = p.shift[1] = shift;
     p.wimg[0] = p.wimg[1] = u->img_fwd[1][0];
     p.out16[0] = planes(0);
     p.rows = rows;
     p.im2col = nullptr;
     return umma2::launch_umma2("conv1_fwd", p, rows * kP1 * kP1, kC1, 1, st, false);
+  };
+  int rc = with_hist(n->cfg.history_length, [&](auto h) {
+    constexpr int H = decltype(h)::value;
+    if (crop) {
+      V2Conv1FwdCrop<H> p{};
+      p.crop[0] = p.crop[1] = crop;
+      return conv1(p);
+    }
+    V2Conv1Fwd<H> p{};
+    return conv1(p);
   });
   if (rc) return rc;
   if (rows <= kConv23MaxRows) {

@@ -22,15 +22,17 @@ int umma_target_synced(b200dqn_net* n, cudaStream_t st);    // target <- online
 // release_early: the launches are links of the single-GPU critical chain; the kernels that gain from it let their
 // successor pre-launch right after their own dependency wait
 // trunk_only (IQN head): conv1..conv3 only, with the fp32 H3 of slots 0 and 1 kept for the modulation; no fc1
+// crop (random_shift): [nb][2] crop offsets of frame sources 0 and 1, or nullptr for unshifted states
 int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* const idx[2], const int shift[2],
-                 int nets, int rows, cudaStream_t st, bool release_early, bool trunk_only = false);
+                 const int32_t* const crop[2], int nets, int rows, cudaStream_t st, bool release_early,
+                 bool trunk_only = false);
 // IQN head: fc1's forward on the modulated rows X (n->d_x16 planes) at `rows` expanded rows with `splits` k-splits
 int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_t st);
 int umma_fc1_splits(int rows);
 // the Munchausen target pass: the target network on the frames src/idx/shift (the prestates), into slot 2's planes and
-// fc1 partials (nets = 1, no fp32 activations)
-int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, int rows,
-                            cudaStream_t st);
+// fc1 partials (nets = 1, no fp32 activations); crop: the prestates' crop offsets (slot 0's), or nullptr
+int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, const int32_t* crop,
+                            int rows, cudaStream_t st);
 // RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel
 int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false);
 // fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tensor-core path

@@ -14,6 +14,7 @@
 #pragma once
 #include <stdlib.h>
 #include <type_traits>
+#include <utility>
 
 #include "umma.cuh"
 
@@ -63,7 +64,8 @@ __device__ __forceinline__ void split8_planes(const float v[8], __half* hi_dst, 
 //   static constexpr int kAMode, kBMode;                         (OperandMode)
 //   static constexpr bool kARowMajorThreads, kBRowMajorThreads;  (thread -> chunk mapping, as in umma.cuh)
 //   int M(z), N(z); void krange(z, kb0, kb1);
-//   kReg  : const uint8_t* a_row_ptr(z, m)  (once per row; nullptr = row outside the problem)
+//   kReg  : const uint8_t* a_row_ptr(z, m)  (once per row; nullptr = row outside the problem; a problem may return
+//           any other per-row type instead, e.g. with the row's crop offsets)
 //           uint2 a_raw8(row_ptr, k0)  8 raw bytes;  static void cvt8(uint2, float v[8])      (A only)
 //   kAsync: RowCtx a_row(z, m)  — once per (thread, tile row): everything that depends on the row only
 //           bool   a_chunk(z, row, kk, int64_t& off) — per k-block: element offset of the 8-wide chunk
@@ -104,6 +106,13 @@ __device__ __forceinline__ void issue_bulk_stage(const P& p, int z, int mtile, i
   if constexpr (P::kBMode == kBulk)
     tma_bulk_g2s(st_gen + C::kAStage, p.b_tile(z, ntile, kb), 2 * C::kBBytes, bar);
 }
+
+template <class P, class = void>   // what a kReg problem's a_row_ptr returns
+struct ARegRow { using type = const uint8_t*; };
+template <class P>
+struct ARegRow<P, std::void_t<decltype(std::declval<const P&>().a_row_ptr(0, 0))>> {
+  using type = decltype(std::declval<const P&>().a_row_ptr(0, 0));
+};
 
 template <class P, class = void>
 struct StagesOf { static constexpr int value = 0; };
@@ -234,7 +243,7 @@ __global__ void __launch_bounds__(kThreads2, 1) k_umma2(const P p, const int tra
   if (release_early) pdl_launch_dependents();
   // kReg operands: per-row source pointers, once per kernel (they may depend on upstream data — the
   // sampled indexes — so they are built after the wait, but not again for every k-block)
-  const uint8_t* areg[kACh];
+  typename ARegRow<P>::type areg[kACh];
   if constexpr (P::kAMode == kReg) {
 #pragma unroll
     for (int i = 0; i < kACh; ++i) {

@@ -31,6 +31,15 @@ def tau_seed(random_seed):
     return (int(random_seed) * 0x9E3779B97F4A7C15 + 0x632BE59BD9B4E019) % (1 << 64)
 
 
+def shift_seed(random_seed):
+    """The random-shift augmentation's uint64 shift_seed for args.random_seed: like tau_seed, with another odd
+    multiplier and offset, so the crops and the IQN head's tau never share a stream; a fresh random one when the seed is
+    None."""
+    if random_seed is None:
+        return int.from_bytes(os.urandom(8), "little")
+    return (int(random_seed) * 0xD1B54A32D192ED03 + 0x8CB92BA72F3D8DD7) % (1 << 64)
+
+
 class DeepQNetwork:
     def __init__(self, num_actions, args, device=None, math_mode=None, stream=None):
         # remember parameters (:17-26)
@@ -115,6 +124,14 @@ class DeepQNetwork:
             cfg.num_quantile_samples = int(_arg(args, "num_quantile_samples", 32))
             assert cfg.num_tau_samples >= 1, "num_tau_samples %d: the IQN head needs 1..64" % cfg.num_tau_samples
             cfg.tau_seed = tau_seed(_arg(args, "random_seed", None))
+        # random-shift augmentation (DrQ, Kostrikov et al., 2020): a new capability, off unless args.random_shift = p > 0
+        # (DrQ uses 4).  Every train step trains on states padded by p with their edge pixels and cropped back to
+        # 84x84 at offsets the device draws from shift_seed, derived from random_seed, and a device-resident counter.
+        # predict and the stored frames are never shifted.
+        self.random_shift = int(_arg(args, "random_shift", 0))
+        if self.random_shift:
+            cfg.random_shift = self.random_shift
+            cfg.shift_seed = self.shift_seed = shift_seed(_arg(args, "random_seed", None))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -341,6 +358,18 @@ class DeepQNetwork:
 
     def _iqn_rows(self):
         return self.batch_size * max(self.num_tau_samples, self.num_quantile_samples)
+
+    # ---- random-shift augmentation (random_shift = p > 0)
+    def last_shifts(self):
+        """The crop offsets (dy, dx) of the last train step, (2, batch, 2) int32: slot 0 the prestates, slot 1 the
+        poststates.  Shifted pixel (y, x) is stored pixel (clip(y + dy, 0, 83), clip(x + dx, 0, 83))."""
+        return L.download(self.device, self.device_view(L.NET_PTR_SHIFT_OFFSETS, (2, self.batch_size, 2)).ptr,
+                          (2, self.batch_size, 2), np.int32, self._stream)
+
+    def shift_draws(self):
+        """The shift's draw counter: train steps that have drawn offsets; the next one draws with this value."""
+        return int(L.download(self.device, self.device_view(L.NET_PTR_SHIFT_DRAWS, (1,)).ptr, (1,), np.uint64,
+                              self._stream)[0])
 
     # ---- Munchausen target (munchausen = True)
     def last_target_q_pre(self):

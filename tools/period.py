@@ -21,6 +21,7 @@ QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (
 MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target (extra target pass on the prestates)
 IQN = int(os.environ.get("IQN", "0"))   # IQN head with this many tau samples per train row; 0: off
 IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per predict row
+SHIFT = int(os.environ.get("SHIFT", "0"))   # random-shift augmentation with this pad p (DrQ: 4); 0: off
 
 
 def args():
@@ -35,6 +36,7 @@ def args():
     a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
     a.munchausen = MUNCHAUSEN
     a.implicit_quantiles, a.num_tau_samples, a.num_quantile_samples = IQN > 0, IQN, IQN_K
+    a.random_shift = SHIFT
     return a
 
 
@@ -60,6 +62,6 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d munchausen %d iqn %d period_us min %.2f median %.2f  "
-      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, MUNCHAUSEN, IQN, min(res), float(np.median(res)),
+print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d munchausen %d iqn %d shift %d period_us min %.2f median %.2f  "
+      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, MUNCHAUSEN, IQN, SHIFT, min(res), float(np.median(res)),
                   " ".join("%.2f" % r for r in res)))

@@ -15,6 +15,7 @@ QUANTILES = int(os.environ.get("QUANTILES", "0"))   # quantile-regression head (
 MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target (extra target pass on the prestates)
 IQN = int(os.environ.get("IQN", "0"))   # IQN head with this many tau samples per train row; 0: off
 IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per predict row
+SHIFT = int(os.environ.get("SHIFT", "0"))   # random-shift augmentation with this pad p (DrQ: 4); 0: off
 
 
 def net_args():
@@ -24,6 +25,7 @@ def net_args():
     a.quantile_regression, a.num_quantiles = QUANTILES > 0, QUANTILES
     a.munchausen = MUNCHAUSEN
     a.implicit_quantiles, a.num_tau_samples, a.num_quantile_samples = IQN > 0, IQN, IQN_K
+    a.random_shift = SHIFT
     return a
 
 
