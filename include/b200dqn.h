@@ -364,6 +364,37 @@ typedef struct b200dqn_net_config {
    *       read slot 1's.  The stored frames, and what getMinibatch returns, are never shifted. */
   int random_shift;
   uint64_t shift_seed;
+  /* Random ensemble mixture head (REM, Agarwal, Schuurmans and Norouzi, 2020; new capability, no reference counterpart),
+   * off when num_heads = 0 (the default).  Otherwise K = num_heads in 1..200 (other values are EINVAL) Q-value heads
+   * per action, mixed by one random convex combination per train step.  EINVAL with num_atoms, num_quantiles or
+   * num_tau_samples (a net has one head), ENOTIMPL with dueling or munchausen; b200dqn_net_comm_init returns ENOTIMPL
+   * and the DELTAS selector is EINVAL on such a net.  Every fp32 operation below is rounded on its own (no
+   * contraction) unless marked fp64; a is the taken action, z the slot (0 online on the prestates, 1 target on the
+   * poststates, 2 online on the poststates under Double DQN):
+   *    1. mixture draw, once per train step: u_k = (2 m_k + 1) 2^-24, m_k = h >> 9 where h is the high 32 bits of
+   *         x = mix(mix(rem_seed + 0x9E3779B97F4A7C15 (ctr + 1)) ^ k)
+   *       (the IQN head's tau hash at z = 0, b = 0, j = k), ctr the mixture's device-resident draw counter;
+   *       S = sum_k double(u_k) in fp64, k order; alpha_k = float(double(u_k) / S).  The same alpha serves every sample
+   *       and slot of the step.  Every train step, on every train entry point, draws with the counter's value and then
+   *       advances it by one, on the device, so replayed step graphs draw fresh alpha; predict neither reads nor
+   *       advances it; the replay sampler's MT19937 stream is not touched;
+   *    2. fc2: theta[z][b][a K + k] = sum_i H4[z][b][i] W5[i][a K + k], i = 0..511 in order, as the distributional
+   *       head's logits (Neon shape (A K, 512), row a K + k);
+   *    3. train-step Q: Q[z][a] = sum_k alpha_k theta[z][b][a K + k] in k order (each product rounded, then each sum).
+   *       The Q rows of a train step, the greedy target and the Double DQN choice use this Q;
+   *    4. predict Q: Q[a] = (sum_k theta[a][k] in k order) / float(K), the quantile-regression head's rule 3;
+   *    5. the TD step is the scalar head's on the rule-3 Q: the clipped (or n-step) return, the maximum of slot 1's Q
+   *       (slot 1's Q at the first maximum of slot 2's with Double DQN), y = R + g maxq (one fused multiply-add on the
+   *       one-step step, a separately rounded product and sum on the n-step step), target = float(y),
+   *       delta = Q[0][a] - target; the row cost 0.5 delta delta (times the importance weight w on a prioritized ring,
+   *       whose TD error is delta); d = clamp(delta, -clip_error, clip_error) (no clip when clip_error = 0), times w on
+   *       a prioritized ring;
+   *    6. dtheta[a][k] = alpha_k d at the taken action, 0 for every other action;
+   *    7. dZ4 and its fp16 planes, and fc2's per-row gradient partials, as for the distributional head with the logit
+   *       gradient replaced by dtheta; fc2's gradient is summed as for the distributional head (block width K), then
+   *       the configured optimizer applies it. */
+  int num_heads;
+  uint64_t rem_seed;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -515,7 +546,12 @@ enum {
   B200DQN_NET_PTR_IQN_TAU_COUNTER,  /* u64 the draw counter (the next forward draws with this value)                 */
   /* Random-shift augmentation only (random_shift > 0; EINVAL otherwise). */
   B200DQN_NET_PTR_SHIFT_OFFSETS,    /* (2, batch, 2) i32 (dy, dx) of the last train step: prestates, then poststates */
-  B200DQN_NET_PTR_SHIFT_DRAWS       /* u64 the shift's draw counter (the next train step draws with this value)      */
+  B200DQN_NET_PTR_SHIFT_DRAWS,      /* u64 the shift's draw counter (the next train step draws with this value)      */
+  /* Random ensemble mixture head only (num_heads > 0; EINVAL otherwise).  Slots as for the distributional head. */
+  B200DQN_NET_PTR_REM_HEADS,        /* (3, batch, A * num_heads) f32 fc2 outputs theta of the last forward           */
+  B200DQN_NET_PTR_REM_ALPHAS,       /* (num_heads,) f32 the mixture alpha of the last train step                     */
+  B200DQN_NET_PTR_REM_GRADS,        /* (batch, num_heads) f32 gradient dtheta on the taken action's heads            */
+  B200DQN_NET_PTR_REM_COUNTER       /* u64 the mixture's draw counter (the next train step draws with this value)    */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

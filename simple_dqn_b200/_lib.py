@@ -19,7 +19,8 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
  NET_PTR_LOGIT_GRADS, NET_PTR_DZ4_PLANES, NET_PTR_DUELING_VA, NET_PTR_QUANTILES, NET_PTR_TARGET_QUANTILES,
  NET_PTR_QUANTILE_GRADS, NET_PTR_Q_TARGET_PRE, NET_PTR_TD_TARGETS, NET_PTR_IQN_TAUS, NET_PTR_IQN_COS, NET_PTR_IQN_PHI,
  NET_PTR_IQN_X, NET_PTR_IQN_QUANTILES, NET_PTR_IQN_TARGET_QUANTILES, NET_PTR_IQN_QUANTILE_GRADS, NET_PTR_IQN_DX,
- NET_PTR_IQN_DPHI, NET_PTR_IQN_TAU_COUNTER, NET_PTR_SHIFT_OFFSETS, NET_PTR_SHIFT_DRAWS) = range(40)
+ NET_PTR_IQN_DPHI, NET_PTR_IQN_TAU_COUNTER, NET_PTR_SHIFT_OFFSETS, NET_PTR_SHIFT_DRAWS, NET_PTR_REM_HEADS,
+ NET_PTR_REM_ALPHAS, NET_PTR_REM_GRADS, NET_PTR_REM_COUNTER) = range(44)
 
 
 class B200DQNError(RuntimeError):
@@ -37,7 +38,8 @@ class NetConfig(C.Structure):
                 ("v_max", C.c_double), ("dueling", C.c_int), ("num_quantiles", C.c_int),
                 ("munchausen", C.c_int), ("munchausen_alpha", C.c_double), ("munchausen_tau", C.c_double),
                 ("munchausen_clip", C.c_double), ("num_tau_samples", C.c_int), ("num_quantile_samples", C.c_int),
-                ("tau_seed", C.c_uint64), ("random_shift", C.c_int), ("shift_seed", C.c_uint64)]
+                ("tau_seed", C.c_uint64), ("random_shift", C.c_int), ("shift_seed", C.c_uint64),
+                ("num_heads", C.c_int), ("rem_seed", C.c_uint64)]
 
 
 _P = C.c_void_p

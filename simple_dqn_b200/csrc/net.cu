@@ -1046,6 +1046,137 @@ k_shift_draw(unsigned long long* ctr, unsigned long long seed, int pad, int rows
   kt_end(kt);
 }
 
+// ------------------------------------------------------------------------------------------
+// Random ensemble mixture head (REM, Agarwal, Schuurmans and Norouzi 2020; b200dqn.h has the rules).  fc2's outputs
+// theta[z][b][a * K + k] come from k_fc2_dist unchanged, fc2's gradient goes through k_opt_fc2_dist unchanged with K as
+// the block width, and predict's Q is k_head_qr<1, false>'s mean over the K heads.  The new kernels:
+//   k_rem_alpha   one CTA: the step's mixture alpha from the stated hash at the draw counter, then the counter + 1
+//   k_head_rem    one CTA per sample: Q under alpha, the scalar head's TD step, dtheta, dZ4 (+ fp16 planes) and the
+//                 compact dW5 row partial [512][K] of the taken action
+// No expf / logf: every stage is +, -, *, / and comparisons, each rounded on its own.
+// ------------------------------------------------------------------------------------------
+// alpha_k = float(u_k / S) with u_k from k_iqn_tau's hash at (z, b, j) = (0, 0, k) and S = sum_k u_k in fp64, k order.
+// One CTA, so the counter advance after the barrier cannot race a read: every thread has read it by then, and the step's
+// head reads alpha, never the counter.
+__global__ void __launch_bounds__(256)
+k_rem_alpha(unsigned long long* ctr, unsigned long long seed, int K, float* alpha, const KTrace kt) {
+  __shared__ double s_u[kMaxRemHeads];
+  __shared__ double s_sum;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const int t = threadIdx.x;
+  const unsigned long long c = *ctr;
+  if (t < K) {
+    const unsigned long long base = iqn_mix(seed + 0x9E3779B97F4A7C15ull * (c + 1ull));
+    const unsigned m = unsigned(iqn_mix(base ^ (unsigned long long)unsigned(t)) >> 32) >> 9;   // top 23 bits
+    s_u[t] = double(__fmul_rn(float(2u * m + 1u), 5.9604644775390625e-08f));   // (2m + 1) 2^-24, exact
+  }
+  __syncthreads();
+  if (t == 0) {
+    double S = 0.0;
+    for (int k = 0; k < K; ++k) S = __dadd_rn(S, s_u[k]);
+    s_sum = S;
+    *ctr = c + 1ull;
+  }
+  __syncthreads();
+  if (t < K) alpha[t] = float(__ddiv_rn(s_u[t], s_sum));
+  kt_end(kt);
+}
+
+// One CTA (512 threads) per sample b of a train step.  Thread r < nets * A owns row (slot z, action a):
+// Q = sum_k alpha_k theta_k in k order.  Thread 0 runs k_head's TD step on these Q; thread k < K forms dtheta_k =
+// alpha_k d; every thread its dZ4 element and a stride of the dW5 row partial.  The TD scalars and Adam's step scalar
+// come from head_td_scalars, before the dependency wait.
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_rem(const float* __restrict__ theta, int ld, int nets, const float* __restrict__ h4_online,
+           const float* __restrict__ w5_online, float* q_online, float* q_target, float* q_online_post, int A, int K,
+           const float* __restrict__ alpha, float* rgrad, int32_t* act_rows, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  __shared__ float s_q[kSlots][kMaxActions];
+  __shared__ float s_al[kMaxRemHeads], s_g[kMaxRemHeads], s_h4[kHidden];
+  __shared__ float s_d;
+  __shared__ int s_a;
+  const int b = blockIdx.x, t = threadIdx.x, ncols = A * K;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  pdl_wait();
+  pdl_launch_dependents();
+  s_h4[t] = h4_online[b * kHidden + t];
+  if (t < K) s_al[t] = alpha[t];
+  __syncthreads();
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float* th = theta + (int64_t(z) * ld + b) * ncols + a * K;
+    float q = 0.f;
+    for (int k = 0; k < K; ++k) q = __fadd_rn(q, __fmul_rn(s_al[k], th[k]));
+    s_q[z][a] = q;
+    (z == 0 ? q_online : z == 2 ? q_online_post : q_target)[b * A + a] = q;
+  }
+  __syncthreads();
+  if (t == 0) {   // k_head's TD step on the mixed Q, with its contractions made explicit
+    const int a = td_a;
+    const double rr = fmin(fmax(double(td_r), td.min_reward), td.max_reward);
+    float maxq;
+    if constexpr (kSlots == 3) {
+      int best = 0;
+      for (int j = 1; j < A; ++j)
+        if (s_q[2][j] > s_q[2][best]) best = j;
+      maxq = s_q[1][best];
+    } else {
+      maxq = s_q[1][0];
+      for (int j = 1; j < A; ++j) maxq = fmaxf(maxq, s_q[1][j]);
+    }
+    double y;
+    if constexpr (kNstep) y = td_term ? td_ret : __dadd_rn(td_ret, __dmul_rn(td_g, double(maxq)));
+    else y = td_term ? rr : __fma_rn(td.discount, double(maxq), rr);
+    const float target = static_cast<float>(y);
+    float d = __fsub_rn(s_q[0][a], target);
+    if (td.isw) {
+      const float wb = td.isw[b];
+      td.td_err[b] = d;
+      td.row_cost[b] = __fmul_rn(wb, __fmul_rn(__fmul_rn(0.5f, d), d));
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+      d = __fmul_rn(d, wb);
+    } else {
+      td.row_cost[b] = __fmul_rn(__fmul_rn(0.5f, d), d);
+      if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+    }
+    s_d = d;
+    s_a = a;
+    act_rows[b] = a;
+  }
+  __syncthreads();
+  const int a = s_a;
+  if (t < K) {
+    const float g = __fmul_rn(s_al[t], s_d);
+    s_g[t] = g;
+    rgrad[b * K + t] = g;
+  }
+  __syncthreads();
+  {
+    const float hv = s_h4[t];
+    const float* w = w5_online + int64_t(t) * ncols + a * K;
+    float o = 0.f;
+    if (hv > 0.f)
+      for (int k = 0; k < K; ++k) o = __fadd_rn(o, __fmul_rn(w[k], s_g[k]));
+    td.dz4[b * kHidden + t] = o;
+    if (td.dz4_hi) {
+      const __half hh = __float2half_rn(o);
+      const __half ll = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+      td.dz4_hi[b * kHidden + t] = hh;
+      td.dz4_hi[td.dz4_lo_off + b * kHidden + t] = ll;
+    }
+  }
+  float* dw = td.dw5_rows + int64_t(b) * kHidden * K;
+  for (int e = t; e < kHidden * K; e += kHidden) dw[e] = __fmul_rn(s_h4[e / K], s_g[e % K]);
+  kt_end(kt);
+}
+
 // grid (cdiv(rows, 16), nets).  c[r][i] = float(cos((pi i) tau_r)) in fp64, stored for the embedding's gradient; then
 // thread t takes columns t, t + 256, ... and accumulates the CTA's 16 rows of column col in i order.
 __global__ void __launch_bounds__(256)
@@ -1563,7 +1694,8 @@ static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t 
 
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
 // for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
-// join (Munchausen train step on a stream): the event of the target pass's branch, waited for before the head.
+// join (Munchausen or REM train step on a stream): the event of the target pass's or the mixture draw's branch, waited
+// for before the head.
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
                    const HeadTrainArgs& td, cudaEvent_t join = nullptr) {
   if (n->iqn_n) return forward_iqn(n, fs, nets, rows, st, td);
@@ -1634,6 +1766,36 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
                              (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, qa, td,
                              ktrace_slot("head_qr")));
     B2_PROF(td.enable ? "head_qr(td+fc2_bwd)" : "head_qr", st);
+    return B200DQN_OK;
+  }
+  if (n->rem_k) {
+    const int ncols = n->fc2_cols();
+    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
+                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
+                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_theta, ncols, ktrace_slot("fc2_dist")));
+    B2_PROF("fc2_dist", st);
+    if (!td.enable) {   // predict: the mean over the K heads, the quantile-regression head's Q
+      const QrArgs qa{n->rem_k, 0.f, nullptr, nullptr, nullptr};
+      B2_CHECK_CUDA(launch_pdl(k_head_qr<1, false>, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb,
+                               nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A,
+                               qa, td, ktrace_slot("head_qr")));
+      B2_PROF("head_qr", st);
+      return B200DQN_OK;
+    }
+    const bool prev = g_pdl_suppressed;
+    if (join) {   // the mixture draw's branch joins here: the head gets ordinary dependencies on both
+      B2_CHECK_CUDA(cudaStreamWaitEvent(st, join, 0));
+      g_pdl_suppressed = true;
+    }
+    auto* kern = nets == 3 ? (nstep ? k_head_rem<3, true> : k_head_rem<3, false>)
+                           : (nstep ? k_head_rem<2, true> : k_head_rem<2, false>);
+    const cudaError_t e = launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
+                                     (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A,
+                                     n->rem_k, (const float*)n->d_rem_alpha, n->d_rem_grad, n->d_act_rows, td,
+                                     ktrace_slot("head_rem"));
+    g_pdl_suppressed = prev;
+    B2_CHECK_CUDA(e);
+    B2_PROF("head_rem(td+fc2_bwd)", st);
     return B200DQN_OK;
   }
   if (n->munchausen && td.enable) {   // predict takes the scalar head below
@@ -2280,6 +2442,30 @@ static int train_step(b200dqn_net* n, const FrameSource& fs_in, const uint8_t* a
       B2_TRY(forward_target_pre(n, fs, rows, st));
     }
   }
+  if (n->rem_k) {
+    // The mixture draw reads only its counter, so on a stream it runs on its own branch from here and joins before the
+    // head; on the serial schedule it runs in line, ahead of the forward.
+    const bool branch = n->use_branches && st != nullptr && !g_prof_on;
+    cudaStream_t sR = branch ? n->side[0] : st;
+    if (branch) {
+      B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
+      B2_CHECK_CUDA(cudaStreamWaitEvent(sR, n->ev[15], 0));
+    }
+    {
+      const bool prev = g_pdl_suppressed;
+      g_pdl_suppressed = prev || branch;
+      const cudaError_t e = launch_pdl(k_rem_alpha, dim3(1), dim3(256), 0, sR, n->d_rem_ctr,
+                                       (unsigned long long)n->cfg.rem_seed, n->rem_k, n->d_rem_alpha,
+                                       ktrace_slot("rem_alpha"));
+      g_pdl_suppressed = prev;
+      B2_CHECK_CUDA(e);
+    }
+    B2_PROF("rem_alpha", sR);
+    if (branch) {
+      B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sR));
+      join = n->ev[16];
+    }
+  }
   B2_TRY(forward(n, fs, nets, rows, st, td, join));
   return backward_and_update(n, fs, rows, st, true);
 }
@@ -2346,6 +2532,8 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->tau_seed = 0;
   cfg->random_shift = 0;         // no augmentation; DrQ's pad is 4
   cfg->shift_seed = 0;
+  cfg->num_heads = 0;            // no random ensemble mixture head
+  cfg->rem_seed = 0;
   return B200DQN_OK;
 }
 
@@ -2414,6 +2602,15 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   B2_REQUIRE(cfg->random_shift >= 0 && cfg->random_shift <= kMaxCropPad, B200DQN_EINVAL,
              "net_create: random_shift %d is neither 0 (no augmentation) nor in [1,%d]", cfg->random_shift, kMaxCropPad);
+  B2_REQUIRE(cfg->num_heads >= 0 && cfg->num_heads <= kMaxRemHeads, B200DQN_EINVAL,
+             "net_create: num_heads %d is neither 0 (no REM head) nor in [1,%d]", cfg->num_heads, kMaxRemHeads);
+  if (cfg->num_heads) {
+    B2_REQUIRE(!cfg->num_atoms && !cfg->num_quantiles && !cfg->num_tau_samples, B200DQN_EINVAL,
+               "net_create: num_heads (REM) with num_atoms, num_quantiles or num_tau_samples asks for two heads; a net "
+               "has one");
+    B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
+               "net_create: the REM head with a dueling network or the Munchausen target is not implemented");
+  }
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -2425,6 +2622,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->A = cfg->num_actions;
   n->atoms = cfg->num_atoms;
   n->quantiles = cfg->num_quantiles;
+  n->rem_k = cfg->num_heads;
   n->dueling = cfg->dueling != 0;
   n->munchausen = cfg->munchausen != 0;
   n->hidden = n->dueling ? kDuelHidden : kHidden;
@@ -2458,7 +2656,7 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     else
       lt.splits[l] = l < 3 ? int(cdiv(kred[l], wgrad_chunk(kred[l], base[l]))) : 1;
     lt.part_off[l] = po;
-    if (l == 4 && n->fc2_block())   // distributional / quantile / IQN head: the taken action's [512][block] per row
+    if (l == 4 && n->fc2_block())   // distributional / quantile / IQN / REM head: the taken action's [512][block] per row
       po += int64_t(n->iqn_n ? n->iqn_rows : nb) * kHidden * n->fc2_block();
     else
       po += int64_t(lt.splits[l]) * (lt.off[l + 1] - lt.off[l]);
@@ -2520,6 +2718,15 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_CHECK_CUDA(fmalloc(&n->d_theta, size_t(3) * nb * A * n->quantiles));
     B2_CHECK_CUDA(fmalloc(&n->d_tquant, size_t(nb) * n->quantiles));
     B2_CHECK_CUDA(fmalloc(&n->d_qgrad, size_t(nb) * n->quantiles));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
+    B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
+  }
+  if (n->rem_k) {
+    B2_CHECK_CUDA(fmalloc(&n->d_theta, size_t(3) * nb * A * n->rem_k));
+    B2_CHECK_CUDA(fmalloc(&n->d_rem_alpha, n->rem_k));
+    B2_CHECK_CUDA(fmalloc(&n->d_rem_grad, size_t(nb) * n->rem_k));
+    B2_CHECK_CUDA(cudaMalloc(&n->d_rem_ctr, sizeof(unsigned long long)));
+    B2_CHECK_CUDA(cudaMemset(n->d_rem_ctr, 0, sizeof(unsigned long long)));
     B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
     B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
   }
@@ -2622,6 +2829,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_logits); cudaFree(n->d_probs); cudaFree(n->d_tdist); cudaFree(n->d_lgrad); cudaFree(n->d_act_rows);
   cudaFree(n->d_va);
   cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
+  cudaFree(n->d_rem_ctr); cudaFree(n->d_rem_alpha); cudaFree(n->d_rem_grad);
   cudaFree(n->d_tdtarget);
   if (n->d_twe != n->d_we) { cudaFree(n->d_twe); cudaFree(n->d_twes); }
   cudaFree(n->d_crop_ctr); cudaFree(n->d_crop);
@@ -3130,6 +3338,7 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       B2_REQUIRE(!n->atoms, B200DQN_EINVAL, "net_device_ptr: a distributional head has no scalar delta");
       B2_REQUIRE(!n->quantiles, B200DQN_EINVAL, "net_device_ptr: a quantile-regression head has no scalar delta");
       B2_REQUIRE(!n->iqn_n, B200DQN_EINVAL, "net_device_ptr: an IQN head has no scalar delta");
+      B2_REQUIRE(!n->rem_k, B200DQN_EINVAL, "net_device_ptr: a REM head has no scalar delta per action");
       p = n->d_delta;
       b = size_t(n->nb) * n->A * 4;
       break;
@@ -3234,6 +3443,18 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
         b = sizeof(unsigned long long);
       }
       break;
+    case B200DQN_NET_PTR_REM_HEADS:
+    case B200DQN_NET_PTR_REM_ALPHAS:
+    case B200DQN_NET_PTR_REM_GRADS:
+    case B200DQN_NET_PTR_REM_COUNTER:
+      B2_REQUIRE(n->rem_k, B200DQN_EINVAL, "net_device_ptr: selector %d needs a REM head", which);
+      switch (which) {
+        case B200DQN_NET_PTR_REM_HEADS: p = n->d_theta; b = size_t(3) * n->nb * n->A * n->rem_k * 4; break;
+        case B200DQN_NET_PTR_REM_ALPHAS: p = n->d_rem_alpha; b = size_t(n->rem_k) * 4; break;
+        case B200DQN_NET_PTR_REM_GRADS: p = n->d_rem_grad; b = size_t(n->nb) * n->rem_k * 4; break;
+        default: p = n->d_rem_ctr; b = sizeof(unsigned long long); break;
+      }
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -3331,9 +3552,10 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
     // target with a separate target network repeats the forward's launches for its pass
     // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient;
-    // random-shift augmentation adds its draw
+    // random-shift augmentation and the REM head add their draws
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
                 (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->crop_pad ? 1 : 0) +
+                (n->rem_k ? 1 : 0) +
                 (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
   }
   return B200DQN_OK;

@@ -15,6 +15,7 @@ constexpr int kLayers = 5;
 constexpr int kMaxActions = 32;
 constexpr int kMaxAtoms = 64;             // distributional head: atoms per action
 constexpr int kMaxQuantiles = 200;        // quantile-regression head: quantiles per action
+constexpr int kMaxRemHeads = 200;         // random ensemble mixture head: heads per action
 constexpr int kCostRing = 1024;
 constexpr int kHostCosts = 60;            // per-step costs mirrored in host-mapped memory
 constexpr int kHostQ = 64, kHostQFloats = 960;   // word offset / capacity of the Q rows in the host-mapped block
@@ -88,8 +89,8 @@ struct b200dqn_net {
   // step scheduling: side streams / events for the independent wgrad + optimizer branches, and the
   // captured CUDA graph of one fused step
   cudaStream_t side[4] = {};   // three wgrad/optimizer branches + the collective stream
-  cudaEvent_t ev[19] = {};   // [15] / [16]: fork / join of the Munchausen target pass (train_step); [17] / [18]: of the
-                             // random-shift draw
+  cudaEvent_t ev[19] = {};   // [15] / [16]: fork / join of the Munchausen target pass, of the IQN tau branch or of the
+                             // REM mixture draw (a net has at most one of them); [17] / [18]: of the random-shift draw
   bool use_graph = true, use_branches = true;
   bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
   bool double_q = false;     // Double DQN target: the online net picks the poststate action, the target net values it
@@ -127,9 +128,15 @@ struct b200dqn_net {
   float* d_theta = nullptr;      // [3][nb][A * quantiles]
   float* d_tquant = nullptr;     // [nb][quantiles] target quantiles
   float* d_qgrad = nullptr;      // [nb][quantiles] gradient on the taken action's quantiles
-  // fc2 outputs per action of a per-action head (C51 atoms or QR quantiles), 0 on the scalar and dueling heads: such
-  // an fc2 is summed and updated by k_opt_fc2_dist from the compact [nb][512][block] partials
-  int fc2_block() const { return atoms ? atoms : quantiles ? quantiles : iqn_n ? 1 : 0; }
+  // random ensemble mixture head (cfg.num_heads > 0; nothing below is allocated otherwise).  fc2 has A * rem_k outputs,
+  // theta in d_theta, and shares the distributional head's compact dW5 partials, d_act_rows and fc2 kernels
+  int rem_k = 0;                             // K
+  unsigned long long* d_rem_ctr = nullptr;   // the mixture's draw counter
+  float* d_rem_alpha = nullptr;              // [K] the mixture alpha of the last train step
+  float* d_rem_grad = nullptr;               // [nb][K] gradient on the taken action's heads
+  // fc2 outputs per action of a per-action head (C51 atoms, QR quantiles or REM heads), 0 on the scalar and dueling
+  // heads: such an fc2 is summed and updated by k_opt_fc2_dist from the compact [nb][512][block] partials
+  int fc2_block() const { return atoms ? atoms : quantiles ? quantiles : iqn_n ? 1 : rem_k; }
   int fc2_cols() const { return fc2_block() ? A * fc2_block() : dueling ? A + 1 : A; }
 
   // dueling network (cfg.dueling): fc1 is kDuelHidden wide (advantage units [0, 512), value units [512, 1024)) and

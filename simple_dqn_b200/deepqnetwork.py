@@ -40,6 +40,14 @@ def shift_seed(random_seed):
     return (int(random_seed) * 0xD1B54A32D192ED03 + 0x8CB92BA72F3D8DD7) % (1 << 64)
 
 
+def rem_seed(random_seed):
+    """The REM head's uint64 rem_seed for args.random_seed: like tau_seed and shift_seed, with another odd multiplier
+    and offset, so the mixture never shares a stream with them; a fresh random one when the seed is None."""
+    if random_seed is None:
+        return int.from_bytes(os.urandom(8), "little")
+    return (int(random_seed) * 0xA0761D6478BD642F + 0xE7037ED1A0B428DB) % (1 << 64)
+
+
 class DeepQNetwork:
     def __init__(self, num_actions, args, device=None, math_mode=None, stream=None):
         # remember parameters (:17-26)
@@ -132,6 +140,16 @@ class DeepQNetwork:
         if self.random_shift:
             cfg.random_shift = self.random_shift
             cfg.shift_seed = self.shift_seed = shift_seed(_arg(args, "random_seed", None))
+        # random ensemble mixture head (REM, Agarwal et al., 2020): a new capability, off unless args.rem is set; K =
+        # num_heads (200) Q-value heads per action, mixed in each train step by a convex combination the device draws
+        # from rem_seed, derived from random_seed, and a device-resident counter; predict takes the mean over the heads.
+        # Fixed here, like the other heads.
+        self.rem = bool(_arg(args, "rem", False))
+        self.num_heads = 0
+        if self.rem:
+            cfg.num_heads = int(_arg(args, "num_heads", 200))
+            assert cfg.num_heads >= 1, "num_heads %d: the REM head needs 1..200" % cfg.num_heads
+            cfg.rem_seed = self.rem_seed = rem_seed(_arg(args, "random_seed", None))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -142,6 +160,8 @@ class DeepQNetwork:
         if self.implicit_quantiles:
             self.num_tau_samples, self.num_quantile_samples = cfg.num_tau_samples, cfg.num_quantile_samples
             self.tau_seed = cfg.tau_seed
+        if self.rem:
+            self.num_heads = cfg.num_heads
         if self.quantile_regression:
             self.num_quantiles = n = cfg.num_quantiles                 # tau_i = (2i + 1) / 2N in fp64, as the device
             self.taus = np.array([(2 * i + 1) / (2 * n) for i in range(n)], dtype=np.float64).astype(np.float32)
@@ -369,6 +389,24 @@ class DeepQNetwork:
     def shift_draws(self):
         """The shift's draw counter: train steps that have drawn offsets; the next one draws with this value."""
         return int(L.download(self.device, self.device_view(L.NET_PTR_SHIFT_DRAWS, (1,)).ptr, (1,), np.uint64,
+                              self._stream)[0])
+
+    # ---- random ensemble mixture head (rem = True): slots as for the distributional head
+    def last_heads(self):
+        """fc2's outputs theta of the last forward, (3, batch, A, num_heads) float32."""
+        return self._read_f32(L.NET_PTR_REM_HEADS, (3, self.batch_size, self.num_actions, self.num_heads))
+
+    def last_mixture(self):
+        """The mixture alpha of the last train step, (num_heads,) float32: positive, summing to 1."""
+        return self._read_f32(L.NET_PTR_REM_ALPHAS, (self.num_heads,))
+
+    def last_head_grads(self):
+        """The gradient on the taken action's heads of the last train(), (batch, num_heads) float32."""
+        return self._read_f32(L.NET_PTR_REM_GRADS, (self.batch_size, self.num_heads))
+
+    def mixture_counter(self):
+        """The mixture's draw counter: train steps that have drawn alpha; the next one draws with this value."""
+        return int(L.download(self.device, self.device_view(L.NET_PTR_REM_COUNTER, (1,)).ptr, (1,), np.uint64,
                               self._stream)[0])
 
     # ---- Munchausen target (munchausen = True)

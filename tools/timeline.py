@@ -16,6 +16,7 @@ MUNCHAUSEN = os.environ.get("MUNCHAUSEN", "0") == "1"   # the Munchausen target 
 IQN = int(os.environ.get("IQN", "0"))   # IQN head with this many tau samples per train row; 0: off
 IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per predict row
 SHIFT = int(os.environ.get("SHIFT", "0"))   # random-shift augmentation with this pad p (DrQ: 4); 0: off
+REM = int(os.environ.get("REM", "0"))   # random ensemble mixture head (REM) with this many heads per action; 0: off
 
 
 def net_args():
@@ -26,6 +27,7 @@ def net_args():
     a.munchausen = MUNCHAUSEN
     a.implicit_quantiles, a.num_tau_samples, a.num_quantile_samples = IQN > 0, IQN, IQN_K
     a.random_shift = SHIFT
+    a.rem, a.num_heads = REM > 0, REM
     return a
 
 
