@@ -395,6 +395,41 @@ typedef struct b200dqn_net_config {
    *       the configured optimizer applies it. */
   int num_heads;
   uint64_t rem_seed;
+  /* Fully parameterized quantile function head (FQF, Yang, Zhao, Lin, Qin, Bian and Liu, 2019; new capability, no
+   * reference counterpart), off when num_fractions = 0 (the default).  Otherwise N = num_fractions in 2..64 with
+   * nb N <= 4096 rows, and fraction_lr (finite, >= 0) is the learning rate of the fraction proposal layer; anything else
+   * is EINVAL before any device work, as are num_atoms, num_quantiles, num_tau_samples or num_heads beside it (a net has
+   * one head) and a non-finite clip_error.  ENOTIMPL with dueling or munchausen; b200dqn_net_set_double_q(n, 1) and
+   * b200dqn_net_comm_init return ENOTIMPL on such a net.  ABI layer 5 is the IQN head's embedding (Neon shape
+   * (3136, 64)), ABI layer 6 the fraction layer W_f (Neon shape (N, 3136), columns in fc1's Neon (c, p, q) input order);
+   * both have optimizer states and belong to each network, and the step reads the online W_f only.  kappa, b, a, z and
+   * the rounding are as for the IQN head; psi is the online network's fp32 H3 of the prestates; every fp64 operation
+   * is rounded on its own except exp, the device's fp64 exp:
+   *    1. logits l[b][k] = sum over col of psi[b][col] W_f[k][col] in fc1's internal (p, q, c) column order, as 32
+   *       lanes: lane j sums the products of columns j, j + 32, ..., j + 3104 in order, then the lanes are combined by
+   *       halving, s_j = s_j + s_{j + h} for h = 16, 8, 4, 2, 1;
+   *    2. proposal in fp64: m = max_k l_k; e_k = exp(double(l_k) - m); C_0 = 0, C_{i+1} = C_i + e_i in i order,
+   *       S = C_N; q_k = float(e_k / S); tau_i = float(C_i / S) (tau_0 = 0, tau_N = 1); tauhat_i =
+   *       float((C_i + C_{i+1}) / (2 S)).  With zero logits tauhat is the quantile-regression head's midpoints;
+   *    3. rows r = b N + i: slot 0 the online network at tauhat on the prestates, slot 1 the target network at the
+   *       same tauhat on the poststates; each slot runs the IQN head's rules 3-6 (c, phi, X = psi phi, fc1, fc2);
+   *    4. Q[a] = sum_i dtau_i theta[b N + i][a] in i order (each product rounded, then each sum), dtau_i =
+   *       tau_{i+1} - tau_i.  Every Q output is this Q: predict, the Q rows, and a* = the first maximum of slot 1's Q
+   *       (a simplification: the target is valued at the prestates' proposal, not at a second proposal on the
+   *       poststates);
+   *    5. the quantile loss, the row cost, the importance weight, the priority (the unweighted row loss), dtheta, dZ4
+   *       and its planes, fc2's gradient, dpsi, dphi and dWe are the IQN head's rules 9-13 with weight tauhat_i; tauhat
+   *       is a constant to this loss and W_f gets no gradient from it;
+   *    6. boundary pass, forward only, on the online network at tau_1..tau_{N-1}: rows b (N - 1) + i - 1 through the
+   *       IQN head's rules 3-6 give theta_bnd; beta_i = theta_bnd[b (N - 1) + i - 1][a];
+   *    7. fraction gradient, i = 1..N-1: g_i = (2 beta_i - theta[0][b N + i][a]) - theta[0][b N + i - 1][a], times
+   *       the importance weight on a prioritized ring; dq_k = sum_{i = k+1..N-1} g_i accumulated from i = N - 1
+   *       downward (dq_{N-1} = 0); s = sum_k q_k dq_k in k order; dl_k = q_k (dq_k - s);
+   *    8. dW_f[k][col] = sum_b dl[b][k] psi[b][col] in b order; the configured optimizer (batch size nb, its other
+   *       hyperparameters and Adam's t the net's) applies it with learning rate fraction_lr.  psi gets no gradient
+   *       from the fraction loss. */
+  int num_fractions;
+  double fraction_lr;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -406,7 +441,8 @@ int b200dqn_net_destroy(b200dqn_net* n);
 
 /* Weights cross the boundary in NEON layout: conv W[C*R*S][K], linear W[nout][nin], fp32,
  * C-contiguous (what Model.get_description / the shipped snapshots hold); host_S is the
- * RMSProp state of the same shape (may be NULL).  layer 0..4 (and 5, the embedding, on an IQN net); which 0 = online,
+ * RMSProp state of the same shape (may be NULL).  layer 0..4 (and 5, the embedding, on an IQN or FQF net; 6, the fraction
+ * layer, on an FQF net); which 0 = online,
  * 1 = target.
  * Replaces Model.load_params / save_params — src/deepqnetwork.py:188-192.  Synchronises. */
 int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, const float* host_W, const float* host_S,
@@ -551,7 +587,15 @@ enum {
   B200DQN_NET_PTR_REM_HEADS,        /* (3, batch, A * num_heads) f32 fc2 outputs theta of the last forward           */
   B200DQN_NET_PTR_REM_ALPHAS,       /* (num_heads,) f32 the mixture alpha of the last train step                     */
   B200DQN_NET_PTR_REM_GRADS,        /* (batch, num_heads) f32 gradient dtheta on the taken action's heads            */
-  B200DQN_NET_PTR_REM_COUNTER       /* u64 the mixture's draw counter (the next train step draws with this value)    */
+  B200DQN_NET_PTR_REM_COUNTER,      /* u64 the mixture's draw counter (the next train step draws with this value)    */
+  /* FQF head only (num_fractions > 0; EINVAL otherwise).  The IQN selectors read its rows (N = K = num_fractions,
+   * IQN_TAUS holding tauhat) except IQN_TAU_COUNTER, which is EINVAL: the head draws nothing. */
+  B200DQN_NET_PTR_FQF_LOGITS,       /* (batch, N) f32 the fraction logits l of the last forward                      */
+  B200DQN_NET_PTR_FQF_PROBS,        /* (batch, N) f32 the proposal q                                                 */
+  B200DQN_NET_PTR_FQF_FRACTIONS,    /* (batch, N + 1) f32 the fractions tau_0 = 0 .. tau_N = 1                       */
+  B200DQN_NET_PTR_FQF_BOUNDARY_QUANTILES, /* (batch (N - 1), A) f32 theta_bnd of the last train step                 */
+  B200DQN_NET_PTR_FQF_FRACTION_GRADS,     /* (batch, N - 1) f32 the fraction gradient g of the last train step       */
+  B200DQN_NET_PTR_FQF_LOGIT_GRADS         /* (batch, N) f32 the logit gradient dl of the last train step             */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

@@ -20,7 +20,8 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
  NET_PTR_QUANTILE_GRADS, NET_PTR_Q_TARGET_PRE, NET_PTR_TD_TARGETS, NET_PTR_IQN_TAUS, NET_PTR_IQN_COS, NET_PTR_IQN_PHI,
  NET_PTR_IQN_X, NET_PTR_IQN_QUANTILES, NET_PTR_IQN_TARGET_QUANTILES, NET_PTR_IQN_QUANTILE_GRADS, NET_PTR_IQN_DX,
  NET_PTR_IQN_DPHI, NET_PTR_IQN_TAU_COUNTER, NET_PTR_SHIFT_OFFSETS, NET_PTR_SHIFT_DRAWS, NET_PTR_REM_HEADS,
- NET_PTR_REM_ALPHAS, NET_PTR_REM_GRADS, NET_PTR_REM_COUNTER) = range(44)
+ NET_PTR_REM_ALPHAS, NET_PTR_REM_GRADS, NET_PTR_REM_COUNTER, NET_PTR_FQF_LOGITS, NET_PTR_FQF_PROBS,
+ NET_PTR_FQF_FRACTIONS, NET_PTR_FQF_BOUNDARY_QUANTILES, NET_PTR_FQF_FRACTION_GRADS, NET_PTR_FQF_LOGIT_GRADS) = range(50)
 
 
 class B200DQNError(RuntimeError):
@@ -39,7 +40,8 @@ class NetConfig(C.Structure):
                 ("munchausen", C.c_int), ("munchausen_alpha", C.c_double), ("munchausen_tau", C.c_double),
                 ("munchausen_clip", C.c_double), ("num_tau_samples", C.c_int), ("num_quantile_samples", C.c_int),
                 ("tau_seed", C.c_uint64), ("random_shift", C.c_int), ("shift_seed", C.c_uint64),
-                ("num_heads", C.c_int), ("rem_seed", C.c_uint64)]
+                ("num_heads", C.c_int), ("rem_seed", C.c_uint64),
+                ("num_fractions", C.c_int), ("fraction_lr", C.c_double)]
 
 
 _P = C.c_void_p

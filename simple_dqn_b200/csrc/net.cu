@@ -1252,15 +1252,27 @@ struct IqnArgs {
   int32_t* act_rows;  // [nb N] taken action of each online row (selects fc2's gradient column)
 };
 
+// The FQF head's additions to k_head_iqn (b200dqn.h's FQF rules 4 and 7)
+struct FqfArgs {
+  const float* frac;    // [nb][N + 1] tau
+  const float* prob;    // [nb][N] q
+  const float* bnd;     // [nb (N - 1)][A] theta_bnd
+  float* g;             // [nb][N - 1]
+  float* dl;            // [nb][N]
+  float adam_flr;       // Adam: fraction_lr, and where this step's l of the fraction layer goes (nullptr otherwise)
+  float* adam_lf;
+};
+
 // One CTA (512 threads) per sample b; its rows are r = b * per + j.  Thread t < nets * A owns (slot z, action a):
-// Q = (sum_j theta[z][r][a], j order) / per.  With td.enable (kSlots = 2): thread 0 picks a* and the fp64 return, thread
-// j < N forms T_j, thread i < N runs k_head_qr's j loop for online row b N + i with the weights tau_i and 1 - tau_i, thread
-// 0 sums the row loss, and thread k writes dZ4 and fc2's row partial of unit k for every online row of the sample.
-template <int kSlots, bool kNstep>
-__global__ void __launch_bounds__(kHidden)
-k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ h4_online,
-           const float* __restrict__ w5_online, float* q_online, float* q_target, int A, const IqnArgs ia,
-           const HeadTrainArgs td, const KTrace kt) {
+// Q = (sum_j theta[z][r][a], j order) / per (FQF: sum_j dtau_j theta[z][r][a]).  With td.enable (kSlots = 2): thread 0
+// picks a* and the fp64 return, thread j < N forms T_j, thread i < N runs k_head_qr's j loop for online row b N + i with
+// the weights tau_i and 1 - tau_i, thread 0 sums the row loss (FQF: and forms g, dq and dl), and thread k writes dZ4 and
+// fc2's row partial of unit k for every online row of the sample.  The body is shared by k_head_iqn and k_head_fqf.
+template <int kSlots, bool kNstep, bool kFqf>
+__device__ __forceinline__ void
+head_iqn_body(const float* __restrict__ theta, int nets, const float* __restrict__ h4_online,
+              const float* __restrict__ w5_online, float* q_online, float* q_target, int A, const IqnArgs& ia,
+              const FqfArgs& fa, const HeadTrainArgs& td, const KTrace& kt) {
   static_assert(kSlots == 1 || kSlots == 2, "predict, or online + target");
   __shared__ float s_q[kSlots][kMaxActions];
   __shared__ float s_t[kIqnMaxPer], s_l[kIqnMaxPer], s_g[kIqnMaxPer];
@@ -1273,14 +1285,28 @@ k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ 
   int64_t td_r = 0;
   double td_ret = 0.0, td_g = 1.0;
   head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  if constexpr (kFqf) {
+    if (td.enable && fa.adam_lf && b == 0 && t == 32) {   // head_td_scalars' Adam scalar at lr = fraction_lr
+      const double tt = double(*td.step) + 1.0;
+      const float a = float(1.0 - pow(0.999, tt)), c = float(1.0 - pow(0.9, tt));
+      *fa.adam_lf = __fdiv_rn(__fmul_rn(fa.adam_flr, __fsqrt_rn(a)), c);
+    }
+  }
   pdl_wait();
   pdl_launch_dependents();
   if (t < nets * A) {
     const int z = t / A, a = t % A;
     const float* th = theta + (z * ld + r0) * A + a;
-    float s = 0.f;
-    for (int j = 0; j < np; ++j) s = __fadd_rn(s, th[int64_t(j) * A]);
-    const float q = __fdiv_rn(s, float(np));
+    float q;
+    if constexpr (kFqf) {
+      const float* fr = fa.frac + int64_t(b) * (np + 1);
+      q = 0.f;
+      for (int j = 0; j < np; ++j) q = __fadd_rn(q, __fmul_rn(__fsub_rn(fr[j + 1], fr[j]), th[int64_t(j) * A]));
+    } else {
+      float s = 0.f;
+      for (int j = 0; j < np; ++j) s = __fadd_rn(s, th[int64_t(j) * A]);
+      q = __fdiv_rn(s, float(np));
+    }
     s_q[z][a] = q;
     (z == 0 ? q_online : q_target)[b * A + a] = q;
   }
@@ -1350,6 +1376,28 @@ k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ 
       } else {
         td.row_cost[b] = l;
       }
+      if constexpr (kFqf) {   // the fraction gradient g, dq and the logit gradient dl (s_t and s_l are free again)
+        const int nb1 = np - 1;
+        const float* th0 = theta + r0 * A + a;
+        const float* bt = fa.bnd + int64_t(b) * nb1 * A + a;
+        for (int i = 1; i < np; ++i) {
+          float gi = __fsub_rn(__fsub_rn(__fmul_rn(2.f, bt[int64_t(i - 1) * A]), th0[int64_t(i) * A]),
+                               th0[int64_t(i - 1) * A]);
+          if (td.isw) gi = __fmul_rn(gi, td.isw[b]);
+          s_t[i] = gi;
+          fa.g[int64_t(b) * nb1 + i - 1] = gi;
+        }
+        float acc = 0.f;
+        s_l[np - 1] = 0.f;
+        for (int k = np - 2; k >= 0; --k) {
+          acc = __fadd_rn(acc, s_t[k + 1]);
+          s_l[k] = acc;
+        }
+        const float* qk = fa.prob + int64_t(b) * np;
+        float s = 0.f;
+        for (int k = 0; k < np; ++k) s = __fadd_rn(s, __fmul_rn(qk[k], s_l[k]));
+        for (int k = 0; k < np; ++k) fa.dl[int64_t(b) * np + k] = __fmul_rn(qk[k], __fsub_rn(s_l[k], s));
+      }
     }
     const float w5a = w5_online[t * A + a];
     for (int i = 0; i < np; ++i) {
@@ -1366,6 +1414,22 @@ k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ 
     }
   }
   kt_end(kt);
+}
+
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_iqn(const float* __restrict__ theta, int nets, const float* __restrict__ h4_online,
+           const float* __restrict__ w5_online, float* q_online, float* q_target, int A, const IqnArgs ia,
+           const HeadTrainArgs td, const KTrace kt) {
+  head_iqn_body<kSlots, kNstep, false>(theta, nets, h4_online, w5_online, q_online, q_target, A, ia, FqfArgs{}, td, kt);
+}
+
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_fqf(const float* __restrict__ theta, int nets, const float* __restrict__ h4_online,
+           const float* __restrict__ w5_online, float* q_online, float* q_target, int A, const IqnArgs ia,
+           const FqfArgs fa, const HeadTrainArgs td, const KTrace kt) {
+  head_iqn_body<kSlots, kNstep, true>(theta, nets, h4_online, w5_online, q_online, q_target, A, ia, fa, td, kt);
 }
 
 // One thread per (sample b, column col) of `rows` samples: dpsi[b][col] = (sum_j dX[r][col] phi[r][col], j order) under
@@ -1449,6 +1513,98 @@ k_iqn_we(const float* __restrict__ cosf, const float* __restrict__ dphi, int row
         w[wi] = wv;
         for (int k = 0; k < opt.nstates; ++k) sst[k * opt.plane + wi] = s[k];
       }
+    }
+  }
+  kt_end(kt);
+}
+
+// ------------------------------------------------------------------------------------------
+// Fully parameterized quantile function head (FQF, Yang et al. 2019; b200dqn.h has the rules).  It is the IQN head with
+// tau = the fraction proposal's tauhat: k_iqn_phi, k_iqn_mod, fc1, k_fc2_dist, k_iqn_mod_bwd and k_iqn_we run unchanged,
+// and the boundary pass runs phi, mod, fc1 and k_fc2_dist once more on the online network at tau_1..tau_{N-1}.  The new
+// kernels:
+//   k_fqf_fraction  one CTA per sample: the logits, the fp64 proposal q, tau and tauhat
+//   k_head_fqf      k_head_iqn's body with the FQF Q rule and, in a train step, the fraction and logit gradients
+//   k_fqf_wf        dW_f and the fraction layer's update at fraction_lr
+// ------------------------------------------------------------------------------------------
+constexpr int kFqfMaxN = 64;
+
+// One CTA (256 threads) per sample b.  Warp w computes the logits k = w, w + 8, ... (rule 1's lane order), thread 0 the
+// fp64 prefix sums, then thread i writes tau_i, q_i and tauhat_i: into both slots of tau (nets = 2) at rows b N + i, and
+// tau_1..tau_{N-1} into btau (a train step; nullptr on predict).
+__global__ void __launch_bounds__(256)
+k_fqf_fraction(const float* __restrict__ psi, const float* __restrict__ wf, int N, int nets, int ld,
+               float* __restrict__ logit, float* __restrict__ prob, float* __restrict__ frac, float* __restrict__ tau,
+               float* __restrict__ btau, const KTrace kt) {
+  __shared__ float s_psi[kFlat];
+  __shared__ float s_l[kFqfMaxN];
+  __shared__ double s_e[kFqfMaxN], s_c[kFqfMaxN + 1];
+  const int b = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  for (int col = t; col < kFlat; col += 256) s_psi[col] = psi[int64_t(b) * kFlat + col];
+  __syncthreads();
+  for (int k = warp; k < N; k += 8) {
+    const float* w = wf + int64_t(k) * kFlat;
+    float acc = 0.f;
+    for (int col = lane; col < kFlat; col += 32) acc = __fadd_rn(acc, __fmul_rn(s_psi[col], w[col]));
+    for (int h = 16; h > 0; h >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, h));
+    if (lane == 0) {
+      s_l[k] = acc;
+      logit[int64_t(b) * N + k] = acc;
+    }
+  }
+  __syncthreads();
+  if (t == 0) {
+    double m = double(s_l[0]);
+    for (int k = 1; k < N; ++k) m = fmax(m, double(s_l[k]));
+    double c = 0.0;
+    s_c[0] = 0.0;
+    for (int k = 0; k < N; ++k) {
+      const double e = exp(__dsub_rn(double(s_l[k]), m));
+      s_e[k] = e;
+      c = __dadd_rn(c, e);
+      s_c[k + 1] = c;
+    }
+  }
+  __syncthreads();
+  const double S = s_c[N];
+  for (int i = t; i <= N; i += 256) {
+    const float ti = float(__ddiv_rn(s_c[i], S));
+    frac[int64_t(b) * (N + 1) + i] = ti;
+    if (btau && i >= 1 && i < N) btau[int64_t(b) * (N - 1) + i - 1] = ti;
+    if (i < N) {
+      prob[int64_t(b) * N + i] = float(__ddiv_rn(s_e[i], S));
+      const float th = float(__ddiv_rn(__dadd_rn(s_c[i], s_c[i + 1]), __dmul_rn(2.0, S)));
+      for (int z = 0; z < nets; ++z) tau[int64_t(z) * ld + int64_t(b) * N + i] = th;
+    }
+  }
+  kt_end(kt);
+}
+
+// dW_f[k][col] = sum_b dl[b][k] psi[b][col] in b order, one thread per (k, col); then (update) the configured optimizer
+// with opt.lr = fraction_lr.
+__global__ void __launch_bounds__(256)
+k_fqf_wf(const float* __restrict__ dl, const float* __restrict__ psi, int rows, int N, float* __restrict__ g_out,
+         float* __restrict__ w, float* __restrict__ sst, int update, const OptArgs opt, const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const int e = blockIdx.x * 256 + threadIdx.x;
+  if (e < N * kFlat) {
+    const int k = e / kFlat, col = e % kFlat;
+    float acc = 0.f;
+    for (int b = 0; b < rows; ++b) acc = __fadd_rn(acc, __fmul_rn(dl[int64_t(b) * N + k], psi[int64_t(b) * kFlat + col]));
+    g_out[e] = acc;
+    if (update) {
+      const float l = opt_step_scalar(opt);
+      float s[3] = {0.f, 0.f, 0.f};
+      for (int q = 0; q < opt.nstates; ++q) s[q] = sst[q * opt.plane + e];
+      float wv = w[e];
+      opt_update1(opt, l, acc, wv, s[0], s[1], s[2]);
+      w[e] = wv;
+      for (int q = 0; q < opt.nstates; ++q) sst[q * opt.plane + e] = s[q];
     }
   }
   kt_end(kt);
@@ -1666,8 +1822,104 @@ static int forward_iqn(b200dqn_net* n, const FrameSource& fs, int nets, int rows
   return B200DQN_OK;
 }
 
+// The FQF forward for `nets` slots of `rows` samples, every launch on st (b200dqn.h's FQF rules): the conv trunk, the
+// fraction proposal from the online psi, then phi, X, fc1 and fc2 of both slots at tauhat, and in a train step the
+// boundary pass (the online network at tau_1..tau_{N-1}) before the head, all in line: tauhat depends on the trunk, and
+// the boundary pass reads the weights the step's updates overwrite, so nothing here can leave the chain.
+static int forward_fqf(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
+                       const HeadTrainArgs& td) {
+  const LayerTable& lt = n->lt;
+  const float* w[3] = {n->d_w, n->d_tw, n->d_w};
+  const int N = n->fqf_n, R = rows * N, ld = n->iqn_rows, Rb = rows * (N - 1);
+  const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
+  // split counts are taken at the full minibatch, so a predict on fewer live rows sums every row as the full one does
+  const int splits = tc ? umma_fc1_splits(n->nb * N) : kFc1Splits;
+  int rc;
+  if (tc) {
+    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1, true))) return rc;
+  } else {
+    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
+    {
+      using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
+      P p;
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
+      p.nb = rows;
+      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
+    }
+    {
+      using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
+      P p;
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
+      p.nb = rows;
+      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
+    }
+  }
+  B2_CHECK_CUDA(launch_pdl(k_fqf_fraction, dim3(rows), dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_wf,
+                           N, nets, ld, n->d_fl, n->d_fq, n->d_ftau, n->d_tau, td.enable ? n->d_btau : nullptr,
+                           ktrace_slot("fqf_fraction")));
+  B2_PROF("fqf_fraction", st);
+  B2_CHECK_CUDA(launch_pdl(k_iqn_phi, dim3(cdiv(R, kIqnTB), nets), dim3(256), 0, st, (const float*)n->d_tau, R, ld,
+                           (const float*)n->d_we, (const float*)n->d_twe, n->d_cos, n->d_phi, ktrace_slot("iqn_phi")));
+  B2_PROF("iqn_phi", st);
+  const int64_t total = int64_t(nets) * R * kFlat;
+  B2_CHECK_CUDA(launch_pdl(k_iqn_mod, dim3(unsigned(std::min<int64_t>(cdiv(total, 256), int64_t(n->sm_count) * 16))),
+                           dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_h3[1], (const float*)n->d_phi,
+                           n->d_x, n->d_x16, nets, R, N, ld, ktrace_slot("iqn_mod")));
+  B2_PROF("iqn_mod", st);
+  if (tc) {
+    if ((rc = umma_fc1_fwd_iqn(n, nets, R, splits, st))) return rc;
+  } else {
+    Fc1Fwd<kHidden> p;
+    for (int z = 0; z < 3; ++z) {
+      p.in[z] = n->d_x + int64_t(z < 2 ? z : 0) * ld * kFlat;
+      p.w[z] = w[z] + lt.off[3];
+    }
+    p.part = n->d_fc1part; p.nb = R; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+    if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, R, kHidden, nets * kFc1Splits, st))) return rc;
+  }
+  B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(R, kDistTB), cdiv(n->A, kDistTN), nets), dim3(256), 0, st,
+                           (const float*)n->d_fc1part, splits, R, ld, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
+                           w[1] + lt.off[4], n->d_iqn_theta, n->A, ktrace_slot("fc2_dist")));
+  B2_PROF("fc2_dist", st);
+  if (td.enable) {   // the boundary pass: the online network at tau_1..tau_{N-1}, on buffers of its own
+    B2_CHECK_CUDA(launch_pdl(k_iqn_phi, dim3(cdiv(Rb, kIqnTB), 1), dim3(256), 0, st, (const float*)n->d_btau, Rb, Rb,
+                             (const float*)n->d_we, (const float*)n->d_we, n->d_bcos, n->d_bphi, ktrace_slot("iqn_phi")));
+    B2_PROF("fqf_bnd_phi", st);
+    B2_CHECK_CUDA(launch_pdl(k_iqn_mod, dim3(unsigned(std::min<int64_t>(cdiv(int64_t(Rb) * kFlat, 256),
+                                                                         int64_t(n->sm_count) * 16))),
+                             dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_h3[0],
+                             (const float*)n->d_bphi, n->d_bx, n->d_bx16, 1, Rb, N - 1, Rb, ktrace_slot("iqn_mod")));
+    B2_PROF("fqf_bnd_mod", st);
+    const int bsplits = tc ? umma_fc1_splits(Rb) : kFc1Splits;
+    if (tc) {
+      if ((rc = umma_fc1_fwd_fqf_boundary(n, Rb, bsplits, st))) return rc;
+    } else {
+      Fc1Fwd<kHidden> p;
+      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_bx; p.w[z] = w[0] + lt.off[3]; }
+      p.part = n->d_fc1part; p.nb = Rb; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+      if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, Rb, kHidden, kFc1Splits, st))) return rc;
+    }
+    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(Rb, kDistTB), cdiv(n->A, kDistTN), 1), dim3(256), 0, st,
+                             (const float*)n->d_fc1part, bsplits, Rb, Rb, n->d_bh4, n->d_bh4, w[0] + lt.off[4],
+                             w[0] + lt.off[4], n->d_btheta, n->A, ktrace_slot("fc2_dist")));
+    B2_PROF("fqf_bnd_fc2", st);
+  }
+  const IqnArgs ia{N, ld, float(n->cfg.clip_error), n->d_tau, n->d_iqn_tq, n->d_iqn_qgrad, n->d_act_rows};
+  const bool adam = n->cfg.optimizer == B200DQN_OPT_ADAM;
+  const FqfArgs fa{n->d_ftau, n->d_fq, n->d_btheta, n->d_fg, n->d_fdl, float(n->cfg.fraction_lr),
+                   adam ? n->d_optscal + 2 : nullptr};
+  const bool nstep = td.enable && td.nstep > 1;
+  auto* kern = nets == 1 ? k_head_fqf<1, false> : nstep ? k_head_fqf<2, true> : k_head_fqf<2, false>;
+  B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_iqn_theta, nets,
+                           (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->A, ia, fa, td,
+                           ktrace_slot("head_fqf")));
+  B2_PROF(td.enable ? "head_fqf(td+fc2_bwd)" : "head_fqf", st);
+  return B200DQN_OK;
+}
+
 // The IQN backward between fc1's dgrad and conv3's (on st): dpsi into dZ3 and dphi; then dWe and the embedding's update,
-// on side stream sW when given (its own branch: nothing later in the step reads We), else in line.
+// on side stream sW when given (its own branch: nothing later in the step reads We), else in line.  An FQF net adds
+// dW_f and the fraction layer's update on the same branch.
 static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t sW, bool update) {
   __half* dpsi16 = nullptr;
   int64_t dpsi_lo = 0;
@@ -1689,6 +1941,16 @@ static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t 
                            (const float*)n->d_dphi, rows * n->iqn_n, n->d_weg, n->d_we, n->d_wes, update ? 1 : 0, o,
                            ktrace_slot("iqn_we")));
   B2_PROF("iqn_we", s);
+  if (n->fqf_n) {
+    OptArgs of = make_opt_args(n, rows);
+    of.lr = float(n->cfg.fraction_lr);
+    of.adam_l = n->d_optscal + 2;   // the FQF head's Adam scalar at fraction_lr
+    of.plane = int64_t(n->fqf_n) * kFlat;
+    B2_CHECK_CUDA(launch_pdl(k_fqf_wf, dim3(cdiv(int64_t(n->fqf_n) * kFlat, 256)), dim3(256), 0, s,
+                             (const float*)n->d_fdl, (const float*)n->d_h3[0], rows, n->fqf_n, n->d_wfg, n->d_wf,
+                             n->d_wfs, update ? 1 : 0, of, ktrace_slot("fqf_wf")));
+    B2_PROF("fqf_wf", s);
+  }
   return B200DQN_OK;
 }
 
@@ -1698,6 +1960,7 @@ static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t 
 // for before the head.
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
                    const HeadTrainArgs& td, cudaEvent_t join = nullptr) {
+  if (n->fqf_n) return forward_fqf(n, fs, nets, rows, st, td);
   if (n->iqn_n) return forward_iqn(n, fs, nets, rows, st, td);
   const LayerTable& lt = n->lt;
   const float* w[3] = {n->d_w, n->d_tw, n->d_w};
@@ -2534,6 +2797,8 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->shift_seed = 0;
   cfg->num_heads = 0;            // no random ensemble mixture head
   cfg->rem_seed = 0;
+  cfg->num_fractions = 0;        // no FQF head
+  cfg->fraction_lr = 2.5e-9;
   return B200DQN_OK;
 }
 
@@ -2611,6 +2876,22 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
                "net_create: the REM head with a dueling network or the Munchausen target is not implemented");
   }
+  B2_REQUIRE(cfg->num_fractions == 0 || (cfg->num_fractions >= 2 && cfg->num_fractions <= kFqfMaxN), B200DQN_EINVAL,
+             "net_create: num_fractions %d is neither 0 (no FQF head) nor in [2,%d]", cfg->num_fractions, kFqfMaxN);
+  if (cfg->num_fractions) {
+    B2_REQUIRE(std::isfinite(cfg->fraction_lr) && cfg->fraction_lr >= 0, B200DQN_EINVAL,
+               "net_create: fraction_lr must be finite and >= 0 (got %g)", cfg->fraction_lr);
+    B2_REQUIRE(int64_t(cfg->batch_size) * cfg->num_fractions <= 4096, B200DQN_EINVAL,
+               "net_create: the FQF head runs fc1 on batch_size x num_fractions = %lld rows; at most 4096 are supported",
+               (long long)cfg->batch_size * cfg->num_fractions);
+    B2_REQUIRE(!cfg->num_atoms && !cfg->num_quantiles && !cfg->num_tau_samples && !cfg->num_heads, B200DQN_EINVAL,
+               "net_create: num_fractions with num_atoms, num_quantiles, num_tau_samples or num_heads asks for two "
+               "heads; a net has one");
+    B2_REQUIRE(std::isfinite(cfg->clip_error), B200DQN_EINVAL,
+               "net_create: the quantile Huber threshold clip_error must be finite (got %g)", cfg->clip_error);
+    B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
+               "net_create: the FQF head with a dueling network or the Munchausen target is not implemented");
+  }
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -2630,6 +2911,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     n->iqn_n = cfg->num_tau_samples;
     n->iqn_k = cfg->num_quantile_samples;
     n->iqn_rows = cfg->batch_size * std::max(n->iqn_n, n->iqn_k);
+  }
+  if (cfg->num_fractions) {   // the IQN head's machinery at N = K = num_fractions rows per sample
+    n->fqf_n = n->iqn_n = n->iqn_k = cfg->num_fractions;
+    n->iqn_rows = cfg->batch_size * n->fqf_n;
   }
   if (n->atoms) n->dz = (cfg->v_max - cfg->v_min) / double(n->atoms - 1);
   const int nb = n->nb, A = n->A, hist = cfg->history_length;
@@ -2751,8 +3036,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
       n->d_twes = n->d_wes;
     }
     B2_CHECK_CUDA(fmalloc(&n->d_weg, we));
-    B2_CHECK_CUDA(cudaMalloc(&n->d_tau_ctr, sizeof(unsigned long long)));
-    B2_CHECK_CUDA(cudaMemset(n->d_tau_ctr, 0, sizeof(unsigned long long)));
+    if (!n->fqf_n) {   // the FQF head draws nothing
+      B2_CHECK_CUDA(cudaMalloc(&n->d_tau_ctr, sizeof(unsigned long long)));
+      B2_CHECK_CUDA(cudaMemset(n->d_tau_ctr, 0, sizeof(unsigned long long)));
+    }
     B2_CHECK_CUDA(fmalloc(&n->d_tau, 2 * R));
     B2_CHECK_CUDA(fmalloc(&n->d_cos, 2 * R * kIqnCos));
     B2_CHECK_CUDA(fmalloc(&n->d_phi, 2 * R * kFlat));
@@ -2767,6 +3054,34 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     if (cfg->math_mode == B200DQN_MATH_TCGEN05) {
       B2_CHECK_CUDA(cudaMalloc(&n->d_x16, 4 * R * kFlat * sizeof(__half)));
       B2_CHECK_CUDA(cudaMemset(n->d_x16, 0, 4 * R * kFlat * sizeof(__half)));
+    }
+  }
+  if (n->fqf_n) {
+    const size_t N = size_t(n->fqf_n), wf = N * kFlat, Rb = size_t(nb) * (N - 1);
+    B2_CHECK_CUDA(fmalloc(&n->d_wf, wf));
+    B2_CHECK_CUDA(fmalloc(&n->d_wfs, wf * n->n_states));
+    if (cfg->target_steps) {
+      B2_CHECK_CUDA(fmalloc(&n->d_twf, wf));
+      B2_CHECK_CUDA(fmalloc(&n->d_twfs, wf * n->n_states));
+    } else {
+      n->d_twf = n->d_wf;
+      n->d_twfs = n->d_wfs;
+    }
+    B2_CHECK_CUDA(fmalloc(&n->d_wfg, wf));
+    B2_CHECK_CUDA(fmalloc(&n->d_fl, size_t(nb) * N));
+    B2_CHECK_CUDA(fmalloc(&n->d_fq, size_t(nb) * N));
+    B2_CHECK_CUDA(fmalloc(&n->d_ftau, size_t(nb) * (N + 1)));
+    B2_CHECK_CUDA(fmalloc(&n->d_fg, size_t(nb) * (N - 1)));
+    B2_CHECK_CUDA(fmalloc(&n->d_fdl, size_t(nb) * N));
+    B2_CHECK_CUDA(fmalloc(&n->d_btau, Rb));
+    B2_CHECK_CUDA(fmalloc(&n->d_bcos, Rb * kIqnCos));
+    B2_CHECK_CUDA(fmalloc(&n->d_bphi, Rb * kFlat));
+    B2_CHECK_CUDA(fmalloc(&n->d_bx, Rb * kFlat));
+    B2_CHECK_CUDA(fmalloc(&n->d_bh4, Rb * kHidden));
+    B2_CHECK_CUDA(fmalloc(&n->d_btheta, Rb * A));
+    if (cfg->math_mode == B200DQN_MATH_TCGEN05) {
+      B2_CHECK_CUDA(cudaMalloc(&n->d_bx16, 2 * Rb * kFlat * sizeof(__half)));
+      B2_CHECK_CUDA(cudaMemset(n->d_bx16, 0, 2 * Rb * kFlat * sizeof(__half)));
     }
   }
   const size_t state_bytes = size_t(nb) * hist * kFrameBytes;
@@ -2836,6 +3151,10 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_we); cudaFree(n->d_wes); cudaFree(n->d_weg); cudaFree(n->d_tau_ctr); cudaFree(n->d_tau);
   cudaFree(n->d_cos); cudaFree(n->d_phi); cudaFree(n->d_x); cudaFree(n->d_iqn_theta); cudaFree(n->d_iqn_tq);
   cudaFree(n->d_iqn_qgrad); cudaFree(n->d_dx); cudaFree(n->d_dphi); cudaFree(n->d_x16);
+  if (n->d_twf != n->d_wf) { cudaFree(n->d_twf); cudaFree(n->d_twfs); }
+  cudaFree(n->d_wf); cudaFree(n->d_wfs); cudaFree(n->d_wfg); cudaFree(n->d_fl); cudaFree(n->d_fq); cudaFree(n->d_ftau);
+  cudaFree(n->d_fg); cudaFree(n->d_fdl); cudaFree(n->d_btau); cudaFree(n->d_bcos); cudaFree(n->d_bphi); cudaFree(n->d_bx);
+  cudaFree(n->d_bh4); cudaFree(n->d_btheta); cudaFree(n->d_bx16);
   cudaFreeHost(n->h_pin);
   cudaFreeHost(const_cast<uint32_t*>(n->h_res));
   delete n;
@@ -2866,8 +3185,39 @@ static int xfer_we(b200dqn_net* n, float* dev_base, float* host, bool to_device,
 
 static bool is_we(const b200dqn_net* n, int layer) { return layer == kLayers && n->iqn_n; }
 
+// ABI layer 6, the FQF fraction layer: Neon W_f[k][n], n = fc1's input column in (c, p, q) order <-> internal
+// W_f[k][(p, q, c)]
+static int xfer_wf(b200dqn_net* n, float* dev_base, float* host, bool to_device, cudaStream_t st) {
+  const int64_t cnt = int64_t(n->fqf_n) * kFlat;
+  std::vector<float> tmp(cnt);
+  auto at = [](int64_t i) {
+    const int k = int(i / kFlat), nn = int(i % kFlat);
+    const int c = nn / 49, p = (nn / 7) % 7, q = nn % 7;
+    return int64_t(k) * kFlat + (p * 7 + q) * kC3 + c;
+  };
+  if (to_device) {
+    for (int64_t i = 0; i < cnt; ++i) tmp[at(i)] = host[i];
+    B2_CHECK_CUDA(cudaMemcpyAsync(dev_base, tmp.data(), cnt * sizeof(float), cudaMemcpyHostToDevice, st));
+    B2_CHECK_CUDA(cudaStreamSynchronize(st));
+  } else {
+    B2_CHECK_CUDA(cudaMemcpyAsync(tmp.data(), dev_base, cnt * sizeof(float), cudaMemcpyDeviceToHost, st));
+    B2_CHECK_CUDA(cudaStreamSynchronize(st));
+    for (int64_t i = 0; i < cnt; ++i) host[i] = tmp[at(i)];
+  }
+  return B200DQN_OK;
+}
+
+static bool is_wf(const b200dqn_net* n, int layer) { return layer == kLayers + 1 && n->fqf_n; }
+// a layer index valid on this net: the five of every net, the embedding (IQN, FQF), the fraction layer (FQF)
+static bool layer_ok(const b200dqn_net* n, int layer) { return layer >= 0 && (layer < kLayers || is_we(n, layer) || is_wf(n, layer)); }
+
 extern "C" int b200dqn_net_layer_shape(const b200dqn_net* n, int layer, int* rows, int* cols) {
-  B2_REQUIRE(n && layer >= 0 && (layer < kLayers || is_we(n, layer)), B200DQN_EINVAL, "net_layer_shape: bad layer");
+  B2_REQUIRE(n && layer_ok(n, layer), B200DQN_EINVAL, "net_layer_shape: bad layer");
+  if (layer == kLayers + 1) {
+    if (rows) *rows = n->fqf_n;
+    if (cols) *cols = kFlat;
+    return B200DQN_OK;
+  }
   if (layer == kLayers) {
     if (rows) *rows = kFlat;
     if (cols) *cols = kIqnCos;
@@ -2898,10 +3248,15 @@ static int xfer_params(b200dqn_net* n, float* dev_base, int layer, float* host, 
 
 extern "C" int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, const float* host_W,
                                        const float* host_S, void* stream) {
-  B2_REQUIRE(n && host_W && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1),
-             B200DQN_EINVAL, "net_set_weights: bad argument");
+  B2_REQUIRE(n && host_W && layer_ok(n, layer) && (which == 0 || which == 1), B200DQN_EINVAL,
+             "net_set_weights: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers + 1) {
+    B2_TRY(xfer_wf(n, which ? n->d_twf : n->d_wf, const_cast<float*>(host_W), true, st));
+    if (host_S) B2_TRY(xfer_wf(n, which ? n->d_twfs : n->d_wfs, const_cast<float*>(host_S), true, st));
+    return B200DQN_OK;
+  }
   if (layer == kLayers) {
     B2_TRY(xfer_we(n, which ? n->d_twe : n->d_we, const_cast<float*>(host_W), true, st));
     if (host_S) B2_TRY(xfer_we(n, which ? n->d_twes : n->d_wes, const_cast<float*>(host_S), true, st));
@@ -2915,10 +3270,14 @@ extern "C" int b200dqn_net_set_weights(b200dqn_net* n, int which, int layer, con
 
 extern "C" int b200dqn_net_get_weights(b200dqn_net* n, int which, int layer, float* host_W, float* host_S,
                                        void* stream) {
-  B2_REQUIRE(n && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1), B200DQN_EINVAL,
-             "net_get_weights: bad argument");
+  B2_REQUIRE(n && layer_ok(n, layer) && (which == 0 || which == 1), B200DQN_EINVAL, "net_get_weights: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers + 1) {
+    if (host_W) B2_TRY(xfer_wf(n, which ? n->d_twf : n->d_wf, host_W, false, st));
+    if (host_S) B2_TRY(xfer_wf(n, which ? n->d_twfs : n->d_wfs, host_S, false, st));
+    return B200DQN_OK;
+  }
   if (layer == kLayers) {
     if (host_W) B2_TRY(xfer_we(n, which ? n->d_twe : n->d_we, host_W, false, st));
     if (host_S) B2_TRY(xfer_we(n, which ? n->d_twes : n->d_wes, host_S, false, st));
@@ -2937,9 +3296,12 @@ extern "C" int b200dqn_net_num_states(const b200dqn_net* n, int* count) {
 }
 
 extern "C" int b200dqn_net_set_state(b200dqn_net* n, int which, int layer, int k, const float* host_S, void* stream) {
-  B2_REQUIRE(n && host_S && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1) && k >= 0 &&
-             k < n->n_states, B200DQN_EINVAL, "net_set_state: bad argument");
+  B2_REQUIRE(n && host_S && layer_ok(n, layer) && (which == 0 || which == 1) && k >= 0 && k < n->n_states,
+             B200DQN_EINVAL, "net_set_state: bad argument");
   DeviceGuard g(n->device);
+  if (layer == kLayers + 1)
+    return xfer_wf(n, (which ? n->d_twfs : n->d_wfs) + int64_t(k) * n->fqf_n * kFlat, const_cast<float*>(host_S), true,
+                   as_stream(stream));
   if (layer == kLayers)
     return xfer_we(n, (which ? n->d_twes : n->d_wes) + int64_t(k) * kIqnCos * kFlat, const_cast<float*>(host_S), true,
                    as_stream(stream));
@@ -2948,9 +3310,11 @@ extern "C" int b200dqn_net_set_state(b200dqn_net* n, int which, int layer, int k
 }
 
 extern "C" int b200dqn_net_get_state(b200dqn_net* n, int which, int layer, int k, float* host_S, void* stream) {
-  B2_REQUIRE(n && host_S && layer >= 0 && (layer < kLayers || is_we(n, layer)) && (which == 0 || which == 1) && k >= 0 &&
-             k < n->n_states, B200DQN_EINVAL, "net_get_state: bad argument");
+  B2_REQUIRE(n && host_S && layer_ok(n, layer) && (which == 0 || which == 1) && k >= 0 && k < n->n_states,
+             B200DQN_EINVAL, "net_get_state: bad argument");
   DeviceGuard g(n->device);
+  if (layer == kLayers + 1)
+    return xfer_wf(n, (which ? n->d_twfs : n->d_wfs) + int64_t(k) * n->fqf_n * kFlat, host_S, false, as_stream(stream));
   if (layer == kLayers)
     return xfer_we(n, (which ? n->d_twes : n->d_wes) + int64_t(k) * kIqnCos * kFlat, host_S, false, as_stream(stream));
   return xfer_params(n, (which ? n->d_ts : n->d_s) + int64_t(k) * n->n_params, layer, host_S, false, as_stream(stream));
@@ -2967,6 +3331,11 @@ extern "C" int b200dqn_net_sync_target(b200dqn_net* n, void* stream) {
     const size_t we = size_t(kIqnCos) * kFlat * sizeof(float);
     B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twe, n->d_we, we, cudaMemcpyDeviceToDevice, st));
     B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twes, n->d_wes, we * n->n_states, cudaMemcpyDeviceToDevice, st));
+  }
+  if (n->fqf_n) {   // and so is the fraction layer
+    const size_t wf = size_t(n->fqf_n) * kFlat * sizeof(float);
+    B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twf, n->d_wf, wf, cudaMemcpyDeviceToDevice, st));
+    B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twfs, n->d_wfs, wf * n->n_states, cudaMemcpyDeviceToDevice, st));
   }
   return umma_target_synced(n, st);
 }
@@ -3417,6 +3786,8 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_IQN_DPHI:
     case B200DQN_NET_PTR_IQN_TAU_COUNTER: {
       B2_REQUIRE(n->iqn_n, B200DQN_EINVAL, "net_device_ptr: selector %d needs an IQN head", which);
+      B2_REQUIRE(!(n->fqf_n && which == B200DQN_NET_PTR_IQN_TAU_COUNTER), B200DQN_EINVAL,
+                 "net_device_ptr: the FQF head draws nothing and has no counter");
       const size_t R = size_t(n->iqn_rows), nbn = size_t(n->nb) * n->iqn_n;
       switch (which) {
         case B200DQN_NET_PTR_IQN_TAUS: p = n->d_tau; b = 2 * R * 4; break;
@@ -3455,6 +3826,24 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
         default: p = n->d_rem_ctr; b = sizeof(unsigned long long); break;
       }
       break;
+    case B200DQN_NET_PTR_FQF_LOGITS:
+    case B200DQN_NET_PTR_FQF_PROBS:
+    case B200DQN_NET_PTR_FQF_FRACTIONS:
+    case B200DQN_NET_PTR_FQF_BOUNDARY_QUANTILES:
+    case B200DQN_NET_PTR_FQF_FRACTION_GRADS:
+    case B200DQN_NET_PTR_FQF_LOGIT_GRADS: {
+      B2_REQUIRE(n->fqf_n, B200DQN_EINVAL, "net_device_ptr: selector %d needs an FQF head", which);
+      const size_t nb = size_t(n->nb), N = size_t(n->fqf_n);
+      switch (which) {
+        case B200DQN_NET_PTR_FQF_LOGITS: p = n->d_fl; b = nb * N * 4; break;
+        case B200DQN_NET_PTR_FQF_PROBS: p = n->d_fq; b = nb * N * 4; break;
+        case B200DQN_NET_PTR_FQF_FRACTIONS: p = n->d_ftau; b = nb * (N + 1) * 4; break;
+        case B200DQN_NET_PTR_FQF_BOUNDARY_QUANTILES: p = n->d_btheta; b = nb * (N - 1) * n->A * 4; break;
+        case B200DQN_NET_PTR_FQF_FRACTION_GRADS: p = n->d_fg; b = nb * (N - 1) * 4; break;
+        default: p = n->d_fdl; b = nb * N * 4; break;
+      }
+      break;
+    }
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -3503,6 +3892,7 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   if (on) {
     B2_REQUIRE(!n->munchausen, B200DQN_EINVAL,
                "net_set_double_q: the Munchausen target makes no greedy choice for Double DQN to change");
+    B2_REQUIRE(!n->fqf_n, B200DQN_ENOTIMPL, "net_set_double_q: the Double DQN target with the FQF head is not implemented");
     B2_REQUIRE(!n->iqn_n, B200DQN_ENOTIMPL, "net_set_double_q: the Double DQN target with the IQN head is not implemented");
     B2_REQUIRE(!n->nccl_comm, B200DQN_ENOTIMPL,
                "net_set_double_q: the Double DQN target is implemented for a single learner only (comm_init has run)");
@@ -3515,10 +3905,10 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
 }
 
 extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream) {
-  B2_REQUIRE(n && host_dW && layer >= 0 && (layer < kLayers || is_we(n, layer)), B200DQN_EINVAL,
-             "net_get_grads: bad argument");
+  B2_REQUIRE(n && host_dW && layer_ok(n, layer), B200DQN_EINVAL, "net_get_grads: bad argument");
   DeviceGuard g(n->device);
   cudaStream_t st = as_stream(stream);
+  if (layer == kLayers + 1) return xfer_wf(n, n->d_wfg, host_dW, false, st);   // written whole by k_fqf_wf
   if (layer == kLayers) return xfer_we(n, n->d_weg, host_dW, false, st);   // written whole by k_iqn_we
   const int64_t n4 = n->n_params / 4;
   if (n->world == 1) {  // partials of the last step are still in scratch; sum them into d_g
@@ -3552,9 +3942,11 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
     // target with a separate target network repeats the forward's launches for its pass
     // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient;
-    // random-shift augmentation and the REM head add their draws
+    // random-shift augmentation and the REM head add their draws; an FQF head replaces the tau draw by the fraction
+    // proposal and adds the boundary pass (phi, the modulation, fc1 and fc2) and the fraction layer's gradient
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
-                (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->crop_pad ? 1 : 0) +
+                (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->fqf_n ? 5 : 0) +
+                (n->crop_pad ? 1 : 0) +
                 (n->rem_k ? 1 : 0) +
                 (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
   }

@@ -175,6 +175,28 @@ struct b200dqn_net {
   // rows one fc1 / fc2 pass runs at for `rows` samples: rows N in a train step, rows K on predict
   int expanded(int rows, bool train) const { return iqn_n ? rows * (train ? iqn_n : iqn_k) : rows; }
 
+  // fully parameterized quantile function head (cfg.num_fractions > 0): an IQN net (iqn_n = iqn_k = N) whose tau is the
+  // fraction proposal tauhat instead of a draw (d_tau_ctr stays unallocated), plus the fraction layer and the boundary
+  // pass at tau_1..tau_{N-1}, which runs phi, X, fc1 and fc2 on buffers of its own (nb (N - 1) rows)
+  int fqf_n = 0;                 // N
+  float* d_wf = nullptr;         // online fraction layer [N][3136] (internal column order); d_wfs: its n_states planes
+  float* d_wfs = nullptr;
+  float* d_twf = nullptr;        // target fraction layer and states (== d_wf / d_wfs when target_steps == 0)
+  float* d_twfs = nullptr;
+  float* d_wfg = nullptr;        // dW_f of the last train step
+  float* d_fl = nullptr;         // [nb][N] logits l
+  float* d_fq = nullptr;         // [nb][N] proposal q
+  float* d_ftau = nullptr;       // [nb][N + 1] fractions tau
+  float* d_fg = nullptr;         // [nb][N - 1] fraction gradient g
+  float* d_fdl = nullptr;        // [nb][N] logit gradient dl
+  float* d_btau = nullptr;       // boundary pass, rows nb (N - 1): tau_1..tau_{N-1}, c, phi, X, H4, theta_bnd
+  float* d_bcos = nullptr;
+  float* d_bphi = nullptr;
+  float* d_bx = nullptr;
+  float* d_bh4 = nullptr;
+  float* d_btheta = nullptr;
+  __half* d_bx16 = nullptr;      // tensor-core engine: fp16 planes of the boundary X [hi | lo]
+
   // random-shift augmentation (cfg.random_shift > 0; nothing below is allocated otherwise): every train step draws
   // crop offsets on the device and conv1 reads its frames through them
   int crop_pad = 0;                       // p

@@ -1257,6 +1257,16 @@ int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_
   return umma2::launch_umma2("fc1_fwd", p, kHidden, rows, nets * splits, st, false);
 }
 
+int umma_fc1_fwd_fqf_boundary(b200dqn_net* n, int rows, int splits, cudaStream_t st) {
+  UmmaState* u = ust(n);
+  V2Fc1Fwd<kHidden> p;   // the online network only (nets = 1)
+  p.wimg[0] = p.wimg[1] = u->img_fwd[0][3];
+  const PlanePair x{n->d_bx16, int64_t(n->nb) * (n->fqf_n - 1) * kFlat};
+  for (int z = 0; z < 3; ++z) p.in16[z] = x;
+  p.part = n->d_fc1part; p.rows = rows; p.splits = splits;
+  return umma2::launch_umma2("fc1_fwd", p, kHidden, rows, splits, st, false);
+}
+
 // The Munchausen target pass: umma_forward's launches with one network slot (nets = 1) and remapped pointers.  Device
 // slot 0 reads the target network's weight images and the prestates (slot 0's frames) and writes the third slot's
 // fp16 planes and fc1 partials; no fp32 activation is kept.  The kernels specialise slot 0 in two places: conv1_fwd

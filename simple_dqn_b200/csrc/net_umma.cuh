@@ -28,6 +28,8 @@ int umma_forward(b200dqn_net* n, const uint8_t* const src[2], const int32_t* con
                  bool trunk_only = false);
 // IQN head: fc1's forward on the modulated rows X (n->d_x16 planes) at `rows` expanded rows with `splits` k-splits
 int umma_fc1_fwd_iqn(b200dqn_net* n, int nets, int rows, int splits, cudaStream_t st);
+// FQF head: the online network's fc1 forward on the boundary pass's X planes (n->d_bx16) at `rows` rows
+int umma_fc1_fwd_fqf_boundary(b200dqn_net* n, int rows, int splits, cudaStream_t st);
 int umma_fc1_splits(int rows);
 // the Munchausen target pass: the target network on the frames src/idx/shift (the prestates), into slot 2's planes and
 // fc1 partials (nets = 1, no fp32 activations); crop: the prestates' crop offsets (slot 0's), or nullptr

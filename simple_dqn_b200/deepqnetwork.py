@@ -150,6 +150,16 @@ class DeepQNetwork:
             cfg.num_heads = int(_arg(args, "num_heads", 200))
             assert cfg.num_heads >= 1, "num_heads %d: the REM head needs 1..200" % cfg.num_heads
             cfg.rem_seed = self.rem_seed = rem_seed(_arg(args, "random_seed", None))
+        # fully parameterized quantile function head (FQF, Yang et al., 2019): a new capability, off unless args.fqf is
+        # set; N = num_fractions (32) fractions per sample, proposed from the online network's conv3 output by a seventh
+        # layer W_f trained at fraction_lr (this project's default 2.5e-9).  It is an IQN net whose tau is the proposal
+        # (no draw, no seed).  Fixed here, like the other heads.
+        self.fqf = bool(_arg(args, "fqf", False))
+        self.num_fractions = 0
+        if self.fqf:
+            cfg.num_fractions = int(_arg(args, "num_fractions", 32))
+            cfg.fraction_lr = float(_arg(args, "fraction_lr", 2.5e-9))
+            assert cfg.num_fractions >= 2, "num_fractions %d: the FQF head needs 2..64" % cfg.num_fractions
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -162,16 +172,20 @@ class DeepQNetwork:
             self.tau_seed = cfg.tau_seed
         if self.rem:
             self.num_heads = cfg.num_heads
+        if self.fqf:   # the IQN accessors read its rows: N = K = num_fractions
+            self.num_fractions = self.num_tau_samples = self.num_quantile_samples = cfg.num_fractions
+            self.fraction_lr = cfg.fraction_lr
         if self.quantile_regression:
             self.num_quantiles = n = cfg.num_quantiles                 # tau_i = (2i + 1) / 2N in fp64, as the device
             self.taus = np.array([(2 * i + 1) / (2 * n) for i in range(n)], dtype=np.float64).astype(np.float32)
 
         # model.initialize (:49, :70): Xavier draws from one numpy RandomState(random_seed) —
         # online layers first, then the separately-initialised target model.  An IQN embedding is drawn after fc2 of
-        # its network, with fan_in 64.
+        # its network, with fan_in 64.  The FQF fraction layer takes no draw and stays zero: the first proposal is
+        # uniform, and layers 0-5 are drawn as on an IQN net.
         rng = np.random.RandomState(_arg(args, "random_seed", None))
         for which in ((0, 1) if cfg.target_steps else (0,)):
-            for layer, shp in enumerate(self.layer_shapes()):
+            for layer, shp in enumerate(self.layer_shapes()[:6]):
                 fan_in = shp[0] if layer < 3 else shp[1]               # Xavier(local=True / False) (:79-80)
                 scale = np.sqrt(3.0 / fan_in)
                 w = rng.uniform(-scale, scale, shp).astype(np.float32)
@@ -195,7 +209,7 @@ class DeepQNetwork:
     # ---- weights in Neon layout
     def layer_shapes(self):
         out = []
-        for layer in range(6 if self.implicit_quantiles else 5):
+        for layer in range(7 if self.fqf else 6 if self.implicit_quantiles else 5):
             r, c = C.c_int(), C.c_int()
             L.call("b200dqn_net_layer_shape", self._h, layer, C.byref(r), C.byref(c))
             out.append((r.value, c.value))
@@ -375,6 +389,33 @@ class DeepQNetwork:
     def last_iqn_quantile_grads(self):
         """The gradient dtheta on the taken action of each online row of the last train(), (batch, N) float32."""
         return self._read_f32(L.NET_PTR_IQN_QUANTILE_GRADS, (self.batch_size, self.num_tau_samples))
+
+    # ---- fully parameterized quantile function head (fqf = True).  Its rows are the IQN head's at N = K = num_fractions:
+    # last_taus() holds tauhat
+    def last_fraction_logits(self):
+        """The fraction logits l of the last forward, (batch, N) float32."""
+        return self._read_f32(L.NET_PTR_FQF_LOGITS, (self.batch_size, self.num_fractions))
+
+    def last_fraction_probs(self):
+        """The proposal q = softmax(l) of the last forward, (batch, N) float32."""
+        return self._read_f32(L.NET_PTR_FQF_PROBS, (self.batch_size, self.num_fractions))
+
+    def last_fractions(self):
+        """The fractions tau_0 = 0 < ... < tau_N = 1 of the last forward, (batch, N + 1) float32."""
+        return self._read_f32(L.NET_PTR_FQF_FRACTIONS, (self.batch_size, self.num_fractions + 1))
+
+    def last_boundary_quantiles(self):
+        """The online network's theta at tau_1..tau_{N-1} of the last train(), (batch, N - 1, A) float32."""
+        return self._read_f32(L.NET_PTR_FQF_BOUNDARY_QUANTILES,
+                              (self.batch_size, self.num_fractions - 1, self.num_actions))
+
+    def last_fraction_grads(self):
+        """The fraction gradient g_1..g_{N-1} of the last train(), (batch, N - 1) float32."""
+        return self._read_f32(L.NET_PTR_FQF_FRACTION_GRADS, (self.batch_size, self.num_fractions - 1))
+
+    def last_fraction_logit_grads(self):
+        """The logit gradient dl of the last train(), (batch, N) float32."""
+        return self._read_f32(L.NET_PTR_FQF_LOGIT_GRADS, (self.batch_size, self.num_fractions))
 
     def _iqn_rows(self):
         return self.batch_size * max(self.num_tau_samples, self.num_quantile_samples)
@@ -558,7 +599,10 @@ class DeepQNetwork:
             ls = d["layer_params_states"]
         else:
             ls = [l for l in d["model"]["config"]["layers"] if "params" in l]
-        if self.implicit_quantiles:
+        if self.fqf:
+            assert len(ls) == 7, ("checkpoint holds %d weight layers; an FQF net needs seven: the five of "
+                                  "deepqnetwork.py:77-92, the tau embedding and the fraction layer" % len(ls))
+        elif self.implicit_quantiles:
             assert len(ls) == 6, ("checkpoint holds %d weight layers; an IQN net needs six: the five of "
                                   "deepqnetwork.py:77-92 and the tau embedding" % len(ls))
         else:

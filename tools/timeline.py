@@ -17,6 +17,7 @@ IQN = int(os.environ.get("IQN", "0"))   # IQN head with this many tau samples pe
 IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per predict row
 SHIFT = int(os.environ.get("SHIFT", "0"))   # random-shift augmentation with this pad p (DrQ: 4); 0: off
 REM = int(os.environ.get("REM", "0"))   # random ensemble mixture head (REM) with this many heads per action; 0: off
+FQF = int(os.environ.get("FQF", "0"))   # FQF head with this many fractions per sample; 0: off
 
 
 def net_args():
@@ -28,6 +29,7 @@ def net_args():
     a.implicit_quantiles, a.num_tau_samples, a.num_quantile_samples = IQN > 0, IQN, IQN_K
     a.random_shift = SHIFT
     a.rem, a.num_heads = REM > 0, REM
+    a.fqf, a.num_fractions = FQF > 0, FQF
     return a
 
 
