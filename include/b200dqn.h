@@ -430,6 +430,42 @@ typedef struct b200dqn_net_config {
    *       from the fraction loss. */
   int num_fractions;
   double fraction_lr;
+  /* Bootstrapped DQN heads (Osband, Blundell, Pritzel and Van Roy, 2016; new capability, no reference counterpart), off
+   * when bootstrap_heads = 0 (the default).  Otherwise K = bootstrap_heads in 1..200 Q-value heads per action on the
+   * shared network, each trained on its own target and masked by its own bootstrap mask, with mask probability p =
+   * bootstrap_p, finite, in (0, 1].  A bad K or p is EINVAL before any device work, as are num_atoms, num_quantiles,
+   * num_tau_samples, num_heads or num_fractions beside it (a net has one head); ENOTIMPL with dueling or munchausen.
+   * b200dqn_net_comm_init returns ENOTIMPL on such a net, and the DELTAS, REM_ALPHAS and REM_COUNTER selectors are
+   * EINVAL; REM_HEADS and REM_GRADS read theta and dtheta.  With p < 1, b200dqn_net_train and b200dqn_net_train_device
+   * return ENOTIMPL (their rows are no ring slots, so they carry no mask); at p = 1 they train.  Every fp32 operation
+   * below is rounded on its own (no contraction) unless marked fp64; b is the sample, a the taken action, z the slot
+   * (0 online on the prestates, 1 target on the poststates, 2 online on the poststates under Double DQN), i the ring
+   * slot the step reads the sample's transition from:
+   *    1. masks: m_k(b) = [double(u) < p] with u = (2 (h >> 9) + 1) 2^-24, h the high 32 bits of
+   *         x = mix(mix(bootstrap_seed + 0x9E3779B97F4A7C15 (i + 1)) ^ k)
+   *       (the REM head's draw at counter i).  The mask belongs to the ring slot: every step that draws slot i, on any
+   *       entry point, in any graph replay, sees the same mask; at p = 1 every mask is 1;
+   *    2. fc2: theta[z][b][a K + k] as the REM head's rule 2 (Neon shape (A K, 512));
+   *    3. per-head targets: a*_k = the first maximum over a of slot 1's theta[a K + k] (slot 2's with Double DQN);
+   *       y_k = R + g theta[1][b][a*_k K + k] (one fused multiply-add on the one-step step, a separately rounded
+   *       product and sum on the n-step step, R at a terminal) with the scalar head's clipped (or n-step) return R and
+   *       g, target_k = float(y_k), delta_k = theta[0][b][a K + k] - target_k;
+   *    4. loss: row cost = (sum_k m_k 0.5 delta_k delta_k in k order) / float(K), times the importance weight w on a
+   *       prioritized ring, whose TD error is (sum_k |delta_k| in k order) / float(K) over every head, masked or not;
+   *       d_k = clamp(delta_k, -clip_error, clip_error) (no clip when clip_error = 0), times w on a prioritized ring;
+   *       dtheta[a][k] = m_k ? d_k : 0 at the taken action, 0 for every other action;
+   *    5. backward: dZ4[t] = H4[t] > 0 ? (sum_k W5[t][a K + k] dtheta_k in k order) / float(K) : 0 (the gradient
+   *       entering the shared network is the mean over the heads), with the fp16 planes every head writes; fc2's
+   *       per-row partials are H4[t] dtheta_k, summed as for the REM head (block width K), then the configured
+   *       optimizer applies them;
+   *    6. the Q rows of a train step are rule 7's at h = -1 (nothing in the step reads them);
+   *    7. predict at the active head h (a device-resident int32, -1 after creation): h = -1 gives Q[a] = (sum_k
+   *       theta[a][k] in k order) / float(K), the REM head's predict Q; h >= 0 gives Q[a] = theta[a][h].  A predict
+   *       enqueued after b200dqn_net_set_active_head sees its h, on every predict entry point, including a replay
+   *       of the captured fast-path graph, which is not recaptured. */
+  int bootstrap_heads;
+  double bootstrap_p;
+  uint64_t bootstrap_seed;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -595,7 +631,12 @@ enum {
   B200DQN_NET_PTR_FQF_FRACTIONS,    /* (batch, N + 1) f32 the fractions tau_0 = 0 .. tau_N = 1                       */
   B200DQN_NET_PTR_FQF_BOUNDARY_QUANTILES, /* (batch (N - 1), A) f32 theta_bnd of the last train step                 */
   B200DQN_NET_PTR_FQF_FRACTION_GRADS,     /* (batch, N - 1) f32 the fraction gradient g of the last train step       */
-  B200DQN_NET_PTR_FQF_LOGIT_GRADS         /* (batch, N) f32 the logit gradient dl of the last train step             */
+  B200DQN_NET_PTR_FQF_LOGIT_GRADS,        /* (batch, N) f32 the logit gradient dl of the last train step             */
+  /* Bootstrapped heads only (bootstrap_heads > 0; EINVAL otherwise).  REM_HEADS and REM_GRADS read theta and dtheta. */
+  B200DQN_NET_PTR_BOOT_MASKS,       /* (batch, K) u8 the bootstrap masks m_k of the last train step                  */
+  B200DQN_NET_PTR_BOOT_TARGETS,     /* (batch, K) f32 the per-head targets float(y_k) of the last train step         */
+  B200DQN_NET_PTR_BOOT_DELTAS,      /* (batch, K) f32 the per-head TD errors delta_k of the last train step          */
+  B200DQN_NET_PTR_BOOT_ACTIVE_HEAD  /* i32 the head predict acts on (-1: the mean over the heads)                    */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well
@@ -609,6 +650,11 @@ int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep);
  * (synchronises the device).  Captured step graphs are rebuilt.  ENOTIMPL once b200dqn_net_comm_init has run;
  * b200dqn_net_comm_init returns ENOTIMPL while it is on.  EINVAL on a net with the Munchausen target. */
 int b200dqn_net_set_double_q(b200dqn_net* n, int on);
+/* The head predict acts on, on a net with bootstrapped heads: h in 0..K-1 picks head h, h = -1 the mean over the heads.
+ * The word lives on the device and is written in stream order: a predict enqueued on `stream` after this call sees h,
+ * one enqueued before does not, and a captured fast-path predict graph reads it at every replay.  EINVAL for h outside
+ * -1..K-1 and on a net without bootstrapped heads.  Asynchronous. */
+int b200dqn_net_set_active_head(b200dqn_net* n, int h, void* stream);
 /* Last summed gradient of `layer` converted to NEON layout (tests).  Synchronises. */
 int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream);
 /* Number of kernels one fused train step launches (bench.py's gpu_launches). */

@@ -21,7 +21,8 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
  NET_PTR_IQN_X, NET_PTR_IQN_QUANTILES, NET_PTR_IQN_TARGET_QUANTILES, NET_PTR_IQN_QUANTILE_GRADS, NET_PTR_IQN_DX,
  NET_PTR_IQN_DPHI, NET_PTR_IQN_TAU_COUNTER, NET_PTR_SHIFT_OFFSETS, NET_PTR_SHIFT_DRAWS, NET_PTR_REM_HEADS,
  NET_PTR_REM_ALPHAS, NET_PTR_REM_GRADS, NET_PTR_REM_COUNTER, NET_PTR_FQF_LOGITS, NET_PTR_FQF_PROBS,
- NET_PTR_FQF_FRACTIONS, NET_PTR_FQF_BOUNDARY_QUANTILES, NET_PTR_FQF_FRACTION_GRADS, NET_PTR_FQF_LOGIT_GRADS) = range(50)
+ NET_PTR_FQF_FRACTIONS, NET_PTR_FQF_BOUNDARY_QUANTILES, NET_PTR_FQF_FRACTION_GRADS, NET_PTR_FQF_LOGIT_GRADS,
+ NET_PTR_BOOT_MASKS, NET_PTR_BOOT_TARGETS, NET_PTR_BOOT_DELTAS, NET_PTR_BOOT_ACTIVE_HEAD) = range(54)
 
 
 class B200DQNError(RuntimeError):
@@ -41,7 +42,8 @@ class NetConfig(C.Structure):
                 ("munchausen_clip", C.c_double), ("num_tau_samples", C.c_int), ("num_quantile_samples", C.c_int),
                 ("tau_seed", C.c_uint64), ("random_shift", C.c_int), ("shift_seed", C.c_uint64),
                 ("num_heads", C.c_int), ("rem_seed", C.c_uint64),
-                ("num_fractions", C.c_int), ("fraction_lr", C.c_double)]
+                ("num_fractions", C.c_int), ("fraction_lr", C.c_double),
+                ("bootstrap_heads", C.c_int), ("bootstrap_p", C.c_double), ("bootstrap_seed", C.c_uint64)]
 
 
 _P = C.c_void_p
@@ -113,6 +115,7 @@ SIGNATURES = {
     "b200dqn_net_device_ptr": [_P, C.c_int, C.POINTER(_P), C.POINTER(C.c_size_t)],
     "b200dqn_net_set_keep_grads": [_P, C.c_int],
     "b200dqn_net_set_double_q": [_P, C.c_int],
+    "b200dqn_net_set_active_head": [_P, C.c_int, _P],
     "b200dqn_net_get_grads": [_P, C.c_int, _P, _P],
     "b200dqn_net_launches_per_step": [_P, C.POINTER(C.c_int)],
     "b200dqn_debug_trace": [_P, C.c_int],

@@ -1177,6 +1177,162 @@ k_head_rem(const float* __restrict__ theta, int ld, int nets, const float* __res
   kt_end(kt);
 }
 
+// ------------------------------------------------------------------------------------------
+// Bootstrapped DQN heads (Osband, Blundell, Pritzel and Van Roy 2016; b200dqn.h has the rules).  The REM head's K-headed
+// fc2 (k_fc2_dist, and k_opt_fc2_dist with K as the block width, both unchanged) with one TD step per head in place of
+// the mixture.  The new kernels:
+//   k_head_boot      one CTA per sample: the masks of the sample's ring slot, each head's target, delta and masked
+//                    gradient, the mean-over-heads Q rows, dZ4 (+ fp16 planes) and the compact dW5 row partial [512][K]
+//   k_boot_predict   one CTA per row: Q at the device-resident active head, or the mean over the heads
+//   k_boot_set_head  one thread: writes the active head in stream order
+// No expf / logf: every stage is +, -, *, / and comparisons, each rounded on its own.
+// ------------------------------------------------------------------------------------------
+struct BootArgs {
+  unsigned long long seed;
+  double p;             // the mask probability
+  uint8_t* mask;        // [ld][K] m_k
+  float* y;             // [ld][K] float(y_k)
+  float* delta;         // [ld][K] delta_k
+  float* grad;          // [ld][K] dtheta on the taken action's heads
+  int32_t* act_rows;    // [ld]
+};
+
+// One CTA (512 threads) per sample b of a train step.  Thread k < K hashes head k's mask from the ring slot midx[b]
+// (before the dependency wait: it depends on the sampler alone, as the TD scalars do) and runs head k's TD step;
+// thread r < nets * A writes the Q row (slot z, action a) as the mean over the heads; thread 0 sums the row cost and
+// the TD error; every thread forms its dZ4 element and a stride of the dW5 row partial.
+template <int kSlots, bool kNstep>
+__global__ void __launch_bounds__(kHidden)
+k_head_boot(const float* __restrict__ theta, int ld, int nets, const float* __restrict__ h4_online,
+            const float* __restrict__ w5_online, float* q_online, float* q_target, float* q_online_post, int A, int K,
+            const BootArgs ba, const HeadTrainArgs td, const KTrace kt) {
+  static_assert(kSlots == 2 || kSlots == 3, "online + target, or Double DQN's three slots");
+  __shared__ float s_h4[kHidden], s_g[kMaxRemHeads], s_c[kMaxRemHeads], s_e[kMaxRemHeads];
+  __shared__ double s_ret, s_gam;
+  __shared__ int s_a, s_term;
+  const int b = blockIdx.x, t = threadIdx.x, ncols = A * K;
+  kt_begin(kt);
+  int td_a = 0, td_term = 0;
+  int64_t td_r = 0;
+  double td_ret = 0.0, td_g = 1.0;
+  head_td_scalars<kNstep>(td, b, t, td_a, td_r, td_term, td_ret, td_g);
+  bool m = false;
+  if (t < K) {   // u = (2 (h >> 9) + 1) 2^-24 from the REM draw's hash at counter value midx[b]; exact in fp64
+    const unsigned long long slot = (unsigned long long)td.midx[b];
+    const unsigned long long base = iqn_mix(ba.seed + 0x9E3779B97F4A7C15ull * (slot + 1ull));
+    const unsigned h = unsigned(iqn_mix(base ^ (unsigned long long)unsigned(t)) >> 32);
+    m = __dmul_rn(double(2u * (h >> 9) + 1u), 5.9604644775390625e-08) < ba.p;
+  }
+  pdl_wait();
+  pdl_launch_dependents();
+  s_h4[t] = h4_online[b * kHidden + t];
+  if (t < nets * A) {
+    const int z = t / A, a = t % A;
+    const float* th = theta + (int64_t(z) * ld + b) * ncols + a * K;
+    float s = 0.f;
+    for (int k = 0; k < K; ++k) s = __fadd_rn(s, th[k]);
+    (z == 0 ? q_online : z == 2 ? q_online_post : q_target)[b * A + a] = __fdiv_rn(s, float(K));
+  }
+  if (t == 0) {
+    if constexpr (kNstep) {
+      s_ret = td_ret;
+      s_gam = td_g;
+    } else {
+      s_ret = fmin(fmax(double(td_r), td.min_reward), td.max_reward);   // np.clip as the scalar head
+      s_gam = td.discount;
+    }
+    s_term = td_term;
+    s_a = td_a;
+    ba.act_rows[b] = td_a;
+  }
+  __syncthreads();
+  const int a = s_a;
+  if (t < K) {   // head k = t: a*_k over slot 1's (slot 2's) column k, y_k, delta_k, the masked clipped gradient
+    const float* th1 = theta + (int64_t(ld) + b) * ncols + t;
+    const float* thc = kSlots == 3 ? theta + (int64_t(2) * ld + b) * ncols + t : th1;
+    int best = 0;
+    for (int j = 1; j < A; ++j)
+      if (thc[j * K] > thc[best * K]) best = j;
+    const double maxq = double(th1[best * K]);
+    double y;
+    if constexpr (kNstep) y = s_term ? s_ret : __dadd_rn(s_ret, __dmul_rn(s_gam, maxq));
+    else y = s_term ? s_ret : __fma_rn(s_gam, maxq, s_ret);
+    const float target = static_cast<float>(y);
+    const float dl = __fsub_rn(theta[int64_t(b) * ncols + a * K + t], target);
+    float d = dl;
+    if (td.clip > 0.f) d = fminf(fmaxf(d, -td.clip), td.clip);
+    if (td.isw) d = __fmul_rn(d, td.isw[b]);
+    const float g = m ? d : 0.f;
+    s_c[t] = m ? __fmul_rn(__fmul_rn(0.5f, dl), dl) : 0.f;
+    s_e[t] = fabsf(dl);
+    s_g[t] = g;
+    ba.mask[b * K + t] = m ? 1 : 0;
+    ba.y[b * K + t] = target;
+    ba.delta[b * K + t] = dl;
+    ba.grad[b * K + t] = g;
+  }
+  __syncthreads();
+  if (t == 0) {   // the row cost over the unmasked heads and the TD error over every head, k order, then / K
+    float c = 0.f, e = 0.f;
+    for (int k = 0; k < K; ++k) {
+      c = __fadd_rn(c, s_c[k]);
+      e = __fadd_rn(e, s_e[k]);
+    }
+    c = __fdiv_rn(c, float(K));
+    if (td.isw) {
+      td.td_err[b] = __fdiv_rn(e, float(K));
+      c = __fmul_rn(td.isw[b], c);
+    }
+    td.row_cost[b] = c;
+  }
+  {   // the shared network's gradient is the mean over the heads; the heads get their full dtheta
+    const float hv = s_h4[t];
+    const float* w = w5_online + int64_t(t) * ncols + a * K;
+    float o = 0.f;
+    if (hv > 0.f) {
+      for (int k = 0; k < K; ++k) o = __fadd_rn(o, __fmul_rn(w[k], s_g[k]));
+      o = __fdiv_rn(o, float(K));
+    }
+    td.dz4[b * kHidden + t] = o;
+    if (td.dz4_hi) {
+      const __half hh = __float2half_rn(o);
+      const __half ll = __float2half_rn((o - __half2float(hh)) * 2048.0f);
+      td.dz4_hi[b * kHidden + t] = hh;
+      td.dz4_hi[td.dz4_lo_off + b * kHidden + t] = ll;
+    }
+  }
+  float* dw = td.dw5_rows + int64_t(b) * kHidden * K;
+  for (int e = t; e < kHidden * K; e += kHidden) dw[e] = __fmul_rn(s_h4[e / K], s_g[e % K]);
+  kt_end(kt);
+}
+
+// One CTA of 32 threads per predict row b; thread a < A writes Q[b][a] at the active head read at run time, so a
+// captured predict graph follows b200dqn_net_set_active_head without recapture.  h = -1: k_head_qr<1, false>'s mean.
+__global__ void __launch_bounds__(32)
+k_boot_predict(const float* __restrict__ theta, int A, int K, const int32_t* __restrict__ head, float* q,
+               const KTrace kt) {
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  const int b = blockIdx.x, a = threadIdx.x;
+  if (a < A) {
+    const int h = *head;
+    const float* th = theta + (int64_t(b) * A + a) * K;
+    float v;
+    if (h >= 0) {
+      v = th[h];
+    } else {
+      float s = 0.f;
+      for (int k = 0; k < K; ++k) s = __fadd_rn(s, th[k]);
+      v = __fdiv_rn(s, float(K));
+    }
+    q[b * A + a] = v;
+  }
+  kt_end(kt);
+}
+
+__global__ void k_boot_set_head(int32_t* head, int h) { *head = h; }
+
 // grid (cdiv(rows, 16), nets).  c[r][i] = float(cos((pi i) tau_r)) in fp64, stored for the embedding's gradient; then
 // thread t takes columns t, t + 256, ... and accumulates the CTA's 16 rows of column col in i order.
 __global__ void __launch_bounds__(256)
@@ -2037,6 +2193,23 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
                              (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
                              w[0] + lt.off[4], w[1] + lt.off[4], n->d_theta, ncols, ktrace_slot("fc2_dist")));
     B2_PROF("fc2_dist", st);
+    if (!td.enable && n->boot) {   // predict at the active head, read on the device
+      B2_CHECK_CUDA(launch_pdl(k_boot_predict, dim3(rows), dim3(32), 0, st, (const float*)n->d_theta, n->A, n->rem_k,
+                               (const int32_t*)n->d_boot_head, n->d_q[0], ktrace_slot("boot_predict")));
+      B2_PROF("boot_predict", st);
+      return B200DQN_OK;
+    }
+    if (n->boot) {
+      const BootArgs ba{(unsigned long long)n->cfg.bootstrap_seed, n->cfg.bootstrap_p, n->d_boot_mask, n->d_boot_y,
+                        n->d_boot_delta, n->d_rem_grad, n->d_act_rows};
+      auto* kern = nets == 3 ? (nstep ? k_head_boot<3, true> : k_head_boot<3, false>)
+                             : (nstep ? k_head_boot<2, true> : k_head_boot<2, false>);
+      B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
+                               (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A,
+                               n->rem_k, ba, td, ktrace_slot("head_boot")));
+      B2_PROF("head_boot(td+fc2_bwd)", st);
+      return B200DQN_OK;
+    }
     if (!td.enable) {   // predict: the mean over the K heads, the quantile-regression head's Q
       const QrArgs qa{n->rem_k, 0.f, nullptr, nullptr, nullptr};
       B2_CHECK_CUDA(launch_pdl(k_head_qr<1, false>, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb,
@@ -2705,7 +2878,7 @@ static int train_step(b200dqn_net* n, const FrameSource& fs_in, const uint8_t* a
       B2_TRY(forward_target_pre(n, fs, rows, st));
     }
   }
-  if (n->rem_k) {
+  if (n->rem_k && !n->boot) {
     // The mixture draw reads only its counter, so on a stream it runs on its own branch from here and joins before the
     // head; on the serial schedule it runs in line, ahead of the forward.
     const bool branch = n->use_branches && st != nullptr && !g_prof_on;
@@ -2799,6 +2972,9 @@ extern "C" int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actio
   cfg->rem_seed = 0;
   cfg->num_fractions = 0;        // no FQF head
   cfg->fraction_lr = 2.5e-9;
+  cfg->bootstrap_heads = 0;      // no bootstrapped heads; this project's mask probability when they are on
+  cfg->bootstrap_p = 0.5;
+  cfg->bootstrap_seed = 0;
   return B200DQN_OK;
 }
 
@@ -2892,6 +3068,19 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
                "net_create: the FQF head with a dueling network or the Munchausen target is not implemented");
   }
+  B2_REQUIRE(cfg->bootstrap_heads >= 0 && cfg->bootstrap_heads <= kMaxRemHeads, B200DQN_EINVAL,
+             "net_create: bootstrap_heads %d is neither 0 (no bootstrapped heads) nor in [1,%d]", cfg->bootstrap_heads,
+             kMaxRemHeads);
+  if (cfg->bootstrap_heads) {
+    B2_REQUIRE(std::isfinite(cfg->bootstrap_p) && cfg->bootstrap_p > 0 && cfg->bootstrap_p <= 1, B200DQN_EINVAL,
+               "net_create: the bootstrap mask probability bootstrap_p must be in (0, 1] (got %g)", cfg->bootstrap_p);
+    B2_REQUIRE(!cfg->num_atoms && !cfg->num_quantiles && !cfg->num_tau_samples && !cfg->num_heads &&
+               !cfg->num_fractions, B200DQN_EINVAL,
+               "net_create: bootstrap_heads with num_atoms, num_quantiles, num_tau_samples, num_heads or num_fractions "
+               "asks for two heads; a net has one");
+    B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
+               "net_create: bootstrapped heads with a dueling network or the Munchausen target are not implemented");
+  }
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -2904,6 +3093,10 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   n->atoms = cfg->num_atoms;
   n->quantiles = cfg->num_quantiles;
   n->rem_k = cfg->num_heads;
+  if (cfg->bootstrap_heads) {   // the REM head's K-headed fc2 and buffers, trained per head
+    n->rem_k = cfg->bootstrap_heads;
+    n->boot = true;
+  }
   n->dueling = cfg->dueling != 0;
   n->munchausen = cfg->munchausen != 0;
   n->hidden = n->dueling ? kDuelHidden : kHidden;
@@ -3008,10 +3201,19 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   if (n->rem_k) {
     B2_CHECK_CUDA(fmalloc(&n->d_theta, size_t(3) * nb * A * n->rem_k));
-    B2_CHECK_CUDA(fmalloc(&n->d_rem_alpha, n->rem_k));
     B2_CHECK_CUDA(fmalloc(&n->d_rem_grad, size_t(nb) * n->rem_k));
-    B2_CHECK_CUDA(cudaMalloc(&n->d_rem_ctr, sizeof(unsigned long long)));
-    B2_CHECK_CUDA(cudaMemset(n->d_rem_ctr, 0, sizeof(unsigned long long)));
+    if (n->boot) {
+      B2_CHECK_CUDA(cudaMalloc(&n->d_boot_mask, size_t(nb) * n->rem_k));
+      B2_CHECK_CUDA(cudaMemset(n->d_boot_mask, 0, size_t(nb) * n->rem_k));
+      B2_CHECK_CUDA(fmalloc(&n->d_boot_y, size_t(nb) * n->rem_k));
+      B2_CHECK_CUDA(fmalloc(&n->d_boot_delta, size_t(nb) * n->rem_k));
+      B2_CHECK_CUDA(cudaMalloc(&n->d_boot_head, sizeof(int32_t)));
+      B2_CHECK_CUDA(cudaMemset(n->d_boot_head, 0xff, sizeof(int32_t)));   // -1: the mean over the heads
+    } else {
+      B2_CHECK_CUDA(fmalloc(&n->d_rem_alpha, n->rem_k));
+      B2_CHECK_CUDA(cudaMalloc(&n->d_rem_ctr, sizeof(unsigned long long)));
+      B2_CHECK_CUDA(cudaMemset(n->d_rem_ctr, 0, sizeof(unsigned long long)));
+    }
     B2_CHECK_CUDA(cudaMalloc(&n->d_act_rows, nb * sizeof(int32_t)));
     B2_CHECK_CUDA(cudaMemset(n->d_act_rows, 0, nb * sizeof(int32_t)));
   }
@@ -3145,6 +3347,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_va);
   cudaFree(n->d_theta); cudaFree(n->d_tquant); cudaFree(n->d_qgrad);
   cudaFree(n->d_rem_ctr); cudaFree(n->d_rem_alpha); cudaFree(n->d_rem_grad);
+  cudaFree(n->d_boot_mask); cudaFree(n->d_boot_y); cudaFree(n->d_boot_delta); cudaFree(n->d_boot_head);
   cudaFree(n->d_tdtarget);
   if (n->d_twe != n->d_we) { cudaFree(n->d_twe); cudaFree(n->d_twes); }
   cudaFree(n->d_crop_ctr); cudaFree(n->d_crop);
@@ -3436,11 +3639,21 @@ extern "C" int b200dqn_net_predict(b200dqn_net* n, const uint8_t* host_states, f
   return B200DQN_OK;
 }
 
+// A host-supplied minibatch names its rows 0..nb-1, not ring slots, so it has no bootstrap mask of its own; at p = 1
+// every mask is 1 and the rows need none.
+static int check_host_rows_maskable(const b200dqn_net* n, const char* who) {
+  B2_REQUIRE(!n->boot || n->cfg.bootstrap_p >= 1.0, B200DQN_ENOTIMPL,
+             "%s: bootstrapped heads with bootstrap_p = %g < 1 mask each transition by its ring slot; a host-supplied "
+             "minibatch has none (train from the replay ring)", who, n->cfg.bootstrap_p);
+  return B200DQN_OK;
+}
+
 extern "C" int b200dqn_net_train_device(b200dqn_net* n, const uint8_t* dev_pre, const uint8_t* dev_actions,
                                         const int64_t* dev_rewards, const uint8_t* dev_post,
                                         const uint8_t* dev_terminals, void* stream) {
   B2_REQUIRE(n && dev_pre && dev_actions && dev_rewards && dev_post && dev_terminals, B200DQN_EINVAL,
              "net_train_device: null argument");
+  B2_TRY(check_host_rows_maskable(n, "net_train_device"));
   DeviceGuard g(n->device);
   FrameSource fs{{dev_pre, dev_post}, {n->d_iota4, n->d_iota4}, {0, 0}};
   B2_TRY(train_step(n, fs, dev_actions, dev_rewards, dev_terminals, n->d_iota1, as_stream(stream)));
@@ -3453,6 +3666,7 @@ extern "C" int b200dqn_net_train(b200dqn_net* n, const uint8_t* host_pre, const 
                                  float* host_cost, void* stream) {
   B2_REQUIRE(n && host_pre && host_actions && host_rewards && host_post && host_terminals, B200DQN_EINVAL,
              "net_train: null argument");
+  B2_TRY(check_host_rows_maskable(n, "net_train"));
   for (int i = 0; i < n->nb; ++i)
     B2_REQUIRE(host_actions[i] < n->A, B200DQN_EINVAL, "net_train: action %d >= num_actions %d", host_actions[i], n->A);
   DeviceGuard g(n->device);
@@ -3707,6 +3921,7 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       B2_REQUIRE(!n->atoms, B200DQN_EINVAL, "net_device_ptr: a distributional head has no scalar delta");
       B2_REQUIRE(!n->quantiles, B200DQN_EINVAL, "net_device_ptr: a quantile-regression head has no scalar delta");
       B2_REQUIRE(!n->iqn_n, B200DQN_EINVAL, "net_device_ptr: an IQN head has no scalar delta");
+      B2_REQUIRE(!n->boot, B200DQN_EINVAL, "net_device_ptr: bootstrapped heads have no scalar delta per action");
       B2_REQUIRE(!n->rem_k, B200DQN_EINVAL, "net_device_ptr: a REM head has no scalar delta per action");
       p = n->d_delta;
       b = size_t(n->nb) * n->A * 4;
@@ -3819,6 +4034,8 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
     case B200DQN_NET_PTR_REM_GRADS:
     case B200DQN_NET_PTR_REM_COUNTER:
       B2_REQUIRE(n->rem_k, B200DQN_EINVAL, "net_device_ptr: selector %d needs a REM head", which);
+      B2_REQUIRE(!n->boot || which == B200DQN_NET_PTR_REM_HEADS || which == B200DQN_NET_PTR_REM_GRADS, B200DQN_EINVAL,
+                 "net_device_ptr: bootstrapped heads draw no REM mixture (selector %d)", which);
       switch (which) {
         case B200DQN_NET_PTR_REM_HEADS: p = n->d_theta; b = size_t(3) * n->nb * n->A * n->rem_k * 4; break;
         case B200DQN_NET_PTR_REM_ALPHAS: p = n->d_rem_alpha; b = size_t(n->rem_k) * 4; break;
@@ -3841,6 +4058,20 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
         case B200DQN_NET_PTR_FQF_BOUNDARY_QUANTILES: p = n->d_btheta; b = nb * (N - 1) * n->A * 4; break;
         case B200DQN_NET_PTR_FQF_FRACTION_GRADS: p = n->d_fg; b = nb * (N - 1) * 4; break;
         default: p = n->d_fdl; b = nb * N * 4; break;
+      }
+      break;
+    }
+    case B200DQN_NET_PTR_BOOT_MASKS:
+    case B200DQN_NET_PTR_BOOT_TARGETS:
+    case B200DQN_NET_PTR_BOOT_DELTAS:
+    case B200DQN_NET_PTR_BOOT_ACTIVE_HEAD: {
+      B2_REQUIRE(n->boot, B200DQN_EINVAL, "net_device_ptr: selector %d needs bootstrapped heads", which);
+      const size_t nk = size_t(n->nb) * n->rem_k;
+      switch (which) {
+        case B200DQN_NET_PTR_BOOT_MASKS: p = n->d_boot_mask; b = nk; break;
+        case B200DQN_NET_PTR_BOOT_TARGETS: p = n->d_boot_y; b = nk * 4; break;
+        case B200DQN_NET_PTR_BOOT_DELTAS: p = n->d_boot_delta; b = nk * 4; break;
+        default: p = n->d_boot_head; b = sizeof(int32_t); break;
       }
       break;
     }
@@ -3904,6 +4135,16 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   return B200DQN_OK;
 }
 
+extern "C" int b200dqn_net_set_active_head(b200dqn_net* n, int h, void* stream) {
+  B2_REQUIRE(n, B200DQN_EINVAL, "null net");
+  B2_REQUIRE(n->boot, B200DQN_EINVAL, "net_set_active_head: the net has no bootstrapped heads");
+  B2_REQUIRE(h >= -1 && h < n->rem_k, B200DQN_EINVAL, "net_set_active_head: head %d not in [-1,%d]", h, n->rem_k - 1);
+  DeviceGuard g(n->device);
+  k_boot_set_head<<<1, 1, 0, as_stream(stream)>>>(n->d_boot_head, h);
+  B2_LAUNCH_CHECK();
+  return B200DQN_OK;
+}
+
 extern "C" int b200dqn_net_get_grads(b200dqn_net* n, int layer, float* host_dW, void* stream) {
   B2_REQUIRE(n && host_dW && layer_ok(n, layer), B200DQN_EINVAL, "net_get_grads: bad argument");
   DeviceGuard g(n->device);
@@ -3942,12 +4183,12 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     // a distributional or quantile head adds k_fc2_dist, and on the SIMT engine fc2's own update; the Munchausen
     // target with a separate target network repeats the forward's launches for its pass
     // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient;
-    // random-shift augmentation and the REM head add their draws; an FQF head replaces the tau draw by the fraction
+    // random-shift augmentation and the REM head add their draws (bootstrapped heads draw nothing); an FQF head replaces the tau draw by the fraction
     // proposal and adds the boundary pass (phi, the modulation, fc1 and fc2) and the fraction layer's gradient
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
                 (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->fqf_n ? 5 : 0) +
                 (n->crop_pad ? 1 : 0) +
-                (n->rem_k ? 1 : 0) +
+                (n->rem_k && !n->boot ? 1 : 0) +
                 (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
   }
   return B200DQN_OK;

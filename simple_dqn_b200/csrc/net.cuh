@@ -134,6 +134,13 @@ struct b200dqn_net {
   unsigned long long* d_rem_ctr = nullptr;   // the mixture's draw counter
   float* d_rem_alpha = nullptr;              // [K] the mixture alpha of the last train step
   float* d_rem_grad = nullptr;               // [nb][K] gradient on the taken action's heads
+  // bootstrapped heads (cfg.bootstrap_heads > 0): the REM head's K-headed fc2 (rem_k = K, d_theta, d_rem_grad, the fc2
+  // kernels) trained by k_head_boot; the mixture's counter and alpha are not allocated.  Nothing below is otherwise.
+  bool boot = false;
+  uint8_t* d_boot_mask = nullptr;            // [nb][K] bootstrap masks of the last train step
+  float* d_boot_y = nullptr;                 // [nb][K] per-head targets float(y_k)
+  float* d_boot_delta = nullptr;             // [nb][K] per-head TD errors delta_k
+  int32_t* d_boot_head = nullptr;            // the head predict acts on (-1: the mean over the heads)
   // fc2 outputs per action of a per-action head (C51 atoms, QR quantiles or REM heads), 0 on the scalar and dueling
   // heads: such an fc2 is summed and updated by k_opt_fc2_dist from the compact [nb][512][block] partials
   int fc2_block() const { return atoms ? atoms : quantiles ? quantiles : iqn_n ? 1 : rem_k; }

@@ -48,6 +48,14 @@ def rem_seed(random_seed):
     return (int(random_seed) * 0xA0761D6478BD642F + 0xE7037ED1A0B428DB) % (1 << 64)
 
 
+def bootstrap_seed(random_seed):
+    """The bootstrapped heads' uint64 bootstrap_seed for args.random_seed: like rem_seed, with another odd multiplier and
+    offset, so the masks never share a stream with the other draws; a fresh random one when the seed is None."""
+    if random_seed is None:
+        return int.from_bytes(os.urandom(8), "little")
+    return (int(random_seed) * 0xE7037ED1A0B428DB + 0x8EBC6AF09C88C6E3) % (1 << 64)
+
+
 class DeepQNetwork:
     def __init__(self, num_actions, args, device=None, math_mode=None, stream=None):
         # remember parameters (:17-26)
@@ -160,6 +168,17 @@ class DeepQNetwork:
             cfg.num_fractions = int(_arg(args, "num_fractions", 32))
             cfg.fraction_lr = float(_arg(args, "fraction_lr", 2.5e-9))
             assert cfg.num_fractions >= 2, "num_fractions %d: the FQF head needs 2..64" % cfg.num_fractions
+        # bootstrapped DQN heads (Osband et al., 2016): a new capability, off unless args.bootstrapped is set; K =
+        # bootstrap_heads (10) Q-value heads per action on the shared network, each trained on its own target with a
+        # Bernoulli(bootstrap_p) mask (0.5) the device hashes from bootstrap_seed, derived from random_seed, and the
+        # transition's ring slot.  predict acts on the active head (set_active_head / sample_head), or on the mean over
+        # the heads (-1, the default).  Fixed here, like the other heads.
+        self.bootstrapped = bool(_arg(args, "bootstrapped", False))
+        if self.bootstrapped:
+            cfg.bootstrap_heads = int(_arg(args, "bootstrap_heads", 10))
+            cfg.bootstrap_p = float(_arg(args, "bootstrap_p", 0.5))
+            assert cfg.bootstrap_heads >= 1, "bootstrap_heads %d: bootstrapped heads need 1..200" % cfg.bootstrap_heads
+            cfg.bootstrap_seed = self.bootstrap_seed = bootstrap_seed(_arg(args, "random_seed", None))
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -172,6 +191,9 @@ class DeepQNetwork:
             self.tau_seed = cfg.tau_seed
         if self.rem:
             self.num_heads = cfg.num_heads
+        if self.bootstrapped:   # the REM head's fc2 and readers, K = bootstrap_heads
+            self.num_heads, self.bootstrap_p = cfg.bootstrap_heads, cfg.bootstrap_p
+            self._head_rng = np.random.RandomState(self.bootstrap_seed % (1 << 32))
         if self.fqf:   # the IQN accessors read its rows: N = K = num_fractions
             self.num_fractions = self.num_tau_samples = self.num_quantile_samples = cfg.num_fractions
             self.fraction_lr = cfg.fraction_lr
@@ -450,6 +472,37 @@ class DeepQNetwork:
         return int(L.download(self.device, self.device_view(L.NET_PTR_REM_COUNTER, (1,)).ptr, (1,), np.uint64,
                               self._stream)[0])
 
+    # ---- bootstrapped heads (bootstrapped = True); last_heads() and last_head_grads() read theta and dtheta
+    @property
+    def active_head(self):
+        """The head predict acts on, read from the device: 0..K-1, or -1 for the mean over the heads."""
+        return int(L.download(self.device, self.device_view(L.NET_PTR_BOOT_ACTIVE_HEAD, (1,)).ptr, (1,), np.int32,
+                              self._stream)[0])
+
+    def set_active_head(self, h):
+        """Act on head h (0..K-1), or on the mean over the heads (-1): every predict issued after this call."""
+        L.call("b200dqn_net_set_active_head", self._h, int(h), self._stream)
+
+    def sample_head(self):
+        """Draw the next episode's head uniformly from this net's own RandomState and act on it; returns it."""
+        assert self.bootstrapped, "sample_head needs bootstrapped heads"
+        h = int(self._head_rng.randint(self.num_heads))
+        self.set_active_head(h)
+        return h
+
+    def last_bootstrap_masks(self):
+        """The bootstrap masks of the last train step, (batch, K) uint8."""
+        return L.download(self.device, self.device_view(L.NET_PTR_BOOT_MASKS, (1,)).ptr,
+                          (self.batch_size, self.num_heads), np.uint8, self._stream)
+
+    def last_head_targets(self):
+        """The per-head targets float(y_k) of the last train step, (batch, K) float32."""
+        return self._read_f32(L.NET_PTR_BOOT_TARGETS, (self.batch_size, self.num_heads))
+
+    def last_head_deltas(self):
+        """The per-head TD errors delta_k of the last train step, (batch, K) float32."""
+        return self._read_f32(L.NET_PTR_BOOT_DELTAS, (self.batch_size, self.num_heads))
+
     # ---- Munchausen target (munchausen = True)
     def last_target_q_pre(self):
         """The target network's Q on the prestates of the last train(), (batch, A) float32: the row whose log-policy
@@ -476,9 +529,12 @@ class DeepQNetwork:
     def train(self, minibatch, epoch=0):
         """deepqnetwork.py:107-172.  A pristine DeviceMinibatch is trained in place from the ring, and so is one from a
         prioritized or n-step ring even once it has been looked at (the importance weights, the priority update and
-        the n-step window live there).  A host tuple is always the uniform, unweighted one-step step."""
+        the n-step window live there), and so is every one on a net with bootstrapped heads at bootstrap_p < 1 (the
+        masks belong to the ring slots).  A host tuple is always the uniform, unweighted one-step step, and such a net
+        refuses it (NotImplementedError)."""
+        ring_masks = self.bootstrapped and self.bootstrap_p < 1
         if isinstance(minibatch, DeviceMinibatch) and (not minibatch.materialised or minibatch._mem.prioritized or
-                                                       minibatch._mem.n_step > 1):
+                                                       minibatch._mem.n_step > 1 or ring_masks):
             minibatch._check_current()
             mem = minibatch._mem
             cost = C.c_float()

@@ -18,6 +18,8 @@ IQN_K = int(os.environ.get("IQN_K", "32"))   # the IQN head's tau samples per pr
 SHIFT = int(os.environ.get("SHIFT", "0"))   # random-shift augmentation with this pad p (DrQ: 4); 0: off
 REM = int(os.environ.get("REM", "0"))   # random ensemble mixture head (REM) with this many heads per action; 0: off
 FQF = int(os.environ.get("FQF", "0"))   # FQF head with this many fractions per sample; 0: off
+BOOT = int(os.environ.get("BOOT", "0"))   # bootstrapped DQN heads, this many per action; 0: off
+BOOT_P = float(os.environ.get("BOOT_P", "0.5"))   # the bootstrapped heads' mask probability
 
 
 def net_args():
@@ -30,6 +32,7 @@ def net_args():
     a.random_shift = SHIFT
     a.rem, a.num_heads = REM > 0, REM
     a.fqf, a.num_fractions = FQF > 0, FQF
+    a.bootstrapped, a.bootstrap_heads, a.bootstrap_p = BOOT > 0, BOOT, BOOT_P
     return a
 
 
