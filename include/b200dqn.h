@@ -466,6 +466,22 @@ typedef struct b200dqn_net_config {
   int bootstrap_heads;
   double bootstrap_p;
   uint64_t bootstrap_seed;
+  /* Soft (Polyak-averaged) target-network update (new capability, no reference counterpart; SB3's and CleanRL's `tau`),
+   * off when soft_target_tau = 0 (the default).  Otherwise tau = soft_target_tau, finite, in (0, 1] (anything else is
+   * EINVAL, as is tau > 0 with target_steps = 0: there is no separate target to blend; both before any device work),
+   * and every train step, on every train entry point, ends by blending each layer of the target network towards the
+   * online one.  b200dqn_net_comm_init returns ENOTIMPL on such a net.  Both engines.  Per element, every operation
+   * rounded on its own (no contraction):
+   *    1. c = float(1 - tau), 1 - tau formed in fp64 from the config double; t = float(tau);
+   *    2. theta_target' = fl(fl(c theta_target) + fl(t theta)), theta the online weight after this step's optimizer
+   *       update;
+   *    3. it covers layers 0-4, the IQN / FQF embedding (layer 5) and the FQF fraction layer (layer 6); the target's
+   *       optimizer state planes are not touched (only b200dqn_net_sync_target copies them);
+   *    4. on the tensor-core engine the target's forward tile images after the step are the packing of the new fp32
+   *       target weights, the images b200dqn_net_set_weights(which = 1) builds.
+   * At tau = 1 the target equals the online weights in value (c = 0, t = 1; an online -0 may land as +0).  The hard
+   * copy b200dqn_net_sync_target keeps working beside it. */
+  double soft_target_tau;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -494,6 +510,11 @@ int b200dqn_net_get_state(b200dqn_net* n, int which, int layer, int k, float* ho
 
 /* DeepQNetwork.update_target_network — src/deepqnetwork.py:102-105 (weights and optimizer state). */
 int b200dqn_net_sync_target(b200dqn_net* n, void* stream);
+/* One soft target update at tau outside a train step, by the rule of b200dqn_net_config::soft_target_tau and its
+ * kernels (with tau in place of soft_target_tau): the interval form, a blend every k-th train step.  Any net with a
+ * separate target network, whatever its soft_target_tau.  EINVAL unless tau is finite in (0, 1], and with
+ * target_steps = 0.  Asynchronous, in stream order. */
+int b200dqn_net_soft_update_target(b200dqn_net* n, double tau, void* stream);
 
 /* DeepQNetwork.predict(states) — src/deepqnetwork.py:174-186.  host_states (batch,hist,h,w) u8,
  * host_q (batch,A) f32 (already transposed as `qvalues.T`).  H2D + forward + D2H; synchronises. */

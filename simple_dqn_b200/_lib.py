@@ -43,7 +43,8 @@ class NetConfig(C.Structure):
                 ("tau_seed", C.c_uint64), ("random_shift", C.c_int), ("shift_seed", C.c_uint64),
                 ("num_heads", C.c_int), ("rem_seed", C.c_uint64),
                 ("num_fractions", C.c_int), ("fraction_lr", C.c_double),
-                ("bootstrap_heads", C.c_int), ("bootstrap_p", C.c_double), ("bootstrap_seed", C.c_uint64)]
+                ("bootstrap_heads", C.c_int), ("bootstrap_p", C.c_double), ("bootstrap_seed", C.c_uint64),
+                ("soft_target_tau", C.c_double)]
 
 
 _P = C.c_void_p
@@ -101,6 +102,7 @@ SIGNATURES = {
     "b200dqn_net_set_state": [_P, C.c_int, C.c_int, C.c_int, _P, _P],
     "b200dqn_net_get_state": [_P, C.c_int, C.c_int, C.c_int, _P, _P],
     "b200dqn_net_sync_target": [_P, _P],
+    "b200dqn_net_soft_update_target": [_P, C.c_double, _P],
     "b200dqn_net_predict": [_P, _P, _P, _P],
     "b200dqn_net_predict_device": [_P, _P, C.c_int, _P, _P],
     "b200dqn_net_predict_device_host": [_P, _P, C.c_int, _P, _P],

@@ -1824,6 +1824,24 @@ k_optimizer(const LayerTable lt, const float* __restrict__ part, float* __restri
   kt_end(kt);
 }
 
+// Soft target update of a parameter range (b200dqn_net_config::soft_target_tau): tw <- fl(fl(c tw) + fl(t w)), four
+// elements per thread.  The only update of fc2, the IQN / FQF embedding and the FQF fraction layer, and of every layer
+// on the SIMT engine; the tensor-core engine fuses conv1..fc1 into their image packs (umma_soft_pack).
+__global__ void __launch_bounds__(256)
+k_soft_blend(const float* __restrict__ w, float* __restrict__ tw, int64_t n4, float c, float t, const KTrace kt) {
+  const int64_t i4 = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (i4 < n4) {
+    const float4 a = reinterpret_cast<const float4*>(tw)[i4];
+    const float4 b = reinterpret_cast<const float4*>(w)[i4];
+    reinterpret_cast<float4*>(tw)[i4] = make_float4(soft_blend1(a.x, b.x, c, t), soft_blend1(a.y, b.y, c, t),
+                                                    soft_blend1(a.z, b.z, c, t), soft_blend1(a.w, b.w, c, t));
+  }
+  kt_end(kt);
+}
+
 __global__ void k_iota(int32_t* a, int32_t* b, int n, int mult) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
@@ -2471,6 +2489,34 @@ static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
     if (rc__) return rc__;    \
   } while (0)
 
+// Soft target update of `elems` parameters at w / tw (elems a multiple of 4).
+static int soft_blend_range(b200dqn_net* n, const float* w, float* tw, int64_t elems, float c, float t, cudaStream_t st,
+                            const char* label) {
+  const int64_t n4 = elems / 4;
+  B2_CHECK_CUDA(launch_pdl(k_soft_blend, dim3(cdiv(n4, 256)), dim3(256), 0, st, w, tw, n4, c, t, ktrace_slot(label)));
+  B2_PROF(label, st);
+  return B200DQN_OK;
+}
+
+// Soft target update of layers [l0, l1] on st: on the tensor-core engine conv1..fc1 one fused blend-and-pack launch
+// each, the fp32-only layers (fc2; every layer on the SIMT engine) one blend over their contiguous range.
+static int soft_update_layers(b200dqn_net* n, int l0, int l1, float c, float t, cudaStream_t st) {
+  const LayerTable& lt = n->lt;
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
+    for (; l0 <= l1 && l0 < 4; ++l0) B2_TRY(umma_soft_pack(n, l0, c, t, st));
+  if (l0 > l1) return B200DQN_OK;
+  static const char* const one[kLayers] = {"soft_c1", "soft_c2", "soft_c3", "soft_fc1", "soft_fc2"};
+  return soft_blend_range(n, n->d_w + lt.off[l0], n->d_tw + lt.off[l0], lt.off[l1 + 1] - lt.off[l0], c, t, st,
+                          l0 == l1 ? one[l0] : l0 == 3 ? "soft_fc" : "soft_layers");
+}
+
+// Soft target update of the IQN / FQF embedding and the FQF fraction layer on st (nothing on other nets).
+static int soft_update_extra(b200dqn_net* n, float c, float t, cudaStream_t st) {
+  if (n->iqn_n) B2_TRY(soft_blend_range(n, n->d_we, n->d_twe, int64_t(kIqnCos) * kFlat, c, t, st, "soft_we"));
+  if (n->fqf_n) B2_TRY(soft_blend_range(n, n->d_wf, n->d_twf, int64_t(n->fqf_n) * kFlat, c, t, st, "soft_wf"));
+  return B200DQN_OK;
+}
+
 // Model.bprop + optimizer.optimize for the online network (src/deepqnetwork.py:162-165).
 //
 // The dgrad chain fc1 -> conv3 -> conv2 is the critical path; every wgrad only needs the dZ of its
@@ -2733,6 +2779,10 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
       B2_TRY(optimizer_range(n, 0, kLayers - 1, 4, rows, st, "optimizer"));
     } else {
       B2_TRY(update_range(n, 0, kLayers - 1, rows, st, "optimizer"));
+      if (n->soft) {   // every layer is updated by now (the embedding and fraction layer in iqn_backward above)
+        B2_TRY(soft_update_layers(n, 0, kLayers - 1, n->soft_c, n->soft_t, st));
+        B2_TRY(soft_update_extra(n, n->soft_c, n->soft_t, st));
+      }
     }
     return B200DQN_OK;
   }
@@ -2749,10 +2799,19 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     // fourth branch: the scalar cost and the 512 x A layer — nothing later in the step reads W5, and nothing here
     // sits in front of the fc1 optimizer any more (the SIMT engine's scalar fc2 rides with fc1 in opt_fc)
     B2_TRY(cost_finish_on(n, rows, sN));
-    if (tc || n->fc2_block()) B2_TRY(opt_fc2_small(n, rows, sN));
+    if (tc || n->fc2_block()) {
+      B2_TRY(opt_fc2_small(n, rows, sN));
+      if (n->soft) B2_TRY(soft_update_layers(n, 4, 4, n->soft_c, n->soft_t, sN));
+    }
   }
   B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
-  if (n->iqn_n) B2_TRY(iqn_backward(n, rows, st, sN, true));   // dZ3 is dpsi
+  if (n->iqn_n) {
+    B2_TRY(iqn_backward(n, rows, st, sN, true));   // dZ3 is dpsi
+    if (n->soft) {                                   // behind the embedding's and fraction layer's updates on sN
+      NoPdlScope side;
+      B2_TRY(soft_update_extra(n, n->soft_c, n->soft_t, sN));
+    }
+  }
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
   {
@@ -2764,6 +2823,8 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
       B2_TRY(umma_opt_fc1(n, rows, sA));                       // smem-free: co-resides with the dgrad chain
     }
     else B2_TRY(optimizer_range(n, 3, n->fc2_block() ? 3 : 4, 1 | 4, rows, sA, "opt_fc"));
+    // fc1's soft target update (with the SIMT engine's scalar fc2, which rides with it in opt_fc)
+    if (n->soft) B2_TRY(soft_update_layers(n, 3, tc || n->fc2_block() ? 3 : 4, n->soft_c, n->soft_t, sA));
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
@@ -2774,6 +2835,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     NoPdlScope side;
     if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 2, rows, sB, "opt_conv3"));
     else B2_TRY(optimizer_range(n, 2, 2, 1 | 4, rows, sB, "opt_conv3"));
+    if (n->soft) B2_TRY(soft_update_layers(n, 2, 2, n->soft_c, n->soft_t, sB));
   }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[2], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv2Wgrad, sC)); }
@@ -2784,10 +2846,12 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     NoPdlScope side;
     if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 1, rows, sC, "opt_conv2"));
     else B2_TRY(optimizer_range(n, 1, 1, 1 | 4, rows, sC, "opt_conv2"));
+    if (n->soft) B2_TRY(soft_update_layers(n, 1, 1, n->soft_c, n->soft_t, sC));
   }
   B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st, true));
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 0, rows, st, "opt_conv1"));
   else B2_TRY(optimizer_range(n, 0, 0, 1 | 4, rows, st, "opt_conv1"));
+  if (n->soft) B2_TRY(soft_update_layers(n, 0, 0, n->soft_c, n->soft_t, st));
   B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));
   B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
   B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
@@ -3081,6 +3145,12 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
     B2_REQUIRE(!cfg->dueling && !cfg->munchausen, B200DQN_ENOTIMPL,
                "net_create: bootstrapped heads with a dueling network or the Munchausen target are not implemented");
   }
+  B2_REQUIRE(std::isfinite(cfg->soft_target_tau) && cfg->soft_target_tau >= 0 && cfg->soft_target_tau <= 1,
+             B200DQN_EINVAL, "net_create: the soft target update's soft_target_tau must be finite and in [0, 1] (got %g)",
+             cfg->soft_target_tau);
+  B2_REQUIRE(cfg->soft_target_tau == 0 || cfg->target_steps != 0, B200DQN_EINVAL,
+             "net_create: a soft target update (soft_target_tau %g) needs a separate target network; target_steps = 0 "
+             "makes the target the online network", cfg->soft_target_tau);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -3099,6 +3169,11 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   n->dueling = cfg->dueling != 0;
   n->munchausen = cfg->munchausen != 0;
+  if (cfg->soft_target_tau > 0) {
+    n->soft = true;
+    n->soft_c = float(1.0 - cfg->soft_target_tau);
+    n->soft_t = float(cfg->soft_target_tau);
+  }
   n->hidden = n->dueling ? kDuelHidden : kHidden;
   if (cfg->num_tau_samples) {
     n->iqn_n = cfg->num_tau_samples;
@@ -3541,6 +3616,19 @@ extern "C" int b200dqn_net_sync_target(b200dqn_net* n, void* stream) {
     B2_CHECK_CUDA(cudaMemcpyAsync(n->d_twfs, n->d_wfs, wf * n->n_states, cudaMemcpyDeviceToDevice, st));
   }
   return umma_target_synced(n, st);
+}
+
+extern "C" int b200dqn_net_soft_update_target(b200dqn_net* n, double tau, void* stream) {
+  B2_REQUIRE(n, B200DQN_EINVAL, "null net");
+  B2_REQUIRE(std::isfinite(tau) && tau > 0 && tau <= 1, B200DQN_EINVAL,
+             "net_soft_update_target: tau must be finite and in (0, 1] (got %g)", tau);
+  B2_REQUIRE(n->d_tw != n->d_w, B200DQN_EINVAL,
+             "net_soft_update_target: target_steps = 0 makes the target the online network; there is nothing to blend");
+  DeviceGuard g(n->device);
+  cudaStream_t st = as_stream(stream);
+  const float c = float(1.0 - tau), t = float(tau);
+  B2_TRY(soft_update_layers(n, 0, kLayers - 1, c, t, st));
+  return soft_update_extra(n, c, t, st);
 }
 
 extern "C" int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_states, int live_rows, float* dev_q,
@@ -4185,11 +4273,14 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
     // an IQN head adds the tau draw, the embedding, the modulation, its backward and the embedding's gradient;
     // random-shift augmentation and the REM head add their draws (bootstrapped heads draw nothing); an FQF head replaces the tau draw by the fraction
     // proposal and adds the boundary pass (phi, the modulation, fc1 and fc2) and the fraction layer's gradient
+    // a soft target update adds one blend per update launch: conv1, conv2, conv3, fc1 (with the SIMT engine's scalar
+    // fc2), fc2 where it is updated on its own, the embedding and the fraction layer
     *launches = 1 + 4 + 1 + 7 + (n->world > 1 ? (tc ? 7 : 2) : (tc ? 6 : 4)) + (n->fc2_block() ? (tc ? 1 : 2) : 0) +
                 (n->munchausen && n->d_tw != n->d_w ? 4 : 0) + (n->iqn_n ? 5 : 0) + (n->fqf_n ? 5 : 0) +
                 (n->crop_pad ? 1 : 0) +
                 (n->rem_k && !n->boot ? 1 : 0) +
-                (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0);   // IQN: the chunked fc1 wgrad and its reduction
+                (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0) +   // IQN: the chunked fc1 wgrad and its reduction
+                (n->soft ? 4 + (tc || n->fc2_block() ? 1 : 0) + (n->iqn_n ? 1 : 0) + (n->fqf_n ? 1 : 0) : 0);
   }
   return B200DQN_OK;
 }

@@ -211,6 +211,11 @@ struct b200dqn_net {
   int32_t* d_crop = nullptr;              // [2][nb][2] (dy, dx) of the last train step: prestates, then poststates
   bool crop_forked = false;               // the step's draw was launched on its own branch (ev[17] / ev[18])
 
+  // soft target update (cfg.soft_target_tau > 0): every train step blends the target towards the online network with
+  // these factors, c = float(1 - tau), t = float(tau)
+  bool soft = false;
+  float soft_c = 1.f, soft_t = 0.f;
+
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 
   // multi-GPU

@@ -735,29 +735,72 @@ struct WFc1WgradGather {
 };
 
 // ---- weight tile-image sources (k_pack_image) --------------------------------------------------
+// at(tile, row, k): the element of w behind image element (tile, row, k), -1 for padding; kContig8: the 8 elements of
+// a chunk (k0 .. k0 + 7) are consecutive in w
 template <int K, int N>
 struct PackFwdConv {   // B operand of a forward conv: rows = output channel n, K = filter taps
   static constexpr bool kRowMajorThreads = false;
+  static constexpr bool kContig8 = false;
   const float* w;      // [K][N]
   __host__ __device__ int tiles() const { return 1; }
   __host__ __device__ int rows() const { return N; }
   __host__ __device__ int kblocks() const { return K / 64; }
+  __device__ int at(int, int r, int k) const { return k * N + r; }
   __device__ void src8(int, int r, int k0, float v[8]) const {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = w[(k0 + j) * N + r];
+    for (int j = 0; j < 8; ++j) v[j] = w[at(0, r, k0 + j)];
   }
 };
 template <int W>
 struct PackFc1Dgrad {  // the fc1 image: rows = flat index m, 64 hidden units per row (dgrad: K-major A; forward: MN-major A)
   static constexpr bool kRowMajorThreads = true;
+  static constexpr bool kContig8 = true;
   const float* w;
   __host__ __device__ int tiles() const { return (kFlat + 127) / 128; }
   __host__ __device__ int rows() const { return 128; }
   __host__ __device__ int kblocks() const { return W / 64; }
+  __device__ int at(int tile, int r, int k) const {
+    const int m = tile * 128 + r;
+    return m < kFlat ? m * W + k : -1;
+  }
   __device__ void src8(int tile, int r, int k0, float v[8]) const {
     const int m = tile * 128 + r;
     if (m >= kFlat) { zero8(v); return; }
     ld8(w + m * W + k0, v);
+  }
+};
+// Soft target update fused into the pack of the target's forward image (b200dqn_net_config::soft_target_tau): the
+// source blends each master weight of a chunk on load, tw <- fl(fl(c tw) + fl(t w)), stores it back and hands the new
+// value to the packer.  P (a packer over the target layer) supplies the tiling, so every target weight is read and
+// written once, by the thread that packs it.
+template <class P>
+struct SoftBlendSrc {
+  static constexpr bool kRowMajorThreads = P::kRowMajorThreads;
+  P tgt;               // the packer over the target layer (tgt.w == tw)
+  float* tw;           // the target layer, updated in place
+  const float* w;      // the online layer, after this step's optimizer update
+  float c, t;
+  __host__ __device__ int tiles() const { return tgt.tiles(); }
+  __host__ __device__ int rows() const { return tgt.rows(); }
+  __host__ __device__ int kblocks() const { return tgt.kblocks(); }
+  __device__ void src8(int tile, int r, int k0, float v[8]) const {
+    if constexpr (P::kContig8) {
+      const int i = tgt.at(tile, r, k0);
+      if (i < 0) { zero8(v); return; }
+      float a[8], b[8];
+      ld8(tw + i, a);
+      ld8(w + i, b);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = soft_blend1(a[j], b[j], c, t);
+      st8(tw + i, v);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int i = tgt.at(tile, r, k0 + j);
+        v[j] = soft_blend1(tw[i], w[i], c, t);
+        tw[i] = v[j];
+      }
+    }
   }
 };
 template <int H, int C, int R, int ST, int KO>
@@ -1032,6 +1075,40 @@ int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st)
     }
   }
   return rc;
+}
+
+// soft target update of layer l (0..3) fused with the rebuild of the target's forward image: one pass over the layer
+// reads the online and target weights, writes the target weights and the image.  The target has no dgrad images.
+int umma_soft_pack(b200dqn_net* n, int l, float c, float t, cudaStream_t st) {
+  UmmaState* u = ust(n);
+  const LayerTable& lt = n->lt;
+  float* tw = n->d_tw + lt.off[l];
+  const float* w = n->d_w + lt.off[l];
+  uint8_t* img = u->img_fwd[1][l];
+  switch (l) {
+    case 0:
+      return with_hist(n->cfg.history_length, [&](auto h) {
+        constexpr int H = decltype(h)::value;
+        using P = PackFwdConv<64 * H, kC1>;
+        return umma2::launch_pack("soft_c1", SoftBlendSrc<P>{P{tw}, tw, w, c, t}, img, st);
+      });
+    case 1: {
+      using P = PackFwdConv<kK2, kC2>;
+      return umma2::launch_pack("soft_c2", SoftBlendSrc<P>{P{tw}, tw, w, c, t}, img, st);
+    }
+    case 2: {
+      using P = PackFwdConv<kK3, kC3>;
+      return umma2::launch_pack("soft_c3", SoftBlendSrc<P>{P{tw}, tw, w, c, t}, img, st);
+    }
+    default:
+      if (n->dueling) {
+        using P = PackFc1Dgrad<kDuelHidden>;
+        return umma2::launch_pack("soft_fc1", SoftBlendSrc<P>{P{tw}, tw, w, c, t}, img, st);
+      } else {
+        using P = PackFc1Dgrad<kHidden>;
+        return umma2::launch_pack("soft_fc1", SoftBlendSrc<P>{P{tw}, tw, w, c, t}, img, st);
+      }
+  }
 }
 
 // fc1 forward split-K over blockIdx.z (the head kernel sums the partials): 49 k-blocks of 64 -> 7 per CTA,

@@ -42,6 +42,9 @@ int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false)
 int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* label, bool from_g = false);
 // rebuild the fp16 hi/lo tile images of layers [l0, l1] of network `which` (0 online, 1 target)
 int umma_pack_layers(b200dqn_net* n, int which, int l0, int l1, cudaStream_t st);
+// soft target update of layer l (0..3): target <- fl(fl(c target) + fl(t online)) and the target's forward image of
+// the result, in one pass
+int umma_soft_pack(b200dqn_net* n, int l, float c, float t, cudaStream_t st);
 // fp16 hi plane of dZ4 and the offset of its lo plane (nullptr when math_mode != TCGEN05)
 void umma_dz4_planes(b200dqn_net* n, __half** hi, int64_t* lo_off);
 // fp16 hi plane of dZ3 (conv3's output gradient) and the offset of its lo plane (nullptr when math_mode != TCGEN05)

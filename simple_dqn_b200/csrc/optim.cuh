@@ -94,6 +94,11 @@ __device__ __forceinline__ void opt_update_vec(const OptArgs& o, float l, const 
             make_float4(sv[k][4 * v], sv[k][4 * v + 1], sv[k][4 * v + 2], sv[k][4 * v + 3]);
     }
 }
+
+// soft target update of one weight (b200dqn_net_config::soft_target_tau): fl(fl(c tw) + fl(t w)), no contraction
+__device__ __forceinline__ float soft_blend1(float tw, float w, float c, float t) {
+  return __fadd_rn(__fmul_rn(c, tw), __fmul_rn(t, w));
+}
 #endif
 
 }  // namespace b200

@@ -179,6 +179,11 @@ class DeepQNetwork:
             cfg.bootstrap_p = float(_arg(args, "bootstrap_p", 0.5))
             assert cfg.bootstrap_heads >= 1, "bootstrap_heads %d: bootstrapped heads need 1..200" % cfg.bootstrap_heads
             cfg.bootstrap_seed = self.bootstrap_seed = bootstrap_seed(_arg(args, "random_seed", None))
+        # soft (Polyak-averaged) target update: a new capability, off unless args.soft_target_tau = tau > 0 (SB3's and
+        # CleanRL's `tau`; BBF uses 0.005).  Every train step ends with target <- (1 - tau) target + tau online on the
+        # device; update_target_network() keeps its hard copy.  It needs a separate target network (target_steps > 0).
+        cfg.soft_target_tau = float(_arg(args, "soft_target_tau", 0.0) or 0.0)
+        self.soft_target_tau = cfg.soft_target_tau
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -523,8 +528,14 @@ class DeepQNetwork:
         return self._read_f32(L.NET_PTR_DUELING_VA, (3, self.batch_size, self.num_actions + 1))[..., -1]
 
     # ---- reference methods
-    def update_target_network(self):
-        L.call("b200dqn_net_sync_target", self._h, self._stream)        # :102-105
+    def update_target_network(self, tau=None):
+        """tau None: the reference's hard copy of the online network, optimizer states included (:102-105).  A float
+        tau in (0, 1]: one soft update, target <- (1 - tau) target + tau online, weights only (the interval form of the
+        soft target update, a blend every k-th train step)."""
+        if tau is None:
+            L.call("b200dqn_net_sync_target", self._h, self._stream)    # :102-105
+        else:
+            L.call("b200dqn_net_soft_update_target", self._h, float(tau), self._stream)
 
     def train(self, minibatch, epoch=0):
         """deepqnetwork.py:107-172.  A pristine DeviceMinibatch is trained in place from the ring, and so is one from a

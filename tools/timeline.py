@@ -20,6 +20,7 @@ REM = int(os.environ.get("REM", "0"))   # random ensemble mixture head (REM) wit
 FQF = int(os.environ.get("FQF", "0"))   # FQF head with this many fractions per sample; 0: off
 BOOT = int(os.environ.get("BOOT", "0"))   # bootstrapped DQN heads, this many per action; 0: off
 BOOT_P = float(os.environ.get("BOOT_P", "0.5"))   # the bootstrapped heads' mask probability
+TAU = float(os.environ.get("TAU", "0"))   # soft target update: blend the target towards the online net by TAU every step
 
 
 def net_args():
@@ -33,6 +34,7 @@ def net_args():
     a.rem, a.num_heads = REM > 0, REM
     a.fqf, a.num_fractions = FQF > 0, FQF
     a.bootstrapped, a.bootstrap_heads, a.bootstrap_p = BOOT > 0, BOOT, BOOT_P
+    a.soft_target_tau = TAU
     return a
 
 
