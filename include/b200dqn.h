@@ -252,7 +252,7 @@ typedef struct b200dqn_net_config {
    *   - the TD step (delta, clip, cost, prioritized and n-step targets) is the scalar head's; backward: g = delta / A,
    *     dA_j = (j == a ? delta - g : -g), dV = delta, dZ4 = (sum_j dA_j W5[j][k], j order) on advantage unit k and
    *     delta W5[A][k] on value unit k, under the H4 mask.  The paper's 1/sqrt(2) rescale of the gradient entering the
-   *     convolutions and its gradient-norm clipping are not applied.
+   *     convolutions is not applied; its gradient-norm clipping (at 10) is the separate opt-in max_grad_norm.
    * Both engines.  ENOTIMPL with num_atoms > 0; b200dqn_net_comm_init returns ENOTIMPL on such a net. */
   int dueling;
   /* Quantile-regression value head (QR-DQN, Dabney, Rowland, Bellemare and Munos, 2018; new capability, no reference
@@ -482,6 +482,30 @@ typedef struct b200dqn_net_config {
    * At tau = 1 the target equals the online weights in value (c = 0, t = 1; an online -0 may land as +0).  The hard
    * copy b200dqn_net_sync_target keeps working beside it. */
   double soft_target_tau;
+  /* Global gradient-norm clipping (new capability, no reference counterpart; SB3's `max_grad_norm`, OpenAI baselines'
+   * `grad_norm_clipping`, the dueling paper's clip at 10), off when max_grad_norm = 0 (the default): the step is then
+   * exactly the unclipped step.  A negative, NaN or infinite value is EINVAL before any device work.
+   * b200dqn_net_comm_init returns ENOTIMPL on such a net.  Both engines, every head, every train entry point (train,
+   * train_device, train_fused, step_host, replayed graphs), both schedules.  With M = max_grad_norm > 0 each train step:
+   *    1. for every parameter of layers 0-4 and of the IQN / FQF embedding (layer 5) forms gg = fl32(g / bsz), exactly
+   *       the value the unclipped update forms: g is the summed gradient the unclipped update reads (what
+   *       b200dqn_net_get_grads returns), bsz the optimizer's batch size (nb on every layer, the expanded IQN / FQF
+   *       layers included);
+   *    2. S_l = sum of double(gg)^2 over layer l in fp64 (the products are exact), in an order fixed by the
+   *       implementation (no floating-point atomics: two runs give the same bits); S_5 = 0 without an embedding;
+   *    3. N = sqrt(S_0 + S_1 + ... + S_5) in fp64, summed in layer order;
+   *    4. c = M / (N + 1e-6) in fp64, c32 = (c < 1.0) ? float(c) : 1.0f (torch's clip_grad_norm_ coefficient; a NaN N
+   *       gives c32 = 1, so NaN gradients pass through as they do unclipped; an infinite N gives c32 = 0);
+   *    5. gg' = fl32(gg c32), and the configured optimizer continues from gg' in its usual operation order (Adam's step
+   *       scalar is unchanged).  At c32 = 1, gg' = gg: a net whose norm never reaches M trains bit for bit like a net
+   *       without clipping;
+   *    6. the FQF fraction layer (layer 6) is neither counted nor scaled: it has its own learning rate (in the FQF
+   *       paper its own optimizer) and updates exactly as unclipped.
+   * b200dqn_net_get_grads keeps returning the pre-clip g; soft target blends follow the clipped update.  The GRAD_SQ,
+   * GRAD_NORM and CLIP_SCALE selectors read S_l, N and c32 of the last train step.  This follows torch and SB3, not
+   * Neon: Neon's gradient_clip_norm scales only the step and divides the norm by the batch size, and its
+   * gradient_clip_value clips each element; neither is what the configurations this field ports mean. */
+  double max_grad_norm;
 } b200dqn_net_config;
 
 int b200dqn_net_config_default(b200dqn_net_config* cfg, int num_actions);
@@ -657,7 +681,11 @@ enum {
   B200DQN_NET_PTR_BOOT_MASKS,       /* (batch, K) u8 the bootstrap masks m_k of the last train step                  */
   B200DQN_NET_PTR_BOOT_TARGETS,     /* (batch, K) f32 the per-head targets float(y_k) of the last train step         */
   B200DQN_NET_PTR_BOOT_DELTAS,      /* (batch, K) f32 the per-head TD errors delta_k of the last train step          */
-  B200DQN_NET_PTR_BOOT_ACTIVE_HEAD  /* i32 the head predict acts on (-1: the mean over the heads)                    */
+  B200DQN_NET_PTR_BOOT_ACTIVE_HEAD, /* i32 the head predict acts on (-1: the mean over the heads)                    */
+  /* Gradient-norm clipping only (max_grad_norm > 0; EINVAL otherwise). */
+  B200DQN_NET_PTR_GRAD_SQ,          /* (6,) f64 S_0..S_5, the per-layer sums of squares of the last train step       */
+  B200DQN_NET_PTR_GRAD_NORM,        /* f64 N, the global gradient norm of the last train step                         */
+  B200DQN_NET_PTR_CLIP_SCALE        /* f32 c32, the clip coefficient of the last train step                           */
 };
 int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr, size_t* bytes);
 /* The tensor-core dgrads write only the fp16 planes of dZ3/dZ2/dZ1; ask them to keep the fp32 copies as well

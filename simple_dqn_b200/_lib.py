@@ -22,7 +22,8 @@ OPT_RMSPROP, OPT_ADAM, OPT_ADADELTA = 0, 1, 2
  NET_PTR_IQN_DPHI, NET_PTR_IQN_TAU_COUNTER, NET_PTR_SHIFT_OFFSETS, NET_PTR_SHIFT_DRAWS, NET_PTR_REM_HEADS,
  NET_PTR_REM_ALPHAS, NET_PTR_REM_GRADS, NET_PTR_REM_COUNTER, NET_PTR_FQF_LOGITS, NET_PTR_FQF_PROBS,
  NET_PTR_FQF_FRACTIONS, NET_PTR_FQF_BOUNDARY_QUANTILES, NET_PTR_FQF_FRACTION_GRADS, NET_PTR_FQF_LOGIT_GRADS,
- NET_PTR_BOOT_MASKS, NET_PTR_BOOT_TARGETS, NET_PTR_BOOT_DELTAS, NET_PTR_BOOT_ACTIVE_HEAD) = range(54)
+ NET_PTR_BOOT_MASKS, NET_PTR_BOOT_TARGETS, NET_PTR_BOOT_DELTAS, NET_PTR_BOOT_ACTIVE_HEAD, NET_PTR_GRAD_SQ,
+ NET_PTR_GRAD_NORM, NET_PTR_CLIP_SCALE) = range(57)
 
 
 class B200DQNError(RuntimeError):
@@ -44,7 +45,7 @@ class NetConfig(C.Structure):
                 ("num_heads", C.c_int), ("rem_seed", C.c_uint64),
                 ("num_fractions", C.c_int), ("fraction_lr", C.c_double),
                 ("bootstrap_heads", C.c_int), ("bootstrap_p", C.c_double), ("bootstrap_seed", C.c_uint64),
-                ("soft_target_tau", C.c_double)]
+                ("soft_target_tau", C.c_double), ("max_grad_norm", C.c_double)]
 
 
 _P = C.c_void_p

@@ -497,6 +497,8 @@ extern "C" int b200dqn_net_comm_init(b200dqn_net* n, const void* id128, int rank
   B2_REQUIRE(!n->boot, B200DQN_ENOTIMPL,
              "net_comm_init: bootstrapped heads are implemented for a single learner only");
   B2_REQUIRE(!n->rem_k, B200DQN_ENOTIMPL, "net_comm_init: the REM head is implemented for a single learner only");
+  B2_REQUIRE(!n->clip, B200DQN_ENOTIMPL,
+             "net_comm_init: gradient-norm clipping is implemented for a single learner only");
   B2_REQUIRE(!n->soft, B200DQN_ENOTIMPL,
              "net_comm_init: the soft target update is implemented for a single learner only");
   B2_REQUIRE(!n->crop_pad, B200DQN_ENOTIMPL,

@@ -1842,6 +1842,94 @@ k_soft_blend(const float* __restrict__ w, float* __restrict__ tw, int64_t n4, fl
   kt_end(kt);
 }
 
+// ------------------------------------------------------------------------------------------
+// Global gradient-norm clipping (b200dqn_net_config::max_grad_norm; b200dqn.h has the rule).  Three kernels:
+//   k_grad_sq     one layer's sum of squares of gg = fl(g / bsz) in fp64, one partial per CTA of kSqChunk elements
+//   k_clip_scale  one CTA: each layer's partials in slot order into S_l, then N and c32
+//   k_opt_clip    the clipped update of a parameter range from its summed gradient (every layer but the tensor-core
+//                 engine's fc1, which k_opt_fc1_clip updates and repacks in one pass; its conv layers are repacked after)
+// Every sum runs in a fixed order (per thread, then the warp's xor butterfly, then the warps in order): no atomics, so
+// two runs give the same bits.
+// ------------------------------------------------------------------------------------------
+constexpr int kSqChunk = 4096;   // elements per k_grad_sq CTA: 256 threads x 4 float4
+
+__device__ __forceinline__ double block_sum_f64(double acc, double* s_w) {
+  for (int h = 16; h > 0; h >>= 1) acc = __dadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, h));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  double s = s_w[0];
+  for (int w = 1; w < int(blockDim.x >> 5); ++w) s = __dadd_rn(s, s_w[w]);
+  return s;
+}
+
+__global__ void __launch_bounds__(256)
+k_grad_sq(const float* __restrict__ g, int64_t n4, float bsz, double* __restrict__ part, const KTrace kt) {
+  __shared__ double s_w[8];
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  double acc = 0.0;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int64_t i4 = int64_t(blockIdx.x) * (kSqChunk / 4) + u * 256 + threadIdx.x;
+    if (i4 < n4) {
+      const float4 v = reinterpret_cast<const float4*>(g)[i4];
+      const double a = __fdiv_rn(v.x, bsz), b = __fdiv_rn(v.y, bsz), c = __fdiv_rn(v.z, bsz), d = __fdiv_rn(v.w, bsz);
+      acc = __dadd_rn(acc, __dmul_rn(a, a));
+      acc = __dadd_rn(acc, __dmul_rn(b, b));
+      acc = __dadd_rn(acc, __dmul_rn(c, c));
+      acc = __dadd_rn(acc, __dmul_rn(d, d));
+    }
+  }
+  const double s = block_sum_f64(acc, s_w);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+  kt_end(kt);
+}
+
+// clip: [0, 6) S_l, [6] N, [7] c32 (as f32), then the partials; layer l's are slots 8 + base[l] .. 8 + base[l + 1] - 1
+struct SqLayout { int64_t base[7]; };
+
+__global__ void __launch_bounds__(256)
+k_clip_scale(double* __restrict__ clip, const SqLayout lay, double max_norm, const KTrace kt) {
+  __shared__ double s_w[8];
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  double S = 0.0;
+  for (int l = 0; l < 6; ++l) {
+    double acc = 0.0;
+    for (int64_t j = lay.base[l] + threadIdx.x; j < lay.base[l + 1]; j += 256) acc = __dadd_rn(acc, clip[8 + j]);
+    const double Sl = block_sum_f64(acc, s_w);
+    if (threadIdx.x == 0) clip[l] = Sl;
+    S = __dadd_rn(S, Sl);
+  }
+  if (threadIdx.x == 0) {
+    const double N = __dsqrt_rn(S);
+    const double c = __ddiv_rn(max_norm, __dadd_rn(N, 1e-6));
+    clip[6] = N;
+    reinterpret_cast<float*>(clip + 7)[0] = c < 1.0 ? __double2float_rn(c) : 1.f;   // NaN: 1
+  }
+  kt_end(kt);
+}
+
+__global__ void __launch_bounds__(256)
+k_opt_clip(const float* __restrict__ g, float* __restrict__ w, float* __restrict__ s, int64_t n4, const OptArgs opt,
+           const float* __restrict__ clip, const KTrace kt) {
+  const int64_t i4 = blockIdx.x * int64_t(blockDim.x) + threadIdx.x;
+  kt_begin(kt);
+  pdl_wait();
+  pdl_launch_dependents();
+  if (i4 < n4) {
+    const int64_t i = i4 * 4;
+    const float4 gv = *reinterpret_cast<const float4*>(g + i);
+    float nw[4];
+    opt_update_vec<4, true>(opt, opt_step_scalar(opt), reinterpret_cast<const float*>(&gv), nw, w + i, s + i,
+                            __ldcg(clip));
+  }
+  kt_end(kt);
+}
+
 __global__ void k_iota(int32_t* a, int32_t* b, int n, int mult) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) {
@@ -2093,7 +2181,8 @@ static int forward_fqf(b200dqn_net* n, const FrameSource& fs, int nets, int rows
 
 // The IQN backward between fc1's dgrad and conv3's (on st): dpsi into dZ3 and dphi; then dWe and the embedding's update,
 // on side stream sW when given (its own branch: nothing later in the step reads We), else in line.  An FQF net adds
-// dW_f and the fraction layer's update on the same branch.
+// dW_f and the fraction layer's update on the same branch.  Under gradient-norm clipping the embedding's update waits
+// for c32 (clip_apply); the fraction layer's does not.
 static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t sW, bool update) {
   __half* dpsi16 = nullptr;
   int64_t dpsi_lo = 0;
@@ -2112,7 +2201,7 @@ static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t 
   OptArgs o = make_opt_args(n, rows);
   o.plane = int64_t(kIqnCos) * kFlat;
   B2_CHECK_CUDA(launch_pdl(k_iqn_we, dim3(cdiv(kFlat, kWeCols)), dim3(256), 0, s, (const float*)n->d_cos,
-                           (const float*)n->d_dphi, rows * n->iqn_n, n->d_weg, n->d_we, n->d_wes, update ? 1 : 0, o,
+                           (const float*)n->d_dphi, rows * n->iqn_n, n->d_weg, n->d_we, n->d_wes, update && !n->clip ? 1 : 0, o,
                            ktrace_slot("iqn_we")));
   B2_PROF("iqn_we", s);
   if (n->fqf_n) {
@@ -2517,6 +2606,72 @@ static int soft_update_extra(b200dqn_net* n, float c, float t, cudaStream_t st) 
   return B200DQN_OK;
 }
 
+// ---- global gradient-norm clipping (cfg.max_grad_norm > 0).  Layer 5 is the IQN / FQF embedding.
+static int64_t clip_layer_size(const b200dqn_net* n, int l) {
+  return l == kLayers ? int64_t(kIqnCos) * kFlat : n->lt.off[l + 1] - n->lt.off[l];
+}
+
+// the summed gradient of layer l the clipped step reads: the tensor-core engine's fc1 from its single wgrad partial (as
+// umma_opt_fc1 reads it), the embedding from d_weg (k_iqn_we), every other layer from d_g after clip_layer_end's reduce
+static const float* clip_grad_src(const b200dqn_net* n, int l) {
+  if (l == kLayers) return n->d_weg;
+  if (l == 3 && n->cfg.math_mode == B200DQN_MATH_TCGEN05 && n->lt.splits[3] == 1) return n->d_part + n->lt.part_off[3];
+  return n->d_g + n->lt.off[l];
+}
+
+// the end of layer l's branch in a clipped step: its partials summed into d_g, then its sum of squares
+static int clip_layer_end(b200dqn_net* n, int l, int rows, cudaStream_t st) {
+  static const char* const red[kLayers] = {"reduce_conv1", "reduce_conv2", "reduce_conv3", "reduce_fc1", "reduce_fc2"};
+  static const char* const sq[kLayers + 1] = {"grad_sq_c1", "grad_sq_c2", "grad_sq_c3", "grad_sq_fc1", "grad_sq_fc2",
+                                              "grad_sq_we"};
+  if (l == 4 && n->fc2_block()) B2_TRY(opt_fc2_dist(n, rows, 2, st, "reduce_fc2_dist"));
+  else if (l < kLayers && clip_grad_src(n, l) == n->d_g + n->lt.off[l])
+    B2_TRY(optimizer_range(n, l, l, 1 | 2, rows, st, red[l]));
+  const int64_t n4 = clip_layer_size(n, l) / 4;
+  B2_CHECK_CUDA(launch_pdl(k_grad_sq, dim3(cdiv(n4 * 4, kSqChunk)), dim3(256), 0, st, clip_grad_src(n, l), n4,
+                           make_opt_args(n, rows).bsz, n->d_clip + 8 + n->sq_base[l], ktrace_slot(sq[l])));
+  B2_PROF(sq[l], st);
+  return B200DQN_OK;
+}
+
+// N and c32 from every layer's partials (one CTA), once every clip_layer_end of the step has run
+static int clip_scale(b200dqn_net* n, cudaStream_t st) {
+  SqLayout lay{};
+  for (int l = 0; l < 7; ++l) lay.base[l] = n->sq_base[l];
+  B2_CHECK_CUDA(launch_pdl(k_clip_scale, dim3(1), dim3(256), 0, st, n->d_clip, lay, n->cfg.max_grad_norm,
+                           ktrace_slot("clip_scale")));
+  B2_PROF("clip_scale", st);
+  return B200DQN_OK;
+}
+
+// the clipped update of layer l from clip_grad_src(n, l), with the tensor-core engine's image refresh: fc1 in one pass
+// (k_opt_fc1_clip), the conv layers by their packers after k_opt_clip
+static int clip_apply(b200dqn_net* n, int l, int rows, cudaStream_t st) {
+  static const char* const lbl[kLayers + 1] = {"opt_conv1_clip", "opt_conv2_clip", "opt_conv3_clip", "opt_fc1_clip",
+                                               "opt_fc2_clip", "opt_we_clip"};
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05 && l == 3)
+    return umma_opt_fc1(n, rows, st, n->lt.splits[3] > 1, n->d_clip_c());
+  OptArgs o = make_opt_args(n, rows);
+  float* w = n->d_we, *s = n->d_wes;
+  if (l == kLayers) o.plane = clip_layer_size(n, l);
+  else w = n->d_w + n->lt.off[l], s = n->d_s + n->lt.off[l];
+  const int64_t n4 = clip_layer_size(n, l) / 4;
+  B2_CHECK_CUDA(launch_pdl(k_opt_clip, dim3(cdiv(n4, 256)), dim3(256), 0, st, clip_grad_src(n, l), w, s, n4, o,
+                           (const float*)n->d_clip_c(), ktrace_slot(lbl[l])));
+  B2_PROF(lbl[l], st);
+  // the tensor-core engine's conv layers: their tile images from the new weights (forward; conv2 and conv3 also dgrad)
+  return l < 3 ? umma_pack_layers(n, 0, l, l, st) : B200DQN_OK;
+}
+
+// the serial form: every layer's end, c32, then every clipped update, in order on st
+static int clip_step_serial(b200dqn_net* n, int rows, cudaStream_t st) {
+  const int last = n->iqn_n ? kLayers : kLayers - 1;
+  for (int l = 0; l <= last; ++l) B2_TRY(clip_layer_end(n, l, rows, st));
+  B2_TRY(clip_scale(n, st));
+  for (int l = 0; l <= last; ++l) B2_TRY(clip_apply(n, l, rows, st));
+  return B200DQN_OK;
+}
+
 // Model.bprop + optimizer.optimize for the online network (src/deepqnetwork.py:162-165).
 //
 // The dgrad chain fc1 -> conv3 -> conv2 is the critical path; every wgrad only needs the dZ of its
@@ -2759,6 +2914,80 @@ static int backward_and_update_multi(b200dqn_net* n, const FrameSource& fs, int 
   return B200DQN_OK;
 }
 
+// The rest of the branches schedule under gradient-norm clipping, from fc1's dgrad on (ev[1] recorded, sA waiting on
+// it): each branch ends with its layer's reduce and sum of squares instead of its update; main joins every branch,
+// forms c32 and fans the clipped updates (with their image refreshes and soft target blends) back out over the same
+// branches; the caller's end-of-step join follows.
+//   main : ... conv2_dgrad . conv1_wgrad . end(conv1) . [join] clip_scale . opt(conv1)
+//   sA   : fc1_wgrad ... [after fc1_dgrad] end(fc1)            [fan-out] opt(fc1)
+//   sB   : conv3_wgrad .. [after conv3_dgrad] end(conv3)       [fan-out] opt(conv3)
+//   sC   : conv2_wgrad .. [after conv2_dgrad] end(conv2)       [fan-out] opt(conv2)
+//   sN   : cost . end(fc2) . end(embedding)                    [fan-out] opt(fc2) . opt(embedding)
+static int clip_branches(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
+  cudaStream_t sA = g_prof_on ? st : n->side[0], sB = g_prof_on ? st : n->side[1], sC = g_prof_on ? st : n->side[2];
+  cudaStream_t sN = g_prof_on ? st : n->side[3];
+  cudaEvent_t* ev = n->ev;
+  const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
+  const bool fc2_on_sn = tc || n->fc2_block();   // else the SIMT engine's scalar fc2 rides with fc1 on sA
+  {
+    NoPdlScope side;
+    B2_TRY(clip_layer_end(n, 3, rows, sA));
+    if (!fc2_on_sn) B2_TRY(clip_layer_end(n, 4, rows, sA));
+  }
+  B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[1], 0));
+  { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv3Wgrad, sB)); }
+  B2_TRY(bwd_op(n, fs, rows, kConv3Dgrad, st, true));
+  B2_CHECK_CUDA(cudaEventRecord(ev[2], st));                 // dZ2 ready, W3 no longer needed
+  B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[2], 0));
+  { NoPdlScope side; B2_TRY(clip_layer_end(n, 2, rows, sB)); }
+  B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[2], 0));
+  { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv2Wgrad, sC)); }
+  B2_TRY(bwd_op(n, fs, rows, kConv2Dgrad, st, true));
+  B2_CHECK_CUDA(cudaEventRecord(ev[3], st));                 // dZ1 ready, W2 no longer needed
+  B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[3], 0));
+  { NoPdlScope side; B2_TRY(clip_layer_end(n, 1, rows, sC)); }
+  B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st, true));
+  NoPdlScope tail;   // the join and the fan-out use ordinary dependencies
+  B2_TRY(clip_layer_end(n, 0, rows, st));
+  B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));                 // join: every S_l partial is written
+  B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
+  B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
+  B2_CHECK_CUDA(cudaEventRecord(ev[7], sN));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[4], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[5], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[6], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[7], 0));
+  B2_TRY(clip_scale(n, st));
+  B2_CHECK_CUDA(cudaEventRecord(ev[9], st));                 // c32 ready
+  for (cudaStream_t s : {sA, sB, sC, sN}) B2_CHECK_CUDA(cudaStreamWaitEvent(s, ev[9], 0));
+  B2_TRY(clip_apply(n, 3, rows, sA));
+  if (!fc2_on_sn) B2_TRY(clip_apply(n, 4, rows, sA));
+  if (n->soft) B2_TRY(soft_update_layers(n, 3, fc2_on_sn ? 3 : 4, n->soft_c, n->soft_t, sA));
+  B2_TRY(clip_apply(n, 2, rows, sB));
+  if (n->soft) B2_TRY(soft_update_layers(n, 2, 2, n->soft_c, n->soft_t, sB));
+  B2_TRY(clip_apply(n, 1, rows, sC));
+  if (n->soft) B2_TRY(soft_update_layers(n, 1, 1, n->soft_c, n->soft_t, sC));
+  if (fc2_on_sn) {
+    B2_TRY(clip_apply(n, 4, rows, sN));
+    if (n->soft) B2_TRY(soft_update_layers(n, 4, 4, n->soft_c, n->soft_t, sN));
+  }
+  if (n->iqn_n) {
+    B2_TRY(clip_apply(n, kLayers, rows, sN));
+    if (n->soft) B2_TRY(soft_update_extra(n, n->soft_c, n->soft_t, sN));
+  }
+  B2_TRY(clip_apply(n, 0, rows, st));
+  if (n->soft) B2_TRY(soft_update_layers(n, 0, 0, n->soft_c, n->soft_t, st));
+  B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));
+  B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
+  B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
+  B2_CHECK_CUDA(cudaEventRecord(ev[7], sN));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[4], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[5], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[6], 0));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[7], 0));
+  return B200DQN_OK;
+}
+
 static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st, bool update) {
   if (update && n->world > 1 && !g_prof_on && n->use_branches && st != nullptr &&
       n->cfg.math_mode == B200DQN_MATH_TCGEN05)
@@ -2778,7 +3007,8 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
       B2_PROF("allreduce", st);
       B2_TRY(optimizer_range(n, 0, kLayers - 1, 4, rows, st, "optimizer"));
     } else {
-      B2_TRY(update_range(n, 0, kLayers - 1, rows, st, "optimizer"));
+      if (n->clip) B2_TRY(clip_step_serial(n, rows, st));
+      else B2_TRY(update_range(n, 0, kLayers - 1, rows, st, "optimizer"));
       if (n->soft) {   // every layer is updated by now (the embedding and fraction layer in iqn_backward above)
         B2_TRY(soft_update_layers(n, 0, kLayers - 1, n->soft_c, n->soft_t, st));
         B2_TRY(soft_update_extra(n, n->soft_c, n->soft_t, st));
@@ -2799,7 +3029,9 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     // fourth branch: the scalar cost and the 512 x A layer — nothing later in the step reads W5, and nothing here
     // sits in front of the fc1 optimizer any more (the SIMT engine's scalar fc2 rides with fc1 in opt_fc)
     B2_TRY(cost_finish_on(n, rows, sN));
-    if (tc || n->fc2_block()) {
+    if (n->clip) {
+      if (tc || n->fc2_block()) B2_TRY(clip_layer_end(n, 4, rows, sN));
+    } else if (tc || n->fc2_block()) {
       B2_TRY(opt_fc2_small(n, rows, sN));
       if (n->soft) B2_TRY(soft_update_layers(n, 4, 4, n->soft_c, n->soft_t, sN));
     }
@@ -2807,13 +3039,14 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   B2_TRY(bwd_op(n, fs, rows, kFc1Dgrad, st, true));
   if (n->iqn_n) {
     B2_TRY(iqn_backward(n, rows, st, sN, true));   // dZ3 is dpsi
-    if (n->soft) {                                   // behind the embedding's and fraction layer's updates on sN
-      NoPdlScope side;
+    NoPdlScope side;
+    if (n->clip) B2_TRY(clip_layer_end(n, kLayers, rows, sN));   // dWe, written by k_iqn_we on sN
+    else if (n->soft)                                   // behind the embedding's and fraction layer's updates on sN
       B2_TRY(soft_update_extra(n, n->soft_c, n->soft_t, sN));
-    }
   }
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
+  if (n->clip) return clip_branches(n, fs, rows, st);
   {
     NoPdlScope side;
     if (tc && n->lt.splits[3] > 1) {                           // IQN: sum fc1's wgrad partials first
@@ -3151,6 +3384,8 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   B2_REQUIRE(cfg->soft_target_tau == 0 || cfg->target_steps != 0, B200DQN_EINVAL,
              "net_create: a soft target update (soft_target_tau %g) needs a separate target network; target_steps = 0 "
              "makes the target the online network", cfg->soft_target_tau);
+  B2_REQUIRE(std::isfinite(cfg->max_grad_norm) && cfg->max_grad_norm >= 0, B200DQN_EINVAL,
+             "net_create: gradient-norm clipping's max_grad_norm must be finite and >= 0 (got %g)", cfg->max_grad_norm);
   DeviceGuard g(device);
   auto* n = new (std::nothrow) b200dqn_net();
   B2_REQUIRE(n, B200DQN_EINVAL, "out of host memory");
@@ -3294,6 +3529,13 @@ extern "C" int b200dqn_net_create(int device, const b200dqn_net_config* cfg, b20
   }
   if (n->dueling) B2_CHECK_CUDA(fmalloc(&n->d_va, size_t(3) * nb * (A + 1)));
   if (n->munchausen) B2_CHECK_CUDA(fmalloc(&n->d_tdtarget, nb));
+  if (cfg->max_grad_norm > 0) {   // S_l, N, c32, then k_grad_sq's partials of layers 0-4 and the embedding
+    n->clip = true;
+    for (int l = 0; l <= kLayers; ++l)
+      n->sq_base[l + 1] = n->sq_base[l] + (l < kLayers || n->iqn_n ? cdiv(clip_layer_size(n, l), kSqChunk) : 0);
+    B2_CHECK_CUDA(cudaMalloc(&n->d_clip, size_t(8 + n->sq_base[kLayers + 1]) * sizeof(double)));
+    B2_CHECK_CUDA(cudaMemset(n->d_clip, 0, size_t(8 + n->sq_base[kLayers + 1]) * sizeof(double)));
+  }
   if (cfg->random_shift) {
     n->crop_pad = cfg->random_shift;
     B2_CHECK_CUDA(cudaMalloc(&n->d_crop_ctr, sizeof(unsigned long long)));
@@ -3426,6 +3668,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   cudaFree(n->d_tdtarget);
   if (n->d_twe != n->d_we) { cudaFree(n->d_twe); cudaFree(n->d_twes); }
   cudaFree(n->d_crop_ctr); cudaFree(n->d_crop);
+  cudaFree(n->d_clip);
   cudaFree(n->d_we); cudaFree(n->d_wes); cudaFree(n->d_weg); cudaFree(n->d_tau_ctr); cudaFree(n->d_tau);
   cudaFree(n->d_cos); cudaFree(n->d_phi); cudaFree(n->d_x); cudaFree(n->d_iqn_theta); cudaFree(n->d_iqn_tq);
   cudaFree(n->d_iqn_qgrad); cudaFree(n->d_dx); cudaFree(n->d_dphi); cudaFree(n->d_x16);
@@ -4163,6 +4406,16 @@ extern "C" int b200dqn_net_device_ptr(b200dqn_net* n, int which, void** dev_ptr,
       }
       break;
     }
+    case B200DQN_NET_PTR_GRAD_SQ:
+    case B200DQN_NET_PTR_GRAD_NORM:
+    case B200DQN_NET_PTR_CLIP_SCALE:
+      B2_REQUIRE(n->clip, B200DQN_EINVAL, "net_device_ptr: selector %d needs gradient-norm clipping", which);
+      switch (which) {
+        case B200DQN_NET_PTR_GRAD_SQ: p = n->d_clip; b = 6 * sizeof(double); break;
+        case B200DQN_NET_PTR_GRAD_NORM: p = n->d_clip + 6; b = sizeof(double); break;
+        default: p = n->d_clip_c(); b = sizeof(float); break;
+      }
+      break;
     default: B2_REQUIRE(false, B200DQN_EINVAL, "net_device_ptr: unknown selector %d", which);
   }
   *dev_ptr = p;
@@ -4280,7 +4533,12 @@ extern "C" int b200dqn_net_launches_per_step(const b200dqn_net* n, int* launches
                 (n->crop_pad ? 1 : 0) +
                 (n->rem_k && !n->boot ? 1 : 0) +
                 (tc && n->lt.splits[3] > 1 ? n->lt.splits[3] : 0) +   // IQN: the chunked fc1 wgrad and its reduction
-                (n->soft ? 4 + (tc || n->fc2_block() ? 1 : 0) + (n->iqn_n ? 1 : 0) + (n->fqf_n ? 1 : 0) : 0);
+                (n->soft ? 4 + (tc || n->fc2_block() ? 1 : 0) + (n->iqn_n ? 1 : 0) + (n->fqf_n ? 1 : 0) : 0) +
+                // gradient-norm clipping: a reduce per layer whose update read partials (not the tensor-core fc1's
+                // single partial), a sum of squares per layer, clip_scale, and one update launch per layer in place
+                // of the per-branch ones (tensor-core conv layers: plus their 5 image packs); the embedding adds its
+                // sum of squares and its update
+                (n->clip ? (tc ? 15 : n->fc2_block() ? 11 : 12) + (n->iqn_n ? 2 : 0) : 0);
   }
   return B200DQN_OK;
 }

@@ -216,6 +216,13 @@ struct b200dqn_net {
   bool soft = false;
   float soft_c = 1.f, soft_t = 0.f;
 
+  // global gradient-norm clipping (cfg.max_grad_norm > 0): d_clip holds S_0..S_5 (f64), N (f64), c32 (f32 in slot 7),
+  // then k_grad_sq's per-CTA partial sums, layer l's (5: the IQN / FQF embedding) from slot 8 + sq_base[l]
+  bool clip = false;
+  double* d_clip = nullptr;
+  int64_t sq_base[7] = {};
+  float* d_clip_c() const { return reinterpret_cast<float*>(d_clip + 7); }
+
   void* umma_state = nullptr;  // tensor-core engine: fp16 operand planes + weight tile images (net_umma.cu)
 
   // multi-GPU

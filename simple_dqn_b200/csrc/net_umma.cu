@@ -928,21 +928,23 @@ k_opt_conv(const float* __restrict__ part, int splits, float* __restrict__ w, fl
 // column-oriented (forward) image is rebuilt by k_pack_image right after.  Both kernels are smem-free,
 // light on registers and launched on a CAPPED grid (2 CTAs per SM, grid-stride loop) so that they
 // co-reside with the tensor-core kernels of the critical chain instead of locking them out of the SMs.
-template <int W>
-__global__ void __launch_bounds__(256)
-k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
-          const OptArgs opt, const KTrace kt) {
+template <int W, bool CLIP>
+__device__ __forceinline__ void opt_fc1_body(const float* __restrict__ dw, float* __restrict__ w,
+                                             float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
+                                             const OptArgs& opt, const float* __restrict__ clip, const KTrace& kt) {
   kt_begin(kt);
   pdl_wait();
   pdl_launch_dependents();
   constexpr int kNB = W / 8;
   const float l_step = opt_step_scalar(opt);
+  float c = 1.f;
+  if constexpr (CLIP) c = __ldcg(clip);
   for (int id = blockIdx.x * blockDim.x + threadIdx.x; id < kFlat * kNB; id += gridDim.x * blockDim.x) {
     const int m = id / kNB, n0 = (id % kNB) * 8;
     const int64_t i = int64_t(m) * W + n0;
     float g[8], wv[8];
     ld8(dw + i, g);
-    opt_update_vec<8>(opt, l_step, g, wv, w + i, sst + i);   // the configured Neon optimizer (optim.cuh)
+    opt_update_vec<8, CLIP>(opt, l_step, g, wv, w + i, sst + i, c);   // the configured Neon optimizer (optim.cuh)
     uint4 hi, lo;
     umma::split8(wv, hi, lo);
     uint8_t* base = img_dgr + (int64_t(m / 128) * (W / 64) + n0 / 64) * (128 * 256) +
@@ -953,7 +955,22 @@ k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict
   kt_end(kt);
 }
 
-int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g) {
+template <int W>
+__global__ void __launch_bounds__(256)
+k_opt_fc1(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst, uint8_t* __restrict__ img_dgr,
+          const OptArgs opt, const KTrace kt) {
+  opt_fc1_body<W, false>(dw, w, sst, img_dgr, opt, nullptr, kt);
+}
+
+// the same under global gradient-norm clipping, with the coefficient c32 read from *clip
+template <int W>
+__global__ void __launch_bounds__(256)
+k_opt_fc1_clip(const float* __restrict__ dw, float* __restrict__ w, float* __restrict__ sst,
+               uint8_t* __restrict__ img_dgr, const OptArgs opt, const float* __restrict__ clip, const KTrace kt) {
+  opt_fc1_body<W, true>(dw, w, sst, img_dgr, opt, clip, kt);
+}
+
+int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g, const float* clip) {
   UmmaState* u = ust(n);
   const LayerTable& lt = n->lt;
   const float* dw = from_g ? n->d_g + lt.off[3] : n->d_part + lt.part_off[3];
@@ -962,6 +979,13 @@ int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g) {
   // 6.4 MB written per step, 5 us at the end of the fc1 branch) are gone.
   // capped grid (2 CTAs per SM, grid-stride): the kernel shares the SMs — and the L2 — with the dgrad chain
   const int ctas = 2 * n->sm_count;
+  if (clip) {
+    B2_CHECK_CUDA(launch_pdl(n->dueling ? k_opt_fc1_clip<kDuelHidden> : k_opt_fc1_clip<kHidden>, dim3(ctas), dim3(256),
+                             0, st, dw, n->d_w + lt.off[3], n->d_s + lt.off[3], u->img_dgr[0], make_opt_args(n, rows),
+                             clip, ktrace_slot("opt_fc1_clip")));
+    B2_PROF("opt_fc1_clip", st);
+    return B200DQN_OK;
+  }
   B2_CHECK_CUDA(launch_pdl(n->dueling ? k_opt_fc1<kDuelHidden> : k_opt_fc1<kHidden>, dim3(ctas), dim3(256), 0, st, dw,
                            n->d_w + lt.off[3],
                            n->d_s + lt.off[3], u->img_dgr[0], make_opt_args(n, rows), ktrace_slot("opt_fc1")));

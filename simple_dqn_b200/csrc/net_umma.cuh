@@ -35,8 +35,9 @@ int umma_fc1_splits(int rows);
 // fc1 partials (nets = 1, no fp32 activations); crop: the prestates' crop offsets (slot 0's), or nullptr
 int umma_forward_target_pre(b200dqn_net* n, const uint8_t* src, const int32_t* idx, int shift, const int32_t* crop,
                             int rows, cudaStream_t st);
-// RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel
-int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false);
+// RMSProp of the fc1 layer + refresh of its tile image in one smem-free kernel; clip (non-null): the update under global
+// gradient-norm clipping, with the coefficient c32 read from *clip on the device
+int umma_opt_fc1(b200dqn_net* n, int rows, cudaStream_t st, bool from_g = false, const float* clip = nullptr);
 // fused split-K reduction + RMSProp + tile-image refresh of conv layer l (0..2), single-GPU tensor-core path
 // from_g: read the (all-reduced) gradient from d_g instead of the split-K partials
 int umma_opt_conv(b200dqn_net* n, int l, int rows, cudaStream_t st, const char* label, bool from_g = false);

@@ -27,10 +27,9 @@ __device__ __forceinline__ float opt_step_scalar(const OptArgs& o) {
   return o.kind == B200DQN_OPT_ADAM ? __ldcg(o.adam_l) : 0.f;
 }
 
-// one parameter: g = raw summed gradient, w = weight, s0..s2 = its state planes (unused ones untouched)
-__device__ __forceinline__ void opt_update1(const OptArgs& o, float l, float g, float& w, float& s0, float& s1,
-                                            float& s2) {
-  const float gg = __fdiv_rn(g, o.bsz);
+// one parameter's rule from its gradient gg = g / bsz: w = weight, s0..s2 = its state planes (unused ones untouched)
+__device__ __forceinline__ void opt_rule1(const OptArgs& o, float l, float gg, float& w, float& s0, float& s1,
+                                          float& s2) {
   if (o.kind == B200DQN_OPT_RMSPROP) {
     // state = decay*state + square(grad)*(1-decay);  param = param - (grad*lrate) / (sqrt(state+eps) + eps)
     const float ns = __fadd_rn(__fmul_rn(o.decay, s0), __fmul_rn(__fmul_rn(gg, gg), o.one_m_decay));
@@ -56,10 +55,24 @@ __device__ __forceinline__ void opt_update1(const OptArgs& o, float l, float g, 
   }
 }
 
-// N consecutive parameters at element offset i: load the live state planes, update, store
-template <int N>
+// one parameter: g = raw summed gradient, w = weight, s0..s2 = its state planes (unused ones untouched)
+__device__ __forceinline__ void opt_update1(const OptArgs& o, float l, float g, float& w, float& s0, float& s1,
+                                            float& s2) {
+  opt_rule1(o, l, __fdiv_rn(g, o.bsz), w, s0, s1, s2);
+}
+
+// the same under global gradient-norm clipping (b200dqn_net_config::max_grad_norm): gg' = fl(fl(g / bsz) c), c the
+// step's clip coefficient c32
+__device__ __forceinline__ void opt_update1_clip(const OptArgs& o, float l, float g, float c, float& w, float& s0,
+                                                 float& s1, float& s2) {
+  opt_rule1(o, l, __fmul_rn(__fdiv_rn(g, o.bsz), c), w, s0, s1, s2);
+}
+
+// N consecutive parameters at element offset i: load the live state planes, update, store.  kClip: the clipped rule
+// (opt_update1_clip) with coefficient c.
+template <int N, bool kClip = false>
 __device__ __forceinline__ void opt_update_vec(const OptArgs& o, float l, const float* g, float* w_out, float* w_ptr,
-                                               float* s_ptr) {
+                                               float* s_ptr, float c = 1.f) {
   static_assert(N == 4 || N == 8, "vector width");
   float sv[3][N];
 #pragma unroll
@@ -81,7 +94,10 @@ __device__ __forceinline__ void opt_update_vec(const OptArgs& o, float l, const 
     w_out[4 * v] = t.x; w_out[4 * v + 1] = t.y; w_out[4 * v + 2] = t.z; w_out[4 * v + 3] = t.w;
   }
 #pragma unroll
-  for (int j = 0; j < N; ++j) opt_update1(o, l, g[j], w_out[j], sv[0][j], sv[1][j], sv[2][j]);
+  for (int j = 0; j < N; ++j) {
+    if constexpr (kClip) opt_update1_clip(o, l, g[j], c, w_out[j], sv[0][j], sv[1][j], sv[2][j]);
+    else opt_update1(o, l, g[j], w_out[j], sv[0][j], sv[1][j], sv[2][j]);
+  }
 #pragma unroll
   for (int v = 0; v < N / 4; ++v)
     *reinterpret_cast<float4*>(w_ptr + 4 * v) = make_float4(w_out[4 * v], w_out[4 * v + 1], w_out[4 * v + 2], w_out[4 * v + 3]);

@@ -184,6 +184,11 @@ class DeepQNetwork:
         # device; update_target_network() keeps its hard copy.  It needs a separate target network (target_steps > 0).
         cfg.soft_target_tau = float(_arg(args, "soft_target_tau", 0.0) or 0.0)
         self.soft_target_tau = cfg.soft_target_tau
+        # global gradient-norm clipping: a new capability, off unless args.max_grad_norm = M > 0 (SB3's name; SB3 uses
+        # 10, as do OpenAI baselines' Atari DQN and the dueling paper).  Every train step scales the whole update by
+        # min(1, M / (||g / bsz|| + 1e-6)) on the device (b200dqn.h states the rule).  Fixed at creation.
+        cfg.max_grad_norm = float(_arg(args, "max_grad_norm", 0.0) or 0.0)
+        self.max_grad_norm = cfg.max_grad_norm or None
         h = C.c_void_p()
         L.call("b200dqn_net_create", self.device, C.byref(cfg), C.byref(h))
         self._h = h
@@ -313,6 +318,23 @@ class DeepQNetwork:
 
     def _read_f32(self, which, shape):
         return L.download(self.device, self.device_view(which, shape).ptr, shape, np.float32, self._stream)
+
+    def _read_clip(self, which, shape, dtype):
+        if not self.max_grad_norm:
+            raise ValueError("the net has no gradient-norm clipping (max_grad_norm)")
+        return L.download(self.device, self.device_view(which, shape).ptr, shape, dtype, self._stream)
+
+    def last_grad_sq(self):
+        """(6,) float64 per-layer sums of squares S_l of g / bsz of the last train step (layer 5: the embedding)."""
+        return self._read_clip(L.NET_PTR_GRAD_SQ, (6,), np.float64)
+
+    def last_grad_norm(self):
+        """The global gradient norm N (float64) of the last train step."""
+        return float(self._read_clip(L.NET_PTR_GRAD_NORM, (1,), np.float64)[0])
+
+    def last_clip_scale(self):
+        """The clip coefficient c32 (float32) the last train step scaled its update by."""
+        return self._read_clip(L.NET_PTR_CLIP_SCALE, (1,), np.float32)[0]
 
     def last_q(self):
         """(preq, postq) of the last train() as (batch, A) arrays (deepqnetwork.py:120,129)."""

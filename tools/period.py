@@ -27,6 +27,7 @@ FQF = int(os.environ.get("FQF", "0"))   # FQF head with this many fractions per 
 BOOT = int(os.environ.get("BOOT", "0"))   # bootstrapped DQN heads, this many per action; 0: off
 BOOT_P = float(os.environ.get("BOOT_P", "0.5"))   # the bootstrapped heads' mask probability
 TAU = float(os.environ.get("TAU", "0"))   # soft target update: blend the target towards the online net by TAU every step
+MAX_GRAD_NORM = float(os.environ.get("MAX_GRAD_NORM", "0"))   # global gradient-norm clipping at this norm; 0: off
 
 
 def args():
@@ -46,6 +47,7 @@ def args():
     a.fqf, a.num_fractions = FQF > 0, FQF
     a.bootstrapped, a.bootstrap_heads, a.bootstrap_p = BOOT > 0, BOOT, BOOT_P
     a.soft_target_tau = TAU
+    a.max_grad_norm = MAX_GRAD_NORM
     return a
 
 
@@ -71,6 +73,6 @@ for _ in range(2):
     st.synchronize()
     t = time.time(); net.train_fused(mem, 300); t_enq = time.time() - t; st.synchronize(); t_all = time.time() - t
     print("300 steps: host enqueue %.1f us/step, until done %.1f us/step" % (t_enq / 300 * 1e6, t_all / 300 * 1e6))
-print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d munchausen %d iqn %d shift %d rem %d fqf %d boot %d boot_p %g tau %g period_us min %.2f median %.2f  "
-      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, MUNCHAUSEN, IQN, SHIFT, REM, FQF, BOOT, BOOT_P, TAU, min(res), float(np.median(res)),
+print("math %s batch %d hist %d double %d per %d nstep %d actions %d atoms %d dueling %d quantiles %d munchausen %d iqn %d shift %d rem %d fqf %d boot %d boot_p %g tau %g max_grad_norm %g period_us min %.2f median %.2f  "
+      "all %s" % (net.math_mode, B, HIST, DOUBLE, PER, NSTEP, NACT, ATOMS, DUELING, QUANTILES, MUNCHAUSEN, IQN, SHIFT, REM, FQF, BOOT, BOOT_P, TAU, MAX_GRAD_NORM, min(res), float(np.median(res)),
                   " ".join("%.2f" % r for r in res)))

@@ -21,6 +21,7 @@ FQF = int(os.environ.get("FQF", "0"))   # FQF head with this many fractions per 
 BOOT = int(os.environ.get("BOOT", "0"))   # bootstrapped DQN heads, this many per action; 0: off
 BOOT_P = float(os.environ.get("BOOT_P", "0.5"))   # the bootstrapped heads' mask probability
 TAU = float(os.environ.get("TAU", "0"))   # soft target update: blend the target towards the online net by TAU every step
+MAX_GRAD_NORM = float(os.environ.get("MAX_GRAD_NORM", "0"))   # global gradient-norm clipping at this norm; 0: off
 
 
 def net_args():
@@ -35,6 +36,7 @@ def net_args():
     a.fqf, a.num_fractions = FQF > 0, FQF
     a.bootstrapped, a.bootstrap_heads, a.bootstrap_p = BOOT > 0, BOOT, BOOT_P
     a.soft_target_tau = TAU
+    a.max_grad_norm = MAX_GRAD_NORM
     return a
 
 
