@@ -597,8 +597,8 @@ extern "C" int b200dqn_net_comm_destroy(b200dqn_net* n) {
   DeviceGuard g(n->device);
   cudaDeviceSynchronize();
   // captured steps hold nodes of this communicator
-  if (n->graph_exec) { cudaGraphExecDestroy(n->graph_exec); n->graph_exec = nullptr; }
-  if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
+  n->graph_step.drop();
+  n->graph_train.drop();
   comm_destroy(n);
   return B200DQN_OK;
 }

@@ -4,6 +4,7 @@
 
 #include <cmath>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_fp16.h>
@@ -1946,6 +1947,12 @@ __global__ void k_zero_rows(float* q, int from, int to, int A) {
 static inline unsigned cdiv(int64_t a, int64_t b) { return unsigned((a + b - 1) / b); }
 static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
+#define B2_TRY(expr)          \
+  do {                        \
+    int rc__ = (expr);        \
+    if (rc__) return rc__;    \
+  } while (0)
+
 template <class P, int BM, int BN, int BK, int TM, int TN>
 static int launch_gemm(const char* label, const P& p, int M, int N, int Z, cudaStream_t st) {
   dim3 grid(cdiv(M, BM), cdiv(N, BN), Z);
@@ -1989,6 +1996,23 @@ static int conv1_fwd_simt(b200dqn_net* n, const FrameSource& fs, const float* co
   return launch_gemm<Conv1Fwd, 64, 32, 16, 4, 2>("conv1_fwd", p, rows * kP1 * kP1, kC1, nets, st);
 }
 
+// conv2 and conv3's forward on the SIMT engine for `nets` slots
+static int conv23_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int rows, cudaStream_t st) {
+  const LayerTable& lt = n->lt;
+  {
+    using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
+    P p;
+    for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
+    p.nb = rows;
+    B2_TRY((launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st)));
+  }
+  using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
+  P p;
+  for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
+  p.nb = rows;
+  return launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st);
+}
+
 // fc1's forward on the SIMT engine at width W (kHidden, or kDuelHidden on a dueling net)
 template <int W>
 static int fc1_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int rows, cudaStream_t st) {
@@ -1996,6 +2020,106 @@ static int fc1_fwd_simt(b200dqn_net* n, const float* const w[3], int nets, int r
   for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h3[z]; p.w[z] = w[z] + n->lt.off[3]; }
   p.part = n->d_fc1part; p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
   return launch_gemm<Fc1Fwd<W>, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, W, nets * kFc1Splits, st);
+}
+
+// fc1's forward on the SIMT engine on IQN / FQF modulated rows: `nets` slots of `rows` rows, slot z's at in[z]
+static int fc1_fwd_x_simt(b200dqn_net* n, const float* const in[3], const float* const w[3], int nets, int rows,
+                          cudaStream_t st) {
+  Fc1Fwd<kHidden> p;
+  for (int z = 0; z < 3; ++z) { p.in[z] = in[z]; p.w[z] = w[z] + n->lt.off[3]; }
+  p.part = n->d_fc1part; p.nb = rows; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
+  return launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, rows, kHidden, nets * kFc1Splits, st);
+}
+
+// fc1's forward on the IQN / FQF modulated rows X: `nets` slots (slot 1's X at ld rows past slot 0's) of `rows`
+// expanded rows, `splits` the k-split count the tensor-core engine was given
+static int fc1_fwd_x(b200dqn_net* n, int nets, int rows, int ld, int splits, cudaStream_t st) {
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) return umma_fc1_fwd_iqn(n, nets, rows, splits, st);
+  const float* x[3] = {n->d_x, n->d_x + int64_t(ld) * kFlat, n->d_x};
+  const float* w[3] = {n->d_w, n->d_tw, n->d_w};
+  return fc1_fwd_x_simt(n, x, w, nets, rows, st);
+}
+
+// The conv trunk for `nets` network slots of `rows` samples, and fc1 on H3 unless trunk_only (an IQN or FQF head runs
+// fc1 on its modulated rows instead), on whichever engine math_mode selects.  One GPU: the tensor-core forward launches
+// are links of the critical chain (umma_forward picks the ones that release early).
+static int forward_trunk(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st, bool trunk_only) {
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05)
+    return umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1, trunk_only);
+  const float* w[3] = {n->d_w, n->d_tw, n->d_w};
+  B2_TRY(conv1_fwd_simt(n, fs, w, nets, rows, st));
+  B2_TRY(conv23_fwd_simt(n, w, nets, rows, st));
+  if (trunk_only) return B200DQN_OK;
+  return n->dueling ? fc1_fwd_simt<kDuelHidden>(n, w, nets, rows, st) : fc1_fwd_simt<kHidden>(n, w, nets, rows, st);
+}
+
+// fc2 of a per-action head (C51, QR, REM) or of the IQN / FQF rows: `nets` slots of `rows` rows from the fc1 partials
+// at `splits` k-splits, slot z's H4 at h4[z] and weights at w[z], into out (slot stride ld rows) at `ncols` columns
+static int fc2_dist(b200dqn_net* n, int nets, int rows, int ld, int splits, float* const h4[2],
+                    const float* const w[2], float* out, int ncols, const char* prof, cudaStream_t st) {
+  const int64_t o = n->lt.off[4];
+  B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
+                           (const float*)n->d_fc1part, splits, rows, ld, h4[0], h4[1], w[0] + o, w[1] + o, out, ncols,
+                           ktrace_slot("fc2_dist")));
+  B2_PROF(prof, st);
+  return B200DQN_OK;
+}
+
+// Calls f(std::integral_constant<int, S>{}, std::bool_constant<N>{}) with the instantiation <S, N> of a head kernel
+// for `slots` network slots and the n-step flag.  Every head is instantiated at S = 2; kOther lists the other slot
+// counts it has: 3 (Double DQN, the Munchausen target pass) and 1 (predict, one-step only).  An unlisted count takes 2.
+// The instantiations are made in the order 3, 2, 1, the order of the kernels in the library.
+template <int... kOther, class F>
+static auto with_head(int slots, bool nstep, F&& f) {
+  auto at = [&](auto s) { return nstep ? f(s, std::true_type{}) : f(s, std::false_type{}); };
+  if constexpr (((kOther == 3) || ...)) {
+    if (slots == 3) return at(std::integral_constant<int, 3>{});
+  }
+  if constexpr (((kOther == 1) || ...)) {
+    if (slots != 1) return at(std::integral_constant<int, 2>{});
+    return f(std::integral_constant<int, 1>{}, std::false_type{});
+  } else {
+    return at(std::integral_constant<int, 2>{});
+  }
+}
+
+// Side branches of a step on a stream: a draw that reads only its counter, or the Munchausen target pass, which reads
+// only weights and frames, forks from st onto a side stream and joins st later, overlapping the chain.  Work on a branch
+// gets ordinary dependencies (see NoPdlScope).  Branches are off without a stream, on the serial schedule and under the
+// event profiler.
+static bool branches_on(const b200dqn_net* n, cudaStream_t st) { return n->use_branches && st != nullptr && !g_prof_on; }
+
+// body(s) on a branch forked from st when `on`: on n->side[side], between events ev[e] (the fork, on st) and ev[e + 1]
+// (its end, on the branch, returned in *done).  Otherwise body(st) runs in line and *done is nullptr.
+template <class F>
+static int fork_branch(b200dqn_net* n, cudaStream_t st, bool on, int side, int e, cudaEvent_t* done, F&& body) {
+  *done = nullptr;
+  if (!on) return body(st);
+  cudaStream_t s = n->side[side];
+  B2_CHECK_CUDA(cudaEventRecord(n->ev[e], st));
+  B2_CHECK_CUDA(cudaStreamWaitEvent(s, n->ev[e], 0));
+  {
+    NoPdlScope branch;
+    B2_TRY(body(s));
+  }
+  B2_CHECK_CUDA(cudaEventRecord(n->ev[e + 1], s));
+  *done = n->ev[e + 1];
+  return B200DQN_OK;
+}
+
+// st waits for a branch's end `done` (nothing when the branch ran in line)
+static int join_branch(cudaStream_t st, cudaEvent_t done) {
+  if (done) B2_CHECK_CUDA(cudaStreamWaitEvent(st, done, 0));
+  return B200DQN_OK;
+}
+
+// ... and launch(), the first launch on st that reads the branch's work, gets ordinary dependencies on both
+template <class F>
+static int join_branch(cudaStream_t st, cudaEvent_t done, F&& launch) {
+  B2_TRY(join_branch(st, done));
+  if (!done) return launch();
+  NoPdlScope joined;
+  return launch();
 }
 
 // The IQN forward for `nets` slots of `rows` samples: tau and phi, the conv trunk at `rows`, then X = psi
@@ -2006,80 +2130,37 @@ static int forward_iqn(b200dqn_net* n, const FrameSource& fs, int nets, int rows
   const LayerTable& lt = n->lt;
   const float* w[3] = {n->d_w, n->d_tw, n->d_w};
   const int per = td.enable ? n->iqn_n : n->iqn_k, R = rows * per, ld = n->iqn_rows;
-  const bool branch = n->use_branches && st != nullptr && !g_prof_on;
-  cudaStream_t sP = branch ? n->side[0] : st;
-  const bool prev = g_pdl_suppressed;
-  if (branch) {
-    B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
-    B2_CHECK_CUDA(cudaStreamWaitEvent(sP, n->ev[15], 0));
-    g_pdl_suppressed = true;
-  }
-  cudaError_t e = launch_pdl(k_iqn_tau, dim3(1), dim3(1024), 0, sP, n->d_tau_ctr, (unsigned long long)n->cfg.tau_seed,
-                             nets, rows, per, ld, n->d_tau, ktrace_slot("iqn_tau"));
-  if (e == cudaSuccess)
-    e = launch_pdl(k_iqn_phi, dim3(cdiv(R, kIqnTB), nets), dim3(256), 0, sP, (const float*)n->d_tau, R, ld,
-                   (const float*)n->d_we, (const float*)n->d_twe, n->d_cos, n->d_phi, ktrace_slot("iqn_phi"));
-  g_pdl_suppressed = prev;
-  B2_CHECK_CUDA(e);
-  B2_PROF("iqn_tau+phi", sP);
-  if (branch) B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sP));
+  cudaEvent_t embedded;
+  B2_TRY(fork_branch(n, st, branches_on(n, st), 0, 15, &embedded, [&](cudaStream_t sP) {
+    B2_CHECK_CUDA(launch_pdl(k_iqn_tau, dim3(1), dim3(1024), 0, sP, n->d_tau_ctr, (unsigned long long)n->cfg.tau_seed,
+                             nets, rows, per, ld, n->d_tau, ktrace_slot("iqn_tau")));
+    B2_CHECK_CUDA(launch_pdl(k_iqn_phi, dim3(cdiv(R, kIqnTB), nets), dim3(256), 0, sP, (const float*)n->d_tau, R, ld,
+                             (const float*)n->d_we, (const float*)n->d_twe, n->d_cos, n->d_phi, ktrace_slot("iqn_phi")));
+    B2_PROF("iqn_tau+phi", sP);
+    return B200DQN_OK;
+  }));
   const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
   // the tensor-core fc1 picks its split count by row count; it is taken at the full minibatch, so a predict on fewer
   // live rows sums every row as the full one does
   const int splits = tc ? umma_fc1_splits(n->nb * per) : kFc1Splits;
-  int rc;
-  if (tc) {
-    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1, true))) return rc;
-  } else {
-    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
-    {
-      using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
-    }
-    {
-      using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
-    }
-  }
-  if (branch) {   // the embedding's branch joins here: the modulation gets ordinary dependencies on both
-    B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[16], 0));
-    g_pdl_suppressed = true;
-  }
+  B2_TRY(forward_trunk(n, fs, nets, rows, st, true));
   const int64_t total = int64_t(nets) * R * kFlat;
-  e = launch_pdl(k_iqn_mod, dim3(unsigned(std::min<int64_t>(cdiv(total, 256), int64_t(n->sm_count) * 16))), dim3(256), 0,
-                 st, (const float*)n->d_h3[0], (const float*)n->d_h3[1], (const float*)n->d_phi, n->d_x, n->d_x16, nets,
-                 R, per, ld, ktrace_slot("iqn_mod"));
-  g_pdl_suppressed = prev;
-  B2_CHECK_CUDA(e);
+  B2_TRY(join_branch(st, embedded, [&] {
+    B2_CHECK_CUDA(launch_pdl(k_iqn_mod, dim3(unsigned(std::min<int64_t>(cdiv(total, 256), int64_t(n->sm_count) * 16))),
+                             dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_h3[1],
+                             (const float*)n->d_phi, n->d_x, n->d_x16, nets, R, per, ld, ktrace_slot("iqn_mod")));
+    return B200DQN_OK;
+  }));
   B2_PROF("iqn_mod", st);
-  if (tc) {
-    if ((rc = umma_fc1_fwd_iqn(n, nets, R, splits, st))) return rc;
-  } else {
-    Fc1Fwd<kHidden> p;
-    for (int z = 0; z < 3; ++z) {
-      p.in[z] = n->d_x + int64_t(z < 2 ? z : 0) * ld * kFlat;
-      p.w[z] = w[z] + lt.off[3];
-    }
-    p.part = n->d_fc1part; p.nb = R; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
-    if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, R, kHidden, nets * kFc1Splits, st))) return rc;
-  }
-  B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(R, kDistTB), cdiv(n->A, kDistTN), nets), dim3(256), 0, st,
-                           (const float*)n->d_fc1part, splits, R, ld, n->d_h4[0],
-                           n->d_h4[1], w[0] + lt.off[4],
-                           w[1] + lt.off[4], n->d_iqn_theta, n->A, ktrace_slot("fc2_dist")));
-  B2_PROF("fc2_dist", st);
+  B2_TRY(fc1_fwd_x(n, nets, R, ld, splits, st));
+  B2_TRY(fc2_dist(n, nets, R, ld, splits, n->d_h4, w, n->d_iqn_theta, n->A, "fc2_dist", st));
   const IqnArgs ia{per, ld, float(n->cfg.clip_error), n->d_tau, n->d_iqn_tq, n->d_iqn_qgrad, n->d_act_rows};
   const bool nstep = td.enable && td.nstep > 1;
-  auto* kern = nets == 1 ? k_head_iqn<1, false> : nstep ? k_head_iqn<2, true> : k_head_iqn<2, false>;
-  B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_iqn_theta, nets,
-                           (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->A, ia, td,
-                           ktrace_slot("head_iqn")));
+  B2_CHECK_CUDA(with_head<1>(nets, nstep, [&](auto s, auto ns) {
+    return launch_pdl(k_head_iqn<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                      (const float*)n->d_iqn_theta, nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0],
+                      n->d_q[1], n->A, ia, td, ktrace_slot("head_iqn"));
+  }));
   B2_PROF(td.enable ? "head_iqn(td+fc2_bwd)" : "head_iqn", st);
   return B200DQN_OK;
 }
@@ -2096,26 +2177,7 @@ static int forward_fqf(b200dqn_net* n, const FrameSource& fs, int nets, int rows
   const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
   // split counts are taken at the full minibatch, so a predict on fewer live rows sums every row as the full one does
   const int splits = tc ? umma_fc1_splits(n->nb * N) : kFc1Splits;
-  int rc;
-  if (tc) {
-    if ((rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1, true))) return rc;
-  } else {
-    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
-    {
-      using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
-    }
-    {
-      using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
-    }
-  }
+  B2_TRY(forward_trunk(n, fs, nets, rows, st, true));
   B2_CHECK_CUDA(launch_pdl(k_fqf_fraction, dim3(rows), dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_wf,
                            N, nets, ld, n->d_fl, n->d_fq, n->d_ftau, n->d_tau, td.enable ? n->d_btau : nullptr,
                            ktrace_slot("fqf_fraction")));
@@ -2128,21 +2190,8 @@ static int forward_fqf(b200dqn_net* n, const FrameSource& fs, int nets, int rows
                            dim3(256), 0, st, (const float*)n->d_h3[0], (const float*)n->d_h3[1], (const float*)n->d_phi,
                            n->d_x, n->d_x16, nets, R, N, ld, ktrace_slot("iqn_mod")));
   B2_PROF("iqn_mod", st);
-  if (tc) {
-    if ((rc = umma_fc1_fwd_iqn(n, nets, R, splits, st))) return rc;
-  } else {
-    Fc1Fwd<kHidden> p;
-    for (int z = 0; z < 3; ++z) {
-      p.in[z] = n->d_x + int64_t(z < 2 ? z : 0) * ld * kFlat;
-      p.w[z] = w[z] + lt.off[3];
-    }
-    p.part = n->d_fc1part; p.nb = R; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
-    if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, R, kHidden, nets * kFc1Splits, st))) return rc;
-  }
-  B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(R, kDistTB), cdiv(n->A, kDistTN), nets), dim3(256), 0, st,
-                           (const float*)n->d_fc1part, splits, R, ld, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
-                           w[1] + lt.off[4], n->d_iqn_theta, n->A, ktrace_slot("fc2_dist")));
-  B2_PROF("fc2_dist", st);
+  B2_TRY(fc1_fwd_x(n, nets, R, ld, splits, st));
+  B2_TRY(fc2_dist(n, nets, R, ld, splits, n->d_h4, w, n->d_iqn_theta, n->A, "fc2_dist", st));
   if (td.enable) {   // the boundary pass: the online network at tau_1..tau_{N-1}, on buffers of its own
     B2_CHECK_CUDA(launch_pdl(k_iqn_phi, dim3(cdiv(Rb, kIqnTB), 1), dim3(256), 0, st, (const float*)n->d_btau, Rb, Rb,
                              (const float*)n->d_we, (const float*)n->d_we, n->d_bcos, n->d_bphi, ktrace_slot("iqn_phi")));
@@ -2153,28 +2202,22 @@ static int forward_fqf(b200dqn_net* n, const FrameSource& fs, int nets, int rows
                              (const float*)n->d_bphi, n->d_bx, n->d_bx16, 1, Rb, N - 1, Rb, ktrace_slot("iqn_mod")));
     B2_PROF("fqf_bnd_mod", st);
     const int bsplits = tc ? umma_fc1_splits(Rb) : kFc1Splits;
-    if (tc) {
-      if ((rc = umma_fc1_fwd_fqf_boundary(n, Rb, bsplits, st))) return rc;
-    } else {
-      Fc1Fwd<kHidden> p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_bx; p.w[z] = w[0] + lt.off[3]; }
-      p.part = n->d_fc1part; p.nb = Rb; p.splits = kFc1Splits; p.kchunk = kFc1Chunk;
-      if ((rc = launch_gemm<Fc1Fwd<kHidden>, 32, 64, 16, 2, 4>("fc1_fwd", p, Rb, kHidden, kFc1Splits, st))) return rc;
-    }
-    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(Rb, kDistTB), cdiv(n->A, kDistTN), 1), dim3(256), 0, st,
-                             (const float*)n->d_fc1part, bsplits, Rb, Rb, n->d_bh4, n->d_bh4, w[0] + lt.off[4],
-                             w[0] + lt.off[4], n->d_btheta, n->A, ktrace_slot("fc2_dist")));
-    B2_PROF("fqf_bnd_fc2", st);
+    const float* bx[3] = {n->d_bx, n->d_bx, n->d_bx};
+    const float* bw[3] = {w[0], w[0], w[0]};
+    B2_TRY(tc ? umma_fc1_fwd_fqf_boundary(n, Rb, bsplits, st) : fc1_fwd_x_simt(n, bx, bw, 1, Rb, st));
+    float* bh4[2] = {n->d_bh4, n->d_bh4};
+    B2_TRY(fc2_dist(n, 1, Rb, Rb, bsplits, bh4, bw, n->d_btheta, n->A, "fqf_bnd_fc2", st));
   }
   const IqnArgs ia{N, ld, float(n->cfg.clip_error), n->d_tau, n->d_iqn_tq, n->d_iqn_qgrad, n->d_act_rows};
   const bool adam = n->cfg.optimizer == B200DQN_OPT_ADAM;
   const FqfArgs fa{n->d_ftau, n->d_fq, n->d_btheta, n->d_fg, n->d_fdl, float(n->cfg.fraction_lr),
                    adam ? n->d_optscal + 2 : nullptr};
   const bool nstep = td.enable && td.nstep > 1;
-  auto* kern = nets == 1 ? k_head_fqf<1, false> : nstep ? k_head_fqf<2, true> : k_head_fqf<2, false>;
-  B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_iqn_theta, nets,
-                           (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->A, ia, fa, td,
-                           ktrace_slot("head_fqf")));
+  B2_CHECK_CUDA(with_head<1>(nets, nstep, [&](auto s, auto ns) {
+    return launch_pdl(k_head_fqf<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                      (const float*)n->d_iqn_theta, nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0],
+                      n->d_q[1], n->A, ia, fa, td, ktrace_slot("head_fqf"));
+  }));
   B2_PROF(td.enable ? "head_fqf(td+fc2_bwd)" : "head_fqf", st);
   return B200DQN_OK;
 }
@@ -2219,87 +2262,51 @@ static int iqn_backward(b200dqn_net* n, int rows, cudaStream_t st, cudaStream_t 
 
 // Model.fprop for `nets` network slots on `rows` samples: z = 0 online (prestates), z = 1 target (poststates) and,
 // for a Double DQN train step (nets = 3), z = 2 online on slot 1's frames (the poststates).
-// join (Munchausen or REM train step on a stream): the event of the target pass's or the mixture draw's branch, waited
-// for before the head.
+// join (Munchausen or REM train step on a stream): the end of the target pass's or the mixture draw's branch, joined
+// before the head.
 static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cudaStream_t st,
                    const HeadTrainArgs& td, cudaEvent_t join = nullptr) {
   if (n->fqf_n) return forward_fqf(n, fs, nets, rows, st, td);
   if (n->iqn_n) return forward_iqn(n, fs, nets, rows, st, td);
   const LayerTable& lt = n->lt;
   const float* w[3] = {n->d_w, n->d_tw, n->d_w};
-  int rc;
-  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
-    // one GPU: the forward launches are links of the critical chain (umma_forward picks the ones that release early)
-    rc = umma_forward(n, fs.src, fs.idx, fs.shift, fs.crop, nets, rows, st, n->world == 1);
-    if (rc) return rc;
-  } else {
-    if ((rc = conv1_fwd_simt(n, fs, w, nets, rows, st))) return rc;
-    {
-      using P = ConvFwd<kP1, kC1, 4, 2, kC2>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h1[z]; p.w[z] = w[z] + lt.off[1]; p.out[z] = n->d_h2[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv2_fwd", p, rows * kP2 * kP2, kC2, nets, st))) return rc;
-    }
-    {
-      using P = ConvFwd<kP2, kC2, 3, 1, kC3>;
-      P p;
-      for (int z = 0; z < 3; ++z) { p.in[z] = n->d_h2[z]; p.w[z] = w[z] + lt.off[2]; p.out[z] = n->d_h3[z]; }
-      p.nb = rows;
-      if ((rc = launch_gemm<P, 32, 64, 16, 2, 4>("conv3_fwd", p, rows * kP3 * kP3, kC3, nets, st))) return rc;
-    }
-    if ((rc = n->dueling ? fc1_fwd_simt<kDuelHidden>(n, w, nets, rows, st) : fc1_fwd_simt<kHidden>(n, w, nets, rows, st)))
-      return rc;
-  }
+  B2_TRY(forward_trunk(n, fs, nets, rows, st, false));
   const int fc1_splits = n->cfg.math_mode == B200DQN_MATH_TCGEN05 ? umma_fc1_splits(rows) : kFc1Splits;
   const bool nstep = td.enable && td.nstep > 1;
   if (n->dueling) {
-    B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head_duel<3, true> : k_head_duel<3, false>)
-                                       : (nstep ? k_head_duel<2, true> : k_head_duel<2, false>),
-                             dim3(rows), dim3(kDuelHidden), 0, st, (const float*)n->d_fc1part, fc1_splits, rows, nets,
-                             n->nb, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1],
-                             n->d_q[2], n->d_va, n->A, td, ktrace_slot("head_duel")));
+    B2_CHECK_CUDA(with_head<3>(nets, nstep, [&](auto s, auto ns) {
+      return launch_pdl(k_head_duel<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kDuelHidden), 0, st,
+                        (const float*)n->d_fc1part, fc1_splits, rows, nets, n->nb, n->d_h4[0], n->d_h4[1],
+                        w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->d_va, n->A, td,
+                        ktrace_slot("head_duel"));
+    }));
     B2_PROF(td.enable ? "head_duel(td+fc2_bwd)" : "head_duel", st);
     return B200DQN_OK;
   }
   if (n->atoms) {
-    const int ncols = n->fc2_cols();
-    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
-                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
-                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_logits, ncols, ktrace_slot("fc2_dist")));
-    B2_PROF("fc2_dist", st);
+    B2_TRY(fc2_dist(n, nets, rows, n->nb, fc1_splits, n->d_h4, w, n->d_logits, n->fc2_cols(), "fc2_dist", st));
     const DistArgs da{n->atoms, n->cfg.v_min, n->cfg.v_max, n->dz, n->d_probs, n->d_tdist, n->d_lgrad, n->d_act_rows};
-    auto* kern = nets == 1 ? k_head_dist<1, false>
-               : nets == 3 ? (nstep ? k_head_dist<3, true> : k_head_dist<3, false>)
-                           : (nstep ? k_head_dist<2, true> : k_head_dist<2, false>);
-    B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_logits, n->nb, nets,
-                             (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, da, td,
-                             ktrace_slot("head_dist")));
+    B2_CHECK_CUDA((with_head<3, 1>(nets, nstep, [&](auto s, auto ns) {
+      return launch_pdl(k_head_dist<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                        (const float*)n->d_logits, n->nb, nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0],
+                        n->d_q[1], n->d_q[2], n->A, da, td, ktrace_slot("head_dist"));
+    })));
     B2_PROF(td.enable ? "head_dist(td+fc2_bwd)" : "head_dist", st);
     return B200DQN_OK;
   }
   if (n->quantiles) {
-    const int ncols = n->fc2_cols();
-    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
-                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
-                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_theta, ncols, ktrace_slot("fc2_dist")));
-    B2_PROF("fc2_dist", st);
+    B2_TRY(fc2_dist(n, nets, rows, n->nb, fc1_splits, n->d_h4, w, n->d_theta, n->fc2_cols(), "fc2_dist", st));
     const QrArgs qa{n->quantiles, float(n->cfg.clip_error), n->d_tquant, n->d_qgrad, n->d_act_rows};
-    auto* kern = nets == 1 ? k_head_qr<1, false>
-               : nets == 3 ? (nstep ? k_head_qr<3, true> : k_head_qr<3, false>)
-                           : (nstep ? k_head_qr<2, true> : k_head_qr<2, false>);
-    B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
-                             (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, qa, td,
-                             ktrace_slot("head_qr")));
+    B2_CHECK_CUDA((with_head<3, 1>(nets, nstep, [&](auto s, auto ns) {
+      return launch_pdl(k_head_qr<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                        (const float*)n->d_theta, n->nb, nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0],
+                        n->d_q[1], n->d_q[2], n->A, qa, td, ktrace_slot("head_qr"));
+    })));
     B2_PROF(td.enable ? "head_qr(td+fc2_bwd)" : "head_qr", st);
     return B200DQN_OK;
   }
   if (n->rem_k) {
-    const int ncols = n->fc2_cols();
-    B2_CHECK_CUDA(launch_pdl(k_fc2_dist, dim3(cdiv(rows, kDistTB), cdiv(ncols, kDistTN), nets), dim3(256), 0, st,
-                             (const float*)n->d_fc1part, fc1_splits, rows, n->nb, n->d_h4[0], n->d_h4[1],
-                             w[0] + lt.off[4], w[1] + lt.off[4], n->d_theta, ncols, ktrace_slot("fc2_dist")));
-    B2_PROF("fc2_dist", st);
+    B2_TRY(fc2_dist(n, nets, rows, n->nb, fc1_splits, n->d_h4, w, n->d_theta, n->fc2_cols(), "fc2_dist", st));
     if (!td.enable && n->boot) {   // predict at the active head, read on the device
       B2_CHECK_CUDA(launch_pdl(k_boot_predict, dim3(rows), dim3(32), 0, st, (const float*)n->d_theta, n->A, n->rem_k,
                                (const int32_t*)n->d_boot_head, n->d_q[0], ktrace_slot("boot_predict")));
@@ -2309,11 +2316,11 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     if (n->boot) {
       const BootArgs ba{(unsigned long long)n->cfg.bootstrap_seed, n->cfg.bootstrap_p, n->d_boot_mask, n->d_boot_y,
                         n->d_boot_delta, n->d_rem_grad, n->d_act_rows};
-      auto* kern = nets == 3 ? (nstep ? k_head_boot<3, true> : k_head_boot<3, false>)
-                             : (nstep ? k_head_boot<2, true> : k_head_boot<2, false>);
-      B2_CHECK_CUDA(launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
-                               (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A,
-                               n->rem_k, ba, td, ktrace_slot("head_boot")));
+      B2_CHECK_CUDA(with_head<3>(nets, nstep, [&](auto s, auto ns) {
+        return launch_pdl(k_head_boot<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                          (const float*)n->d_theta, n->nb, nets, (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0],
+                          n->d_q[1], n->d_q[2], n->A, n->rem_k, ba, td, ktrace_slot("head_boot"));
+      }));
       B2_PROF("head_boot(td+fc2_bwd)", st);
       return B200DQN_OK;
     }
@@ -2325,19 +2332,15 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
       B2_PROF("head_qr", st);
       return B200DQN_OK;
     }
-    const bool prev = g_pdl_suppressed;
-    if (join) {   // the mixture draw's branch joins here: the head gets ordinary dependencies on both
-      B2_CHECK_CUDA(cudaStreamWaitEvent(st, join, 0));
-      g_pdl_suppressed = true;
-    }
-    auto* kern = nets == 3 ? (nstep ? k_head_rem<3, true> : k_head_rem<3, false>)
-                           : (nstep ? k_head_rem<2, true> : k_head_rem<2, false>);
-    const cudaError_t e = launch_pdl(kern, dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_theta, n->nb, nets,
-                                     (const float*)n->d_h4[0], w[0] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A,
-                                     n->rem_k, (const float*)n->d_rem_alpha, n->d_rem_grad, n->d_act_rows, td,
-                                     ktrace_slot("head_rem"));
-    g_pdl_suppressed = prev;
-    B2_CHECK_CUDA(e);
+    B2_TRY(join_branch(st, join, [&] {   // the mixture draw's branch
+      return with_head<3>(nets, nstep, [&](auto s, auto ns) {
+        B2_CHECK_CUDA(launch_pdl(k_head_rem<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                                 (const float*)n->d_theta, n->nb, nets, (const float*)n->d_h4[0], w[0] + lt.off[4],
+                                 n->d_q[0], n->d_q[1], n->d_q[2], n->A, n->rem_k, (const float*)n->d_rem_alpha,
+                                 n->d_rem_grad, n->d_act_rows, td, ktrace_slot("head_rem")));
+        return B200DQN_OK;
+      });
+    }));
     B2_PROF("head_rem(td+fc2_bwd)", st);
     return B200DQN_OK;
   }
@@ -2345,26 +2348,23 @@ static int forward(b200dqn_net* n, const FrameSource& fs, int nets, int rows, cu
     // slot 2, the target network on the prestates, exists with a separate target network only (train_step's pass)
     const bool pre = n->d_tw != n->d_w;
     const MdqnArgs ma{n->cfg.munchausen_alpha, n->cfg.munchausen_tau, n->cfg.munchausen_clip, n->d_q[2], n->d_tdtarget};
-    const bool prev = g_pdl_suppressed;
-    if (join) {   // the pass's branch joins here: the head gets ordinary dependencies on both
-      B2_CHECK_CUDA(cudaStreamWaitEvent(st, join, 0));
-      g_pdl_suppressed = true;
-    }
-    const cudaError_t e = launch_pdl(pre ? (nstep ? k_head_mdqn<3, true> : k_head_mdqn<3, false>)
-                                         : (nstep ? k_head_mdqn<2, true> : k_head_mdqn<2, false>),
-                                     dim3(rows), dim3(kHidden), 0, st, (const float*)n->d_fc1part, fc1_splits, rows,
-                                     n->d_h4[0], n->d_h4[1], w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1],
-                                     n->A, ma, td, ktrace_slot("head_mdqn"));
-    g_pdl_suppressed = prev;
-    B2_CHECK_CUDA(e);
+    B2_TRY(join_branch(st, join, [&] {   // the target pass's branch
+      return with_head<3>(pre ? 3 : 2, nstep, [&](auto s, auto ns) {
+        B2_CHECK_CUDA(launch_pdl(k_head_mdqn<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0,
+                                 st, (const float*)n->d_fc1part, fc1_splits, rows, n->d_h4[0], n->d_h4[1],
+                                 w[0] + lt.off[4], w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->A, ma, td,
+                                 ktrace_slot("head_mdqn")));
+        return B200DQN_OK;
+      });
+    }));
     B2_PROF("head_mdqn(td+fc2_bwd)", st);
     return B200DQN_OK;
   }
-  B2_CHECK_CUDA(launch_pdl(nets == 3 ? (nstep ? k_head<3, true> : k_head<3, false>)
-                                     : (nstep ? k_head<2, true> : k_head<2, false>),
-                           dim3(rows), dim3(kHidden), 0, st,
-                           (const float*)n->d_fc1part, fc1_splits, rows, nets, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
-                           w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, td, ktrace_slot("head")));
+  B2_CHECK_CUDA(with_head<3>(nets, nstep, [&](auto s, auto ns) {
+    return launch_pdl(k_head<decltype(s)::value, decltype(ns)::value>, dim3(rows), dim3(kHidden), 0, st,
+                      (const float*)n->d_fc1part, fc1_splits, rows, nets, n->d_h4[0], n->d_h4[1], w[0] + lt.off[4],
+                      w[1] + lt.off[4], n->d_q[0], n->d_q[1], n->d_q[2], n->A, td, ktrace_slot("head"));
+  }));
   B2_PROF(td.enable ? "head(fc2+td+fc2_bwd)" : "fc2_fwd", st);
   return B200DQN_OK;
 }
@@ -2572,12 +2572,6 @@ static int opt_fc2_small(b200dqn_net* n, int rows, cudaStream_t s) {
   return B200DQN_OK;
 }
 
-#define B2_TRY(expr)          \
-  do {                        \
-    int rc__ = (expr);        \
-    if (rc__) return rc__;    \
-  } while (0)
-
 // Soft target update of `elems` parameters at w / tw (elems a multiple of 4).
 static int soft_blend_range(b200dqn_net* n, const float* w, float* tw, int64_t elems, float c, float t, cudaStream_t st,
                             const char* label) {
@@ -2693,7 +2687,8 @@ static int clip_step_serial(b200dqn_net* n, int rows, cudaStream_t st) {
 // the moment its wgrad has finished, on that layer's own branch, and only conv1's 32 KB exchange is left
 // on the critical chain:  wgrad -> partial sums -> exchange (in place, all ranks) -> RMSProp from d_g.
 static void destroy_step_graphs(b200dqn_net* n) {
-  if (n->graph_exec) { cudaGraphExecDestroy(n->graph_exec); n->graph_exec = nullptr; }
+  n->graph_step.drop();
+  n->graph_train.drop();
 }
 
 static int backward_and_update_xchg(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
@@ -2914,6 +2909,29 @@ static int backward_and_update_multi(b200dqn_net* n, const FrameSource& fs, int 
   return B200DQN_OK;
 }
 
+// The branch streams of the single-GPU step: fc1 (sA), conv3 (sB), conv2 (sC) and the fourth branch (sN)
+struct StepBranches {
+  cudaStream_t sA, sB, sC, sN;
+};
+
+// the single-GPU step's end: every branch joins the main stream
+static int join_branches(b200dqn_net* n, cudaStream_t st, const StepBranches& br) {
+  const cudaStream_t s[4] = {br.sA, br.sB, br.sC, br.sN};
+  for (int i = 0; i < 4; ++i) B2_CHECK_CUDA(cudaEventRecord(n->ev[4 + i], s[i]));
+  for (int i = 0; i < 4; ++i) B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[4 + i], 0));
+  return B200DQN_OK;
+}
+
+// conv layer l's update on the single-GPU branch schedule, on whichever engine math_mode selects, then its soft target
+// blend
+static int update_conv(b200dqn_net* n, int l, int rows, cudaStream_t s) {
+  static const char* const lbl[3] = {"opt_conv1", "opt_conv2", "opt_conv3"};
+  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, l, rows, s, lbl[l]));
+  else B2_TRY(optimizer_range(n, l, l, 1 | 4, rows, s, lbl[l]));
+  if (n->soft) B2_TRY(soft_update_layers(n, l, l, n->soft_c, n->soft_t, s));
+  return B200DQN_OK;
+}
+
 // The rest of the branches schedule under gradient-norm clipping, from fc1's dgrad on (ev[1] recorded, sA waiting on
 // it): each branch ends with its layer's reduce and sum of squares instead of its update; main joins every branch,
 // forms c32 and fans the clipped updates (with their image refreshes and soft target blends) back out over the same
@@ -2923,9 +2941,8 @@ static int backward_and_update_multi(b200dqn_net* n, const FrameSource& fs, int 
 //   sB   : conv3_wgrad .. [after conv3_dgrad] end(conv3)       [fan-out] opt(conv3)
 //   sC   : conv2_wgrad .. [after conv2_dgrad] end(conv2)       [fan-out] opt(conv2)
 //   sN   : cost . end(fc2) . end(embedding)                    [fan-out] opt(fc2) . opt(embedding)
-static int clip_branches(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st) {
-  cudaStream_t sA = g_prof_on ? st : n->side[0], sB = g_prof_on ? st : n->side[1], sC = g_prof_on ? st : n->side[2];
-  cudaStream_t sN = g_prof_on ? st : n->side[3];
+static int clip_branches(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st, const StepBranches& br) {
+  const auto [sA, sB, sC, sN] = br;
   cudaEvent_t* ev = n->ev;
   const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
   const bool fc2_on_sn = tc || n->fc2_block();   // else the SIMT engine's scalar fc2 rides with fc1 on sA
@@ -2949,14 +2966,7 @@ static int clip_branches(b200dqn_net* n, const FrameSource& fs, int rows, cudaSt
   B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st, true));
   NoPdlScope tail;   // the join and the fan-out use ordinary dependencies
   B2_TRY(clip_layer_end(n, 0, rows, st));
-  B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));                 // join: every S_l partial is written
-  B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
-  B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
-  B2_CHECK_CUDA(cudaEventRecord(ev[7], sN));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[4], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[5], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[6], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[7], 0));
+  B2_TRY(join_branches(n, st, br));   // every S_l partial is written
   B2_TRY(clip_scale(n, st));
   B2_CHECK_CUDA(cudaEventRecord(ev[9], st));                 // c32 ready
   for (cudaStream_t s : {sA, sB, sC, sN}) B2_CHECK_CUDA(cudaStreamWaitEvent(s, ev[9], 0));
@@ -2977,15 +2987,7 @@ static int clip_branches(b200dqn_net* n, const FrameSource& fs, int rows, cudaSt
   }
   B2_TRY(clip_apply(n, 0, rows, st));
   if (n->soft) B2_TRY(soft_update_layers(n, 0, 0, n->soft_c, n->soft_t, st));
-  B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));
-  B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
-  B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
-  B2_CHECK_CUDA(cudaEventRecord(ev[7], sN));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[4], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[5], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[6], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[7], 0));
-  return B200DQN_OK;
+  return join_branches(n, st, br);
 }
 
 static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, cudaStream_t st, bool update) {
@@ -3016,8 +3018,9 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
     }
     return B200DQN_OK;
   }
-  cudaStream_t sA = g_prof_on ? st : n->side[0], sB = g_prof_on ? st : n->side[1], sC = g_prof_on ? st : n->side[2];
-  cudaStream_t sN = g_prof_on ? st : n->side[3];
+  const StepBranches br{g_prof_on ? st : n->side[0], g_prof_on ? st : n->side[1], g_prof_on ? st : n->side[2],
+                        g_prof_on ? st : n->side[3]};
+  const auto [sA, sB, sC, sN] = br;
   cudaEvent_t* ev = n->ev;
   const bool tc = n->cfg.math_mode == B200DQN_MATH_TCGEN05;
   B2_CHECK_CUDA(cudaEventRecord(ev[0], st));                 // dZ4, the dW5 partials and the per-sample costs are ready
@@ -3046,7 +3049,7 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   }
   B2_CHECK_CUDA(cudaEventRecord(ev[1], st));                 // dZ3 ready, W4 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sA, ev[1], 0));
-  if (n->clip) return clip_branches(n, fs, rows, st);
+  if (n->clip) return clip_branches(n, fs, rows, st, br);
   {
     NoPdlScope side;
     if (tc && n->lt.splits[3] > 1) {                           // IQN: sum fc1's wgrad partials first
@@ -3064,69 +3067,42 @@ static int backward_and_update(b200dqn_net* n, const FrameSource& fs, int rows, 
   B2_TRY(bwd_op(n, fs, rows, kConv3Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[2], st));                 // dZ2 ready, W3 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sB, ev[2], 0));
-  {
-    NoPdlScope side;
-    if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 2, rows, sB, "opt_conv3"));
-    else B2_TRY(optimizer_range(n, 2, 2, 1 | 4, rows, sB, "opt_conv3"));
-    if (n->soft) B2_TRY(soft_update_layers(n, 2, 2, n->soft_c, n->soft_t, sB));
-  }
+  { NoPdlScope side; B2_TRY(update_conv(n, 2, rows, sB)); }
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[2], 0));
   { NoPdlScope side; B2_TRY(bwd_op(n, fs, rows, kConv2Wgrad, sC)); }
   B2_TRY(bwd_op(n, fs, rows, kConv2Dgrad, st, true));
   B2_CHECK_CUDA(cudaEventRecord(ev[3], st));                 // dZ1 ready, W2 no longer needed
   B2_CHECK_CUDA(cudaStreamWaitEvent(sC, ev[3], 0));
-  {
-    NoPdlScope side;
-    if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 1, rows, sC, "opt_conv2"));
-    else B2_TRY(optimizer_range(n, 1, 1, 1 | 4, rows, sC, "opt_conv2"));
-    if (n->soft) B2_TRY(soft_update_layers(n, 1, 1, n->soft_c, n->soft_t, sC));
-  }
+  { NoPdlScope side; B2_TRY(update_conv(n, 1, rows, sC)); }
   B2_TRY(bwd_op(n, fs, rows, kConv1Wgrad, st, true));
-  if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) B2_TRY(umma_opt_conv(n, 0, rows, st, "opt_conv1"));
-  else B2_TRY(optimizer_range(n, 0, 0, 1 | 4, rows, st, "opt_conv1"));
-  if (n->soft) B2_TRY(soft_update_layers(n, 0, 0, n->soft_c, n->soft_t, st));
-  B2_CHECK_CUDA(cudaEventRecord(ev[4], sA));
-  B2_CHECK_CUDA(cudaEventRecord(ev[5], sB));
-  B2_CHECK_CUDA(cudaEventRecord(ev[6], sC));
-  B2_CHECK_CUDA(cudaEventRecord(ev[7], sN));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[4], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[5], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[6], 0));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(st, ev[7], 0));
+  B2_TRY(update_conv(n, 0, rows, st));
+  return join_branches(n, st, br);
+}
+
+static int shift_draw(b200dqn_net* n, cudaStream_t s) {
+  B2_CHECK_CUDA(launch_pdl(k_shift_draw, dim3(1), dim3(1024), 0, s, n->d_crop_ctr,
+                           (unsigned long long)n->cfg.shift_seed, n->crop_pad, n->nb, n->d_crop,
+                           ktrace_slot("shift_draw")));
+  B2_PROF("shift_draw", s);
   return B200DQN_OK;
 }
 
 // The random-shift draw of a train step on its own branch from the head of the step (on a stream; the serial schedule
 // draws in line, in shift_join).  It reads only the counter, so it overlaps the sampler.
 static int shift_fork(b200dqn_net* n, cudaStream_t st) {
-  if (!n->crop_pad || n->crop_forked || !n->use_branches || st == nullptr || g_prof_on) return B200DQN_OK;
-  cudaStream_t sD = n->side[1];
-  B2_CHECK_CUDA(cudaEventRecord(n->ev[17], st));
-  B2_CHECK_CUDA(cudaStreamWaitEvent(sD, n->ev[17], 0));
-  {
-    NoPdlScope side;
-    B2_CHECK_CUDA(launch_pdl(k_shift_draw, dim3(1), dim3(1024), 0, sD, n->d_crop_ctr,
-                             (unsigned long long)n->cfg.shift_seed, n->crop_pad, n->nb, n->d_crop,
-                             ktrace_slot("shift_draw")));
-  }
-  B2_PROF("shift_draw", sD);
-  B2_CHECK_CUDA(cudaEventRecord(n->ev[18], sD));
+  if (!n->crop_pad || n->crop_forked || !branches_on(n, st)) return B200DQN_OK;
+  cudaEvent_t done;
+  B2_TRY(fork_branch(n, st, true, 1, 17, &done, [&](cudaStream_t sD) { return shift_draw(n, sD); }));
   n->crop_forked = true;
   return B200DQN_OK;
 }
 
-// The draw is complete on st from here on: its branch joins, or it runs here, in line.
+// The draw is complete on st from here on: its branch joins (the forward's first launch after it keeps its PDL), or it
+// runs here, in line.
 static int shift_join(b200dqn_net* n, cudaStream_t st) {
-  if (n->crop_forked) {
-    n->crop_forked = false;
-    B2_CHECK_CUDA(cudaStreamWaitEvent(st, n->ev[18], 0));
-    return B200DQN_OK;
-  }
-  B2_CHECK_CUDA(launch_pdl(k_shift_draw, dim3(1), dim3(1024), 0, st, n->d_crop_ctr,
-                           (unsigned long long)n->cfg.shift_seed, n->crop_pad, n->nb, n->d_crop,
-                           ktrace_slot("shift_draw")));
-  B2_PROF("shift_draw", st);
-  return B200DQN_OK;
+  if (!n->crop_forked) return shift_draw(n, st);
+  n->crop_forked = false;
+  return join_branch(st, n->ev[18]);
 }
 
 // One DeepQNetwork.train on device-resident inputs (the caller counts train_iterations, :168).
@@ -3161,43 +3137,18 @@ static int train_step(b200dqn_net* n, const FrameSource& fs_in, const uint8_t* a
     // The Munchausen target needs the target network on the prestates.  The pass reads only weights and frames, so on
     // a stream it forks into its own branch here, after the sampler, overlaps the forward and joins before the head;
     // on the serial schedule it runs in line, ahead of the forward.
-    if (n->use_branches && st != nullptr && !g_prof_on) {
-      cudaStream_t sP = n->side[0];
-      B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
-      B2_CHECK_CUDA(cudaStreamWaitEvent(sP, n->ev[15], 0));
-      {
-        NoPdlScope side;
-        B2_TRY(forward_target_pre(n, fs, rows, sP));
-      }
-      B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sP));
-      join = n->ev[16];
-    } else {
-      B2_TRY(forward_target_pre(n, fs, rows, st));
-    }
+    B2_TRY(fork_branch(n, st, branches_on(n, st), 0, 15, &join,
+                       [&](cudaStream_t sP) { return forward_target_pre(n, fs, rows, sP); }));
   }
   if (n->rem_k && !n->boot) {
     // The mixture draw reads only its counter, so on a stream it runs on its own branch from here and joins before the
     // head; on the serial schedule it runs in line, ahead of the forward.
-    const bool branch = n->use_branches && st != nullptr && !g_prof_on;
-    cudaStream_t sR = branch ? n->side[0] : st;
-    if (branch) {
-      B2_CHECK_CUDA(cudaEventRecord(n->ev[15], st));
-      B2_CHECK_CUDA(cudaStreamWaitEvent(sR, n->ev[15], 0));
-    }
-    {
-      const bool prev = g_pdl_suppressed;
-      g_pdl_suppressed = prev || branch;
-      const cudaError_t e = launch_pdl(k_rem_alpha, dim3(1), dim3(256), 0, sR, n->d_rem_ctr,
-                                       (unsigned long long)n->cfg.rem_seed, n->rem_k, n->d_rem_alpha,
-                                       ktrace_slot("rem_alpha"));
-      g_pdl_suppressed = prev;
-      B2_CHECK_CUDA(e);
-    }
-    B2_PROF("rem_alpha", sR);
-    if (branch) {
-      B2_CHECK_CUDA(cudaEventRecord(n->ev[16], sR));
-      join = n->ev[16];
-    }
+    B2_TRY(fork_branch(n, st, branches_on(n, st), 0, 15, &join, [&](cudaStream_t sR) {
+      B2_CHECK_CUDA(launch_pdl(k_rem_alpha, dim3(1), dim3(256), 0, sR, n->d_rem_ctr, (unsigned long long)n->cfg.rem_seed,
+                               n->rem_k, n->d_rem_alpha, ktrace_slot("rem_alpha")));
+      B2_PROF("rem_alpha", sR);
+      return B200DQN_OK;
+    }));
   }
   B2_TRY(forward(n, fs, nets, rows, st, td, join));
   return backward_and_update(n, fs, rows, st, true);
@@ -3645,8 +3596,7 @@ extern "C" int b200dqn_net_destroy(b200dqn_net* n) {
   comm_destroy(n);
   umma_net_destroy(n);
   destroy_step_graphs(n);
-  if (n->graph_train_exec) cudaGraphExecDestroy(n->graph_train_exec);
-  if (n->graph_predict_exec) cudaGraphExecDestroy(n->graph_predict_exec);
+  n->graph_predict.drop();
   for (auto& sd : n->side) if (sd) cudaStreamDestroy(sd);
   for (auto& e : n->ev) if (e) cudaEventDestroy(e);
   if (n->d_tw != n->d_w) { cudaFree(n->d_tw); cudaFree(n->d_ts); }
@@ -3874,6 +3824,23 @@ extern "C" int b200dqn_net_soft_update_target(b200dqn_net* n, double tau, void* 
   return soft_update_extra(n, c, t, st);
 }
 
+// Captures what enqueue() puts on key.stream into a CUDA graph held by c, unless c already holds one captured at key.
+template <class F>
+static int graph_cached(GraphCache& c, const GraphKey& key, F&& enqueue) {
+  if (c.exec && c.key == key) return B200DQN_OK;
+  c.drop();
+  cudaGraph_t graph = nullptr;
+  B2_CHECK_CUDA(cudaStreamBeginCapture(key.stream, cudaStreamCaptureModeThreadLocal));
+  const int rc = enqueue();
+  cudaError_t e = cudaStreamEndCapture(key.stream, &graph);
+  if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
+  B2_CHECK_CUDA(e);
+  B2_CHECK_CUDA(cudaGraphInstantiate(&c.exec, graph, 0));
+  cudaGraphDestroy(graph);
+  c.key = key;
+  return B200DQN_OK;
+}
+
 extern "C" int b200dqn_net_predict_device(b200dqn_net* n, const uint8_t* dev_states, int live_rows, float* dev_q,
                                           void* stream) {
   B2_REQUIRE(n && dev_states && dev_q && live_rows >= 1 && live_rows <= n->nb, B200DQN_EINVAL,
@@ -3923,11 +3890,9 @@ extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* de
     B2_CHECK_CUDA(cudaStreamSynchronize(st));
     return B200DQN_OK;
   }
-  if (!n->graph_predict_exec || n->graph_predict_states != dev_states || n->graph_predict_rows != live_rows ||
-      n->graph_predict_stream != st) {
-    if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  GraphKey key;
+  key.src = dev_states; key.rows = live_rows; key.stream = st;
+  B2_TRY(graph_cached(n->graph_predict, key, [&] {
     FrameSource fs{{dev_states, dev_states}, {n->d_iota4, n->d_iota4}, {0, 0}};
     HeadTrainArgs no_td{};
     int rc = forward(n, fs, 1, live_rows, st, no_td);
@@ -3935,14 +3900,9 @@ extern "C" int b200dqn_net_predict_device_host(b200dqn_net* n, const uint8_t* de
       k_publish_q_counter<<<1, 64, 0, st>>>(n->d_q[0], count, n->h_res, n->d_optscal_u32());
       if (cudaGetLastError() != cudaSuccess) rc = B200DQN_ECUDA;
     }
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    B2_CHECK_CUDA(e);
-    B2_CHECK_CUDA(cudaGraphInstantiate(&n->graph_predict_exec, graph, 0));
-    cudaGraphDestroy(graph);
-    n->graph_predict_states = dev_states; n->graph_predict_rows = live_rows; n->graph_predict_stream = st;
-  }
-  B2_CHECK_CUDA(cudaGraphLaunch(n->graph_predict_exec, st));
+    return rc;
+  }));
+  B2_CHECK_CUDA(cudaGraphLaunch(n->graph_predict.exec, st));
   n->predicts_launched += 1;
   int rc = poll_mapped_seq(n->h_res + 2, n->predicts_launched, st, "predict result");
   if (rc) return rc;
@@ -4057,29 +4017,20 @@ static int train_on_ring(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   return rc;
 }
 
+// what a step graph on ring r and stream st is captured at
+static GraphKey step_graph_key(const b200dqn_net* n, const b200dqn_replay* r, cudaStream_t st) {
+  GraphKey k;
+  k.src = r; k.serial = r->serial; k.stream = st; k.world = n->world; k.trace_gen = g_ktrace_gen;
+  k.per_gen = r->per_gen; k.nstep = r->nstep;
+  return k;
+}
+
 // train_on_ring through a cached CUDA graph (the sampler is NOT part of it: the indexes are already in r)
 static int train_sampled_launch(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (!use_graph) return train_on_ring(n, r, st);
-  if (!n->graph_train_exec || n->graph_train_replay != r || n->graph_train_replay_serial != r->serial ||
-      n->graph_train_stream != st || n->graph_train_world != n->world || n->graph_train_gen != g_ktrace_gen ||
-      n->graph_train_per_gen != r->per_gen || n->graph_train_nstep != r->nstep) {
-    if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-    int rc = train_on_ring(n, r, st);
-    cudaError_t e = cudaStreamEndCapture(st, &graph);
-    if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-    B2_CHECK_CUDA(e);
-    B2_CHECK_CUDA(cudaGraphInstantiate(&n->graph_train_exec, graph, 0));
-    cudaGraphDestroy(graph);
-    n->graph_train_replay = r; n->graph_train_stream = st; n->graph_train_world = n->world;
-    n->graph_train_replay_serial = r->serial;
-    n->graph_train_gen = g_ktrace_gen;
-    n->graph_train_per_gen = r->per_gen;
-    n->graph_train_nstep = r->nstep;
-  }
-  B2_CHECK_CUDA(cudaGraphLaunch(n->graph_train_exec, st));
+  B2_TRY(graph_cached(n->graph_train, step_graph_key(n, r, st), [&] { return train_on_ring(n, r, st); }));
+  B2_CHECK_CUDA(cudaGraphLaunch(n->graph_train.exec, st));
   return B200DQN_OK;
 }
 
@@ -4114,6 +4065,20 @@ extern "C" int b200dqn_net_train_sampled_cost(b200dqn_net* n, b200dqn_replay* r,
   return wait_step_cost(n, as_stream(stream), uint32_t(n->train_iterations), host_cost);
 }
 
+// The head of a fused step: the trace tick, the random-shift draw's fork and the sampler.  The sampler must not start
+// ahead of the tick.
+static int sample_step_head(b200dqn_net* n, b200dqn_replay* r, cudaStream_t st) {
+  auto head = [&] {
+    int rc = shift_fork(n, st);
+    if (!rc) rc = launch_sample(r, st);
+    if (rc) n->crop_forked = false;
+    return rc;
+  };
+  if (!ktrace_tick(st)) return head();
+  NoPdlScope after_tick;
+  return head();
+}
+
 extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int nsteps, void* stream) {
   B2_REQUIRE(n && r && nsteps >= 1, B200DQN_EINVAL, "net_train_fused: bad argument");
   int rc = check_fusable(n, r);
@@ -4128,45 +4093,18 @@ extern "C" int b200dqn_net_train_fused(b200dqn_net* n, b200dqn_replay* r, int ns
   // and replayed: one graph launch per step instead of ~17 stream operations.
   const bool use_graph = n->use_graph && !g_prof_on && st != nullptr;
   if (use_graph) {
-    if (n->graph_replay != r || n->graph_replay_serial != r->serial || n->graph_stream != st ||
-        n->graph_world != n->world || n->graph_trace_gen != g_ktrace_gen || n->graph_per_gen != r->per_gen ||
-        n->graph_nstep != r->nstep) {
-      destroy_step_graphs(n);
-      n->graph_replay = r; n->graph_stream = st; n->graph_world = n->world; n->graph_trace_gen = g_ktrace_gen;
-      n->graph_replay_serial = r->serial;
-      n->graph_per_gen = r->per_gen;
-      n->graph_nstep = r->nstep;
-    }
-    if (!n->graph_exec) {
-      cudaGraph_t graph = nullptr;
-      B2_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+    B2_TRY(graph_cached(n->graph_step, step_graph_key(n, r, st), [&] {
       const long long launches_before = g_launch_count;
-      {
-        const bool prev = g_pdl_suppressed;
-        if (ktrace_tick(st)) g_pdl_suppressed = true;   // the sampler must not start ahead of the tick
-        rc = shift_fork(n, st);
-        if (!rc) rc = launch_sample(r, st);
-        g_pdl_suppressed = prev;
-      }
+      int rc = sample_step_head(n, r, st);
       if (!rc) rc = train_on_ring(n, r, st);
-      n->crop_forked = false;
       n->graph_launches = int(g_launch_count - launches_before);
-      cudaError_t e = cudaStreamEndCapture(st, &graph);
-      if (rc) { if (graph) cudaGraphDestroy(graph); return rc; }
-      B2_CHECK_CUDA(e);
-      B2_CHECK_CUDA(cudaGraphInstantiate(&n->graph_exec, graph, 0));
-      cudaGraphDestroy(graph);
-    }
-    for (int i = 0; i < nsteps; ++i) B2_CHECK_CUDA(cudaGraphLaunch(n->graph_exec, st));
+      return rc;
+    }));
+    for (int i = 0; i < nsteps; ++i) B2_CHECK_CUDA(cudaGraphLaunch(n->graph_step.exec, st));
   } else {
     for (int i = 0; i < nsteps; ++i) {
-      const bool prev = g_pdl_suppressed;
-      if (ktrace_tick(st)) g_pdl_suppressed = true;
-      rc = shift_fork(n, st);
-      if (!rc) rc = launch_sample(r, st);
-      g_pdl_suppressed = prev;
-      if (rc) { n->crop_forked = false; return rc; }
-      if ((rc = train_on_ring(n, r, st))) return rc;
+      B2_TRY(sample_step_head(n, r, st));
+      B2_TRY(train_on_ring(n, r, st));
     }
   }
   n->train_iterations += nsteps;
@@ -4427,7 +4365,6 @@ extern "C" int b200dqn_net_set_keep_grads(b200dqn_net* n, int keep) {
   B2_REQUIRE(n, B200DQN_EINVAL, "null net");
   n->keep_grads = keep != 0;
   destroy_step_graphs(n);   // parameters are baked in
-  if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
   return B200DQN_OK;
 }
 
@@ -4443,7 +4380,7 @@ static int double_q_alloc(b200dqn_net* n) {
   B2_CHECK_CUDA(cudaMemset(part, 0, size_t(3) * kFc1Splits * nb * n->hidden * sizeof(float)));
   cudaFree(n->d_fc1part);
   n->d_fc1part = part;
-  if (n->graph_predict_exec) { cudaGraphExecDestroy(n->graph_predict_exec); n->graph_predict_exec = nullptr; }
+  n->graph_predict.drop();
   if (n->cfg.math_mode == B200DQN_MATH_TCGEN05) {
     int rc = umma_double_q_alloc(n);
     if (rc) return rc;
@@ -4472,7 +4409,6 @@ extern "C" int b200dqn_net_set_double_q(b200dqn_net* n, int on) {
   }
   n->double_q = on != 0;
   destroy_step_graphs(n);   // the number of network slots is baked in
-  if (n->graph_train_exec) { cudaGraphExecDestroy(n->graph_train_exec); n->graph_train_exec = nullptr; }
   return B200DQN_OK;
 }
 

@@ -31,6 +31,29 @@ struct LayerTable {
   int splits[kLayers];
 };
 
+// What a captured CUDA graph was captured at: a step graph at a ring, a predict graph at a state window and row count.
+// A graph is stale as soon as one field differs.
+struct GraphKey {
+  const void* src = nullptr;   // the ring (a step) or the device-resident state window (predict)
+  uint64_t serial = 0;         // b200dqn_replay::serial: the pointer alone can name a newer ring
+  cudaStream_t stream = nullptr;
+  int world = 0, trace_gen = 0, rows = 0;
+  uint32_t per_gen = 0;        // b200dqn_replay::per_gen
+  int nstep = 1;               // b200dqn_replay::nstep
+  bool operator==(const GraphKey& o) const {
+    return src == o.src && serial == o.serial && stream == o.stream && world == o.world && trace_gen == o.trace_gen &&
+           rows == o.rows && per_gen == o.per_gen && nstep == o.nstep;
+  }
+};
+
+struct GraphCache {
+  cudaGraphExec_t exec = nullptr;
+  GraphKey key{};
+  void drop() {
+    if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
+  }
+};
+
 }  // namespace b200
 
 struct b200dqn_net {
@@ -70,10 +93,7 @@ struct b200dqn_net {
   // [64 ..) Q rows of the last fast-path predict (k_publish_q)
   volatile uint32_t* h_res = nullptr;
   uint32_t predicts_launched = 0;
-  cudaGraphExec_t graph_predict_exec = nullptr;   // forward on a device-resident state window + result publish
-  const uint8_t* graph_predict_states = nullptr;
-  int graph_predict_rows = 0;
-  cudaStream_t graph_predict_stream = nullptr;
+  b200::GraphCache graph_predict;   // forward on a device-resident state window + result publish
   b200dqn_replay* step_replay = nullptr;   // set while a step that samples from a ring is being enqueued / captured
 
   // unfused-mode staging (host minibatch -> device)
@@ -95,20 +115,9 @@ struct b200dqn_net {
   bool keep_grads = false;   // tensor-core dgrads also write the fp32 dZ3/dZ2/dZ1 (tests)
   bool double_q = false;     // Double DQN target: the online net picks the poststate action, the target net values it
   bool double_q_alloc = false;   // the third network slot's buffers exist
-  cudaGraphExec_t graph_exec = nullptr;
-  b200dqn_replay* graph_replay = nullptr;
-  cudaStream_t graph_stream = nullptr;
-  int graph_world = 0;
-  int graph_trace_gen = 0;
-  int graph_launches = 0;   // kernels launched by one captured step
-  cudaGraphExec_t graph_train_exec = nullptr;   // same step without the sampler (train on pre-sampled indexes)
-  b200dqn_replay* graph_train_replay = nullptr;
-  cudaStream_t graph_train_stream = nullptr;
-  int graph_train_world = 0, graph_train_gen = 0;
-  uint32_t graph_per_gen = 0, graph_train_per_gen = 0;   // b200dqn_replay::per_gen the step graphs were captured at
-  // b200dqn_replay::serial of the ring the step graphs were captured on: the pointer alone can name a newer ring
-  uint64_t graph_replay_serial = 0, graph_train_replay_serial = 0;
-  int graph_nstep = 1, graph_train_nstep = 1;   // b200dqn_replay::nstep the step graphs were captured at
+  b200::GraphCache graph_step;    // the fused step (sampler + train step)
+  int graph_launches = 0;         // kernels launched by one captured fused step
+  b200::GraphCache graph_train;   // same step without the sampler (train on pre-sampled indexes)
   int ring_nstep = 1;   // n-step length of the ring this net last trained from (comm_init refuses N > 1)
   float* d_td_err = nullptr;   // [nb] TD errors before the clip (prioritized replay; allocated at its first step)
 
